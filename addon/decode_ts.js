@@ -1,5 +1,5 @@
 // Node harness: decode an MPEG-TS file through the reference's OWN demuxer and interfaces with the
-// B200 decoder plugged in where the WASM decoder would be.  NOT RUN IN THIS REPOSITORY'S IMAGE (no
+// CUDA decoder plugged in where the WASM decoder would be.  NOT RUN IN THIS REPOSITORY'S IMAGE (no
 // Node); the Python twin of this script is what the tests execute (INTEGRATION.md).
 //
 //   node addon/decode_ts.js /path/to/jsmpeg/src clip.ts

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- MPEG-1 video decode throughput (frames/s, Gpix/s) on N B200s vs the reference on host cores.
+"""bench.py -- MPEG-1 video decode throughput (frames/s, Gpix/s) on N H100s vs the reference on host cores.
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA, through the C ABI)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's own C on the host cores
@@ -22,8 +22,9 @@ reconstruction (stage 2).
          to the CPUs of its GPU's NUMA node first (pinned rings are then node-local).
   verified  after the timed region the LAST picture of every stream of the rank (60 pictures deep into
          the P chains) is read back and its FNV-1a hash compared with the unmodified reference C
-         (oracle/_ref) decoding the same stream on the host; the run FAILS (exit 1) on any difference
-         or if any picture fell back from the lane-parallel walk.
+         (oracle/_ref, where it was built) or else the oracle (oracle/liboracle.so, the CPU restatement the
+         tests pin to the reference) decoding the same stream on the host; the run FAILS (exit 1) on any
+         difference or if any picture fell back from the lane-parallel walk.
   roofline  stage-2 kernel: algorithmic bytes (DESIGN.md) / CUDA-event time of its launches on the
          stream they run on; in the value leg nothing else runs beside them.
   cpu_baseline  oracle/_ref (the unmodified reference C, compiled in place) on the host cores this
@@ -39,6 +40,11 @@ Timing: wall clock between torch.cuda.synchronize() + barrier on both sides of e
 (every step ends host-synchronised), max over ranks; per-kernel times are CUDA events recorded on
 the launching stream inside the library.  Inputs are much larger than L2 (ES ~0.8 GB, records
 ~20 GB per step), so no explicit L2 flush is needed.
+
+  --dump-outputs DIR  after the timed steps, what the value leg's last step left in HBM (the planes a
+         caller receives) as float32 .npy files: the last picture of stream 0 whole (y/cr/cb_stream0),
+         a fixed seeded sample of the last picture of every stream (y/cr/cb_sample, one row per stream),
+         and the FNV-1a 64 of every stream's last picture split in 32-bit halves (last_picture_fnv1a64).
 """
 from __future__ import annotations
 
@@ -132,7 +138,7 @@ def rank_seeds(rank, n=None):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks, power and throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -194,7 +200,7 @@ def measured_peak():
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def recorded_traffic():
@@ -210,24 +216,47 @@ def recorded_traffic():
 # the reference on the host: reference arm / cpu baseline / checker
 
 REF_LIB = os.path.join(ROOT, "oracle", "_ref", "libjsmpeg_ref.so")
+ORACLE_LIB = os.path.join(ROOT, "oracle", "liboracle.so")
 _ref = None
+_oracle = None
+
+
+def _harness(path):
+    """ctypes handle on a library that carries our pthread harness oracle/ref_bench.c."""
+    lib = ctypes.CDLL(path, mode=os.RTLD_LOCAL | os.RTLD_NOW)
+    lib.ref_bench_run.restype = ctypes.c_long
+    lib.ref_bench_run.argtypes = [ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_uint), ctypes.c_int,
+                                  ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_double)]
+    lib.ref_picture_hashes.restype = ctypes.c_long
+    lib.ref_picture_hashes.argtypes = [ctypes.c_char_p, ctypes.c_uint, ctypes.POINTER(ctypes.c_uint64), ctypes.c_long]
+    lib.ref_hash_bytes.restype = ctypes.c_uint64
+    lib.ref_hash_bytes.argtypes = [ctypes.c_uint64, ctypes.c_void_p, ctypes.c_size_t]
+    return lib
 
 
 def ref_library():
-    """oracle/_ref/libjsmpeg_ref.so: the unmodified reference C (built from /root/reference/src/wasm/*.c
-    in the build container; travels with the tree) + our pthread harness oracle/ref_bench.c."""
+    """oracle/_ref/libjsmpeg_ref.so: the unmodified reference C (compiled by oracle/Makefile where the
+    reference tree is present) + our pthread harness oracle/ref_bench.c; None where it was not built."""
     global _ref
     if _ref is None and os.path.exists(REF_LIB):
-        lib = ctypes.CDLL(REF_LIB, mode=os.RTLD_LOCAL | os.RTLD_NOW)
-        lib.ref_bench_run.restype = ctypes.c_long
-        lib.ref_bench_run.argtypes = [ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_uint), ctypes.c_int,
-                                      ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_double)]
-        lib.ref_picture_hashes.restype = ctypes.c_long
-        lib.ref_picture_hashes.argtypes = [ctypes.c_char_p, ctypes.c_uint, ctypes.POINTER(ctypes.c_uint64), ctypes.c_long]
-        lib.ref_hash_bytes.restype = ctypes.c_uint64
-        lib.ref_hash_bytes.argtypes = [ctypes.c_uint64, ctypes.c_void_p, ctypes.c_size_t]
-        _ref = lib
+        _ref = _harness(REF_LIB)
     return _ref
+
+
+def oracle_library():
+    """oracle/liboracle.so: the oracle with the same harness linked in (always built by build())."""
+    global _oracle
+    if _oracle is None:
+        if not os.path.exists(ORACLE_LIB):
+            subprocess.check_call(["make", "-s", "-C", os.path.join(ROOT, "oracle")])
+        _oracle = _harness(ORACLE_LIB)
+    return _oracle
+
+
+def checker_library():
+    """What the GPU output is held against: the compiled reference where it exists, else the oracle."""
+    lib = ref_library()
+    return (lib, "oracle/_ref (unmodified reference C)") if lib is not None else (oracle_library(), "oracle/liboracle.so (oracle)")
 
 
 def run_reference_cpu(clips, threads, loops):
@@ -270,10 +299,8 @@ def run_reference_cpu(clips, threads, loops):
 
 
 def reference_last_hashes(clips, workers):
-    """hash of the LAST picture of each clip, decoded by the reference on `workers` host threads."""
-    lib = ref_library()
-    if lib is None:
-        return None
+    """hash of the LAST picture of each clip, decoded by the checker on `workers` host threads."""
+    lib, _ = checker_library()
     out = [None] * len(clips)
 
     def work(k):
@@ -293,7 +320,7 @@ def reference_last_hashes(clips, workers):
 def fnv1a64_planes(y, cr, cb):
     """FNV-1a 64 of Y | Cr | Cb exactly as oracle/ref_bench.c computes it (the hash is inherently serial;
     Python ints would take seconds per picture, so the byte loop runs in the same C: ref_hash_bytes)."""
-    lib = ref_library()
+    lib = oracle_library()
     h = 1469598103934665603
     for a in (y, cr, cb):
         h = lib.ref_hash_bytes(h, a.ctypes.data, a.size)
@@ -425,8 +452,7 @@ class Legs:
     def verify(self, seeds, workers):
         """The last picture of every stream, as the value leg left it in HBM, against the reference's
         decode of the same stream (FNV-1a 64 over Y | Cr | Cb).  Returns a dict for the JSON line."""
-        if ref_library() is None:
-            return {"verified": None, "why": "oracle/_ref not built on this box"}
+        _, checker = checker_library()
         # distinct clips only once on the host
         uniq = {}
         for i, s in enumerate(seeds):
@@ -443,7 +469,25 @@ class Legs:
                 if n_ref != PICTURES or fnv1a64_planes(y, cr, cb) != h_ref:
                     bad.append(i)
         return {"verified": not bad, "streams_checked": checked, "pictures_deep": PICTURES, "mismatching_streams": bad[:16],
-                "checker": "oracle/_ref (unmodified reference C) on the host, FNV-1a 64 of Y|Cr|Cb of each stream's last picture"}
+                "checker": f"{checker} on the host, FNV-1a 64 of Y|Cr|Cb of each stream's last picture"}
+
+    def dump_outputs(self, out_dir, seed=20240, sample=65536):
+        """The last picture of every stream as the value leg left it in HBM (see --dump-outputs)."""
+        import numpy as np
+        os.makedirs(out_dir, exist_ok=True)
+        planes = [None] * len(self.streams)
+        for dec, g in zip(self.value_decoders, self.vgroups):
+            for j, i in enumerate(g):
+                planes[i] = [np.ascontiguousarray(p).reshape(-1) for p in dec.read_planes(j)]
+        rng = np.random.default_rng(seed)
+        idx_y = np.sort(rng.choice(planes[0][0].size, min(sample, planes[0][0].size), replace=False))
+        idx_c = np.sort(rng.choice(planes[0][1].size, min(sample // 4, planes[0][1].size), replace=False))
+        for k, name in enumerate(("y", "cr", "cb")):
+            np.save(os.path.join(out_dir, f"{name}_stream0.npy"), planes[0][k].astype(np.float32))
+            idx = idx_y if k == 0 else idx_c
+            np.save(os.path.join(out_dir, f"{name}_sample.npy"), np.stack([p[k][idx] for p in planes]).astype(np.float32))
+        h = np.array([fnv1a64_planes(*p) for p in planes], dtype=np.uint64)
+        np.save(os.path.join(out_dir, "last_picture_fnv1a64.npy"), np.stack([h >> np.uint64(32), h & np.uint64(0xFFFFFFFF)], 1).astype(np.float64))
 
 
 def roofline_block(st, peak, peak_src, traffic):
@@ -553,6 +597,7 @@ def main():
     ap.add_argument("--no-e2e", action="store_true", help="value leg only (used for the ncu launch list)")
     ap.add_argument("--no-extras", action="store_true", help="skip config_720p / single_stream_1080p")
     ap.add_argument("--no-verify", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the value leg's last-step output as .npy files (rank 0)")
     args = ap.parse_args()
 
     rank = env_int("RANK", 0)
@@ -566,7 +611,7 @@ def main():
                     f"(BASELINE configs[3]; weak-scaled x N GPUs = configs[4]), GOP 12, one slice per picture",
         "streams_per_gpu": STREAMS_PER_GPU, "pictures_per_stream": PICTURES, "distinct_clips_per_gpu": DISTINCT,
         "parallelism": f"streams sharded {STREAMS_PER_GPU} per GPU, no collective",
-        "l2": "inputs larger than L2 (ES + records per step >> 126 MB); no explicit flush",
+        "l2": "inputs larger than L2 (ES + records per step >> 50 MB); no explicit flush",
     }
 
     if args.impl == "reference":
@@ -628,6 +673,8 @@ def main():
     legs = Legs(streams, WIDTH, HEIGHT, local_rank, world, e2e_groups)
 
     frames, dt, st, clocks = legs.timed(legs.run_device, args.steps, args.warmup, legs.value_decoders)
+    if args.dump_outputs and rank == 0:
+        legs.dump_outputs(args.dump_outputs)
     verdict = {"verified": None, "why": "--no-verify"}
     if not args.no_verify:
         verdict = legs.verify(seeds, per_rank_cores)

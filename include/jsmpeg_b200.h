@@ -1,5 +1,5 @@
 /*
- * jsmpeg_b200.h -- C ABI of libjsmpeg_b200.so: a B200 (sm_100a CUDA) implementation of jsmpeg's
+ * jsmpeg_b200.h -- C ABI of libjsmpeg_b200.so: an H100 (sm_90a CUDA) implementation of jsmpeg's
  * MPEG-1 video decode path.  Plain pointers and sizes only.
  *
  * Part 1 is EXACTLY the ABI the reference's own native plugin boundary binds -- the 15 functions

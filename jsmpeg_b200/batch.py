@@ -75,7 +75,7 @@ def bind_batch_abi(lib):
 
 
 class BatchDecoder:
-    """``n_streams`` independent MPEG-1 video decoders on one B200."""
+    """``n_streams`` independent MPEG-1 video decoders on one GPU."""
 
     def __init__(self, n_streams, device=0, max_slots=0, lib=None, chunk_pictures=None, decode_b=None, slice_walk=None):
         from . import capi

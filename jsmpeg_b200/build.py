@@ -1,4 +1,4 @@
-"""Build libjsmpeg_b200.so (hand-written CUDA for sm_100a + the C ABI) in-tree with nvcc.
+"""Build libjsmpeg_b200.so (hand-written CUDA for sm_90a, H100 + the C ABI) in-tree with nvcc.
 
     python -m jsmpeg_b200.build
 
@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["engine.cu", "parse.cu", "recon.cu", "scan.cu", "tsdemux.cu"]
 OUT = os.path.join(HERE, "libjsmpeg_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def nvcc_path():

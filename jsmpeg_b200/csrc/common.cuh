@@ -1,4 +1,4 @@
-// common.cuh -- task descriptors shared by the kernels and the host engine (sm_100a only).
+// common.cuh -- task descriptors shared by the kernels and the host engine (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -25,8 +25,8 @@
 // followed by the read-back of its picture infos.  The host then takes chunk after chunk: waits for
 // that chunk's infos only, does the acceptance above, and queues the chunk's reconstruct launches on
 // a SECOND stream -- while the parse of the following chunks is running.  Stage 1 (latency-bound, few
-// resident warps) and stage 2 (bandwidth / issue-bound) are natural co-runners; round 1 serialised
-// them with a host synchronisation between the parse wave and the first reconstruct launch.
+// resident warps) and stage 2 (bandwidth / issue-bound) are natural co-runners in principle; without
+// the option the parse wave and the first reconstruct launch are separated by a host synchronisation.
 #include <sched.h>
 
 #include <algorithm>
@@ -1015,7 +1015,7 @@ int env_int(const char *name, int fallback) {
 
 extern "C" {
 
-const char *jsmpeg_b200_version(void) { return "jsmpeg_b200 0.2 (sm_100a)"; }
+const char *jsmpeg_b200_version(void) { return "jsmpeg_b200 0.2 (sm_90a)"; }
 
 jsmpeg_b200_batch_t *jsmpeg_b200_batch_create(int n_streams, int device, unsigned int max_slots) {
 	Batch *b = new Batch();
@@ -1312,8 +1312,7 @@ struct mpeg1_decoder_t {
 
 // Host placement.  The pinned bit buffers and plane rings of a decoder are touched by the host threads
 // that drive it and by the GPU's copy engines; on a two-socket host a GPU hangs off ONE socket, and a
-// ring on the other socket costs every D2H byte a trip over the socket interconnect (round 1: the
-// 8-GPU e2e curve went flat at 4 GPUs).  This binds the CALLING THREAD -- and with it the threads it
+// ring on the other socket costs every D2H byte a trip over the socket interconnect.  This binds the CALLING THREAD -- and with it the threads it
 // creates and the pages it first touches from now on -- to the CPUs of the NUMA node of `device`
 // (sysfs: /sys/bus/pci/devices/<id>/numa_node, /sys/devices/system/node/node<k>/cpulist), intersected
 // with the affinity it already has.  Returns the number of CPUs bound to, 0 if the node is unknown

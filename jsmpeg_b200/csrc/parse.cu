@@ -1,4 +1,4 @@
-// parse.cu -- stage 1: bitstream / VLC parse (sm_100a), in two kernels.
+// parse.cu -- stage 1: bitstream / VLC parse (sm_90a), in two kernels.
 //
 // Replaces, for the bitstream half, the reference's decodePicture / decodeSlice / decodeMacroblock /
 // decodeMotionVectors / decodeBlock (src/mpeg1.js:174-457, 698-811) and its bit reader
@@ -48,10 +48,11 @@ constexpr uint32_t EXPAND_SMEM = EXP_OFF_TILES + CTA_THREADS * TILE_PITCH;
 // 1a: one warp per picture (walk.cuh), serial or lane-parallel with serial fall-back
 
 // the serial walk keeps the allocation it was tuned with (63 registers, no occupancy hint); the
-// lane-parallel walk is held to 64 registers = 4 resident CTAs per SM (measured: 46.4 ms per step
-// against 47.9 ms with the 80 registers it takes unbounded)
+// lane-parallel walk asks for 3 resident CTAs per SM.  Measured on an H100 (64 x 1080p x 60 pictures,
+// tools/time_stages.py, two interleaved runs): walk 16.0 / 15.2 ms and step 49.6 / 51.0 ms with 3,
+// against walk 19.6 / 19.7 ms and step 51.0 / 51.7 ms with 4 and walk 23.0 / 23.0 ms with 5.
 #ifndef JSMPEG_LANES_MIN_CTAS
-#define JSMPEG_LANES_MIN_CTAS 4
+#define JSMPEG_LANES_MIN_CTAS 3
 #endif
 #define LANES_BOUNDS __launch_bounds__(WALK_THREADS, JSMPEG_LANES_MIN_CTAS)
 #define WALK_KERNEL(NAME, LANES, BOUNDS)                                                                          \
@@ -100,10 +101,10 @@ walk_pictures_slices_kernel(const ParseTask *__restrict__ tasks, int n_tasks, co
 // A CTA stages the tables once and then takes EXPAND_GROUPS runs of CTA_THREADS consecutive slots, one after
 // the other: the warps go through their runs independently (tiles are per thread, the tables read-only, so
 // the one barrier is the one after staging), and a thread asks for the next run's inputs before it expands
-// the current block -- the staging, the barrier and the exposed load latency at the start of a CTA were a
-// fifth of the kernel's stall samples when every CTA did one run (profiles/r2_expand.md).
+// the current block -- the staging, the barrier and the exposed load latency at the start of a CTA are paid
+// once per EXPAND_GROUPS runs.
 #ifndef JSMPEG_EXPAND_GROUPS
-#define JSMPEG_EXPAND_GROUPS 4  // measured: 1 -> 4: 8.2 -> 7.5 ms; 8: the same
+#define JSMPEG_EXPAND_GROUPS 4  // H100, step per 64 x 1080p x 60: 1 run 51.6 / 51.6 ms, 4 runs 51.0 / 51.7, 8 runs 51.9 / 52.2
 #endif
 constexpr int EXPAND_GROUPS = JSMPEG_EXPAND_GROUPS;
 
@@ -187,8 +188,8 @@ static const uint16_t *ms_table_for_current_device() {
 	return d;
 }
 
-// JSMPEG_B200_PARSE_GROUPS=1 keeps stage 1 on one stream (used for the ncu launch list: ncu
-// serialises concurrent kernels, so only the unforked run has comparable shares)
+// JSMPEG_B200_PARSE_GROUPS=1 keeps stage 1 on one stream (a profiler that serialises concurrent
+// kernels gives comparable per-kernel shares only for the unforked run)
 static int max_parse_groups() {
 	static const int max_groups = [] {
 		const char *e = getenv("JSMPEG_B200_PARSE_GROUPS");
@@ -219,8 +220,8 @@ void launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size,
 	const int groups = parse_group_count(n_tasks, fork != nullptr);
 	if (groups > 1) CUDA_CHECK(cudaEventRecord(fork->fork, stream));
 	for (int g = 0; g < groups; g++) {
-		// equal groups; measured on the 3840-picture wave: unforked 59.8 ms, 4 groups 52.4, 8 groups 50.5,
-		// 16 groups 80.8 (too many concurrent kernels), a small first group 55.0
+		// equal groups; on an H100 the 3840-picture wave takes the same time unforked, in 4 or in 8 groups
+		// (steps 50.8-52.5 ms, within the run-to-run spread)
 		const int lo = (int)((long)n_tasks * g / groups), hi = (int)((long)n_tasks * (g + 1) / groups);
 		const int n = hi - lo;
 		if (n <= 0) continue;

@@ -37,6 +37,8 @@
 
 namespace {
 
+// H100, 60 launches per 64 x 1080p x 60 step: 20.9 ms with 5 resident CTAs per SM, 21.8 ms with 4, 25.8 ms
+// with 6 (register cap too low)
 #ifndef JSMPEG_RECON_MIN_CTAS
 #define JSMPEG_RECON_MIN_CTAS 5
 #endif

@@ -1,4 +1,4 @@
-// recon.cuh -- stage 2 device code: one 8x8 block = one thread (sm_100a).
+// recon.cuh -- stage 2 device code: one 8x8 block = one thread (sm_90a).
 //
 // Included by recon.cu (kernel shell + launcher).  Like walk.cuh the same text compiles for the host
 // when JSMPEG_WALK_EMU is defined (tests/emu/walk_emu.cpp): the TMA copy and the packed-saturate /
@@ -294,13 +294,12 @@ static inline uint32_t smem_u32(const void *) { return 0; }
 // staging area (one WARP_STAGE per warp), tid = the thread's index in the CTA.
 // WARP-CONVERGENT: the 32 lanes of a warp call it together (collectives inside).
 //
-// Latency plan (round 2; the kernel was stalled on memory it asked for too late -- long-scoreboard 2.7
-// warps per issue at 4.5 resident warps per scheduler, profiles/r2_reconstruct.md):
+// Latency plan (the kernel was stalled on memory it asked for too late):
 //   t0  the header load starts;  the header and the coefficient record of the CTA that will run here two
 //       pictures of the launch later are pulled into L2
 //   t0' header there: the records of the coded blocks are requested (TMA).  (Requesting every slot's record
-//       before the header is known, for pictures with most blocks coded, was built and measured: 11.90 ms per
-//       60 launches against 11.92 -- nothing, for 3.5 % more DRAM traffic; removed.)
+//       before the header is known, for pictures with most blocks coded, gained nothing for more DRAM
+//       traffic; removed.)
 //   t1  header there: the nine reference rows of a predicted block are pulled into L2 (no registers)
 //   t2  records there: IDCT (some 700 instructions) -- the reference rows arrive meanwhile
 //   t3  prediction reads hit L2, + residual, store
@@ -327,8 +326,8 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		if (lane == 0) {
 			asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar));
 			// the initialised barrier must be visible to the async proxy (the TMA unit) before the copies name it:
-			// the proxy fence of the CUDA guide's single-CTA pattern.  (fence.mbarrier_init.release.cluster, used
-			// until round 2, is cluster-scoped: ptxas adds CCTL.IVALL to it, an invalidation of the SM's whole L1.)
+			// the proxy fence of the CUDA guide's single-CTA pattern.  (fence.mbarrier_init.release.cluster is
+			// cluster-scoped: ptxas adds CCTL.IVALL to it, an invalidation of the SM's whole L1.)
 			asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 			asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(128u * (uint32_t)__popc(copy_mask)) : "memory");
 		}
@@ -415,7 +414,7 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 	}
 	if (present && !intra && inside && (!BIDIR || use_f)) {  // t1: the reference rows, into L2, while the records travel and the IDCT runs
 		// (Sharing the rows out among the lanes -- lane l asks for row l & 7 of its own block, two instructions
-		// instead of nine -- was measured: 12.03 ms per 60 launches against 11.87, the neighbours' vectors differ too often.)
+		// instead of nine -- was slower: the neighbours' vectors differ too often.)
 #pragma unroll
 		for (int r = 0; r < 9; r++) prefetch_l2(splane + src + r * stride + 4);
 	}

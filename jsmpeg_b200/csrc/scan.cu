@@ -8,8 +8,8 @@
 // position list; the host sorts the (short) list, picks the picture start codes (fourth byte 00) out
 // of it and hands the whole list back to the device: knowing every picture start up front is what
 // lets stage 1 parse all buffered pictures concurrently, and knowing every prefix is what tells the
-// lane-parallel walk where a slice ends without reading the slice (round 1 and early round 2: a
-// 128-bytes-per-step search over every picture, 6 % of the walk's stall samples and 0.8 GB per step).
+// lane-parallel walk where a slice ends without reading the slice (instead of a 128-bytes-per-step
+// search over every picture's bytes once more).
 #include "common.cuh"
 
 namespace {

@@ -1,5 +1,5 @@
 // walk.cuh -- stage 1 device code: the walk of one picture's bitstream (1a) and the per-block expansion
-// (1b) (sm_100a).
+// (1b) (sm_90a).
 //
 // Included by parse.cu (the kernels, the tables' upload and the launcher live there).  The same text
 // compiles for the host when JSMPEG_WALK_EMU is defined and the including file supplies the few CUDA
@@ -7,10 +7,9 @@
 // lane-parallel walk is checked against the serial one, and both plus stage 1b against the oracle, on
 // machines without a GPU.  Nothing in the product library is built that way.
 //
-// (Three candidates written at the end of round 1 were measured on the B200 at the start of round 2 and
-// deleted: staged relative records + fix-up instead of the second semantic pass: walk 20.5 -> 18.6 ms
-// but stage 1 unchanged at 29.8 ms; the storing pass writing the block records itself, no stage 1b:
-// walk 29.6 ms, stage 1 45 ms; 16-byte register-cached refills: walk 22.9 ms.  profiles/r2_variants.md.)
+// (Three candidates were measured and deleted: staged relative records + fix-up instead of the second
+// semantic pass (a faster walk, the same stage 1); the storing pass writing the block records itself, no
+// stage 1b (slower stage 1); 16-byte register-cached refills (slower walk).)
 #pragma once
 #include "common.cuh"
 
@@ -87,11 +86,10 @@ static inline void sts_s16(uint32_t addr, int v) { const int16_t x = (int16_t)v;
 //
 // RING (the lane-parallel walk): the bytes reach the lane through its own 64-byte ring in shared memory,
 // filled by asynchronous 16-byte global -> shared copies (cp.async, SASS LDGSTS) issued three chunks
-// (48 bytes, some forty look-ups) ahead of the read position.  Round 1 refilled with one 4-byte global
-// load per lane, a single word ahead: with 1024 lanes per SM each on its own stream L1 thrashed (hit rate
-// 46 %) and the load's latency was the walk's top stall -- 35 % of all warp-stall samples sat on that
-// one instruction (profiles/r2_walk.md).  A 16-byte register cache per lane (loads still on demand) had
-// been measured slower; what was missing was distance, not width.
+// (48 bytes, some forty look-ups) ahead of the read position.  Refilling with one 4-byte global load per
+// lane, a single word ahead, left the load's latency exposed: with 1024 lanes per SM each on its own stream
+// L1 thrashes.  A 16-byte register cache per lane (loads still on demand) was slower too; what was missing
+// was distance, not width.
 // PADDED: the bytes behind the data are known to be zero (the product's ES mirror: ES_PAD zeroed bytes)
 // and no reader runs further than a few words past the end, so neither the test against len nor the mask
 // of the last word is needed.  (Host emulation: exact-size buffers under AddressSanitizer, so never.)
@@ -139,8 +137,8 @@ struct BitReaderT {
 	}
 #endif
 	// the next word of a sequential read (w only grows between seeks)
-	// (Measured and rejected in round 1 for the global-load refill: a branch-free variant relying on the zero
-	// pad after the data, 17 % slower; a software prefetch 256 B ahead at every refill, 7 % slower.)
+	// (Rejected for the global-load refill: a branch-free variant relying on the zero pad after the data, and a
+	// software prefetch 256 B ahead at every refill; both were slower.)
 	__device__ __forceinline__ uint32_t load_word(uint32_t w) {
 #if !defined(JSMPEG_WALK_EMU)
 		if (RING) {
@@ -294,9 +292,8 @@ __device__ __forceinline__ bool walk_block_head(BR &br, uint32_t sbase, PictureS
 		                             : lds_u16(sbase + OFF_DC_CHROMA + (w >> 24) * 2u);
 		const int len = e & 31, size = e >> 5;
 		if (len == 0) return false;
-		// (The pointer sends the three predictors to local memory, 5 % of the lane walk's stall samples sit on
-		// those loads.  Selects instead were measured: the state then competes for the 64 registers, spill
-		// instructions went from 12 M to 390 M per wave and the walk from 11.6 to 12.6 ms.)
+		// (The pointer sends the three predictors to local memory.  Selects instead were slower: the state then
+		// competes for the 64 registers and spills far more.)
 		int *pred = block < 4 ? &ps.dc_y : (block == 4 ? &ps.dc_b4 : &ps.dc_b5);
 		int dc = *pred;
 		if (DEFER) {  // code and differential (at most 8 + 8 bits) sit in the same 32-bit peek: the window moves once
@@ -339,8 +336,8 @@ __device__ __forceinline__ bool walk_block(BR &br, uint32_t sbase, PictureState 
 	if (!walk_block_head<false>(br, sbase, ps, intra, block, park, store, n, unused)) return false;
 	for (;;) {
 		const uint32_t w = br.peek32();
-		// (Resolving '10' / '11s' arithmetically before the look-up was measured 8 % SLOWER: it defeats the
-		// combining of several codes per look-up.)
+		// (Resolving '10' / '11s' arithmetically before the look-up was SLOWER: it defeats the combining of
+		// several codes per look-up.)
 		// as many complete codes as fit in the next 13 bits, in one look-up
 		const uint32_t m = lds_u16(sbase + OFF_MS + (w >> (32 - MS_BITS)) * 2u);
 		if (m & 15u) {
@@ -660,8 +657,8 @@ __device__ __forceinline__ uint32_t syn_guess(const SliceConst &sc) { return syn
 // automaton is written in the order of the syntax, one macroblock per trip of the outer loop and one
 // look-up per trip of the coefficient loop, and both loops are closed by a warp vote: the lanes run
 // the same stage at the same time.  (Left to themselves, lanes that leave a loop early never wait for
-// the others: measured on B200, the first version ran with 4 of 32 lanes active on average and its
-// per-lane macroblock loops with ONE.)
+// the others: the first version ran with 4 of 32 lanes active on average and its per-lane macroblock
+// loops with ONE.)
 template <class BR>
 __device__ void syntax_run(BR &br, uint32_t sbase, const SliceConst &sc, bool live, uint32_t limit, uint32_t &st) {
 	int ph = (int)(st & 15u);
@@ -1201,14 +1198,14 @@ __device__ void walk_picture(const ParseTask &t, uint32_t sbase, int lane, uint3
 // parked = {bit offset of the block's first coefficient code, intra dc * 8} from the walk's dense side
 // array, stile = the shared-memory address of this thread's (zeroed) 128-byte tile.
 //
-// The kernel is bound by the integer ALU pipe (87 % busy, profiles/r2_expand.md), so the loop is built to need
+// The kernel is bound by the integer ALU pipe, so the loop is built to need
 // few ALU instructions per code:
 //  * no bit window to maintain: the 32 bits at the current bit POSITION are two word loads (L1 hits: the
 //    blocks of a warp lie side by side in the stream) and one funnel shift -- the loads go to the LSU, the
 //    address to the FMA pipe; the window's shifts, counters and predicated refill were a quarter of the loop.
 //    (Keeping the three words around the position in registers and loading one word per crossing -- the
-//    load off the chain from code to code -- was measured: 8.2 ms against 7.9, the predicated register
-//    moves cost more than the L1 hits.)
+//    load off the chain from code to code -- was slower: the predicated register moves cost more than the
+//    L1 hits.)
 //  * the frequent codes (at most 8 bits) come from a table indexed by the next 8 bits (VLC_DCT_EXPAND_TOP8),
 //    no clz and no second shift; entries hold what a trip needs: bits to consume, run + 1, 2 * level
 //  * dequantisation in sign-magnitude form.  The reference (mpeg1.js:794-807): level <<= 1;
@@ -1297,7 +1294,7 @@ __device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, u
 	}
 	// The finished block leaves as ONE 128-byte TMA bulk store (shared -> global, SASS UBLKCP): whole
 	// lines reach L2, whereas eight 16-byte stores per thread half-fill 32-byte sectors and made L2
-	// read every sector back before merging (ncu: 23.5 GB read for 22 GB written per step).
+	// read every sector back before merging (about as many bytes read as written).
 #ifndef JSMPEG_WALK_EMU
 	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the copy engine
 	asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], 128;" ::"l"(slot), "r"(stile) : "memory");

@@ -1,4 +1,4 @@
-// walk_b.cuh -- stage 1a for B pictures (sm_100a): the opt-in extension, SURVEY 8(f) rank 4.
+// walk_b.cuh -- stage 1a for B pictures (sm_90a): the opt-in extension, SURVEY 8(f) rank 4.
 //
 // The reference skips B pictures (src/mpeg1.js:181-184) although it carries their macroblock-type table
 // (MACROBLOCK_TYPE_B, mpeg1.js:1152-1175 -> VLC_MBTYPE_B, pinned by tests/test_vlc_tables.py).  With the batch

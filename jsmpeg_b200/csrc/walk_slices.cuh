@@ -1,11 +1,11 @@
-// walk_slices.cuh -- stage 1a for pictures cut into many slices (sm_100a): one LANE per slice.
+// walk_slices.cuh -- stage 1a for pictures cut into many slices (sm_90a): one LANE per slice.
 //
 // The lane-parallel walk (walk.cuh) was built for what FFmpeg's mpeg1video encoder writes: ONE slice per picture,
 // whose bits it cuts into 32 sub-sequences that find each other by VLC self-synchronisation.  Streams from
 // encoders that start a slice in every macroblock row (the classic MPEG-1 layout: 45 slices of a few hundred
 // bytes in a 720p picture) defeat that: each slice is too short to cut, so the walk takes the slices one after
-// the other with one or two lanes busy -- measured on the B200: 17.5 ms for 320 such 720p pictures against 7 ms
-// for 3,840 one-slice pictures of the same size (profiles/r2_b_pictures.md).
+// the other with one or two lanes busy: such pictures took several times longer per picture than one-slice
+// pictures of the same size.
 //
 // But slices are the unit the syntax makes independent: every predictor is reset in the slice header
 // (src/mpeg1.js:255-266) and the address comes from the slice's start code.  So here lane i of the picture's warp

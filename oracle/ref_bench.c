@@ -1,8 +1,10 @@
 /*
  * oracle/ref_bench.c -- TEST/BENCH INFRASTRUCTURE ONLY (never linked into the product).
  *
- * A pthread harness around the UNMODIFIED reference decoder (reference src/wasm/mpeg1.c +
- * buffer.c, compiled in place by oracle/Makefile into oracle/_ref/libjsmpeg_ref.so).  It only
+ * A pthread harness around a decoder of the 15-function ABI: the UNMODIFIED reference decoder
+ * (reference src/wasm/mpeg1.c + buffer.c, compiled in place by oracle/Makefile into
+ * oracle/_ref/libjsmpeg_ref.so) and, built with ORACLE_ABI, the oracle (oracle/liboracle.so), so that
+ * the checker and the hash also exist where the reference tree is absent.  It only
  * uses the reference's public 15-function ABI (reference src/wasm/mpeg1.h:10-25), exactly the
  * way the reference's own glue does (src/mpeg1-wasm.js:52-70 write, :103 decode): one decoder
  * per elementary stream, whole stream written once (EXPAND mode), then decode() until it
@@ -14,7 +16,11 @@
 #include <stdlib.h>
 #include <string.h>
 #include <time.h>
+#ifdef ORACLE_ABI
+#include "../include/jsmpeg_b200.h"
+#else
 #include "mpeg1.h"
+#endif
 
 typedef struct {
 	const uint8_t *const *es;

@@ -3,15 +3,23 @@
 modes; every byte the protocol hands out is written, so AddressSanitizer aborts the process on any
 byte the returned pointer does not cover.  Where the REFERENCE's own arithmetic leaves enough room, the
 state (capacity, length, index) must equal that of the compiled reference's bit_buffer_* functions
-(oracle/_ref, src/wasm/buffer.c:48-71, 157-190).  Prints "bitbuffer ok: N writes" on success."""
+(oracle/_ref, src/wasm/buffer.c:48-71, 157-190), as stored in tests/golden/reference/bitbuffer.npy.
+Prints "bitbuffer ok: N writes" on success.
+
+    bitbuffer_check.py LIB GOLDEN.npy                 # compare with the stored reference states
+    bitbuffer_check.py LIB GOLDEN.npy --record REF    # run the compiled reference REF and store them"""
 import ctypes
-import os
 import sys
+import zlib
 
 import numpy as np
 
 lib = ctypes.CDLL(sys.argv[1])
-ref = ctypes.CDLL(sys.argv[2]) if len(sys.argv) > 2 and os.path.exists(sys.argv[2]) else None
+GOLDEN = sys.argv[2]
+ref = ctypes.CDLL(sys.argv[4]) if sys.argv[3:4] == ["--record"] else None
+# one row per write the reference is asked to mirror: trial, step, in domain after its get_write_ptr,
+# capacity, length, index, crc32 of its buffered bytes
+rows = [] if ref is not None else {(int(r[0]), int(r[1])): r for r in np.load(GOLDEN)}
 lib.bbt_create.restype = ctypes.c_void_p
 lib.bbt_create.argtypes = [ctypes.c_uint, ctypes.c_int]
 lib.bbt_destroy.argtypes = [ctypes.c_void_p]
@@ -88,7 +96,7 @@ for trial in range(300):
     cap = int(rng.integers(1, 4000))
     t = lib.bbt_create(cap, mode)
     r = ref.bit_buffer_create(cap, mode) if ref is not None else None
-    in_domain = r is not None
+    in_domain = True
     for step in range(int(rng.integers(1, 40))):
         n = int(rng.integers(0, 3000)) if rng.random() < 0.8 else int(rng.integers(0, 40))
         chunk = bytes(rng.integers(0, 256, n, dtype=np.uint8))
@@ -96,22 +104,31 @@ for trial in range(300):
         writes += 1
         cap_t, len_t, idx_t, _ = state(t)
         assert content(t).endswith(chunk) and len_t <= cap_t
-        if in_domain:
+        if in_domain and ref is not None:
             ref.bit_buffer_get_write_ptr(r, n)
             if r.contents.byte_capacity - r.contents.byte_length < n:
                 in_domain = False  # the reference would now write past its allocation: no parity defined from here on
+                rows.append((trial, step, 0, 0, 0, 0, 0))
             else:
                 ctypes.memmove(ctypes.addressof(r.contents.bytes.contents) + r.contents.byte_length, chunk, n)
                 ref.bit_buffer_did_write(r, n)
-                assert (cap_t, len_t, idx_t) == (r.contents.byte_capacity, r.contents.byte_length, r.contents.index), \
-                    (trial, step, (cap_t, len_t, idx_t), (r.contents.byte_capacity, r.contents.byte_length, r.contents.index))
-                assert content(t) == bytes(r.contents.bytes[:len_t])
+                c = r.contents
+                rows.append((trial, step, 1, c.byte_capacity, c.byte_length, c.index, zlib.crc32(bytes(c.bytes[:c.byte_length]))))
+        if in_domain:
+            _, _, ok, cap_r, len_r, idx_r, crc_r = (int(x) for x in (rows[-1] if ref is not None else rows[(trial, step)]))
+            if not ok:
+                in_domain = False
+            else:
+                assert (cap_t, len_t, idx_t) == (cap_r, len_r, idx_r), (trial, step, (cap_t, len_t, idx_t), (cap_r, len_r, idx_r))
+                assert zlib.crc32(content(t)) == crc_r, (trial, step)
         # the decoder consumes some of what is buffered
         idx = int(rng.integers(idx_t >> 3, len_t + 1)) << 3
         lib.bbt_set_index(t, idx)
-        if in_domain:
+        if in_domain and ref is not None:
             r.contents.index = idx
     lib.bbt_destroy(t)
     if r is not None:
         ref.bit_buffer_destroy(r)
-print("bitbuffer ok:", writes, "writes", "(reference compared)" if ref is not None else "(no reference build)")
+if ref is not None:
+    np.save(GOLDEN, np.array(rows, dtype=np.int64))
+print("bitbuffer ok:", writes, "writes,", len(rows), "reference states", "recorded" if ref is not None else "compared")

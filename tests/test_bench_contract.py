@@ -36,15 +36,13 @@ def test_reference_arm_prints_one_contract_line():
 
 def test_checker_hash_is_fnv1a64_of_the_planes():
     """bench.py's `verified` compares hashes made by oracle/ref_bench.c; pin that function to the textbook
-    FNV-1a 64 on a small buffer, and the reference's per-picture hashes to hashes of its own planes."""
+    FNV-1a 64 on a small buffer, and the checker's per-picture hashes to hashes of its own planes, which are
+    the compiled reference's (stored in tests/golden/reference/decodes.json)."""
     import ctypes
     import numpy as np
     sys.path.insert(0, helpers.ROOT)
     import bench
-    lib = bench.ref_library()
-    if lib is None:
-        import pytest
-        pytest.skip("oracle/_ref not built")
+    lib, _ = bench.checker_library()
     data = np.frombuffer(b"jsmpeg_b200 fnv check", dtype=np.uint8).copy()
     h = 1469598103934665603
     for byte in data.tobytes():
@@ -54,9 +52,11 @@ def test_checker_hash_is_fnv1a64_of_the_planes():
     buf = (ctypes.c_uint64 * 8)()
     n = lib.ref_picture_hashes(es, len(es), buf, 8)
     assert n == 5
-    frames, _, d = helpers.decode_all(helpers.ref_lib(), [(0, es)])
+    frames, idx, d = helpers.decode_all(helpers.oracle_lib(), [(0, es)])
     for k, (y, cr, cb) in enumerate(frames):
         assert bench.fnv1a64_planes(np.ascontiguousarray(y), np.ascontiguousarray(cr), np.ascontiguousarray(cb)) == buf[k]
+    assert [format(buf[k], "016x") for k in range(n)] == helpers.reference_decode([(0, es)])["fnv1a64"]
+    helpers.assert_frames_match_reference(frames, idx, [(0, es)], "checker clip")
     d.destroy()
 
 

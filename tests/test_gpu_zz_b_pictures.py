@@ -78,12 +78,8 @@ def test_extension_off_is_the_reference_behaviour():
     got, got_idx, gd = decode_all(capi.product_library(), [(0, es)])
     assert got_idx == exp_idx
     assert_frames_equal(got, exp, "b_rows, extension off")
-    ref = helpers.ref_lib()
-    if ref is not None:
-        theirs, tidx, rd = decode_all(ref, [(0, es)])
-        assert tidx == got_idx
-        assert_frames_equal(got[1:], theirs[1:], "b_rows, extension off, vs compiled reference")
-        rd.destroy()
+    # the compiled reference's decode (tests/golden/reference/decodes.json); picture 0: its C planes start uninitialised
+    helpers.assert_frames_match_reference(got, got_idx, [(0, es)], "b_rows, extension off, vs compiled reference", first=1)
     od.destroy()
     gd.destroy()
 
@@ -189,8 +185,6 @@ def test_bench_shape_64_streams_720p_every_picture():
 
     import bench
     from test_b_pictures import FIXTURE_720P
-    if bench.ref_library() is None:
-        pytest.skip("oracle/_ref (the hash helper lives there) not built")
     meta = json.load(open(FIXTURE_720P.replace(".m1v", ".json")))
     es = open(FIXTURE_720P, "rb").read()
     n_streams = int(os.environ.get("B_TEST_STREAMS", "64"))

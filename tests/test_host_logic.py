@@ -181,7 +181,7 @@ def test_napi_addon_source_parses():
 
 
 def test_kernels_are_the_measured_ones():
-    """profiles/r2_sass_hashes.txt lists an md5 of every kernel's SASS on the build the round's last GPU runs used
+    """profiles/sass_hashes_sm90a.txt lists an md5 of every kernel's SASS on the build the H100 numbers were taken with
     (tools/sass_hash.py).  Recompiling the tree must give the same machine code: nobody edits a kernel after it was
     measured without this test saying so."""
     import shutil
@@ -191,7 +191,7 @@ def test_kernels_are_the_measured_ones():
     sys.path.insert(0, os.path.join(helpers.ROOT, "tools"))
     import sass_hash
     recorded = {}
-    for line in open(os.path.join(helpers.ROOT, "profiles", "r2_sass_hashes.txt")):
+    for line in open(os.path.join(helpers.ROOT, "profiles", "sass_hashes_sm90a.txt")):
         parts = line.split()
         if len(parts) >= 3 and parts[0].endswith(".cu") and parts[1].endswith("_kernel"):
             recorded[parts[1]] = next(p for p in parts[2:] if len(p) == 32)

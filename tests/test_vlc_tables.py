@@ -1,20 +1,24 @@
 """Pin tools/vlc_tables.py (ISO 11172-2 Annex B form) to the reference's tree tables.
 
-The reference's trees (src/wasm/mpeg1.c:59-680 == src/mpeg1.js:1037-1663) are parsed out of the
-reference source at test time -- nothing is copied into this repo -- and every canonical code is
-walked through them exactly the way read_huffman does (src/wasm/mpeg1.c:1742-1748).
+The reference's trees (src/wasm/mpeg1.c:59-680 == src/mpeg1.js:1037-1663), parsed out of the
+reference source by tools/make_golden.py into tests/golden/reference/tables.json (data only), and every
+canonical code is walked through them exactly the way read_huffman does (src/wasm/mpeg1.c:1742-1748).
 """
+import json
 import os
 import re
 
 import pytest
 
+import helpers
 import vlc_tables as V
-from conftest import REFERENCE
+
+TABLES_GOLDEN = os.path.join(helpers.REFERENCE_DATA, "tables.json")
 
 
-def _ref_arrays():
-    src = open(os.path.join(REFERENCE, "src/wasm/mpeg1.c")).read()
+def parse_reference_arrays(tree):
+    """The named constant arrays of the reference's src/wasm/mpeg1.c (tools/make_golden.py stores them)."""
+    src = open(os.path.join(tree, "src", "wasm", "mpeg1.c")).read()
     out = {}
     for m in re.finditer(r"static const (?:int|uint8_t|float) (\w+)\[\] = \{(.*?)\};", src, re.S):
         body = re.sub(r"//[^\n]*", "", m.group(2))
@@ -25,6 +29,14 @@ def _ref_arrays():
                 vals.append(eval(tok))  # tokens are literals like "13*3", "0x0a", "-1"
         out[m.group(1)] = vals
     return out
+
+
+def _ref_arrays():
+    if helpers.RECORD and helpers.REFERENCE_TREE:
+        with open(TABLES_GOLDEN, "w") as f:
+            json.dump(parse_reference_arrays(helpers.REFERENCE_TREE), f, sort_keys=True)
+            f.write("\n")
+    return json.load(open(TABLES_GOLDEN))
 
 
 def _walk(tree, code):
@@ -43,7 +55,6 @@ def test_prefix_free(name):
     V.check_prefix_free(V.ALL_VLC[name])
 
 
-@pytest.mark.reference
 @pytest.mark.parametrize("name", sorted(V.ALL_VLC))
 def test_codes_match_reference_trees(name):
     tree = _ref_arrays()[name]
@@ -57,7 +68,6 @@ def test_codes_match_reference_trees(name):
     assert leaves == len(table), (name, leaves, len(table))
 
 
-@pytest.mark.reference
 def test_constant_matrices_match_reference():
     ref = _ref_arrays()
     assert ref["ZIG_ZAG"] == V.ZIG_ZAG

@@ -2,10 +2,10 @@
 """Build compile-time variants of the product library side by side and print the one-call A/B command.
 
     python tools/ab_variants.py                      # builds variants/lib_<name>.so for the candidates below
-    gpurun -- '<the printed command>'                # tools/time_stages.py once per library (JSMPEG_B200_LIB)
+    <the printed command>                            # on the GPU: tools/time_stages.py per library (JSMPEG_B200_LIB), twice, interleaved
 
-The candidates are compile-time tuning constants (CTA sizes, occupancy bounds); round 1's macro-gated code
-paths were measured and deleted (profiles/r2_variants.md).  The in-tree library is left alone.
+The candidates are the compile-time tuning constants: the occupancy bounds of the lane-parallel walk and of
+the reconstruct kernel, and the runs per CTA of the expand kernel.  The in-tree library is left alone.
 """
 import os
 import shutil
@@ -18,8 +18,12 @@ from jsmpeg_b200 import build  # noqa: E402
 
 CANDIDATES = {
     "default": "",
-    "groups4": "-DJSMPEG_EXPAND_GROUPS=4",
-    "groups8": "-DJSMPEG_EXPAND_GROUPS=8",
+    "lanes_ctas3": "-DJSMPEG_LANES_MIN_CTAS=3",
+    "lanes_ctas5": "-DJSMPEG_LANES_MIN_CTAS=5",
+    "expand_groups1": "-DJSMPEG_EXPAND_GROUPS=1",
+    "expand_groups8": "-DJSMPEG_EXPAND_GROUPS=8",
+    "recon_ctas4": "-DJSMPEG_RECON_MIN_CTAS=4",
+    "recon_ctas6": "-DJSMPEG_RECON_MIN_CTAS=6",
 }
 
 
@@ -41,7 +45,7 @@ def main():
         os.environ.pop("JSMPEG_B200_NVCC_FLAGS", None)
         if os.path.exists(keep):
             os.replace(keep, build.OUT)
-    print("; ".join(cmds))
+    print("; ".join(cmds + cmds))
     print("\n# parity first, per variant:  JSMPEG_B200_LIB=$PWD/variants/lib_<name>.so python -m pytest tests/test_gpu_parity.py -m gpu -x -q",
           file=sys.stderr)
 

@@ -6,7 +6,8 @@ Content is seeded numpy: low-resolution noise upsampled bicubically (smooth, mov
 a moving disc, and +-noise uniform noise per sample.  cv2 gives no bitrate/GOP control: FFmpeg's
 defaults apply (GOP 12 = 1 I + 11 P, no B pictures, one slice per picture).
 
-Clips are cached under $JSMPEG_B200_CACHE (default /tmp/jsmpeg_b200_cache) because encoding 1080p
+Clips are cached under $JSMPEG_B200_CACHE (default jsmpeg_b200_cache_<uid> in the system temporary
+directory, one per user, so that another user's cache never blocks a write) because encoding 1080p
 takes seconds.
 """
 from __future__ import annotations
@@ -14,10 +15,11 @@ from __future__ import annotations
 import hashlib
 import os
 import sys
+import tempfile
 
 import numpy as np
 
-CACHE = os.environ.get("JSMPEG_B200_CACHE", "/tmp/jsmpeg_b200_cache")
+CACHE = os.environ.get("JSMPEG_B200_CACHE", os.path.join(tempfile.gettempdir(), f"jsmpeg_b200_cache_{os.getuid()}"))
 
 
 def make_clip_ts(width, height, frames, seed=1234, noise=6, fps=30):

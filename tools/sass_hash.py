@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """md5 of the SASS instruction stream of every product kernel (addresses and encodings stripped).
 Used to show that a source change left the machine code of a GPU-verified kernel untouched
-(profiles/README.md lists the hashes of the build the round-end numbers were taken with).
+(profiles/sass_hashes_sm90a.txt lists the hashes of the build the H100 numbers were taken with).
 
     python tools/sass_hash.py [--csrc DIR] [extra nvcc flags...]
 """
@@ -21,7 +21,7 @@ def kernel_hashes(cu, csrc=CSRC, flags=()):
     """{kernel name: (md5, instruction count)} for one .cu file."""
     with tempfile.TemporaryDirectory() as tmp:
         cubin = os.path.join(tmp, "k.cubin")
-        subprocess.check_call(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", *flags,
+        subprocess.check_call(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", *flags,
                                "-cubin", "-o", cubin, os.path.join(csrc, cu)])
         sass = subprocess.run(["cuobjdump", "-sass", cubin], capture_output=True, text=True, check=True).stdout
     out, name, lines = {}, None, []

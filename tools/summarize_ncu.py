@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Turn ncu outputs brought back in gpurun_out/ into the small text summaries kept under profiles/.
+"""Turn Nsight Compute outputs into small text summaries.
 
-    python tools/summarize_ncu.py launches gpurun_out/launches_r1.csv          > profiles/r1_launches.md
-    python tools/summarize_ncu.py kernel   gpurun_out/prof_recon_r1.ncu-rep    > profiles/r1_reconstruct.md
-    python tools/summarize_ncu.py lines    gpurun_out/prof_walk_r2.ncu-rep 25  >> profiles/r2_walk.md   # hottest source lines
+    python tools/summarize_ncu.py launches launches.csv          > launches.md
+    python tools/summarize_ncu.py kernel   prof_recon.ncu-rep    > reconstruct.md
+    python tools/summarize_ncu.py lines    prof_walk.ncu-rep 25  >> walk.md   # hottest source lines
 """
 import csv
 import io

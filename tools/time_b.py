@@ -66,7 +66,6 @@ for decode_b, slice_walk in (((1, 0),) if quick else ((1, 0), (0, 0), (1, 1))): 
     bd.close()
 if quick:
     sys.exit(0)
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-with open(os.path.join(ROOT, "gpurun_out", os.environ.get("TIME_B_OUT", "r2_b_pictures_720p.json")), "w") as f:
+with open(os.environ.get("TIME_B_OUT", "time_b.json"), "w") as f:
     json.dump(out, f, indent=1)
 sys.exit(0 if out.get("verified_last_picture_of_every_stream") and out.get("verified_last_picture_of_every_stream_slice_walk", True) else 1)
