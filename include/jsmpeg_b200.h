@@ -141,6 +141,21 @@ int jsmpeg_b200_batch_stream_info(jsmpeg_b200_batch_t *b, int stream, int *width
 long jsmpeg_b200_batch_write_ts(jsmpeg_b200_batch_t *b, int stream, const uint8_t *ts, size_t n_bytes, int stream_id,
                                 uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes);
 
+/* MPEG program stream in (ISO 11172-1 system stream, .mpg / VCD .dat; ISO 13818-1 program stream, .vob),
+ * demultiplexed on the GPU: the payload of every PES packet with stream id `stream_id` (0xE0..0xEF) is
+ * appended to `stream` exactly as if it had been written with get_write_ptr/did_write.  The stream is
+ * read as a chain of items without gaps -- pack headers of either form, end codes, and packets of
+ * 6 + packet_length bytes (system header, PSM, PES) -- starting at the first valid pack header.  Bytes
+ * that are not an item where one should start are a break: parsing resumes at the next valid pack
+ * header.  The buffer may be cut anywhere: what a call leaves over is kept for the next one, and the
+ * result does not depend on how the bytes are split into calls.  Returns the number of
+ * elementary-stream bytes appended (-1: the decoder is dead; -2: stream_id is not 0xE0..0xEF, nothing
+ * changed).  pts_out / offset_out (capacity n_max, may be NULL) receive, per PES packet of the stream
+ * with a PTS and a non-empty payload, in stream order, its 33-bit PTS in 90 kHz ticks and the byte
+ * offset of its payload in the stream's buffer; *n_pes = their number. */
+long jsmpeg_b200_batch_write_ps(jsmpeg_b200_batch_t *b, int stream, const uint8_t *ps, size_t n_bytes, int stream_id,
+                                uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes);
+
 /* Make everything written so far resident in HBM and indexed (H2D copy of new bytes + start-code
  * scan).  Called implicitly by decode; exposed so that a benchmark can separate it.  Returns the
  * number of picture start codes currently indexed over all streams. */
@@ -189,6 +204,10 @@ int jsmpeg_b200_debug_parse_picture(const uint8_t *es, uint32_t es_len, uint32_t
 int jsmpeg_b200_debug_reconstruct(int mb_width, int mb_height, const void *hdr, const void *coef,
                                   const uint8_t *fwd_y, const uint8_t *fwd_cr, const uint8_t *fwd_cb,
                                   uint8_t *cur_y, uint8_t *cur_cr, uint8_t *cur_cb);
+
+/* Copy the first min(cap, resident) bytes of the stream's elementary stream as it is resident in HBM into
+ * `dst`; returns the resident byte count (-1: the batch is dead). */
+long jsmpeg_b200_debug_read_es(jsmpeg_b200_batch_t *b, int stream, void *dst, size_t cap);
 
 /* NULL while the decoder works, else why it is dead (see mpeg1_decoder_create). */
 const char *jsmpeg_b200_decoder_last_error(mpeg1_decoder_t *self);

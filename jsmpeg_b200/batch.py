@@ -40,6 +40,8 @@ _BATCH_ABI = {
                                                      ctypes.POINTER(ctypes.c_float)]),
     "jsmpeg_b200_batch_write_ts": (ctypes.c_long, [_VP, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int,
                                                    _VP, _VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
+    "jsmpeg_b200_batch_write_ps": (ctypes.c_long, [_VP, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int,
+                                                   _VP, _VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_batch_upload": (ctypes.c_long, [_VP]),
     "jsmpeg_b200_batch_rewind": (None, [_VP]),
     "jsmpeg_b200_batch_reset": (None, [_VP]),
@@ -55,6 +57,7 @@ _BATCH_ABI = {
     "jsmpeg_b200_debug_parse_picture": (ctypes.c_int, [_VP, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int, ctypes.c_int,
                                                        _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_debug_reconstruct": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "jsmpeg_b200_debug_read_es": (ctypes.c_long, [_VP, ctypes.c_int, _VP, ctypes.c_size_t]),
     "jsmpeg_b200_set_default_device": (None, [ctypes.c_int]),
     "jsmpeg_b200_batch_last_error": (ctypes.c_char_p, [_VP]),
     "jsmpeg_b200_batch_set_option": (ctypes.c_int, [_VP, ctypes.c_char_p, ctypes.c_int]),
@@ -128,6 +131,34 @@ class BatchDecoder:
         if total < 0:
             raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ts failed")
         return total, [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
+
+    def write_ps(self, stream, ps_bytes, stream_id=0xE0):
+        """MPEG program stream in (.mpg: ISO 11172-1, .vob: ISO 13818-1), demultiplexed on the GPU (any
+        chunking, resyncs at the next pack header).  Returns (ES bytes appended, [(payload byte offset, pts
+        seconds), ...] per PES packet of `stream_id` with a PTS in it)."""
+        ps_bytes = bytes(ps_bytes)
+        # a table entry needs >= 12 bytes (6 + a 5-byte PTS + 1 payload byte); the call may also finish items
+        # of up to 65,541 bytes that an earlier call left over
+        n_max = (len(ps_bytes) + 65541) // 12 + 1
+        pts = np.zeros(n_max, np.uint64)
+        off = np.zeros(n_max, np.uint32)
+        n = ctypes.c_int()
+        total = self.lib.jsmpeg_b200_batch_write_ps(self.handle, stream, ps_bytes, len(ps_bytes), stream_id,
+                                                    pts.ctypes.data, off.ctypes.data, n_max, ctypes.byref(n))
+        if total == -2:
+            raise ValueError(f"stream_id {stream_id:#x} is not a video stream id (0xE0..0xEF)")
+        if total < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ps failed")
+        return total, [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
+
+    def read_es(self, stream):
+        """The stream's elementary stream as it is resident in HBM (test hook)."""
+        n = self.lib.jsmpeg_b200_debug_read_es(self.handle, stream, None, 0)
+        if n < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_debug_read_es failed")
+        buf = ctypes.create_string_buffer(max(n, 1))
+        self.lib.jsmpeg_b200_debug_read_es(self.handle, stream, buf, n)
+        return buf.raw[:n]
 
     def get_index(self, stream):
         return self.lib.jsmpeg_b200_batch_get_index(self.handle, stream)

@@ -137,3 +137,11 @@ TsScratch *ts_scratch_create();
 void ts_scratch_destroy(TsScratch *s);
 long ts_demux_measure(TsScratch *s, const uint8_t *ts_host, size_t ts_bytes, int stream_id, int16_t *bound, size_t *consumed, cudaStream_t st);
 int ts_demux_gather(TsScratch *s, uint8_t *es, uint32_t es_base, uint64_t *pts_out, uint32_t *offset_out, int n_max, cudaStream_t st);
+
+// device MPEG program stream demux (psdemux.cu)
+struct PsScratch;
+PsScratch *ps_scratch_create();
+void ps_scratch_destroy(PsScratch *s);
+long ps_demux_measure(PsScratch *s, const uint8_t *ps_host, size_t ps_bytes, int stream_id, bool *in_sync, size_t *consumed, cudaStream_t st);
+int ps_demux_gather(PsScratch *s, uint8_t *es, uint32_t es_base, uint64_t *pts_out, uint32_t *offset_out, int n_max, cudaStream_t st);
+uint32_t ps_demux_launches(const PsScratch *s);  // kernels the last measure + gather launched

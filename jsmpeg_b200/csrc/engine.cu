@@ -102,6 +102,8 @@ struct Stream {
 	uint8_t *d_rgba = nullptr;
 	std::vector<int16_t> ts_bound;     // device TS demux: the stream id every PID is bound to, 0 = none (ts.js pidsToStreamIds)
 	std::vector<uint8_t> ts_leftover;  // ... and the bytes the last write_ts left over (ts.js leftoverBytes)
+	std::vector<uint8_t> ps_leftover;  // device PS demux: the bytes the last write_ps left over
+	bool ps_in_sync = false;           // ... and whether they continue the item chain (else: look for a pack header)
 	// parsed-ahead pictures, consecutive, front = next picture decode() consumes
 	std::deque<Parsed> cache;
 };
@@ -158,6 +160,7 @@ struct jsmpeg_b200_batch_t {
 	std::vector<size_t> copy_size;
 	bool batch_copy_ok = true;
 	TsScratch *ts = nullptr;
+	PsScratch *ps = nullptr;
 	jsmpeg_b200_stats_t stats{};
 };
 
@@ -1008,6 +1011,38 @@ int env_int(const char *name, int fallback) {
 	return e && *e ? atoi(e) : fallback;
 }
 
+// The tail of a device demux (write_ts, write_ps): `total` ES bytes that gather(es_base) writes to the HBM
+// mirror at s.d_es + es_base are appended to the stream as if written with get_write_ptr / did_write.
+// gather returns the number of PES starts it listed in pts_out / offset_out (unordered).
+template <typename F>
+long append_demuxed(Batch *b, Stream &s, uint32_t total, F &&gather, uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes) {
+	// room in the host bit buffer (the reference's write protocol, may expand or evict) and in HBM
+	uint8_t *hdst = static_cast<uint8_t *>(stream_get_write_ptr(b, s, total));
+	reserve_device_es(b, s, s.bb.length + total);
+	if (s.d_valid < s.bb.length) {  // bytes written the ordinary way that are not resident yet
+		CUDA_CHECK(cudaMemcpyAsync(s.d_es + s.d_valid, s.bb.bytes + s.d_valid, s.bb.length - s.d_valid, cudaMemcpyHostToDevice, b->st_main));
+		b->stats.h2d_bytes += s.bb.length - s.d_valid;
+		s.d_valid = s.bb.length;
+	}
+	const int count = gather(s.bb.length);
+	// the host keeps a mirror of the ES (sequence header parse, EVICT bookkeeping): copy the new bytes back
+	CUDA_CHECK(cudaMemcpyAsync(hdst, s.d_es + s.bb.length, (size_t)total, cudaMemcpyDeviceToHost, b->st_main));
+	CUDA_CHECK(cudaMemsetAsync(s.d_es + s.bb.length + total, 0, ES_PAD, b->st_main));
+	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+	b->stats.d2h_bytes += (uint64_t)total;
+	stream_did_write(b, s, total);
+	s.d_valid = s.bb.length;
+	if (n_pes) *n_pes = count;
+	if (pts_out && offset_out && count > 1) {  // the device appends PES starts unordered: sort by offset
+		const int m = std::min(count, n_max);
+		std::vector<std::pair<uint32_t, uint64_t>> v(m);
+		for (int i = 0; i < m; i++) v[i] = {offset_out[i], pts_out[i]};
+		std::sort(v.begin(), v.end());
+		for (int i = 0; i < m; i++) { offset_out[i] = v[i].first; pts_out[i] = v[i].second; }
+	}
+	return total;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -1081,6 +1116,7 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b) {
 	if (b->h_rtasks) cudaFreeHost(b->h_rtasks);
 	if (b->d_rtasks) cudaFree(b->d_rtasks);
 	ts_scratch_destroy(b->ts);
+	ps_scratch_destroy(b->ps);
 	cudaEvent_t evs[] = {b->ev_a, b->ev_b, b->ev_mid, b->ev_step, b->ev_round, b->ev_copied[0], b->ev_copied[1], b->fork.fork};
 	for (auto e : evs) if (e) cudaEventDestroy(e);
 	for (auto v : {&b->ev_info, &b->ev_rec0, &b->ev_rec1}) for (auto e : *v) if (e) cudaEventDestroy(e);
@@ -1251,35 +1287,44 @@ long jsmpeg_b200_batch_write_ts(jsmpeg_b200_batch_t *b, int stream, const uint8_
 		size_t consumed = 0;
 		const long total = ts_demux_measure(b->ts, data, n_data, stream_id, s.ts_bound.data(), &consumed, b->st_main);
 		std::vector<uint8_t> rest(data + consumed, data + n_data);  // (data may alias ts_leftover)
-		if (total <= 0) { s.ts_leftover.swap(rest); return total; }
-		// room in the host bit buffer (the reference's write protocol, may expand or evict) and in HBM
-		uint8_t *hdst = static_cast<uint8_t *>(stream_get_write_ptr(b, s, (uint32_t)total));
-		reserve_device_es(b, s, s.bb.length + (uint32_t)total);
-		if (s.d_valid < s.bb.length) {  // bytes written the ordinary way that are not resident yet
-			CUDA_CHECK(cudaMemcpyAsync(s.d_es + s.d_valid, s.bb.bytes + s.d_valid, s.bb.length - s.d_valid, cudaMemcpyHostToDevice, b->st_main));
-			b->stats.h2d_bytes += s.bb.length - s.d_valid;
-			s.d_valid = s.bb.length;
-		}
-		const int count = ts_demux_gather(b->ts, s.d_es, s.bb.length, pts_out, offset_out, n_max, b->st_main);
 		s.ts_leftover.swap(rest);
+		if (total <= 0) return total;
 		b->stats.kernel_launches += 7;
 		b->stats.h2d_bytes += n_data;
-		// the host keeps a mirror of the ES (sequence header parse, EVICT bookkeeping): copy the new bytes back
-		CUDA_CHECK(cudaMemcpyAsync(hdst, s.d_es + s.bb.length, (size_t)total, cudaMemcpyDeviceToHost, b->st_main));
-		CUDA_CHECK(cudaMemsetAsync(s.d_es + s.bb.length + total, 0, ES_PAD, b->st_main));
-		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-		b->stats.d2h_bytes += (uint64_t)total;
-		stream_did_write(b, s, (uint32_t)total);
-		s.d_valid = s.bb.length;
-		if (n_pes) *n_pes = count;
-		if (pts_out && offset_out && count > 1) {  // the device appends PES starts unordered: sort by offset
-			const int m = std::min(count, n_max);
-			std::vector<std::pair<uint32_t, uint64_t>> v(m);
-			for (int i = 0; i < m; i++) v[i] = {offset_out[i], pts_out[i]};
-			std::sort(v.begin(), v.end());
-			for (int i = 0; i < m; i++) { offset_out[i] = v[i].first; pts_out[i] = v[i].second; }
+		return append_demuxed(b, s, (uint32_t)total, [&](uint32_t es_base) {
+			return ts_demux_gather(b->ts, s.d_es, es_base, pts_out, offset_out, n_max, b->st_main);
+		}, pts_out, offset_out, n_max, n_pes);
+	});
+}
+
+long jsmpeg_b200_batch_write_ps(jsmpeg_b200_batch_t *b, int stream, const uint8_t *ps, size_t n_bytes, int stream_id,
+                                uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes) {
+	if (n_pes) *n_pes = 0;
+	return guarded<long>(b, -1, [&]() -> long {
+		if (stream_id < 0xE0 || stream_id > 0xEF) return -2;  // not a video stream id: the caller's mistake, nothing changes
+		use_device(b);
+		Stream &s = b->streams[stream];
+		if (!b->ps) b->ps = ps_scratch_create();
+		// what the previous call left over comes first: an unfinished item, or the tail that may begin a pack header
+		const uint8_t *data = ps;
+		size_t n_data = n_bytes;
+		if (!s.ps_leftover.empty()) {
+			s.ps_leftover.insert(s.ps_leftover.end(), ps, ps + n_bytes);
+			data = s.ps_leftover.data();
+			n_data = s.ps_leftover.size();
 		}
-		return total;
+		size_t consumed = 0;
+		const long total = ps_demux_measure(b->ps, data, n_data, stream_id, &s.ps_in_sync, &consumed, b->st_main);
+		std::vector<uint8_t> rest(data + consumed, data + n_data);  // (data may alias ps_leftover)
+		s.ps_leftover.swap(rest);
+		b->stats.h2d_bytes += n_data;
+		long r = total;
+		if (total > 0)
+			r = append_demuxed(b, s, (uint32_t)total, [&](uint32_t es_base) {
+				return ps_demux_gather(b->ps, s.d_es, es_base, pts_out, offset_out, n_max, b->st_main);
+			}, pts_out, offset_out, n_max, n_pes);
+		b->stats.kernel_launches += ps_demux_launches(b->ps);
+		return r;
 	});
 }
 
@@ -1410,6 +1455,16 @@ bool mpeg1_decoder_decode(mpeg1_decoder_t *self) {
 
 // ================================================================================================
 // test hooks
+
+long jsmpeg_b200_debug_read_es(jsmpeg_b200_batch_t *b, int stream, void *dst, size_t cap) {
+	return guarded<long>(b, -1, [&]() -> long {
+		use_device(b);
+		const Stream &s = b->streams[stream];
+		const size_t n = std::min<size_t>(cap, s.d_valid);
+		if (n) CUDA_CHECK(cudaMemcpy(dst, s.d_es, n, cudaMemcpyDeviceToHost));
+		return (long)s.d_valid;
+	});
+}
 
 int jsmpeg_b200_debug_parse_picture(const uint8_t *es, uint32_t es_len, uint32_t start_byte, int mb_width,
                                     int mb_height, const uint8_t *intra_q, const uint8_t *non_intra_q,

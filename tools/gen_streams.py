@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Synthetic MPEG-1 video test clips (MPEG-TS) encoded with cv2's bundled FFmpeg (mpeg1video encoder +
+"""Synthetic MPEG-1 video test clips (MPEG-TS, program streams, raw ES) encoded with cv2's bundled FFmpeg (mpeg1video encoder +
 mpegts muxer), SURVEY.md section 7 step 0(a) / section 8(d).
 
 Content is seeded numpy: low-resolution noise upsampled bicubically (smooth, moving background),
@@ -24,25 +24,44 @@ CACHE = os.environ.get("JSMPEG_B200_CACHE", os.path.join(tempfile.gettempdir(), 
 
 def make_clip_ts(width, height, frames, seed=1234, noise=6, fps=30):
     """Returns the bytes of an MPEG-TS clip (video PID 0x100, stream id 0xE0)."""
+    return _make_clip("ts", width, height, frames, seed, noise, fps)
+
+
+def make_clip_ps(width, height, frames, seed=1234, noise=6, fps=30, form="mpg"):
+    """The same encode in a program stream: form "mpg" = FFmpeg's mpeg muxer (ISO 11172-1 packs and PES),
+    "vob" = its vob muxer (ISO 13818-1 packs and PES).  Video stream id 0xE0."""
+    if form not in ("mpg", "vob"):
+        raise ValueError(f"form {form!r}: 'mpg' or 'vob'")
+    return _make_clip(form, width, height, frames, seed, noise, fps)
+
+
+def make_clip_m1v(width, height, frames, seed=1234, noise=6, fps=30):
+    """The same encode as a raw MPEG-1 video elementary stream."""
+    return _make_clip("m1v", width, height, frames, seed, noise, fps)
+
+
+def _make_clip(ext, width, height, frames, seed, noise, fps):
+    """Encodes the scene; FFmpeg picks the container from the file extension."""
     import cv2
 
     os.makedirs(CACHE, exist_ok=True)
-    key = hashlib.sha1(f"v2-{width}x{height}-{frames}-{seed}-{noise}-{fps}-{cv2.__version__}".encode()).hexdigest()[:16]
-    path = os.path.join(CACHE, f"clip_{width}x{height}_{frames}f_s{seed}_{key}.ts")
+    tag = "v2" if ext == "ts" else f"v2-{ext}"
+    key = hashlib.sha1(f"{tag}-{width}x{height}-{frames}-{seed}-{noise}-{fps}-{cv2.__version__}".encode()).hexdigest()[:16]
+    path = os.path.join(CACHE, f"clip_{width}x{height}_{frames}f_s{seed}_{key}.{ext}")
     if os.path.exists(path):
         with open(path, "rb") as f:
             return f.read()
     rng = np.random.default_rng(seed)
     lo = rng.integers(0, 256, (height // 32 + 3, width // 32 + 3, 3), dtype=np.uint8)
     base = cv2.resize(lo, (width + 64, height + 64), interpolation=cv2.INTER_CUBIC).astype(np.int16)
-    tmp = path + f".{os.getpid()}.tmp.ts"
+    tmp = path + f".{os.getpid()}.tmp.{ext}"
     devnull = os.open(os.devnull, os.O_WRONLY)
     saved = os.dup(2)
     os.dup2(devnull, 2)  # FFmpeg prints a harmless "tag mpg1 not supported" warning
     try:
         vw = cv2.VideoWriter(tmp, cv2.CAP_FFMPEG, cv2.VideoWriter_fourcc(*"mpg1"), fps, (width, height))
         if not vw.isOpened():
-            raise RuntimeError("cv2/FFmpeg cannot open an mpeg1video MPEG-TS writer")
+            raise RuntimeError(f"cv2/FFmpeg cannot open an mpeg1video .{ext} writer")
         for i in range(frames):
             dx, dy = (i * 3) % 64, (i * 2) % 64
             f = base[dy:dy + height, dx:dx + width].copy()
