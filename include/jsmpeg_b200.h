@@ -188,6 +188,33 @@ int jsmpeg_b200_batch_read_planes(jsmpeg_b200_batch_t *b, int stream, void *y, v
  * stream's last decode() consumed, decoded or skipped; -1 before the first one.  Either pointer may be NULL. */
 int jsmpeg_b200_batch_last_picture(jsmpeg_b200_batch_t *b, int stream, int *picture_type, int *temporal_reference);
 
+/* KEY PICTURES (thumbnails, seek previews, frame sampling): I pictures decoded independently of decode(), any number
+ * of them from any streams in one parallel wave.  Picture k of a stream is the k-th picture start code (00 00 01 00)
+ * in its current buffer (for a buffer that never evicted: the picture the (k+1)-th decode() consumes).  The index
+ * lists picture k when it starts after the stream's first sequence header, its picture_coding_type is 1, and it is
+ * closed: a later start code is in the buffer that is no slice (01..AF), user data (B2) or extension (B5).  A
+ * listed picture decodes to exactly what a fresh decoder gives for the first sequence header + the picture's bytes
+ * up to and including that closing code: where the picture codes every macroblock, what decode() gives at that
+ * point of the stream; a macroblock the picture does not reach is 0 (RGBA: the conversion of those planes, the
+ * odd edge opaque white).  Neither call changes anything decode() observes (bit index, planes, last_picture,
+ * stats -- both make written bytes resident first, and count that upload as decode() would have); decode_intra may
+ * drop parsed-ahead pictures when it needs their record slots (decode() then parses them again). */
+
+/* I pictures of `stream` that decode_intra can decode now; returns how many there are (-1 dead, -2 stream out of
+ * range); the first min(count, n_max) go to the arrays, any of which may be NULL. */
+long jsmpeg_b200_batch_intra_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out,
+                                   uint32_t *byte_pos_out, int32_t *temporal_reference_out, long n_max);
+/* Decode n listed I pictures, of any streams, in as few waves as the record slots allow.  Request i =
+ * picture pictures[i] of stream streams[i] into planes_dst[i]: DEVICE memory of coded_size * 3 / 2 bytes
+ * (Y | Cr | Cb, coded size, like get_planes), 16-byte aligned.  With JSMPEG_B200_OUT_RGBA in flags, rgba_dst[i]
+ * (device, 16-byte aligned, width * height * 4) gets the picture too.  Synchronous: everything is written when it
+ * returns.  n_present_out / error_out (may be NULL) get picture_info_t.n_present / .error per request.  Returns n;
+ * -1 dead; -2 a request is invalid (stream out of range or without sequence header, picture not in the
+ * intra index, NULL or misaligned destination) -- checked before any work, and then nothing changed. */
+long jsmpeg_b200_batch_decode_intra(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                    void *const *planes_dst, void *const *rgba_dst, int flags,
+                                    int32_t *n_present_out, int32_t *error_out);
+
 void jsmpeg_b200_batch_get_stats(jsmpeg_b200_batch_t *b, jsmpeg_b200_stats_t *out);
 void jsmpeg_b200_batch_reset_stats(jsmpeg_b200_batch_t *b);
 

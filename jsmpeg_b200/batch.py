@@ -2,6 +2,7 @@
 one GPU, device-resident planes, one call decodes the next pictures of every stream."""
 from __future__ import annotations
 
+import bisect
 import ctypes
 
 import numpy as np
@@ -52,6 +53,8 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_read_planes": (ctypes.c_int, [_VP, ctypes.c_int, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_read_rgba": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
     "jsmpeg_b200_batch_last_picture": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
+    "jsmpeg_b200_batch_intra_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, ctypes.c_long]),
+    "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
     "jsmpeg_b200_batch_get_stats": (None, [_VP, ctypes.POINTER(Stats)]),
     "jsmpeg_b200_batch_reset_stats": (None, [_VP]),
     "jsmpeg_b200_debug_parse_picture": (ctypes.c_int, [_VP, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int, ctypes.c_int,
@@ -69,6 +72,14 @@ _BATCH_ABI = {
 }
 
 
+def planes_view(t, info):
+    """Y [coded_h, coded_w], Cr and Cb [coded_h / 2, coded_w / 2] as views of a decode_intra planes tensor; `info` is
+    the stream's BatchDecoder.stream_info."""
+    cw, ch = (info["width"] + 15) // 16 * 16, (info["height"] + 15) // 16 * 16
+    n = cw * ch
+    return t[:n].view(ch, cw), t[n:n + n // 4].view(ch // 2, cw // 2), t[n + n // 4:n + n // 2].view(ch // 2, cw // 2)
+
+
 def bind_batch_abi(lib):
     for name, (res, args) in _BATCH_ABI.items():
         fn = getattr(lib, name)
@@ -84,6 +95,9 @@ class BatchDecoder:
         from . import capi
         self.lib = lib if lib is not None else capi.product_library()
         self.n_streams = n_streams
+        self.device = device
+        self._pes = [[] for _ in range(n_streams)]  # per stream: every (payload byte offset, pts seconds) write_ts/write_ps returned
+        self.last_intra_info = []  # per request of the last decode_intra: {"n_present", "error"} (picture_info_t)
         self.handle = self.lib.jsmpeg_b200_batch_create(n_streams, device, max_slots)
         err = self.lib.jsmpeg_b200_batch_last_error(self.handle)
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
@@ -130,7 +144,9 @@ class BatchDecoder:
                                                     pts.ctypes.data, off.ctypes.data, n_max, ctypes.byref(n))
         if total < 0:
             raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ts failed")
-        return total, [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
+        table = [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
+        self._pes[stream] += table
+        return total, table
 
     def write_ps(self, stream, ps_bytes, stream_id=0xE0):
         """MPEG program stream in (.mpg: ISO 11172-1, .vob: ISO 13818-1), demultiplexed on the GPU (any
@@ -149,7 +165,9 @@ class BatchDecoder:
             raise ValueError(f"stream_id {stream_id:#x} is not a video stream id (0xE0..0xEF)")
         if total < 0:
             raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ps failed")
-        return total, [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
+        table = [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
+        self._pes[stream] += table
+        return total, table
 
     def read_es(self, stream):
         """The stream's elementary stream as it is resident in HBM (test hook)."""
@@ -180,6 +198,7 @@ class BatchDecoder:
 
     def reset(self):
         self.lib.jsmpeg_b200_batch_reset(self.handle)
+        self._pes = [[] for _ in range(self.n_streams)]
 
     def decode(self, n_pictures=1, flags=OUT_DEVICE):
         return self.lib.jsmpeg_b200_batch_decode(self.handle, n_pictures, flags)
@@ -217,6 +236,60 @@ class BatchDecoder:
         if self.lib.jsmpeg_b200_batch_read_rgba(self.handle, stream, out.ctypes.data) != 0:
             raise RuntimeError("no RGBA picture (decode with OUT_RGBA first)")
         return out
+
+    def intra_index(self, stream):
+        """The I pictures of `stream` that decode_intra can decode now (include/jsmpeg_b200.h): one dict per picture,
+        {"picture": k, "byte_pos", "temporal_reference", "pts"}.  `pts` (seconds) is that of the last PES packet
+        write_ts / write_ps reported at or before the picture's start code (src/decoder.js:36-47), or None."""
+        n = self.lib.jsmpeg_b200_batch_intra_index(self.handle, stream, None, None, None, 0)
+        if n == -2:
+            raise ValueError(f"stream {stream} out of range")
+        if n < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_intra_index failed")
+        pic, pos, tr = np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.int32)
+        n = self.lib.jsmpeg_b200_batch_intra_index(self.handle, stream, pic.ctypes.data, pos.ctypes.data, tr.ctypes.data, n)
+        pes = self._pes[stream]
+        offsets = [o for o, _ in pes]
+        out = []
+        for i in range(min(n, len(pic))):
+            j = bisect.bisect_right(offsets, int(pos[i])) - 1
+            out.append({"picture": int(pic[i]), "byte_pos": int(pos[i]), "temporal_reference": int(tr[i]),
+                        "pts": pes[j][1] if j >= 0 else None})
+        return out
+
+    def decode_intra(self, requests, rgba=False):
+        """Decode I pictures listed by intra_index, of any streams, in one call: `requests` is an iterable of (stream,
+        picture).  Returns per request a torch.uint8 CUDA tensor of coded_size * 3 // 2 bytes (Y | Cr | Cb, see
+        planes_view), or with rgba=True a pair (planes, rgba [height, width, 4])."""
+        import torch
+        reqs = [(int(s), int(p)) for s, p in requests]
+        n = len(reqs)
+        dev = torch.device("cuda", self.device)
+        planes, images = [], []
+        for s, _ in reqs:
+            if not 0 <= s < self.n_streams:
+                raise ValueError(f"stream {s} out of range")
+            info = self.stream_info(s)
+            if not info["has_sequence_header"]:
+                raise ValueError(f"stream {s} has no sequence header yet")
+            planes.append(torch.empty(info["coded_size"] * 3 // 2, dtype=torch.uint8, device=dev))
+            if rgba:
+                images.append(torch.empty((info["height"], info["width"], 4), dtype=torch.uint8, device=dev))
+        streams = (ctypes.c_int * max(n, 1))(*[s for s, _ in reqs])
+        pictures = (ctypes.c_uint32 * max(n, 1))(*[p for _, p in reqs])
+        planes_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in planes])
+        rgba_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in images]) if rgba else None
+        n_present = (ctypes.c_int32 * max(n, 1))()
+        errors = (ctypes.c_int32 * max(n, 1))()
+        torch.cuda.current_stream(dev).synchronize()  # the allocations are the caller's stream's; the call uses its own
+        got = self.lib.jsmpeg_b200_batch_decode_intra(self.handle, n, streams, pictures, planes_dst, rgba_dst,
+                                                      OUT_RGBA if rgba else OUT_DEVICE, n_present, errors)
+        if got == -2:
+            raise ValueError("a request names a picture that is not in the stream's intra index")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_intra failed")
+        self.last_intra_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
+        return list(zip(planes, images)) if rgba else planes
 
     def last_picture(self, stream):
         """(picture_coding_type, temporal_reference) of the picture the stream's last decode() consumed, or None."""

@@ -77,6 +77,7 @@ struct Stream {
 	float frame_rate = 0.f;
 	int width = 0, height = 0, coded_size = 0;
 	uint32_t seq_end_index = 0;  // bit index right after the sequence header
+	uint32_t seq_floor = 0;      // byte position in the CURRENT buffer from which pictures follow the sequence header
 	SeqParams seq{};
 	SeqParams *d_seq = nullptr;
 	// ES mirror in HBM + start-code index
@@ -161,6 +162,9 @@ struct jsmpeg_b200_batch_t {
 	bool batch_copy_ok = true;
 	TsScratch *ts = nullptr;
 	PsScratch *ps = nullptr;
+	// decode_intra: the forward plane set its reconstruct tasks name, zeroed and never written (DESIGN 3.6)
+	uint8_t *d_intra_fwd = nullptr;
+	size_t intra_fwd_bytes = 0;
 	jsmpeg_b200_stats_t stats{};
 };
 
@@ -216,8 +220,13 @@ void forget_index(Batch *b, Stream &s) {
 // src/wasm/buffer.c:48-65 get_write_ptr, :167-190 evict (bitbuffer.h)
 void *stream_get_write_ptr(Batch *b, Stream &s, uint32_t n) {
 	bool moved = false;
+	const uint32_t old_length = s.bb.length;
 	uint8_t *p = bitbuffer::get_write_ptr(s.bb, n, kPinned, moved);
-	if (moved) forget_index(b, s);  // byte positions changed: the HBM mirror, the index and the look-ahead are void
+	if (moved) {
+		forget_index(b, s);  // byte positions changed: the HBM mirror, the index and the look-ahead are void
+		const uint32_t dropped = old_length - s.bb.length;  // EVICT drops bytes from the front only
+		s.seq_floor = s.seq_floor > dropped ? s.seq_floor - dropped : 0;
+	}
 	if (!p) throw std::runtime_error("jsmpeg_b200: bit buffer cannot hold the write (more than 4 GiB - 1 bytes)");
 	return p;
 }
@@ -260,6 +269,7 @@ void parse_sequence_header(Batch *b, Stream &s, uint32_t bit_index) {
 	seq_fill_xq(s.seq);
 	s.bb.index = hb.idx;
 	s.seq_end_index = hb.idx;
+	s.seq_floor = (hb.idx + 7) >> 3;  // where decode() starts looking for the first picture
 	s.seq.mb_width = (s.width + 15) >> 4;
 	s.seq.mb_height = (s.height + 15) >> 4;
 	s.seq.mb_size = s.seq.mb_width * s.seq.mb_height;
@@ -611,6 +621,52 @@ void copy_out_step(Batch *b, const std::vector<ReconTask> &tasks, const std::vec
 	b->copy_steps++;
 }
 
+// picture_coding_type of picture `pic` of a stream (ISO 11172-2 2.4.2.5: 10 bits temporal_reference, 3 bits
+// picture_coding_type); 0 while its header byte is not in the buffer yet
+int picture_type_of(const Stream &s, uint32_t pic) {
+	const uint32_t pos = s.pics[pic];
+	return (uint64_t)pos + 5 < s.bb.length ? (s.bb.bytes[pos + 5] >> 3) & 7 : 0;
+}
+
+// Which walk kernel takes picture `pic` of a stream: 0 the lane-parallel walk, 1 the slice walk, 2 the B-picture walk
+int walk_kind(const Batch *b, const Stream &s, uint32_t pic) {
+	// the extension: a type 3 picture goes to the B-picture walk; everything else, and everything without it, to the I/P walk
+	const int type = picture_type_of(s, pic);
+	int kind = (b->decode_b && type == 3) ? 2 : 0;
+	if (b->slice_walk && (type == 1 || type == 2)) {  // enough slice start codes between this picture's and the next one's?
+		const uint32_t hi = pic + 1 < s.pic_code.size() ? s.pic_code[pic + 1] : (uint32_t)s.codes.size();
+		int n_slices = 0;
+		for (uint32_t k = s.pic_code[pic] + 1; k < hi && n_slices < SLICE_WALK_MIN_SLICES; k++) {
+			const uint32_t q = s.codes[k];
+			if (q + 3u < s.bb.length && s.bb.bytes[q + 3u] >= 0x01 && s.bb.bytes[q + 3u] <= 0xAF) n_slices++;
+		}
+		if (n_slices >= SLICE_WALK_MIN_SLICES) kind = 1;
+	}
+	return kind;
+}
+
+// The stage-1 task of picture `pic` of stream `si`: records into `slot`, its info into d_info[info_idx]
+ParseTask parse_task(const Batch *b, int si, uint32_t pic, int slot, int info_idx) {
+	const Stream &s = b->streams[si];
+	ParseTask t{};
+	t.es = s.d_es;
+	t.es_len = s.bb.length;
+	t.start_byte = s.pics[pic] + 4;
+	t.seq = s.d_seq;
+	t.hdr = b->d_hdr + (size_t)slot * b->slot_mb;
+	t.coef = b->d_coef + (size_t)slot * b->slot_mb * MB_COEF_INT16;
+	t.park = b->d_park + (size_t)slot * b->slot_mb * 6;
+	t.info = b->d_info + info_idx;
+	t.mb_width = s.seq.mb_width;
+	t.mb_size = s.seq.mb_size;
+	t.stage = b->d_stage + (size_t)slot * stage_entries_for(b->slot_mb) * 4;
+	t.stage_entries = stage_entries_for(b->slot_mb);
+	t.codes = b->d_codes ? b->d_codes + (size_t)si * b->codes_stride : nullptr;
+	t.n_codes = (uint32_t)s.codes.size();
+	t.code_hint = s.pic_code[pic];
+	return t;
+}
+
 // One round: parse ahead what is missing (one wave, queued chunk by chunk), then -- chunk after chunk, as
 // the chunks' infos arrive -- consume up to want[s] pictures per stream in decode() order and queue their
 // reconstruction.  Returns pictures consumed; `progress[s]` gets the per-stream count, `more[s]` whether
@@ -647,21 +703,8 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			b->free_slots.pop_back();
 			s.cache.push_back(p);
 			++next;
-			// the extension: a picture whose header says type 3 (ISO 11172-2 2.4.2.5: 10 bits temporal_reference, 3 bits
-			// picture_coding_type) goes to the B-picture walk; everything else, and everything without it, to the I/P walk
-			const int type = (uint64_t)p.pos + 5 < s.bb.length ? (s.bb.bytes[p.pos + 5] >> 3) & 7 : 0;
 			const uint32_t pic = (uint32_t)(next - 1 - s.pics.begin());
-			int kind = (b->decode_b && type == 3) ? 2 : 0;
-			if (b->slice_walk && (type == 1 || type == 2)) {  // enough slice start codes between this picture's and the next one's?
-				const uint32_t hi = pic + 1 < s.pic_code.size() ? s.pic_code[pic + 1] : (uint32_t)s.codes.size();
-				int n_slices = 0;
-				for (uint32_t k = s.pic_code[pic] + 1; k < hi && n_slices < SLICE_WALK_MIN_SLICES; k++) {
-					const uint32_t q = s.codes[k];
-					if (q + 3u < s.bb.length && s.bb.bytes[q + 3u] >= 0x01 && s.bb.bytes[q + 3u] <= 0xAF) n_slices++;
-				}
-				if (n_slices >= SLICE_WALK_MIN_SLICES) kind = 1;
-			}
-			fresh.push_back({si, s.cache.size() - 1, (next < s.pics.end() ? *next : s.bb.length) - p.pos, 0, pic, kind});
+			fresh.push_back({si, s.cache.size() - 1, (next < s.pics.end() ? *next : s.bb.length) - p.pos, 0, pic, walk_kind(b, s, pic)});
 		}
 	}
 	// ---- 2. chunks by picture ordinal (position in the stream's look-ahead); a small wave stays whole
@@ -686,24 +729,8 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 		for (int c = 0; c < n_chunks; c++) chunk_off[c + 1] += chunk_off[c];
 		ensure_task_caps(b, (int)fresh.size(), 0);
 		for (size_t i = 0; i < fresh.size(); i++) {
-			Stream &s = b->streams[fresh[i].stream];
-			Parsed &p = s.cache[fresh[i].cache_idx];
-			ParseTask &t = b->h_ptasks[i];
-			t.es = s.d_es;
-			t.es_len = s.bb.length;
-			t.start_byte = p.pos + 4;
-			t.seq = s.d_seq;
-			t.hdr = b->d_hdr + (size_t)p.slot * b->slot_mb;
-			t.coef = b->d_coef + (size_t)p.slot * b->slot_mb * MB_COEF_INT16;
-			t.park = b->d_park + (size_t)p.slot * b->slot_mb * 6;
-			t.info = b->d_info + i;
-			t.mb_width = s.seq.mb_width;
-			t.mb_size = s.seq.mb_size;
-			t.stage = b->d_stage + (size_t)p.slot * stage_entries_for(b->slot_mb) * 4;
-			t.stage_entries = stage_entries_for(b->slot_mb);
-			t.codes = b->d_codes ? b->d_codes + (size_t)fresh[i].stream * b->codes_stride : nullptr;
-			t.n_codes = (uint32_t)s.codes.size();
-			t.code_hint = s.pic_code[fresh[i].pic];
+			const Parsed &p = b->streams[fresh[i].stream].cache[fresh[i].cache_idx];
+			b->h_ptasks[i] = parse_task(b, fresh[i].stream, fresh[i].pic, p.slot, (int)i);
 		}
 		if (b->recon_pending) {  // slots freed by the previous round are still being read by its reconstruct launches
 			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_round, 0));
@@ -1006,6 +1033,136 @@ long batch_decode(Batch *b, int n_pictures, int flags) {
 	return total;
 }
 
+// ---- decode_intra: chosen I pictures of any streams, each as a fresh decoder gives it (DESIGN 3.6) -----------------
+
+// The pictures (indices into s.pics) decode_intra can decode now: after the first sequence header, picture_coding_type
+// 1, and closed -- a later start code is resident whose fourth byte is no slice (01..AF), user data (B2) or extension
+// (B5).  The parse of a closed picture stops at or before that code, so later bytes cannot change it.
+std::vector<uint32_t> intra_index(const Stream &s) {
+	std::vector<uint32_t> out;
+	if (!s.has_seq) return out;
+	for (uint32_t k = 0; k < s.pics.size(); k++) {
+		if (s.pics[k] < s.seq_floor || picture_type_of(s, k) != 1) continue;
+		bool closed = false;
+		for (uint32_t c = s.pic_code[k] + 1; c < s.codes_classified && !closed; c++) {
+			const uint8_t code = s.bb.bytes[s.codes[c] + 3u];
+			closed = !(code >= 0x01 && code <= 0xAF) && code != 0xB2 && code != 0xB5;
+		}
+		if (closed) out.push_back(k);
+	}
+	return out;
+}
+
+long batch_decode_intra(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *planes_dst,
+                        void *const *rgba_dst, int flags, int32_t *n_present_out, int32_t *error_out) {
+	use_device(b);
+	const bool rgba = (flags & JSMPEG_B200_OUT_RGBA) != 0;
+	if (n < 0 || (n > 0 && (!streams || !pictures || !planes_dst || (rgba && !rgba_dst)))) return -2;
+	upload_all(b);
+	// ---- every request is checked before anything changes
+	const int S = (int)b->streams.size();
+	std::vector<std::vector<uint32_t>> listed(S);
+	std::vector<char> indexed(S, 0);
+	size_t fwd_bytes = 0;
+	auto aligned = [](const void *p) { return ((uintptr_t)p & 15u) == 0; };  // stage 2 stores 8 and 16 bytes at a time
+	for (int i = 0; i < n; i++) {
+		const int si = streams[i];
+		if (si < 0 || si >= S || !b->streams[si].has_seq || !planes_dst[i] || !aligned(planes_dst[i])) return -2;
+		if (rgba && (!rgba_dst[i] || !aligned(rgba_dst[i]))) return -2;
+		const Stream &s = b->streams[si];
+		if (!indexed[si]) { listed[si] = intra_index(s); indexed[si] = 1; }
+		if (!std::binary_search(listed[si].begin(), listed[si].end(), pictures[i])) return -2;
+		fwd_bytes = std::max(fwd_bytes, (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64);  // parse_sequence_header's slack
+	}
+	if (n == 0) return 0;
+	ensure_pool(b);
+	if (fwd_bytes > b->intra_fwd_bytes) {
+		if (b->d_intra_fwd) {
+			CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+			CUDA_CHECK(cudaFree(b->d_intra_fwd));
+			b->d_intra_fwd = nullptr;
+			b->intra_fwd_bytes = 0;
+		}
+		b->d_intra_fwd = dev_alloc<uint8_t>(fwd_bytes);
+		CUDA_CHECK(cudaMemsetAsync(b->d_intra_fwd, 0, fwd_bytes, b->st_recon));
+		b->intra_fwd_bytes = fwd_bytes;
+	}
+	// record slots: the free ones; when they do not cover the call, the look-ahead's too (decode() parses those again)
+	if ((int)b->free_slots.size() < n)
+		for (auto &s : b->streams) flush_cache(b, s);
+	const int wave_max = (int)b->free_slots.size();
+	ensure_task_caps(b, std::min(n, wave_max), std::min(n, wave_max));
+	struct Req { int idx, kind; uint32_t bytes; };
+	for (int lo = 0; lo < n;) {
+		const int m = std::min(n - lo, wave_max);
+		// ---- stage 1: one wave, grouped by walk kernel and longest first, like decode_round
+		std::vector<Req> wave(m);
+		for (int j = 0; j < m; j++) {
+			const int r = lo + j;
+			const Stream &s = b->streams[streams[r]];
+			const uint32_t pic = pictures[r];
+			const uint32_t end = pic + 1 < s.pics.size() ? s.pics[pic + 1] : s.bb.length;
+			wave[j] = {r, walk_kind(b, s, pic), end - s.pics[pic]};
+		}
+		std::stable_sort(wave.begin(), wave.end(), [](const Req &x, const Req &y) {
+			return x.kind != y.kind ? x.kind < y.kind : x.bytes > y.bytes;
+		});
+		std::vector<int> slot(m);
+		int n_lanes = 0;  // pictures for the lane-parallel walk; the rest go to the slice walk
+		for (int j = 0; j < m; j++) {
+			slot[j] = b->free_slots.back();
+			b->free_slots.pop_back();
+			b->h_ptasks[j] = parse_task(b, streams[wave[j].idx], pictures[wave[j].idx], slot[j], j);
+			n_lanes += wave[j].kind == 0;
+		}
+		if (b->recon_pending) {  // reconstruct launches of an earlier round or wave may still read these slots
+			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_round, 0));
+			b->recon_pending = false;
+		}
+		CUDA_CHECK(cudaMemcpyAsync(b->d_ptasks, b->h_ptasks, m * sizeof(ParseTask), cudaMemcpyHostToDevice, b->st_main));
+		if (n_lanes) launch_parse_pictures(b->d_ptasks, n_lanes, b->slot_mb, b->st_main, nullptr, &b->fork);
+		if (m > n_lanes) launch_parse_pictures_slices(b->d_ptasks + n_lanes, m - n_lanes, b->slot_mb, b->st_main);
+		CUDA_CHECK(cudaMemcpyAsync(b->h_info, b->d_info, m * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		// ---- stage 2: into the caller's planes, predicted (skipped macroblocks) from the zeroed scratch set
+		int n_rec = 0;
+		for (int j = 0; j < m; j++) {
+			const int r = wave[j].idx;
+			const Stream &s = b->streams[streams[r]];
+			const picture_info_t &info = b->h_info[j];
+			if (n_present_out) n_present_out[r] = info.n_present;
+			if (error_out) error_out[r] = info.error;
+			CUDA_CHECK(cudaMemsetAsync(planes_dst[r], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
+			if (rgba) CUDA_CHECK(cudaMemsetAsync(rgba_dst[r], 0xff, (size_t)s.width * s.height * 4, b->st_recon));
+			if (info.status != PIC_DECODED) continue;
+			ReconTask t{};
+			t.hdr = b->d_hdr + (size_t)slot[j] * b->slot_mb;
+			t.coef = b->d_coef + (size_t)slot[j] * b->slot_mb * MB_COEF_INT16;
+			t.cur = plane_set(s, static_cast<uint8_t *>(planes_dst[r]));
+			t.fwd = plane_set(s, b->d_intra_fwd);
+			t.mb_width = s.seq.mb_width;
+			t.mb_size = s.seq.mb_size;
+			t.coded_width = s.seq.coded_width;
+			t.coded_height = s.seq.coded_height;
+			t.rgba = rgba ? static_cast<uint8_t *>(rgba_dst[r]) : nullptr;
+			t.width = s.width;
+			t.height = s.height;
+			b->h_rtasks[n_rec++] = t;
+		}
+		if (n_rec) {
+			if (rgba) launch_reconstruct_rgba(b->h_rtasks, n_rec, b->st_recon);
+			else launch_reconstruct(b->h_rtasks, n_rec, b->st_recon);
+		}
+		CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
+		b->recon_pending = true;
+		for (int j = 0; j < m; j++) release_slot(b, slot[j]);  // reused by the next wave's parse, which waits for ev_round
+		lo += m;
+	}
+	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+	b->recon_pending = false;
+	return n;
+}
+
 int env_int(const char *name, int fallback) {
 	const char *e = getenv(name);
 	return e && *e ? atoi(e) : fallback;
@@ -1115,6 +1272,7 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b) {
 	if (b->d_ptasks) cudaFree(b->d_ptasks);
 	if (b->h_rtasks) cudaFreeHost(b->h_rtasks);
 	if (b->d_rtasks) cudaFree(b->d_rtasks);
+	if (b->d_intra_fwd) cudaFree(b->d_intra_fwd);
 	ts_scratch_destroy(b->ts);
 	ps_scratch_destroy(b->ps);
 	cudaEvent_t evs[] = {b->ev_a, b->ev_b, b->ev_mid, b->ev_step, b->ev_round, b->ev_copied[0], b->ev_copied[1], b->fork.fork};
@@ -1214,6 +1372,7 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 			s.d_last = nullptr;
 			s.last_type = s.last_temporal = 0;
 			s.h_head = -1;
+			s.seq_floor = 0;
 			if (s.has_seq) {
 				for (auto p : s.d_planes) CUDA_CHECK(cudaMemsetAsync(p, 0, (size_t)s.coded_size * 3 / 2, b->st_main));
 				for (auto p : s.d_planes_b) if (p) CUDA_CHECK(cudaMemsetAsync(p, 0, (size_t)s.coded_size * 3 / 2, b->st_main));
@@ -1225,6 +1384,32 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 
 long jsmpeg_b200_batch_decode(jsmpeg_b200_batch_t *b, int n_pictures, int flags) {
 	return guarded<long>(b, 0, [&] { return batch_decode(b, n_pictures, flags); });
+}
+
+long jsmpeg_b200_batch_intra_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out, uint32_t *byte_pos_out,
+                                   int32_t *temporal_reference_out, long n_max) {
+	return guarded<long>(b, -1, [&]() -> long {
+		if (stream < 0 || stream >= (int)b->streams.size()) return -2;
+		use_device(b);
+		upload_all(b);
+		const Stream &s = b->streams[stream];
+		const std::vector<uint32_t> listed = intra_index(s);
+		for (long i = 0; i < std::min<long>((long)listed.size(), n_max); i++) {
+			const uint32_t pos = s.pics[listed[i]];
+			if (picture_out) picture_out[i] = listed[i];
+			if (byte_pos_out) byte_pos_out[i] = pos;
+			if (temporal_reference_out) temporal_reference_out[i] = s.bb.bytes[pos + 4] << 2 | s.bb.bytes[pos + 5] >> 6;
+		}
+		return (long)listed.size();
+	});
+}
+
+long jsmpeg_b200_batch_decode_intra(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                    void *const *planes_dst, void *const *rgba_dst, int flags, int32_t *n_present_out,
+                                    int32_t *error_out) {
+	return guarded<long>(b, -1, [&] {
+		return batch_decode_intra(b, n, streams, pictures, planes_dst, rgba_dst, flags, n_present_out, error_out);
+	});
 }
 
 int jsmpeg_b200_batch_get_planes(jsmpeg_b200_batch_t *b, int stream, void **y, void **cr, void **cb) {
