@@ -215,6 +215,32 @@ long jsmpeg_b200_batch_decode_intra(jsmpeg_b200_batch_t *b, int n, const int *st
                                     void *const *planes_dst, void *const *rgba_dst, int flags,
                                     int32_t *n_present_out, int32_t *error_out);
 
+/* RANDOM ACCESS (seek, frame sampling): any picture decode() would reconstruct, decoded from its chain start,
+ * independently of decode(), many short chains side by side.  The index lists picture k (numbered as above) when it
+ * starts after the first sequence header, is closed (as above), is one decode() reconstructs -- an I picture, a P
+ * picture with forward_f_code != 0, and while the "decode_b" option is on a B picture with both f_codes != 0 -- and
+ * has a chain start: the greatest picture j <= k of the intra index such that at least r pictures of [j, k) are
+ * references (I, or P with forward_f_code != 0), r = 0 for I, 1 for P, 2 for B.  (So j = k for an I picture, the
+ * last I picture before it for a P picture, one GOP further back for a B picture of an open GOP.)  A listed picture
+ * decodes to exactly what get_planes gives after the decode() that consumes it, in a fresh decoder (every plane set
+ * zeroed, the batch's current decode_b) fed the first sequence header + the bytes from picture j up to and including
+ * picture k's closing code.  Where every picture from j through k codes every macroblock, that is what decode()
+ * gives at that point of the stream.  (Damaged input: a walk that runs across a closing code reads the stream's
+ * bytes behind it, as decode() does -- DESIGN 3.7.)  Neither call changes anything decode() observes, as above. */
+
+/* Pictures of `stream` that decode_pictures can decode now; returns how many there are (-1 dead, -2 stream out of
+ * range); the first min(count, n_max) go to the arrays (picture_coding_type to type_out), any of which may be NULL. */
+long jsmpeg_b200_batch_picture_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out,
+                                     uint32_t *byte_pos_out, int32_t *type_out, int32_t *temporal_reference_out,
+                                     uint32_t *chain_start_out, long n_max);
+/* Decode n listed pictures, of any streams; destinations, flags, synchronism and the -2 rule as decode_intra, the
+ * requests checked against the picture index.  status_out[i] (may be NULL) is PIC_DECODED, or 0 when the fresh
+ * decoder never consumes picture k (a damaged earlier picture's walk ran across its start code): its planes are
+ * then 0, its RGBA opaque white, its n_present / error 0.  Duplicate requests each get the picture. */
+long jsmpeg_b200_batch_decode_pictures(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                       void *const *planes_dst, void *const *rgba_dst, int flags,
+                                       int32_t *status_out, int32_t *n_present_out, int32_t *error_out);
+
 void jsmpeg_b200_batch_get_stats(jsmpeg_b200_batch_t *b, jsmpeg_b200_stats_t *out);
 void jsmpeg_b200_batch_reset_stats(jsmpeg_b200_batch_t *b);
 

@@ -55,6 +55,8 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_last_picture": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_batch_intra_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
+    "jsmpeg_b200_batch_picture_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, ctypes.c_long]),
+    "jsmpeg_b200_batch_decode_pictures": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_get_stats": (None, [_VP, ctypes.POINTER(Stats)]),
     "jsmpeg_b200_batch_reset_stats": (None, [_VP]),
     "jsmpeg_b200_debug_parse_picture": (ctypes.c_int, [_VP, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int, ctypes.c_int,
@@ -98,6 +100,7 @@ class BatchDecoder:
         self.device = device
         self._pes = [[] for _ in range(n_streams)]  # per stream: every (payload byte offset, pts seconds) write_ts/write_ps returned
         self.last_intra_info = []  # per request of the last decode_intra: {"n_present", "error"} (picture_info_t)
+        self.last_pictures_info = []  # per request of the last decode_pictures: {"status", "n_present", "error"}
         self.handle = self.lib.jsmpeg_b200_batch_create(n_streams, device, max_slots)
         err = self.lib.jsmpeg_b200_batch_last_error(self.handle)
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
@@ -248,21 +251,59 @@ class BatchDecoder:
             raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_intra_index failed")
         pic, pos, tr = np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.int32)
         n = self.lib.jsmpeg_b200_batch_intra_index(self.handle, stream, pic.ctypes.data, pos.ctypes.data, tr.ctypes.data, n)
-        pes = self._pes[stream]
-        offsets = [o for o, _ in pes]
         out = []
         for i in range(min(n, len(pic))):
-            j = bisect.bisect_right(offsets, int(pos[i])) - 1
             out.append({"picture": int(pic[i]), "byte_pos": int(pos[i]), "temporal_reference": int(tr[i]),
-                        "pts": pes[j][1] if j >= 0 else None})
+                        "pts": self._pts(stream, int(pos[i]))})
+        return out
+
+    def _pts(self, stream, byte_pos):
+        """PTS (seconds) of the last PES packet write_ts / write_ps reported at or before `byte_pos`, or None."""
+        pes = self._pes[stream]
+        j = bisect.bisect_right([o for o, _ in pes], byte_pos) - 1
+        return pes[j][1] if j >= 0 else None
+
+    def picture_index(self, stream):
+        """The pictures of `stream` that decode_pictures can decode now (include/jsmpeg_b200.h): one dict per picture,
+        {"picture": k, "byte_pos", "type" (picture_coding_type), "temporal_reference", "chain_start", "pts"}; `pts`
+        as in intra_index.  Follows the decode_b option's current value."""
+        n = self.lib.jsmpeg_b200_batch_picture_index(self.handle, stream, None, None, None, None, None, 0)
+        if n == -2:
+            raise ValueError(f"stream {stream} out of range")
+        if n < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_picture_index failed")
+        pic, pos, start = np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.uint32)
+        kind, tr = np.zeros(n, np.int32), np.zeros(n, np.int32)
+        n = self.lib.jsmpeg_b200_batch_picture_index(self.handle, stream, pic.ctypes.data, pos.ctypes.data,
+                                                     kind.ctypes.data, tr.ctypes.data, start.ctypes.data, n)
+        return [{"picture": int(pic[i]), "byte_pos": int(pos[i]), "type": int(kind[i]), "temporal_reference": int(tr[i]),
+                 "chain_start": int(start[i]), "pts": self._pts(stream, int(pos[i]))} for i in range(min(n, len(pic)))]
+
+    def decode_pictures(self, requests, rgba=False):
+        """Decode pictures listed by picture_index, of any streams, in one call: `requests` is an iterable of (stream,
+        picture).  Returns what decode_intra returns; last_pictures_info gets {"status", "n_present", "error"} per
+        request (status 1: decoded; 0: the fresh decoder never reached the picture, whose planes are then 0)."""
+        reqs = [(int(s), int(p)) for s, p in requests]
+        status = (ctypes.c_int32 * max(len(reqs), 1))()
+        out, n_present, errors = self._decode_requests(self.lib.jsmpeg_b200_batch_decode_pictures, reqs, rgba, [status],
+                                                       "a request names a picture that is not in the stream's picture index")
+        self.last_pictures_info = [{"status": status[i], "n_present": n_present[i], "error": errors[i]} for i in range(len(reqs))]
         return out
 
     def decode_intra(self, requests, rgba=False):
         """Decode I pictures listed by intra_index, of any streams, in one call: `requests` is an iterable of (stream,
         picture).  Returns per request a torch.uint8 CUDA tensor of coded_size * 3 // 2 bytes (Y | Cr | Cb, see
         planes_view), or with rgba=True a pair (planes, rgba [height, width, 4])."""
-        import torch
         reqs = [(int(s), int(p)) for s, p in requests]
+        out, n_present, errors = self._decode_requests(self.lib.jsmpeg_b200_batch_decode_intra, reqs, rgba, [],
+                                                       "a request names a picture that is not in the stream's intra index")
+        self.last_intra_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(len(reqs))]
+        return out
+
+    def _decode_requests(self, fn, reqs, rgba, extra_out, refused):
+        """Allocate the destinations of (stream, picture) requests and call `fn` (decode_intra / decode_pictures) with
+        `extra_out` before n_present and error.  Returns (outputs, n_present, errors)."""
+        import torch
         n = len(reqs)
         dev = torch.device("cuda", self.device)
         planes, images = [], []
@@ -282,14 +323,13 @@ class BatchDecoder:
         n_present = (ctypes.c_int32 * max(n, 1))()
         errors = (ctypes.c_int32 * max(n, 1))()
         torch.cuda.current_stream(dev).synchronize()  # the allocations are the caller's stream's; the call uses its own
-        got = self.lib.jsmpeg_b200_batch_decode_intra(self.handle, n, streams, pictures, planes_dst, rgba_dst,
-                                                      OUT_RGBA if rgba else OUT_DEVICE, n_present, errors)
+        got = fn(self.handle, n, streams, pictures, planes_dst, rgba_dst, OUT_RGBA if rgba else OUT_DEVICE, *extra_out,
+                 n_present, errors)
         if got == -2:
-            raise ValueError("a request names a picture that is not in the stream's intra index")
+            raise ValueError(refused)
         if got < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_intra failed")
-        self.last_intra_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
-        return list(zip(planes, images)) if rgba else planes
+            raise RuntimeError(self.last_error() or f"{fn.__name__} failed")
+        return (list(zip(planes, images)) if rgba else planes), n_present, errors
 
     def last_picture(self, stream):
         """(picture_coding_type, temporal_reference) of the picture the stream's last decode() consumed, or None."""

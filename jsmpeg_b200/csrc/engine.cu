@@ -162,9 +162,12 @@ struct jsmpeg_b200_batch_t {
 	bool batch_copy_ok = true;
 	TsScratch *ts = nullptr;
 	PsScratch *ps = nullptr;
-	// decode_intra: the forward plane set its reconstruct tasks name, zeroed and never written (DESIGN 3.6)
+	// decode_pictures / decode_intra: the forward plane set a chain of one picture names, zeroed and never written
+	// (DESIGN 3.6); and the pool of the other chains' plane sets, zeroed per chain group (DESIGN 3.7)
 	uint8_t *d_intra_fwd = nullptr;
 	size_t intra_fwd_bytes = 0;
+	uint8_t *d_chain_sets = nullptr;
+	size_t chain_sets_bytes = 0;
 	jsmpeg_b200_stats_t stats{};
 };
 
@@ -587,11 +590,30 @@ bool entry_stale(const Stream &s, const Parsed &e) {
 	return e.len_at_parse != s.bb.length && (uint64_t)e.info.end_bit + 64 >= (uint64_t)e.len_at_parse * 8;
 }
 
+// b->copy_dst / copy_src / copy_size in ONE batched copy call on `st` (cudaMemcpyBatchAsync, CUDA 12.8+); plain
+// copies where the driver has no batched copy
+void copy_batch(Batch *b, cudaStream_t st) {
+	const size_t n_copy = b->copy_dst.size();
+	bool batched = false;
+	if (b->batch_copy_ok && n_copy > 1) {
+		cudaMemcpyAttributes attr{};
+		attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
+		size_t attr_idx = 0, fail_idx = 0;
+		cudaError_t e = cudaMemcpyBatchAsync(b->copy_dst.data(), b->copy_src.data(), b->copy_size.data(), n_copy,
+		                                     &attr, &attr_idx, 1, &fail_idx, st);
+		if (e == cudaSuccess) batched = true;
+		else { (void)cudaGetLastError(); b->batch_copy_ok = false; }  // older driver: plain copies from now on
+	}
+	if (!batched)
+		for (size_t i = 0; i < n_copy; i++)
+			CUDA_CHECK(cudaMemcpyAsync(b->copy_dst[i], b->copy_src[i], b->copy_size[i], cudaMemcpyDefault, st));
+}
+
 // The copy-out of one reconstruct launch's pictures (OUT_HOST), on the copy stream.
 void copy_out_step(Batch *b, const std::vector<ReconTask> &tasks, const std::vector<int> &stream_ids) {
 	CUDA_CHECK(cudaEventRecord(b->ev_step, b->st_recon));
 	CUDA_CHECK(cudaStreamWaitEvent(b->st_copy, b->ev_step, 0));
-	// all pictures of the step leave in ONE batched copy call (cudaMemcpyBatchAsync, CUDA 12.8+)
+	// all pictures of the step leave in one batched copy call
 	const size_t n_copy = tasks.size();
 	b->copy_dst.resize(n_copy);
 	b->copy_src.resize(n_copy);
@@ -604,19 +626,7 @@ void copy_out_step(Batch *b, const std::vector<ReconTask> &tasks, const std::vec
 		b->copy_size[i] = (size_t)s.coded_size * 3 / 2;
 		b->stats.d2h_bytes += b->copy_size[i];
 	}
-	bool batched = false;
-	if (b->batch_copy_ok && n_copy > 1) {
-		cudaMemcpyAttributes attr{};
-		attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
-		size_t attr_idx = 0, fail_idx = 0;
-		cudaError_t e = cudaMemcpyBatchAsync(b->copy_dst.data(), b->copy_src.data(), b->copy_size.data(), n_copy,
-		                                     &attr, &attr_idx, 1, &fail_idx, b->st_copy);
-		if (e == cudaSuccess) batched = true;
-		else { (void)cudaGetLastError(); b->batch_copy_ok = false; }  // older driver: plain copies from now on
-	}
-	if (!batched)
-		for (size_t i = 0; i < n_copy; i++)
-			CUDA_CHECK(cudaMemcpyAsync(b->copy_dst[i], b->copy_src[i], b->copy_size[i], cudaMemcpyDeviceToHost, b->st_copy));
+	copy_batch(b, b->st_copy);
 	CUDA_CHECK(cudaEventRecord(b->ev_copied[b->copy_steps & 1], b->st_copy));
 	b->copy_steps++;
 }
@@ -1033,24 +1043,352 @@ long batch_decode(Batch *b, int n_pictures, int flags) {
 	return total;
 }
 
-// ---- decode_intra: chosen I pictures of any streams, each as a fresh decoder gives it (DESIGN 3.6) -----------------
+// ---- decode_pictures / decode_intra: chosen pictures of any streams, each as a fresh decoder gives it from its chain
+// start (DESIGN 3.6, 3.7) ------------------------------------------------------------------------------------------
+
+// Picture k is closed when a later start code is resident whose fourth byte is no slice (01..AF), user data (B2) or
+// extension (B5).  The parse of a closed picture stops at or before that code, so later bytes cannot change it.
+bool picture_closed(const Stream &s, uint32_t k) {
+	for (uint32_t c = s.pic_code[k] + 1; c < s.codes_classified; c++) {
+		const uint8_t code = s.bb.bytes[s.codes[c] + 3u];
+		if (!(code >= 0x01 && code <= 0xAF) && code != 0xB2 && code != 0xB5) return true;
+	}
+	return false;
+}
 
 // The pictures (indices into s.pics) decode_intra can decode now: after the first sequence header, picture_coding_type
-// 1, and closed -- a later start code is resident whose fourth byte is no slice (01..AF), user data (B2) or extension
-// (B5).  The parse of a closed picture stops at or before that code, so later bytes cannot change it.
+// 1, and closed.
 std::vector<uint32_t> intra_index(const Stream &s) {
 	std::vector<uint32_t> out;
 	if (!s.has_seq) return out;
+	for (uint32_t k = 0; k < s.pics.size(); k++)
+		if (s.pics[k] >= s.seq_floor && picture_type_of(s, k) == 1 && picture_closed(s, k)) out.push_back(k);
+	return out;
+}
+
+// `n` bits of picture `pic`'s header, from bit `bit` after its start code (ISO 11172-2 2.4.2.5: temporal_reference 10,
+// picture_coding_type 3, vbv_delay 16, full_pel_forward_vector 1, forward_f_code 3, full_pel_backward_vector 1,
+// backward_f_code 3).  Bytes beyond the buffer read as 0, as they do to the walks.
+uint32_t picture_header_bits(const Stream &s, uint32_t pic, int bit, int n) {
+	uint32_t v = 0;
+	for (int i = 0; i < n; i++, bit++) {
+		const uint64_t byte = (uint64_t)s.pics[pic] + 4 + (bit >> 3);
+		v = v << 1 | (byte < s.bb.length ? (s.bb.bytes[byte] >> (7 - (bit & 7))) & 1u : 0u);
+	}
+	return v;
+}
+
+// Whether decode() reconstructs picture k (PIC_DECODED), by the walks' rule (walk.cuh, walk_b.cuh): an I picture, a
+// P picture with forward_f_code != 0, and with decode_b a B picture with both f_codes != 0
+bool picture_decoded(const Batch *b, const Stream &s, uint32_t k) {
+	const int type = picture_type_of(s, k);
+	if (type == 1) return true;
+	if (type == 2) return picture_header_bits(s, k, 30, 3) != 0;
+	return type == 3 && b->decode_b && picture_header_bits(s, k, 30, 3) != 0 && picture_header_bits(s, k, 34, 3) != 0;
+}
+
+struct IndexEntry {
+	uint32_t pic, chain_start;
+};
+
+// The pictures decode_pictures can decode now: after the first sequence header, closed, reconstructed by decode(),
+// and with a chain start -- the greatest picture j <= k of the intra index such that at least r(k) pictures of
+// [j, k) are references (I, or P with forward_f_code != 0); r = 0 for I, 1 for P, 2 for B.
+std::vector<IndexEntry> picture_index(const Batch *b, const Stream &s) {
+	std::vector<IndexEntry> out;
+	if (!s.has_seq) return out;
+	std::vector<uint32_t> keys;      // the I pictures after the sequence header so far
+	std::vector<uint32_t> refs_upto;  // refs_upto[k]: references among pictures [0, k)
+	uint32_t refs = 0;
 	for (uint32_t k = 0; k < s.pics.size(); k++) {
-		if (s.pics[k] < s.seq_floor || picture_type_of(s, k) != 1) continue;
-		bool closed = false;
-		for (uint32_t c = s.pic_code[k] + 1; c < s.codes_classified && !closed; c++) {
-			const uint8_t code = s.bb.bytes[s.codes[c] + 3u];
-			closed = !(code >= 0x01 && code <= 0xAF) && code != 0xB2 && code != 0xB5;
-		}
-		if (closed) out.push_back(k);
+		refs_upto.push_back(refs);
+		const int type = picture_type_of(s, k);
+		const bool after = s.pics[k] >= s.seq_floor;
+		if (after && type == 1) keys.push_back(k);
+		refs += type == 1 || (type == 2 && picture_header_bits(s, k, 30, 3) != 0);
+		if (!after || !picture_decoded(b, s, k) || !picture_closed(s, k)) continue;
+		const uint32_t need = type == 1 ? 0 : type - 1;
+		// (every key is a reference: this looks at most three keys back)
+		for (auto j = keys.rbegin(); j != keys.rend(); ++j)
+			if (refs_upto[k] - refs_upto[*j] >= need) {
+				out.push_back({k, *j});
+				break;
+			}
 	}
 	return out;
+}
+
+// One request: picture `pic` of stream `stream`, decoded by a fresh decoder from picture `from` (its chain start) on
+struct PictureRequest {
+	int stream;
+	uint32_t pic, from;
+};
+
+// The schedule behind decode_pictures and decode_intra (DESIGN 3.7).  Requests with the same stream and chain start
+// form a chain: pictures [first, last], parsed in waves over consecutive positions of every chain, consumed on the
+// host by decode()'s rule and reconstructed in launches by depth (launch d: the d-th reconstructed picture of every
+// chain of the wave).  A requested picture is copied to its destination right behind its launch -- or, in a chain
+// that reconstructs nothing else, reconstructed straight into it.  The requests are valid (the caller checked them).
+void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const *planes_dst, void *const *rgba_dst,
+                   bool rgba, int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
+	const int n = (int)req.size();
+	ensure_pool(b);
+	std::vector<int> order(n);  // the requests by stream, chain start and picture
+	for (int i = 0; i < n; i++) order[i] = i;
+	std::sort(order.begin(), order.end(), [&](int x, int y) {
+		const PictureRequest &p = req[x], &q = req[y];
+		return p.stream != q.stream ? p.stream < q.stream : p.from != q.from ? p.from < q.from : p.pic != q.pic ? p.pic < q.pic : x < y;
+	});
+	struct Chain {
+		int stream;
+		uint32_t first, last;  // chain start, last requested picture
+		uint32_t b_end;        // last requested B picture + 1; 0: none (B pictures after it are not reconstructed)
+		int req_lo, req_hi;    // its requests: order[req_lo .. req_hi)
+		int req_next;          // the first of them not consumed yet
+		int n_sets;            // plane sets: 0 (a leaf: it reconstructs the one picture requested), 2 (I/P), 4 (+ B)
+		uint8_t *set[4];
+		int cur, b_cur;        // as Stream::cur / b_cur
+		uint32_t next;         // the picture decode() consumes next; beyond `last`: the chain is done
+		std::vector<picture_info_t> info;  // per picture of the chain, once parsed
+		std::vector<int> slot;
+	};
+	std::vector<Chain> chains;
+	size_t set_bytes = 0, n_tasks = 0;
+	bool leaves = false;
+	for (int lo = 0; lo < n;) {
+		const PictureRequest &r = req[order[lo]];
+		int hi = lo + 1;
+		while (hi < n && req[order[hi]].stream == r.stream && req[order[hi]].from == r.from) hi++;
+		const Stream &s = b->streams[r.stream];
+		Chain c{};
+		c.stream = r.stream;
+		c.first = c.next = r.from;
+		c.last = req[order[hi - 1]].pic;
+		for (int i = lo; i < hi; i++)
+			if (picture_type_of(s, req[order[i]].pic) == 3) c.b_end = req[order[i]].pic + 1;
+		c.req_lo = c.req_next = lo;
+		c.req_hi = hi;
+		c.n_sets = c.last == c.first ? 0 : (c.b_end ? 4 : 2);
+		c.info.resize(c.last - c.first + 1);
+		c.slot.resize(c.last - c.first + 1);
+		leaves |= c.n_sets == 0;
+		// + coded_width + 64: parse_sequence_header's slack; a multiple of 256 keeps every set of the pool aligned
+		set_bytes = std::max(set_bytes, ((size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64 + 255) & ~(size_t)255);
+		n_tasks += c.info.size();
+		chains.push_back(std::move(c));
+		lo = hi;
+	}
+	if (leaves && set_bytes > b->intra_fwd_bytes) {
+		if (b->d_intra_fwd) {
+			CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+			CUDA_CHECK(cudaFree(b->d_intra_fwd));
+			b->d_intra_fwd = nullptr;
+			b->intra_fwd_bytes = 0;
+		}
+		b->d_intra_fwd = dev_alloc<uint8_t>(set_bytes);
+		CUDA_CHECK(cudaMemsetAsync(b->d_intra_fwd, 0, set_bytes, b->st_recon));
+		b->intra_fwd_bytes = set_bytes;
+	}
+	// what a request that is never consumed keeps: planes 0, RGBA opaque white.  A leaf is reconstructed into its
+	// destination, whose absent macroblocks keep that 0; every other destination is written whole by a copy.
+	for (const Chain &c : chains)
+		for (int q = c.req_lo; q < c.req_hi; q++) {
+			const int i = order[q];
+			const Stream &s = b->streams[req[i].stream];
+			if (c.n_sets == 0) CUDA_CHECK(cudaMemsetAsync(planes_dst[i], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
+			if (rgba) CUDA_CHECK(cudaMemsetAsync(rgba_dst[i], 0xff, (size_t)s.width * s.height * 4, b->st_recon));
+		}
+	std::vector<int32_t> status(n, 0), n_present(n, 0), error(n, 0);
+	// record slots: the free ones; when they do not cover the call, the look-ahead's too (decode() parses those again)
+	if (b->free_slots.size() < n_tasks)
+		for (auto &s : b->streams) flush_cache(b, s);
+	const int wave_max = (int)b->free_slots.size();
+	ensure_task_caps(b, (int)std::min<size_t>(n_tasks, (size_t)wave_max), 0);
+	// chain groups: at most wave_max chains (a wave parses at least one picture of each), and plane sets within half
+	// of the free device memory -- a request beyond the device is cut into groups, not refused
+	size_t free_b = 0, total_b = 0;
+	CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+	const size_t max_sets = std::max<size_t>(4, ((size_t)(0.5 * (double)free_b) + b->chain_sets_bytes) / set_bytes);
+	std::vector<std::pair<size_t, size_t>> groups;
+	size_t most_sets = 0;
+	for (size_t lo = 0; lo < chains.size();) {
+		size_t hi = lo, sets = 0;
+		while (hi < chains.size() && hi - lo < (size_t)wave_max && sets + chains[hi].n_sets <= max_sets) sets += chains[hi++].n_sets;
+		groups.push_back({lo, hi});
+		most_sets = std::max(most_sets, sets);
+		lo = hi;
+	}
+	if (most_sets * set_bytes > b->chain_sets_bytes) {
+		if (b->d_chain_sets) {
+			CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+			CUDA_CHECK(cudaFree(b->d_chain_sets));
+			b->d_chain_sets = nullptr;
+			b->chain_sets_bytes = 0;
+		}
+		b->d_chain_sets = dev_alloc<uint8_t>(most_sets * set_bytes);
+		b->chain_sets_bytes = most_sets * set_bytes;
+	}
+	struct Task { int chain; uint32_t pic; int kind; uint32_t bytes; };
+	// per depth: the I/P and B tasks without and with the fused RGBA conversion, then the copies to destinations
+	struct Depth { std::vector<ReconTask> ip, ip_rgba, bi, bi_rgba; std::vector<void *> dst, src; std::vector<size_t> size; };
+	for (const auto &[glo, ghi] : groups) {
+		size_t sets = 0;
+		for (size_t c = glo; c < ghi; c++)
+			for (int k = 0; k < chains[c].n_sets; k++) chains[c].set[k] = b->d_chain_sets + set_bytes * sets++;
+		if (sets)  // a fresh decoder's planes start zeroed, the B sets too (the previous group's copies are queued before)
+			CUDA_CHECK(cudaMemsetAsync(b->d_chain_sets, 0, set_bytes * sets, b->st_recon));
+		const uint32_t width = (uint32_t)std::max<size_t>(1, (size_t)wave_max / (ghi - glo));
+		for (uint32_t lo = 0;; lo += width) {
+			// ---- stage 1: positions [lo, lo + width) of every chain still consuming, grouped by walk kernel and longest
+			// first, like decode_round
+			std::vector<Task> wave;
+			for (size_t c = glo; c < ghi; c++) {
+				const Chain &ch = chains[c];
+				if (ch.next > ch.last) continue;
+				const Stream &s = b->streams[ch.stream];
+				for (uint32_t p = ch.first + lo; p <= ch.last && p - ch.first < lo + width; p++) {
+					const uint32_t end = p + 1 < s.pics.size() ? s.pics[p + 1] : s.bb.length;
+					wave.push_back({(int)c, p, walk_kind(b, s, p), end - s.pics[p]});
+				}
+			}
+			if (wave.empty()) break;
+			std::stable_sort(wave.begin(), wave.end(), [](const Task &x, const Task &y) {
+				return x.kind != y.kind ? x.kind < y.kind : x.bytes > y.bytes;
+			});
+			const int m = (int)wave.size();
+			int cnt[3] = {0, 0, 0};
+			for (int t = 0; t < m; t++) {
+				Chain &ch = chains[wave[t].chain];
+				const int slot = b->free_slots.back();
+				b->free_slots.pop_back();
+				ch.slot[wave[t].pic - ch.first] = slot;
+				b->h_ptasks[t] = parse_task(b, ch.stream, wave[t].pic, slot, t);
+				cnt[wave[t].kind]++;
+			}
+			if (b->recon_pending) {  // reconstruct launches of an earlier round or wave may still read these slots
+				CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_round, 0));
+				b->recon_pending = false;
+			}
+			CUDA_CHECK(cudaMemcpyAsync(b->d_ptasks, b->h_ptasks, m * sizeof(ParseTask), cudaMemcpyHostToDevice, b->st_main));
+			if (cnt[0]) launch_parse_pictures(b->d_ptasks, cnt[0], b->slot_mb, b->st_main, nullptr, &b->fork);
+			if (cnt[1]) launch_parse_pictures_slices(b->d_ptasks + cnt[0], cnt[1], b->slot_mb, b->st_main);
+			if (cnt[2]) launch_parse_pictures_b(b->d_ptasks + cnt[0] + cnt[1], cnt[2], b->slot_mb, b->st_main);
+			CUDA_CHECK(cudaMemcpyAsync(b->h_info, b->d_info, m * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
+			CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+			for (int t = 0; t < m; t++) {
+				Chain &ch = chains[wave[t].chain];
+				ch.info[wave[t].pic - ch.first] = b->h_info[t];
+			}
+			// ---- decode()'s consumption rule over the infos (decode_round): which pictures reconstruct, at which depth
+			std::vector<Depth> depths;
+			for (size_t c = glo; c < ghi; c++) {
+				Chain &ch = chains[c];
+				const Stream &s = b->streams[ch.stream];
+				const uint32_t parsed_end = std::min(ch.last + 1, ch.first + lo + width);
+				size_t d = 0;
+				while (ch.next < parsed_end) {
+					const uint32_t k = ch.next;
+					const picture_info_t &e = ch.info[k - ch.first];
+					while (ch.req_next < ch.req_hi && req[order[ch.req_next]].pic < k) ch.req_next++;  // passed over: status 0
+					const int q_lo = ch.req_next;
+					while (ch.req_next < ch.req_hi && req[order[ch.req_next]].pic == k) ch.req_next++;
+					const int q_hi = ch.req_next;
+					for (int q = q_lo; q < q_hi; q++) {
+						status[order[q]] = e.status;
+						n_present[order[q]] = e.n_present;
+						error[order[q]] = e.error;
+					}
+					const bool is_b = e.picture_type == 3;  // (only the B walk answers PIC_DECODED for one)
+					if (e.status == PIC_DECODED && (!is_b || k < ch.b_end)) {
+						const int slot = ch.slot[k - ch.first];
+						ReconTask t{};
+						t.hdr = b->d_hdr + (size_t)slot * b->slot_mb;
+						t.coef = b->d_coef + (size_t)slot * b->slot_mb * MB_COEF_INT16;
+						const bool leaf = ch.n_sets == 0;
+						if (is_b) {  // the two I/P sets: `cur` the older (forward), `1 - cur` the newer (backward) reference
+							t.cur = plane_set(s, ch.set[2 + ch.b_cur]);
+							t.fwd = plane_set(s, ch.set[ch.cur]);
+							t.bwd = plane_set(s, ch.set[1 - ch.cur]);
+						} else if (leaf) {  // into the destination, predicted (skipped macroblocks) from the zeroed scratch set
+							t.cur = plane_set(s, static_cast<uint8_t *>(planes_dst[order[q_lo]]));
+							t.fwd = plane_set(s, b->d_intra_fwd);
+						} else {
+							t.cur = plane_set(s, ch.set[ch.cur]);
+							t.fwd = plane_set(s, ch.set[1 - ch.cur]);
+						}
+						t.mb_width = s.seq.mb_width;
+						t.mb_size = s.seq.mb_size;
+						t.coded_width = s.seq.coded_width;
+						t.coded_height = s.seq.coded_height;
+						t.width = s.width;
+						t.height = s.height;
+						const bool out = q_hi > q_lo;
+						t.rgba = rgba && out ? static_cast<uint8_t *>(rgba_dst[order[q_lo]]) : nullptr;
+						if (depths.size() <= d) depths.emplace_back();
+						Depth &dp = depths[d++];
+						(is_b ? (t.rgba ? dp.bi_rgba : dp.bi) : (t.rgba ? dp.ip_rgba : dp.ip)).push_back(t);
+						for (int q = q_lo; q < q_hi; q++) {  // the first request gets the picture, duplicates a copy of it
+							if (!leaf || q > q_lo) {
+								dp.dst.push_back(planes_dst[order[q]]);
+								dp.src.push_back(t.cur.y);
+								dp.size.push_back((size_t)s.coded_size * 3 / 2);
+							}
+							if (rgba && q > q_lo) {
+								dp.dst.push_back(rgba_dst[order[q]]);
+								dp.src.push_back(t.rgba);
+								dp.size.push_back((size_t)s.width * s.height * 4);
+							}
+						}
+						if (is_b) ch.b_cur ^= 1;
+						else ch.cur ^= 1;
+					}
+					// the next picture: the first picture start code at or after where this one's parse ended
+					ch.next = (uint32_t)(std::lower_bound(s.pics.begin(), s.pics.end(), (e.end_bit + 7) >> 3) - s.pics.begin());
+				}
+			}
+			// ---- stage 2: one depth after the other on the reconstruct stream, each followed by its copies (a set is
+			// overwritten two references later, by a later launch on the same stream)
+			for (Depth &dp : depths) {
+				if (!dp.ip.empty()) launch_reconstruct(dp.ip.data(), (int)dp.ip.size(), b->st_recon);
+				if (!dp.ip_rgba.empty()) launch_reconstruct_rgba(dp.ip_rgba.data(), (int)dp.ip_rgba.size(), b->st_recon);
+				if (!dp.bi.empty()) launch_reconstruct_b(dp.bi.data(), (int)dp.bi.size(), false, b->st_recon);
+				if (!dp.bi_rgba.empty()) launch_reconstruct_b(dp.bi_rgba.data(), (int)dp.bi_rgba.size(), true, b->st_recon);
+				if (!dp.dst.empty()) {
+					b->copy_dst.swap(dp.dst);
+					b->copy_src.swap(dp.src);
+					b->copy_size.swap(dp.size);
+					copy_batch(b, b->st_recon);
+				}
+			}
+			CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
+			b->recon_pending = true;
+			for (int t = 0; t < m; t++) {  // reused by the next wave's parse, which waits for ev_round
+				const Chain &ch = chains[wave[t].chain];
+				release_slot(b, ch.slot[wave[t].pic - ch.first]);
+			}
+		}
+		for (size_t c = glo; c < ghi; c++)  // never consumed: planes 0 (a copied destination was not zeroed)
+			if (chains[c].n_sets)
+				for (int q = chains[c].req_lo; q < chains[c].req_hi; q++)
+					if (status[order[q]] == 0) {
+						const Stream &s = b->streams[chains[c].stream];
+						CUDA_CHECK(cudaMemsetAsync(planes_dst[order[q]], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
+					}
+	}
+	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+	b->recon_pending = false;
+	for (int i = 0; i < n; i++) {
+		if (status_out) status_out[i] = status[i];
+		if (n_present_out) n_present_out[i] = n_present[i];
+		if (error_out) error_out[i] = error[i];
+	}
+}
+
+// The checks both front ends make of a request before anything changes: stream, sequence header, destinations
+bool request_valid(const Batch *b, int si, void *planes, void *image, bool rgba) {
+	auto aligned = [](const void *p) { return ((uintptr_t)p & 15u) == 0; };  // stage 2 stores 8 and 16 bytes at a time
+	if (si < 0 || si >= (int)b->streams.size() || !b->streams[si].has_seq || !planes || !aligned(planes)) return false;
+	return !rgba || (image && aligned(image));
 }
 
 long batch_decode_intra(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *planes_dst,
@@ -1060,106 +1398,42 @@ long batch_decode_intra(Batch *b, int n, const int *streams, const uint32_t *pic
 	if (n < 0 || (n > 0 && (!streams || !pictures || !planes_dst || (rgba && !rgba_dst)))) return -2;
 	upload_all(b);
 	// ---- every request is checked before anything changes
-	const int S = (int)b->streams.size();
-	std::vector<std::vector<uint32_t>> listed(S);
-	std::vector<char> indexed(S, 0);
-	size_t fwd_bytes = 0;
-	auto aligned = [](const void *p) { return ((uintptr_t)p & 15u) == 0; };  // stage 2 stores 8 and 16 bytes at a time
+	std::vector<std::vector<uint32_t>> listed(b->streams.size());
+	std::vector<char> indexed(b->streams.size(), 0);
+	std::vector<PictureRequest> req(n);
 	for (int i = 0; i < n; i++) {
 		const int si = streams[i];
-		if (si < 0 || si >= S || !b->streams[si].has_seq || !planes_dst[i] || !aligned(planes_dst[i])) return -2;
-		if (rgba && (!rgba_dst[i] || !aligned(rgba_dst[i]))) return -2;
-		const Stream &s = b->streams[si];
-		if (!indexed[si]) { listed[si] = intra_index(s); indexed[si] = 1; }
+		if (!request_valid(b, si, planes_dst[i], rgba ? rgba_dst[i] : nullptr, rgba)) return -2;
+		if (!indexed[si]) { listed[si] = intra_index(b->streams[si]); indexed[si] = 1; }
 		if (!std::binary_search(listed[si].begin(), listed[si].end(), pictures[i])) return -2;
-		fwd_bytes = std::max(fwd_bytes, (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64);  // parse_sequence_header's slack
+		req[i] = {si, pictures[i], pictures[i]};  // an I picture is its own chain start
 	}
 	if (n == 0) return 0;
-	ensure_pool(b);
-	if (fwd_bytes > b->intra_fwd_bytes) {
-		if (b->d_intra_fwd) {
-			CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-			CUDA_CHECK(cudaFree(b->d_intra_fwd));
-			b->d_intra_fwd = nullptr;
-			b->intra_fwd_bytes = 0;
-		}
-		b->d_intra_fwd = dev_alloc<uint8_t>(fwd_bytes);
-		CUDA_CHECK(cudaMemsetAsync(b->d_intra_fwd, 0, fwd_bytes, b->st_recon));
-		b->intra_fwd_bytes = fwd_bytes;
+	decode_chains(b, req, planes_dst, rgba_dst, rgba, nullptr, n_present_out, error_out);
+	return n;
+}
+
+long batch_decode_pictures(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *planes_dst,
+                           void *const *rgba_dst, int flags, int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
+	use_device(b);
+	const bool rgba = (flags & JSMPEG_B200_OUT_RGBA) != 0;
+	if (n < 0 || (n > 0 && (!streams || !pictures || !planes_dst || (rgba && !rgba_dst)))) return -2;
+	upload_all(b);
+	// ---- every request is checked before anything changes
+	std::vector<std::vector<IndexEntry>> listed(b->streams.size());
+	std::vector<char> indexed(b->streams.size(), 0);
+	std::vector<PictureRequest> req(n);
+	for (int i = 0; i < n; i++) {
+		const int si = streams[i];
+		if (!request_valid(b, si, planes_dst[i], rgba ? rgba_dst[i] : nullptr, rgba)) return -2;
+		if (!indexed[si]) { listed[si] = picture_index(b, b->streams[si]); indexed[si] = 1; }
+		auto e = std::lower_bound(listed[si].begin(), listed[si].end(), pictures[i],
+		                          [](const IndexEntry &x, uint32_t k) { return x.pic < k; });
+		if (e == listed[si].end() || e->pic != pictures[i]) return -2;
+		req[i] = {si, pictures[i], e->chain_start};
 	}
-	// record slots: the free ones; when they do not cover the call, the look-ahead's too (decode() parses those again)
-	if ((int)b->free_slots.size() < n)
-		for (auto &s : b->streams) flush_cache(b, s);
-	const int wave_max = (int)b->free_slots.size();
-	ensure_task_caps(b, std::min(n, wave_max), std::min(n, wave_max));
-	struct Req { int idx, kind; uint32_t bytes; };
-	for (int lo = 0; lo < n;) {
-		const int m = std::min(n - lo, wave_max);
-		// ---- stage 1: one wave, grouped by walk kernel and longest first, like decode_round
-		std::vector<Req> wave(m);
-		for (int j = 0; j < m; j++) {
-			const int r = lo + j;
-			const Stream &s = b->streams[streams[r]];
-			const uint32_t pic = pictures[r];
-			const uint32_t end = pic + 1 < s.pics.size() ? s.pics[pic + 1] : s.bb.length;
-			wave[j] = {r, walk_kind(b, s, pic), end - s.pics[pic]};
-		}
-		std::stable_sort(wave.begin(), wave.end(), [](const Req &x, const Req &y) {
-			return x.kind != y.kind ? x.kind < y.kind : x.bytes > y.bytes;
-		});
-		std::vector<int> slot(m);
-		int n_lanes = 0;  // pictures for the lane-parallel walk; the rest go to the slice walk
-		for (int j = 0; j < m; j++) {
-			slot[j] = b->free_slots.back();
-			b->free_slots.pop_back();
-			b->h_ptasks[j] = parse_task(b, streams[wave[j].idx], pictures[wave[j].idx], slot[j], j);
-			n_lanes += wave[j].kind == 0;
-		}
-		if (b->recon_pending) {  // reconstruct launches of an earlier round or wave may still read these slots
-			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_round, 0));
-			b->recon_pending = false;
-		}
-		CUDA_CHECK(cudaMemcpyAsync(b->d_ptasks, b->h_ptasks, m * sizeof(ParseTask), cudaMemcpyHostToDevice, b->st_main));
-		if (n_lanes) launch_parse_pictures(b->d_ptasks, n_lanes, b->slot_mb, b->st_main, nullptr, &b->fork);
-		if (m > n_lanes) launch_parse_pictures_slices(b->d_ptasks + n_lanes, m - n_lanes, b->slot_mb, b->st_main);
-		CUDA_CHECK(cudaMemcpyAsync(b->h_info, b->d_info, m * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
-		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-		// ---- stage 2: into the caller's planes, predicted (skipped macroblocks) from the zeroed scratch set
-		int n_rec = 0;
-		for (int j = 0; j < m; j++) {
-			const int r = wave[j].idx;
-			const Stream &s = b->streams[streams[r]];
-			const picture_info_t &info = b->h_info[j];
-			if (n_present_out) n_present_out[r] = info.n_present;
-			if (error_out) error_out[r] = info.error;
-			CUDA_CHECK(cudaMemsetAsync(planes_dst[r], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
-			if (rgba) CUDA_CHECK(cudaMemsetAsync(rgba_dst[r], 0xff, (size_t)s.width * s.height * 4, b->st_recon));
-			if (info.status != PIC_DECODED) continue;
-			ReconTask t{};
-			t.hdr = b->d_hdr + (size_t)slot[j] * b->slot_mb;
-			t.coef = b->d_coef + (size_t)slot[j] * b->slot_mb * MB_COEF_INT16;
-			t.cur = plane_set(s, static_cast<uint8_t *>(planes_dst[r]));
-			t.fwd = plane_set(s, b->d_intra_fwd);
-			t.mb_width = s.seq.mb_width;
-			t.mb_size = s.seq.mb_size;
-			t.coded_width = s.seq.coded_width;
-			t.coded_height = s.seq.coded_height;
-			t.rgba = rgba ? static_cast<uint8_t *>(rgba_dst[r]) : nullptr;
-			t.width = s.width;
-			t.height = s.height;
-			b->h_rtasks[n_rec++] = t;
-		}
-		if (n_rec) {
-			if (rgba) launch_reconstruct_rgba(b->h_rtasks, n_rec, b->st_recon);
-			else launch_reconstruct(b->h_rtasks, n_rec, b->st_recon);
-		}
-		CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
-		b->recon_pending = true;
-		for (int j = 0; j < m; j++) release_slot(b, slot[j]);  // reused by the next wave's parse, which waits for ev_round
-		lo += m;
-	}
-	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-	b->recon_pending = false;
+	if (n == 0) return 0;
+	decode_chains(b, req, planes_dst, rgba_dst, rgba, status_out, n_present_out, error_out);
 	return n;
 }
 
@@ -1273,6 +1547,7 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b) {
 	if (b->h_rtasks) cudaFreeHost(b->h_rtasks);
 	if (b->d_rtasks) cudaFree(b->d_rtasks);
 	if (b->d_intra_fwd) cudaFree(b->d_intra_fwd);
+	if (b->d_chain_sets) cudaFree(b->d_chain_sets);
 	ts_scratch_destroy(b->ts);
 	ps_scratch_destroy(b->ps);
 	cudaEvent_t evs[] = {b->ev_a, b->ev_b, b->ev_mid, b->ev_step, b->ev_round, b->ev_copied[0], b->ev_copied[1], b->fork.fork};
@@ -1409,6 +1684,35 @@ long jsmpeg_b200_batch_decode_intra(jsmpeg_b200_batch_t *b, int n, const int *st
                                     int32_t *error_out) {
 	return guarded<long>(b, -1, [&] {
 		return batch_decode_intra(b, n, streams, pictures, planes_dst, rgba_dst, flags, n_present_out, error_out);
+	});
+}
+
+long jsmpeg_b200_batch_picture_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out, uint32_t *byte_pos_out,
+                                     int32_t *type_out, int32_t *temporal_reference_out, uint32_t *chain_start_out,
+                                     long n_max) {
+	return guarded<long>(b, -1, [&]() -> long {
+		if (stream < 0 || stream >= (int)b->streams.size()) return -2;
+		use_device(b);
+		upload_all(b);
+		const Stream &s = b->streams[stream];
+		const std::vector<IndexEntry> listed = picture_index(b, s);
+		for (long i = 0; i < std::min<long>((long)listed.size(), n_max); i++) {
+			const uint32_t k = listed[i].pic;
+			if (picture_out) picture_out[i] = k;
+			if (byte_pos_out) byte_pos_out[i] = s.pics[k];
+			if (type_out) type_out[i] = picture_type_of(s, k);
+			if (temporal_reference_out) temporal_reference_out[i] = (int32_t)picture_header_bits(s, k, 0, 10);
+			if (chain_start_out) chain_start_out[i] = listed[i].chain_start;
+		}
+		return (long)listed.size();
+	});
+}
+
+long jsmpeg_b200_batch_decode_pictures(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                       void *const *planes_dst, void *const *rgba_dst, int flags, int32_t *status_out,
+                                       int32_t *n_present_out, int32_t *error_out) {
+	return guarded<long>(b, -1, [&] {
+		return batch_decode_pictures(b, n, streams, pictures, planes_dst, rgba_dst, flags, status_out, n_present_out, error_out);
 	});
 }
 
