@@ -102,10 +102,8 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b);
 /* NULL while the batch works; otherwise the first failure (a CUDA error text).  A dead batch returns
  * 0 / -1 / false from every call and never touches the device again. */
 const char *jsmpeg_b200_batch_last_error(jsmpeg_b200_batch_t *b);
-/* Tuning knobs, 0 on success.  "chunk_pictures" G: a parse wave is queued in chunks of G pictures per
- * stream and chunk k is reconstructed while chunk k+1 is being parsed (0 = one chunk, no overlap;
- * default from the environment variable JSMPEG_B200_CHUNK, else 0).  "lookahead": pictures parsed
- * ahead per stream beyond the ones a decode call asks for.
+/* Tuning knobs, 0 on success, -1 for an unknown name.  "lookahead": pictures parsed ahead per stream
+ * beyond the ones a decode call asks for.
  * "slice_walk" (default 0, or JSMPEG_B200_SLICE_WALK): I/P pictures with at least four slices are parsed by a
  * walk kernel that gives every slice a lane of its own instead of cutting one slice's bits into 32 (streams with a
  * slice per macroblock row); the results are the same bit for bit, only the speed differs.

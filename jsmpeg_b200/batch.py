@@ -93,7 +93,7 @@ def bind_batch_abi(lib):
 class BatchDecoder:
     """``n_streams`` independent MPEG-1 video decoders on one GPU."""
 
-    def __init__(self, n_streams, device=0, max_slots=0, lib=None, chunk_pictures=None, decode_b=None, slice_walk=None):
+    def __init__(self, n_streams, device=0, max_slots=0, lib=None, decode_b=None, slice_walk=None):
         from . import capi
         self.lib = lib if lib is not None else capi.product_library()
         self.n_streams = n_streams
@@ -106,8 +106,6 @@ class BatchDecoder:
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
             self.close()
             raise RuntimeError(err.decode(errors="replace"))
-        if chunk_pictures is not None:
-            self.set_option("chunk_pictures", chunk_pictures)
         if slice_walk is not None:  # I/P pictures of many slices: one lane per slice (same records, another walk kernel)
             self.set_option("slice_walk", slice_walk)
         if decode_b is not None:  # the B-picture extension (the reference skips B pictures, and so does the default)

@@ -106,23 +106,23 @@ struct ScanSpan {
 };
 void launch_scan_start_codes(const ScanSpan *spans, int n_spans, uint32_t longest_span, uint32_t *positions,
                              uint32_t capacity, uint32_t *counts, cudaStream_t stream);
-// Helper streams/events with which stage 1 forks the (size-sorted) wave into groups: the expand of
+// Helper streams/events with which stage 1 forks a (size-sorted) wave of I/P pictures into groups: the expand of
 // a group of small pictures runs while the walk of the bigger pictures is still going.
 constexpr int PARSE_GROUPS = 8;
 struct ParseFork {
 	cudaStream_t side[PARSE_GROUPS];
 	cudaEvent_t fork, join[PARSE_GROUPS];
 };
-void launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream,
-                           cudaEvent_t walk_done = nullptr, const ParseFork *fork = nullptr);
-// how many size groups (walk + expand launch pairs) launch_parse_pictures uses for n_tasks pictures
-int parse_group_count(int n_tasks, bool forked);
-// `tasks_host` is read on the host at launch time: the table travels in the kernel parameters
-void launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
+// Stage 1 of I/P pictures: a walk + an expand launch per size group (one group without `fork`); walk_done, unless
+// nullptr, is recorded behind the first group's walk.  Returns the number of kernels launched.
+int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream,
+                          cudaEvent_t walk_done = nullptr, const ParseFork *fork = nullptr);
+// Stage 2.  `tasks_host` is read on the host at launch time: the table travels in the kernel parameters.  Each
+// launcher returns the number of kernels it launched.
+int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
 // the same with the planar -> RGBA conversion fused in (tasks' rgba / width / height)
-void launch_reconstruct_rgba(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
-// B pictures (every task has `bwd`): prediction from two references; `rgba` = with the fused conversion.
-// Returns the number of kernels launched.
+int launch_reconstruct_rgba(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
+// B pictures (every task has `bwd`): prediction from two references; `rgba` = with the fused conversion
 int launch_reconstruct_b(const ReconTask *tasks_host, int n_tasks, bool rgba, cudaStream_t stream);
 // stage 1 for B pictures: the serial walk with the B-picture macroblock layer (walk_b.cuh) + the same expand
 void launch_parse_pictures_b(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream);

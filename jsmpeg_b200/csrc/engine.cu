@@ -20,13 +20,11 @@
 // one at/after the bit index where picture j's parse ended (otherwise the look-ahead is discarded
 // and re-planned from there).
 //
-// Pipeline.  A round's parse wave can be cut into CHUNKS by picture ordinal (pictures [kG, (k+1)G)
-// of every stream; option "chunk_pictures"); all chunks are queued on the parse stream at once, each
-// followed by the read-back of its picture infos.  The host then takes chunk after chunk: waits for
-// that chunk's infos only, does the acceptance above, and queues the chunk's reconstruct launches on
-// a SECOND stream -- while the parse of the following chunks is running.  Stage 1 (latency-bound, few
-// resident warps) and stage 2 (bandwidth / issue-bound) are natural co-runners in principle; without
-// the option the parse wave and the first reconstruct launch are separated by a host synchronisation.
+// Pipeline.  decode() and decode_pictures / decode_intra share it.  A round plans its pictures, parses
+// them in one stage-1 wave (parse_wave: walk + expand per walk kernel, the kernels beside each other on
+// side streams) and waits for the picture infos; the host then consumes them in decode() order and
+// queues one reconstruct step per picture depth (ReconStep, launch_step) on the reconstruct stream.
+// Cutting the wave into chunks to overlap stage 1 with stage 2 was measured not to pay (DESIGN 8).
 #include <sched.h>
 
 #include <algorithm>
@@ -66,7 +64,6 @@ struct Parsed {
 	uint32_t pos;           // byte position of the 00 00 01 00 start code
 	uint32_t len_at_parse;  // buffer length the parse saw
 	int slot;
-	bool ready;             // `info` has arrived from the device
 	picture_info_t info;
 };
 
@@ -126,8 +123,7 @@ struct jsmpeg_b200_batch_t {
 	uint32_t codes_rows = 0, codes_stride = 0;  // rows = streams, stride = entries per row
 	cudaStream_t st_main = nullptr, st_recon = nullptr, st_copy = nullptr;  // uploads + scan + parse | reconstruct | copy-out
 	cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_mid = nullptr, ev_step = nullptr, ev_round = nullptr, ev_copied[2] = {nullptr, nullptr};
-	std::vector<cudaEvent_t> ev_info;            // per chunk: its picture infos are on the host
-	std::vector<cudaEvent_t> ev_rec0, ev_rec1;   // per chunk: around its reconstruct launches (timing)
+	cudaEvent_t ev_recon[2] = {nullptr, nullptr};  // around a round's reconstruct launches (timing)
 	// record slots
 	unsigned max_slots_req = 0;
 	int slot_mb = 0, n_slots = 0;
@@ -140,25 +136,16 @@ struct jsmpeg_b200_batch_t {
 	int lookahead = 1;
 	bool decode_b = false;       // the B-picture extension: off = B pictures are skipped like the reference does (mpeg1.js:181-184)
 	bool slice_walk = false;     // I/P pictures of >= SLICE_WALK_MIN_SLICES slices go to the one-lane-per-slice walk (walk_slices.cuh)
-	int chunk_pictures = 0;      // G of the pipeline; 0 = the whole wave is one chunk
-	int chunk_min_wave = 256;    // waves with fewer new pictures stay whole
-	int chunk_streams = 3;       // chunks are parsed on this many streams in turn (1 = on the main stream, forked into size groups)
 	// pictures with a walk kernel of their own (B pictures; with "slice_walk", I/P pictures of many slices) are
 	// walked beside the others, on these streams
 	cudaStream_t st_side[2] = {nullptr, nullptr};
 	cudaEvent_t ev_sfork = nullptr, ev_sjoin[2] = {nullptr, nullptr};
-	cudaStream_t st_chunk[4] = {nullptr, nullptr, nullptr, nullptr};
-	cudaEvent_t ev_fed = nullptr, ev_chunk_done[4] = {nullptr, nullptr, nullptr, nullptr};
 	bool recon_pending = false;  // reconstruct launches of an earlier round may still read record slots
-	// task staging
+	// parse task staging
 	ParseTask *h_ptasks = nullptr, *d_ptasks = nullptr;
 	int ptask_cap = 0;
-	ReconTask *h_rtasks = nullptr, *d_rtasks = nullptr;
-	int rtask_cap = 0;
 	uint64_t copy_steps = 0;  // reconstruct launches with a copy-out so far (event parity)
 	ParseFork fork{};
-	std::vector<void *> copy_dst, copy_src;
-	std::vector<size_t> copy_size;
 	bool batch_copy_ok = true;
 	TsScratch *ts = nullptr;
 	PsScratch *ps = nullptr;
@@ -538,43 +525,15 @@ void ensure_pool(Batch *b) {
 	for (int i = (int)n - 1; i >= 0; i--) b->free_slots.push_back(i);
 }
 
-void ensure_task_caps(Batch *b, int n_parse, int n_recon) {
-	if (n_parse > b->ptask_cap) {
-		if (b->h_ptasks) { CUDA_CHECK(cudaFreeHost(b->h_ptasks)); b->h_ptasks = nullptr; }
-		if (b->d_ptasks) { CUDA_CHECK(cudaFree(b->d_ptasks)); b->d_ptasks = nullptr; }
-		const int cap = std::max(n_parse, b->ptask_cap * 2);
-		b->ptask_cap = 0;
-		b->h_ptasks = pinned_alloc<ParseTask>(cap);
-		b->d_ptasks = dev_alloc<ParseTask>(cap);
-		b->ptask_cap = cap;
-	}
-	if (n_recon > b->rtask_cap) {
-		if (b->h_rtasks) { CUDA_CHECK(cudaFreeHost(b->h_rtasks)); b->h_rtasks = nullptr; }
-		if (b->d_rtasks) { CUDA_CHECK(cudaFree(b->d_rtasks)); b->d_rtasks = nullptr; }
-		const int cap = std::max(n_recon, b->rtask_cap * 2);
-		b->rtask_cap = 0;
-		b->h_rtasks = pinned_alloc<ReconTask>(cap);
-		b->d_rtasks = dev_alloc<ReconTask>(cap);
-		b->rtask_cap = cap;
-	}
-}
-
-void ensure_chunk_events(Batch *b, size_t n) {
-	while (b->ev_info.size() < n) {
-		cudaEvent_t e = nullptr;
-		CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-		b->ev_info.push_back(e);
-	}
-	while (b->ev_rec0.size() < n) {
-		cudaEvent_t e = nullptr;
-		CUDA_CHECK(cudaEventCreate(&e));
-		b->ev_rec0.push_back(e);
-	}
-	while (b->ev_rec1.size() < n) {
-		cudaEvent_t e = nullptr;
-		CUDA_CHECK(cudaEventCreate(&e));
-		b->ev_rec1.push_back(e);
-	}
+void ensure_task_caps(Batch *b, int n_parse) {
+	if (n_parse <= b->ptask_cap) return;
+	if (b->h_ptasks) { CUDA_CHECK(cudaFreeHost(b->h_ptasks)); b->h_ptasks = nullptr; }
+	if (b->d_ptasks) { CUDA_CHECK(cudaFree(b->d_ptasks)); b->d_ptasks = nullptr; }
+	const int cap = std::max(n_parse, b->ptask_cap * 2);
+	b->ptask_cap = 0;
+	b->h_ptasks = pinned_alloc<ParseTask>(cap);
+	b->d_ptasks = dev_alloc<ParseTask>(cap);
+	b->ptask_cap = cap;
 }
 
 PlaneSet plane_set(const Stream &s, uint8_t *base) {
@@ -590,43 +549,51 @@ bool entry_stale(const Stream &s, const Parsed &e) {
 	return e.len_at_parse != s.bb.length && (uint64_t)e.info.end_bit + 64 >= (uint64_t)e.len_at_parse * 8;
 }
 
-// b->copy_dst / copy_src / copy_size in ONE batched copy call on `st` (cudaMemcpyBatchAsync, CUDA 12.8+); plain
-// copies where the driver has no batched copy
-void copy_batch(Batch *b, cudaStream_t st) {
-	const size_t n_copy = b->copy_dst.size();
+// dst[i] <- src[i], size[i] bytes, in ONE batched copy call on `st` (cudaMemcpyBatchAsync, CUDA 12.8+); plain copies
+// where the driver has no batched copy
+void copy_batch(Batch *b, std::vector<void *> &dst, std::vector<void *> &src, std::vector<size_t> &size, cudaStream_t st) {
+	const size_t n_copy = dst.size();
 	bool batched = false;
 	if (b->batch_copy_ok && n_copy > 1) {
 		cudaMemcpyAttributes attr{};
 		attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
 		size_t attr_idx = 0, fail_idx = 0;
-		cudaError_t e = cudaMemcpyBatchAsync(b->copy_dst.data(), b->copy_src.data(), b->copy_size.data(), n_copy,
-		                                     &attr, &attr_idx, 1, &fail_idx, st);
+		cudaError_t e = cudaMemcpyBatchAsync(dst.data(), src.data(), size.data(), n_copy, &attr, &attr_idx, 1, &fail_idx, st);
 		if (e == cudaSuccess) batched = true;
 		else { (void)cudaGetLastError(); b->batch_copy_ok = false; }  // older driver: plain copies from now on
 	}
 	if (!batched)
-		for (size_t i = 0; i < n_copy; i++)
-			CUDA_CHECK(cudaMemcpyAsync(b->copy_dst[i], b->copy_src[i], b->copy_size[i], cudaMemcpyDefault, st));
+		for (size_t i = 0; i < n_copy; i++) CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], size[i], cudaMemcpyDefault, st));
 }
 
-// The copy-out of one reconstruct launch's pictures (OUT_HOST), on the copy stream.
-void copy_out_step(Batch *b, const std::vector<ReconTask> &tasks, const std::vector<int> &stream_ids) {
+// The reconstruct launches of one step of decode() (or one depth of decode_chains), by kernel: I/P and B pictures,
+// each without and with the fused RGBA conversion; and the copies of its pictures that follow them
+struct ReconStep {
+	std::vector<ReconTask> ip, ip_rgba, bi, bi_rgba;
+	std::vector<void *> dst, src;
+	std::vector<size_t> size;
+	void add(const ReconTask &t) { (t.bwd.y ? (t.rgba ? bi_rgba : bi) : (t.rgba ? ip_rgba : ip)).push_back(t); }
+	void copy(void *to, void *from, size_t n) {
+		dst.push_back(to);
+		src.push_back(from);
+		size.push_back(n);
+	}
+};
+
+// Queues a step's reconstruct launches on `st`; returns the number of kernels launched
+int launch_step(const ReconStep &r, cudaStream_t st) {
+	int n = launch_reconstruct(r.ip.data(), (int)r.ip.size(), st);
+	n += launch_reconstruct_rgba(r.ip_rgba.data(), (int)r.ip_rgba.size(), st);
+	n += launch_reconstruct_b(r.bi.data(), (int)r.bi.size(), false, st);
+	n += launch_reconstruct_b(r.bi_rgba.data(), (int)r.bi_rgba.size(), true, st);
+	return n;
+}
+
+// The copy-out of one step's pictures (OUT_HOST) on the copy stream, behind the step's launches
+void copy_out_step(Batch *b, ReconStep &r) {
 	CUDA_CHECK(cudaEventRecord(b->ev_step, b->st_recon));
 	CUDA_CHECK(cudaStreamWaitEvent(b->st_copy, b->ev_step, 0));
-	// all pictures of the step leave in one batched copy call
-	const size_t n_copy = tasks.size();
-	b->copy_dst.resize(n_copy);
-	b->copy_src.resize(n_copy);
-	b->copy_size.resize(n_copy);
-	for (size_t i = 0; i < n_copy; i++) {
-		Stream &s = b->streams[stream_ids[i]];
-		s.h_head = (s.h_head + 1) % HOST_RING;
-		b->copy_dst[i] = s.h_planes[s.h_head];
-		b->copy_src[i] = tasks[i].cur.y;
-		b->copy_size[i] = (size_t)s.coded_size * 3 / 2;
-		b->stats.d2h_bytes += b->copy_size[i];
-	}
-	copy_batch(b, b->st_copy);
+	copy_batch(b, r.dst, r.src, r.size, b->st_copy);  // all pictures of the step leave in one batched copy call
 	CUDA_CHECK(cudaEventRecord(b->ev_copied[b->copy_steps & 1], b->st_copy));
 	b->copy_steps++;
 }
@@ -677,20 +644,108 @@ ParseTask parse_task(const Batch *b, int si, uint32_t pic, int slot, int info_id
 	return t;
 }
 
-// One round: parse ahead what is missing (one wave, queued chunk by chunk), then -- chunk after chunk, as
-// the chunks' infos arrive -- consume up to want[s] pictures per stream in decode() order and queue their
-// reconstruction.  Returns pictures consumed; `progress[s]` gets the per-stream count, `more[s]` whether
-// the stream may have further pictures.
+// One picture of a stage-1 wave: picture `pic` of stream `stream`, records into `slot`; `kind` is its walk kernel
+// (walk_kind), `bytes` its length up to the next picture start code
+struct WaveItem {
+	int stream;
+	uint32_t pic;
+	int slot;
+	int kind;
+	uint32_t bytes;
+};
+
+// Stage 1 of `wave` as one wave, for decode() and decode_chains alike.  The tasks are grouped by walk kernel and,
+// within a kernel, longest first: a CTA's warps, and consecutive CTAs (which land on different SMs), then carry
+// similar amounts of work and the walk ends without a long tail.  The first kernel present runs on the main stream;
+// the others have walk kernels of their own (one warp per picture, latency-bound like every walk) and run beside it on
+// side streams, forked after the upload and joined before the infos are read.  On return the infos are on the host,
+// b->h_info[i] that of wave[i], and ev_a / ev_mid / ev_b bracket the wave and its lane-parallel walk.  Returns the
+// number of kernels launched.
+int parse_wave(Batch *b, const std::vector<WaveItem> &wave) {
+	const int n = (int)wave.size();
+	std::vector<int> order(n);
+	for (int i = 0; i < n; i++) order[i] = i;
+	std::stable_sort(order.begin(), order.end(), [&](int x, int y) {
+		return wave[x].kind != wave[y].kind ? wave[x].kind < wave[y].kind : wave[x].bytes > wave[y].bytes;
+	});
+	ensure_task_caps(b, n);
+	int cnt[3] = {0, 0, 0};
+	for (int j = 0; j < n; j++) {
+		const WaveItem &w = wave[order[j]];
+		b->h_ptasks[j] = parse_task(b, w.stream, w.pic, w.slot, order[j]);
+		cnt[w.kind]++;
+	}
+	if (b->recon_pending) {  // slots freed by an earlier round or wave may still be read by its reconstruct launches
+		CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_round, 0));
+		b->recon_pending = false;
+	}
+	CUDA_CHECK(cudaMemcpyAsync(b->d_ptasks, b->h_ptasks, n * sizeof(ParseTask), cudaMemcpyHostToDevice, b->st_main));
+	CUDA_CHECK(cudaEventRecord(b->ev_a, b->st_main));
+	int primary = 0;
+	while (cnt[primary] == 0) primary++;
+	if (cnt[primary] < n) CUDA_CHECK(cudaEventRecord(b->ev_sfork, b->st_main));
+	// the wave's pictures by walk kernel: [0, cnt[0]) lane-parallel walk, then the slice walk's, then the B pictures
+	const int off[3] = {0, cnt[0], cnt[0] + cnt[1]};
+	int launches = 0, n_side = 0;
+	for (int kind = 0; kind < 3; kind++) {
+		if (cnt[kind] == 0) continue;
+		cudaStream_t st = b->st_main;
+		if (kind != primary) {
+			st = b->st_side[n_side];
+			CUDA_CHECK(cudaStreamWaitEvent(st, b->ev_sfork, 0));
+		}
+		if (kind == 0) {
+			launches += launch_parse_pictures(b->d_ptasks, cnt[0], b->slot_mb, st, b->ev_mid, &b->fork);
+		} else {
+			if (kind == 1) launch_parse_pictures_slices(b->d_ptasks + off[1], cnt[1], b->slot_mb, st);
+			else launch_parse_pictures_b(b->d_ptasks + off[2], cnt[2], b->slot_mb, st);
+			launches += 2;  // walk + expand
+		}
+		if (kind != primary) {
+			CUDA_CHECK(cudaEventRecord(b->ev_sjoin[n_side], st));
+			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_sjoin[n_side], 0));
+			n_side++;
+		}
+	}
+	CUDA_CHECK(cudaMemcpyAsync(b->h_info, b->d_info, n * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
+	if (cnt[0] == 0) CUDA_CHECK(cudaEventRecord(b->ev_mid, b->st_main));  // (a wave without the lane-parallel walk)
+	CUDA_CHECK(cudaEventRecord(b->ev_b, b->st_main));
+	CUDA_CHECK(cudaEventSynchronize(b->ev_b));
+	return launches;
+}
+
+// The reconstruct task of a picture of `s` whose records are in `slot`: written into the plane set at `cur`, predicted
+// from `fwd` (and, for a B picture, `bwd`), with the fused RGBA conversion into `rgba` unless that is nullptr
+ReconTask recon_task(const Batch *b, const Stream &s, int slot, uint8_t *cur, uint8_t *fwd, uint8_t *bwd, uint8_t *rgba) {
+	ReconTask t{};
+	t.hdr = b->d_hdr + (size_t)slot * b->slot_mb;
+	t.coef = b->d_coef + (size_t)slot * b->slot_mb * MB_COEF_INT16;
+	t.cur = plane_set(s, cur);
+	t.fwd = plane_set(s, fwd);
+	if (bwd) t.bwd = plane_set(s, bwd);
+	t.mb_width = s.seq.mb_width;
+	t.mb_size = s.seq.mb_size;
+	t.coded_width = s.seq.coded_width;
+	t.coded_height = s.seq.coded_height;
+	t.width = s.width;
+	t.height = s.height;
+	t.rgba = rgba;
+	return t;
+}
+
+// One round: parse ahead what is missing in one wave, then consume up to want[s] pictures per stream in decode()
+// order and queue their reconstruction.  Returns pictures consumed; `progress[s]` gets the per-stream count, `more[s]`
+// whether the stream may have further pictures.
 long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &progress, std::vector<char> &more, int flags) {
 	const int S = (int)b->streams.size();
 	// ---- 1. plan the parse wave
-	// kind: which walk kernel takes the picture -- 0 the lane-parallel walk, 1 the slice walk, 2 the B-picture walk
-	struct NewParse { int stream; size_t cache_idx; uint32_t bytes; int chunk; uint32_t pic; int kind; };
-	std::vector<NewParse> fresh;
+	std::vector<WaveItem> wave;
+	std::vector<size_t> fresh(S, 0);  // per stream: the cache index of its first picture in the wave
 	for (int si = 0; si < S; si++) {
 		Stream &s = b->streams[si];
 		progress[si] = 0;
-		if (!s.has_seq || want[si] <= 0) { more[si] = 0; continue; }
+		more[si] = s.has_seq && want[si] > 0;
+		if (!more[si]) continue;
 		const uint32_t from_byte = (s.bb.index + 7) >> 3;
 		auto it = std::lower_bound(s.pics.begin(), s.pics.end(), from_byte);
 		if (!s.cache.empty() && (it == s.pics.end() || s.cache.front().pos != *it)) flush_cache(b, s);
@@ -700,6 +755,7 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 				break;
 			}
 		}
+		fresh[si] = s.cache.size();
 		if ((int)s.cache.size() >= want[si]) continue;
 		int target = std::max(want[si], b->lookahead);
 		auto next = it + (ptrdiff_t)s.cache.size();
@@ -709,300 +765,125 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			p.pos = *next;
 			p.len_at_parse = s.bb.length;
 			p.slot = b->free_slots.back();
-			p.ready = false;
 			b->free_slots.pop_back();
 			s.cache.push_back(p);
 			++next;
 			const uint32_t pic = (uint32_t)(next - 1 - s.pics.begin());
-			fresh.push_back({si, s.cache.size() - 1, (next < s.pics.end() ? *next : s.bb.length) - p.pos, 0, pic, walk_kind(b, s, pic)});
+			wave.push_back({si, pic, p.slot, walk_kind(b, s, pic), (next < s.pics.end() ? *next : s.bb.length) - p.pos});
 		}
 	}
-	// ---- 2. chunks by picture ordinal (position in the stream's look-ahead); a small wave stays whole
-	const int G = (b->chunk_pictures > 0 && (int)fresh.size() >= b->chunk_min_wave) ? b->chunk_pictures : 0;
-	int n_chunks = 1;
-	if (G > 0) {
-		for (auto &f : fresh) { f.chunk = (int)(f.cache_idx / (size_t)G); n_chunks = std::max(n_chunks, f.chunk + 1); }
-		int max_ordinal = 0;
-		for (int si = 0; si < S; si++) max_ordinal = std::max(max_ordinal, std::max(want[si], 0));
-		n_chunks = std::max(n_chunks, (max_ordinal + G - 1) / G);
-	}
-	ensure_chunk_events(b, (size_t)n_chunks);
-	std::vector<int> chunk_off(n_chunks + 1, 0);
-	if (!fresh.empty()) {
-		// Within a chunk, longest pictures first: a CTA's warps, and consecutive CTAs (which land on different
-		// SMs), then carry similar amounts of work and the chunk's walk ends without a long tail.
-		// (and grouped by the walk kernel that takes them)
-		std::stable_sort(fresh.begin(), fresh.end(), [](const NewParse &x, const NewParse &y) {
-			return x.chunk != y.chunk ? x.chunk < y.chunk : (x.kind != y.kind ? x.kind < y.kind : x.bytes > y.bytes);
-		});
-		for (auto &f : fresh) chunk_off[f.chunk + 1]++;
-		for (int c = 0; c < n_chunks; c++) chunk_off[c + 1] += chunk_off[c];
-		ensure_task_caps(b, (int)fresh.size(), 0);
-		for (size_t i = 0; i < fresh.size(); i++) {
-			const Parsed &p = b->streams[fresh[i].stream].cache[fresh[i].cache_idx];
-			b->h_ptasks[i] = parse_task(b, fresh[i].stream, fresh[i].pic, p.slot, (int)i);
+	// ---- 2. stage 1: the wave, every picture's info on the host before consumption starts
+	if (!wave.empty()) {
+		b->stats.kernel_launches += parse_wave(b, wave);
+		for (size_t i = 0; i < wave.size(); i++) {  // a stream's pictures are in the wave in cache order
+			const int si = wave[i].stream;
+			Parsed &p = b->streams[si].cache[fresh[si]++];
+			p.info = b->h_info[i];
+			if (p.info.error == PARSE_ERR_INVALID_VLC) b->stats.parse_errors++;
+			if (p.info.reserved[0]) b->stats.lane_walk_pictures++;
 		}
-		if (b->recon_pending) {  // slots freed by the previous round are still being read by its reconstruct launches
-			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_round, 0));
-			b->recon_pending = false;
-		}
-		CUDA_CHECK(cudaMemcpyAsync(b->d_ptasks, b->h_ptasks, fresh.size() * sizeof(ParseTask), cudaMemcpyHostToDevice, b->st_main));
-		CUDA_CHECK(cudaEventRecord(b->ev_a, b->st_main));
-		// Chunks are parsed on a few streams in turn: the walk of chunk c + 1 starts while chunk c is still walking or
-		// expanding (a chunk's walk costs its latency floor whatever its size; in a row on one stream the floors add up).
-		const int n_cs = (G > 0 && n_chunks > 1) ? std::min(std::max(b->chunk_streams, 1), 4) : 1;
-		if (n_cs > 1) {
-			for (int k = 0; k < n_cs; k++)
-				if (!b->st_chunk[k]) {
-					CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_chunk[k], cudaStreamNonBlocking));
-					CUDA_CHECK(cudaEventCreateWithFlags(&b->ev_chunk_done[k], cudaEventDisableTiming));
-				}
-			if (!b->ev_fed) CUDA_CHECK(cudaEventCreateWithFlags(&b->ev_fed, cudaEventDisableTiming));
-			CUDA_CHECK(cudaEventRecord(b->ev_fed, b->st_main));  // tasks uploaded, the previous round's reconstruction waited for
-		}
-		bool mid_recorded = false;
-		for (int c = 0; c < n_chunks; c++) {
-			const int lo = chunk_off[c], n = chunk_off[c + 1] - lo;
-			cudaStream_t st = n_cs > 1 ? b->st_chunk[c % n_cs] : b->st_main;
-			if (n_cs > 1 && c < n_cs) CUDA_CHECK(cudaStreamWaitEvent(st, b->ev_fed, 0));
-			if (n > 0) {
-				// the chunk's pictures by walk kernel: [lo, lo + cnt[0]) lane-parallel walk, then the slice walk's, then the B pictures
-				int cnt[3] = {0, 0, 0};
-				for (int i = lo; i < lo + n; i++) cnt[fresh[i].kind]++;
-				const int off[3] = {lo, lo + cnt[0], lo + cnt[0] + cnt[1]};
-				// The first kind present stays on `st`; the others have walk kernels of their own (one warp per picture,
-				// latency-bound like every walk) and run beside it on side streams, forked before anything is queued and
-				// joined before the infos are read.
-				int primary = 0;
-				while (cnt[primary] == 0) primary++;
-				const bool side = cnt[0] + cnt[1] + cnt[2] > cnt[primary];
-				if (side) {
-					if (!b->ev_sfork) {
-						CUDA_CHECK(cudaEventCreateWithFlags(&b->ev_sfork, cudaEventDisableTiming));
-						for (int j = 0; j < 2; j++) {
-							CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_side[j], cudaStreamNonBlocking));
-							CUDA_CHECK(cudaEventCreateWithFlags(&b->ev_sjoin[j], cudaEventDisableTiming));
-						}
-					}
-					CUDA_CHECK(cudaEventRecord(b->ev_sfork, st));
-				}
-				int n_side = 0;
-				for (int kind = 0; kind < 3; kind++) {
-					if (cnt[kind] == 0) continue;
-					cudaStream_t sk = st;
-					if (kind != primary) {
-						sk = b->st_side[n_side];
-						CUDA_CHECK(cudaStreamWaitEvent(sk, b->ev_sfork, 0));
-					}
-					if (kind == 0) {
-						launch_parse_pictures(b->d_ptasks + off[0], cnt[0], b->slot_mb, sk, mid_recorded ? nullptr : b->ev_mid, n_cs > 1 ? nullptr : &b->fork);
-						mid_recorded = true;
-						b->stats.kernel_launches += 2 * parse_group_count(cnt[0], n_cs == 1);  // walk + expand per size group
-					} else {
-						if (kind == 1) launch_parse_pictures_slices(b->d_ptasks + off[1], cnt[1], b->slot_mb, sk);
-						else launch_parse_pictures_b(b->d_ptasks + off[2], cnt[2], b->slot_mb, sk);
-						b->stats.kernel_launches += 2;
-					}
-					if (kind != primary) {
-						CUDA_CHECK(cudaEventRecord(b->ev_sjoin[n_side], sk));
-						CUDA_CHECK(cudaStreamWaitEvent(st, b->ev_sjoin[n_side], 0));
-						n_side++;
-					}
-				}
-				CUDA_CHECK(cudaMemcpyAsync(b->h_info + lo, b->d_info + lo, n * sizeof(picture_info_t), cudaMemcpyDeviceToHost, st));
-			}
-			CUDA_CHECK(cudaEventRecord(b->ev_info[c], st));
-		}
-		if (n_cs > 1)  // everything queued later on the main stream comes after the whole wave
-			for (int k = 0; k < n_cs; k++) {
-				CUDA_CHECK(cudaEventRecord(b->ev_chunk_done[k], b->st_chunk[k]));
-				CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_chunk_done[k], 0));
-			}
-		if (!mid_recorded) CUDA_CHECK(cudaEventRecord(b->ev_mid, b->st_main));  // (a wave of B pictures only)
-		CUDA_CHECK(cudaEventRecord(b->ev_b, b->st_main));
-		b->stats.h2d_bytes += fresh.size() * sizeof(ParseTask);
-		b->stats.d2h_bytes += fresh.size() * sizeof(picture_info_t);
-	}
-	// ---- 3. chunk after chunk: absorb the infos, consume in decode() order, queue the reconstruction
-	long consumed = 0;
-	std::vector<char> open(S, 0);  // stream still consuming in this round
-	std::vector<int> taken(S, 0);  // pictures consumed (= ordinal of the stream's next picture)
-	for (int si = 0; si < S; si++) {
-		const Stream &s = b->streams[si];
-		if (s.has_seq && want[si] > 0) { open[si] = 1; more[si] = 1; }
-	}
-	int rec_chunks = 0;
-	for (int c = 0; c < n_chunks; c++) {
-		const int lo = chunk_off[c], n = chunk_off[c + 1] - lo;
-		if (n > 0) {
-			CUDA_CHECK(cudaEventSynchronize(b->ev_info[c]));
-			for (int i = lo; i < lo + n; i++) {
-				Stream &s = b->streams[fresh[i].stream];
-				// cache indices were taken at planning time; `taken` pictures have left the front since
-				const size_t tk = (size_t)taken[fresh[i].stream];
-				if (fresh[i].cache_idx < tk || fresh[i].cache_idx - tk >= s.cache.size()) continue;  // flushed meanwhile
-				Parsed &p = s.cache[fresh[i].cache_idx - tk];
-				p.info = b->h_info[i];
-				p.ready = true;
-				if (p.info.error == PARSE_ERR_INVALID_VLC) b->stats.parse_errors++;
-				if (p.info.reserved[0]) b->stats.lane_walk_pictures++;
-			}
-		}
-		// step j of a stream -> reconstruct launch j of the chunk
-		std::vector<std::vector<ReconTask>> steps;
-		std::vector<std::vector<int>> step_streams;
-		const int ordinal_end = G > 0 ? (c + 1) * G : 0x7fffffff;
-		for (int si = 0; si < S; si++) {
-			if (!open[si]) continue;
-			Stream &s = b->streams[si];
-			int step = 0;
-			while (taken[si] < want[si] && taken[si] < ordinal_end) {
-				const uint32_t from_byte = (s.bb.index + 7) >> 3;
-				auto it = std::lower_bound(s.pics.begin(), s.pics.end(), from_byte);
-				if (it == s.pics.end()) {  // findStartCode(PICTURE) == -1: index parks at the end (buffer.js:126-127)
-					s.bb.index = s.bb.length << 3;
-					more[si] = 0;
-					open[si] = 0;
-					break;
-				}
-				if (s.cache.empty() || !s.cache.front().ready || s.cache.front().pos != *it || entry_stale(s, s.cache.front())) {
-					// the look-ahead does not match the serial order: re-plan in the next round.  (Entries of later
-					// chunks may still be in flight; their slots are reused only by parses queued behind them.)
-					flush_cache(b, s);
-					open[si] = 0;
-					taken[si] = 0x40000000;  // nothing of this stream's planning-time indices is valid any more
-					break;
-				}
-				const Parsed e = s.cache.front();
-				s.cache.pop_front();
-				s.bb.index = e.info.end_bit;
-				taken[si]++;
-				progress[si]++;
-				consumed++;
-				b->stats.pictures++;
-				b->stats.es_bytes += (e.info.end_bit >> 3) - e.pos;
-				s.last_type = e.info.picture_type;
-				s.last_temporal = (uint64_t)e.pos + 5 < s.bb.length ? (s.bb.bytes[e.pos + 4] << 2 | s.bb.bytes[e.pos + 5] >> 6) : 0;
-				if (e.info.status == PIC_DECODED) {
-					const bool is_b = e.info.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
-					ReconTask t{};
-					t.hdr = b->d_hdr + (size_t)e.slot * b->slot_mb;
-					t.coef = b->d_coef + (size_t)e.slot * b->slot_mb * MB_COEF_INT16;
-					if (is_b) {
-						// after the swaps `cur` holds the older and `1 - cur` the newer of the two most recent I/P pictures:
-						// the B picture's forward (past) and backward (future) reference.  It goes to a set of its own.
-						if (!s.d_planes_b[0]) {
-							const size_t bytes = (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64;
-							for (auto &pb : s.d_planes_b) {
-								pb = dev_alloc<uint8_t>(bytes);
-								CUDA_CHECK(cudaMemsetAsync(pb, 0, bytes, b->st_recon));
-							}
-						}
-						t.cur = plane_set(s, s.d_planes_b[s.b_cur]);
-						t.fwd = plane_set(s, s.d_planes[s.cur]);
-						t.bwd = plane_set(s, s.d_planes[1 - s.cur]);
-					} else {
-						t.cur = plane_set(s, s.d_planes[s.cur]);
-						t.fwd = plane_set(s, s.d_planes[1 - s.cur]);
-					}
-					s.d_last = t.cur.y;
-					t.mb_width = s.seq.mb_width;
-					t.mb_size = s.seq.mb_size;
-					t.coded_width = s.seq.coded_width;
-					t.coded_height = s.seq.coded_height;
-					t.width = s.width;
-					t.height = s.height;
-					t.rgba = nullptr;
-					if (flags & JSMPEG_B200_OUT_RGBA) {
-						if (!s.d_rgba) {  // opaque white, like the canvas the reference creates (canvas2d.js:24-29): the odd edge keeps it
-							s.d_rgba = dev_alloc<uint8_t>((size_t)s.width * s.height * 4);
-							CUDA_CHECK(cudaMemsetAsync(s.d_rgba, 0xff, (size_t)s.width * s.height * 4, b->st_recon));
-						}
-						t.rgba = s.d_rgba;
-					}
-					if ((int)steps.size() <= step) { steps.emplace_back(); step_streams.emplace_back(); }
-					steps[step].push_back(t);
-					step_streams[step].push_back(si);
-					step++;
-					if (is_b) s.b_cur ^= 1;  // no reference: the I/P ping-pong stays as it is
-					else s.cur ^= 1;         // mpeg1.js:221-246: the picture just decoded becomes `forward`
-					b->stats.pictures_decoded++;
-					b->stats.coded_blocks += e.info.n_coded_blocks;
-					b->stats.macroblocks += e.info.n_present;
-					const uint64_t planes = (uint64_t)s.coded_size * 3 / 2;
-					b->stats.algorithmic_bytes += planes + (e.info.picture_type == 2 ? planes : (is_b ? 2 * planes : 0)) +
-					                              (uint64_t)s.seq.mb_size * sizeof(mb_record_t) + (uint64_t)e.info.n_coded_blocks * 128;
-				}
-				release_slot(b, e.slot);  // reused by the NEXT round's parse, which waits for this round's reconstruction (ev_round)
-			}
-			if (open[si] && taken[si] >= want[si]) open[si] = 0;
-		}
-		// ---- 4. reconstruction of the chunk, one launch per step, on the reconstruct stream
-		if (steps.empty()) continue;
-		size_t total = 0;
-		for (auto &v : steps) total += v.size();
-		ensure_task_caps(b, 0, (int)total);
-		size_t off = 0;
-		std::vector<int> step_n_b(steps.size(), 0);
-		for (size_t f = 0; f < steps.size(); f++) {
-			auto &v = steps[f];
-			// the step's B pictures (extension) behind its I/P pictures: they take the two-reference kernel
-			int n_b = 0;
-			for (auto &t : v) n_b += t.bwd.y != nullptr;
-			if (n_b) {
-				std::vector<ReconTask> tv;
-				std::vector<int> sv;
-				for (int pass = 0; pass < 2; pass++)
-					for (size_t i = 0; i < v.size(); i++)
-						if ((v[i].bwd.y != nullptr) == (pass == 1)) { tv.push_back(v[i]); sv.push_back(step_streams[f][i]); }
-				v.swap(tv);
-				step_streams[f].swap(sv);
-			}
-			step_n_b[f] = n_b;
-			memcpy(b->h_rtasks + off, v.data(), v.size() * sizeof(ReconTask));
-			off += v.size();
-		}
-		CUDA_CHECK(cudaEventRecord(b->ev_rec0[rec_chunks], b->st_recon));
-		off = 0;
-		for (size_t f = 0; f < steps.size(); f++) {
-			// A launch overwrites, per stream, the plane set written two of that stream's pictures ago, i.e. by
-			// a launch at least two copy-out launches back: the copy-out recorded two launches ago must be done
-			// (the copy stream is in order, so that covers every earlier one).
-			if ((flags & JSMPEG_B200_OUT_HOST) && b->copy_steps >= 2)
-				CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_copied[b->copy_steps & 1], 0));
-			const int n_ip = (int)steps[f].size() - step_n_b[f];
-			if (n_ip > 0) {
-				if (flags & JSMPEG_B200_OUT_RGBA) launch_reconstruct_rgba(b->h_rtasks + off, n_ip, b->st_recon);  // conversion fused in
-				else launch_reconstruct(b->h_rtasks + off, n_ip, b->st_recon);
-				b->stats.kernel_launches += (n_ip + (flags & JSMPEG_B200_OUT_RGBA ? 59 : 79)) / (flags & JSMPEG_B200_OUT_RGBA ? 60 : 80);
-			}
-			if (step_n_b[f] > 0)
-				b->stats.kernel_launches += launch_reconstruct_b(b->h_rtasks + off + n_ip, step_n_b[f], (flags & JSMPEG_B200_OUT_RGBA) != 0, b->st_recon);
-			b->stats.recon_launches++;
-			if (flags & JSMPEG_B200_OUT_HOST) copy_out_step(b, steps[f], step_streams[f]);  // while the next step reconstructs
-			off += steps[f].size();
-		}
-		CUDA_CHECK(cudaEventRecord(b->ev_rec1[rec_chunks], b->st_recon));
-		rec_chunks++;
-		// h_rtasks is read at launch time only (the table travels in the kernel parameters), so the next chunk may reuse it
-	}
-	if (rec_chunks) {
-		CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
-		b->recon_pending = true;
-		CUDA_CHECK(cudaEventSynchronize(b->ev_rec1[rec_chunks - 1]));
-		for (int k = 0; k < rec_chunks; k++) {
-			float ms = 0;
-			CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_rec0[k], b->ev_rec1[k]));
-			b->stats.recon_ms += ms;
-		}
-	}
-	if (!fresh.empty()) {
-		CUDA_CHECK(cudaEventSynchronize(b->ev_b));
+		b->stats.h2d_bytes += wave.size() * sizeof(ParseTask);
+		b->stats.d2h_bytes += wave.size() * sizeof(picture_info_t);
 		float ms = 0;
 		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_a, b->ev_b));
 		b->stats.parse_ms += ms;
 		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_a, b->ev_mid));
 		b->stats.walk_ms += ms;
+	}
+	// ---- 3. consume in decode() order; the j-th reconstructed picture of a stream goes to step j
+	long consumed = 0;
+	std::vector<ReconStep> steps;
+	for (int si = 0; si < S; si++) {
+		if (!more[si]) continue;
+		Stream &s = b->streams[si];
+		size_t step = 0;
+		while (progress[si] < want[si]) {
+			const uint32_t from_byte = (s.bb.index + 7) >> 3;
+			auto it = std::lower_bound(s.pics.begin(), s.pics.end(), from_byte);
+			if (it == s.pics.end()) {  // findStartCode(PICTURE) == -1: index parks at the end (buffer.js:126-127)
+				s.bb.index = s.bb.length << 3;
+				more[si] = 0;
+				break;
+			}
+			if (s.cache.empty() || s.cache.front().pos != *it || entry_stale(s, s.cache.front())) {
+				flush_cache(b, s);  // the look-ahead does not match the serial order: re-plan in the next round
+				break;
+			}
+			const Parsed e = s.cache.front();
+			s.cache.pop_front();
+			s.bb.index = e.info.end_bit;
+			progress[si]++;
+			consumed++;
+			b->stats.pictures++;
+			b->stats.es_bytes += (e.info.end_bit >> 3) - e.pos;
+			s.last_type = e.info.picture_type;
+			s.last_temporal = (uint64_t)e.pos + 5 < s.bb.length ? (s.bb.bytes[e.pos + 4] << 2 | s.bb.bytes[e.pos + 5] >> 6) : 0;
+			if (e.info.status == PIC_DECODED) {
+				const bool is_b = e.info.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
+				uint8_t *rgba = nullptr;
+				if (flags & JSMPEG_B200_OUT_RGBA) {
+					if (!s.d_rgba) {  // opaque white, like the canvas the reference creates (canvas2d.js:24-29): the odd edge keeps it
+						s.d_rgba = dev_alloc<uint8_t>((size_t)s.width * s.height * 4);
+						CUDA_CHECK(cudaMemsetAsync(s.d_rgba, 0xff, (size_t)s.width * s.height * 4, b->st_recon));
+					}
+					rgba = s.d_rgba;
+				}
+				ReconTask t;
+				if (is_b) {
+					// after the swaps `cur` holds the older and `1 - cur` the newer of the two most recent I/P pictures:
+					// the B picture's forward (past) and backward (future) reference.  It goes to a set of its own.
+					if (!s.d_planes_b[0]) {
+						const size_t bytes = (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64;
+						for (auto &pb : s.d_planes_b) {
+							pb = dev_alloc<uint8_t>(bytes);
+							CUDA_CHECK(cudaMemsetAsync(pb, 0, bytes, b->st_recon));
+						}
+					}
+					t = recon_task(b, s, e.slot, s.d_planes_b[s.b_cur], s.d_planes[s.cur], s.d_planes[1 - s.cur], rgba);
+					s.b_cur ^= 1;  // no reference: the I/P ping-pong stays as it is
+				} else {
+					t = recon_task(b, s, e.slot, s.d_planes[s.cur], s.d_planes[1 - s.cur], nullptr, rgba);
+					s.cur ^= 1;  // mpeg1.js:221-246: the picture just decoded becomes `forward`
+				}
+				s.d_last = t.cur.y;
+				const uint64_t planes = (uint64_t)s.coded_size * 3 / 2;
+				if (steps.size() <= step) steps.emplace_back();
+				steps[step].add(t);
+				if (flags & JSMPEG_B200_OUT_HOST) {  // into the next slot of the stream's host ring
+					s.h_head = (s.h_head + 1) % HOST_RING;
+					steps[step].copy(s.h_planes[s.h_head], t.cur.y, planes);
+					b->stats.d2h_bytes += planes;
+				}
+				step++;
+				b->stats.pictures_decoded++;
+				b->stats.coded_blocks += e.info.n_coded_blocks;
+				b->stats.macroblocks += e.info.n_present;
+				b->stats.algorithmic_bytes += planes + (e.info.picture_type == 2 ? planes : (is_b ? 2 * planes : 0)) +
+				                              (uint64_t)s.seq.mb_size * sizeof(mb_record_t) + (uint64_t)e.info.n_coded_blocks * 128;
+			}
+			release_slot(b, e.slot);  // reused by the NEXT round's parse, which waits for this round's reconstruction (ev_round)
+		}
+	}
+	// ---- 4. reconstruction, one step after the other on the reconstruct stream
+	if (!steps.empty()) {
+		CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
+		for (ReconStep &r : steps) {
+			// A launch overwrites, per stream, the plane set written two of that stream's pictures ago, i.e. by
+			// a launch at least two copy-out launches back: the copy-out recorded two launches ago must be done
+			// (the copy stream is in order, so that covers every earlier one).
+			if ((flags & JSMPEG_B200_OUT_HOST) && b->copy_steps >= 2)
+				CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_copied[b->copy_steps & 1], 0));
+			b->stats.kernel_launches += launch_step(r, b->st_recon);
+			b->stats.recon_launches++;
+			if (flags & JSMPEG_B200_OUT_HOST) copy_out_step(b, r);  // while the next step reconstructs
+		}
+		CUDA_CHECK(cudaEventRecord(b->ev_recon[1], b->st_recon));
+		CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
+		b->recon_pending = true;
+		CUDA_CHECK(cudaEventSynchronize(b->ev_recon[1]));
+		float ms = 0;
+		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_recon[0], b->ev_recon[1]));
+		b->stats.recon_ms += ms;
 	}
 	return consumed;
 }
@@ -1056,13 +937,18 @@ bool picture_closed(const Stream &s, uint32_t k) {
 	return false;
 }
 
-// The pictures (indices into s.pics) decode_intra can decode now: after the first sequence header, picture_coding_type
-// 1, and closed.
-std::vector<uint32_t> intra_index(const Stream &s) {
-	std::vector<uint32_t> out;
+// An entry of an index: picture `pic` (an index into s.pics) and its chain start
+struct IndexEntry {
+	uint32_t pic, chain_start;
+};
+
+// The pictures decode_intra can decode now: after the first sequence header, picture_coding_type 1, and closed.  Each
+// is its own chain start.
+std::vector<IndexEntry> intra_index(const Stream &s) {
+	std::vector<IndexEntry> out;
 	if (!s.has_seq) return out;
 	for (uint32_t k = 0; k < s.pics.size(); k++)
-		if (s.pics[k] >= s.seq_floor && picture_type_of(s, k) == 1 && picture_closed(s, k)) out.push_back(k);
+		if (s.pics[k] >= s.seq_floor && picture_type_of(s, k) == 1 && picture_closed(s, k)) out.push_back({k, k});
 	return out;
 }
 
@@ -1086,10 +972,6 @@ bool picture_decoded(const Batch *b, const Stream &s, uint32_t k) {
 	if (type == 2) return picture_header_bits(s, k, 30, 3) != 0;
 	return type == 3 && b->decode_b && picture_header_bits(s, k, 30, 3) != 0 && picture_header_bits(s, k, 34, 3) != 0;
 }
-
-struct IndexEntry {
-	uint32_t pic, chain_start;
-};
 
 // The pictures decode_pictures can decode now: after the first sequence header, closed, reconstructed by decode(),
 // and with a chain start -- the greatest picture j <= k of the intra index such that at least r(k) pictures of
@@ -1203,7 +1085,6 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 	if (b->free_slots.size() < n_tasks)
 		for (auto &s : b->streams) flush_cache(b, s);
 	const int wave_max = (int)b->free_slots.size();
-	ensure_task_caps(b, (int)std::min<size_t>(n_tasks, (size_t)wave_max), 0);
 	// chain groups: at most wave_max chains (a wave parses at least one picture of each), and plane sets within half
 	// of the free device memory -- a request beyond the device is cut into groups, not refused
 	size_t free_b = 0, total_b = 0;
@@ -1228,9 +1109,6 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 		b->d_chain_sets = dev_alloc<uint8_t>(most_sets * set_bytes);
 		b->chain_sets_bytes = most_sets * set_bytes;
 	}
-	struct Task { int chain; uint32_t pic; int kind; uint32_t bytes; };
-	// per depth: the I/P and B tasks without and with the fused RGBA conversion, then the copies to destinations
-	struct Depth { std::vector<ReconTask> ip, ip_rgba, bi, bi_rgba; std::vector<void *> dst, src; std::vector<size_t> size; };
 	for (const auto &[glo, ghi] : groups) {
 		size_t sets = 0;
 		for (size_t c = glo; c < ghi; c++)
@@ -1239,48 +1117,30 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 			CUDA_CHECK(cudaMemsetAsync(b->d_chain_sets, 0, set_bytes * sets, b->st_recon));
 		const uint32_t width = (uint32_t)std::max<size_t>(1, (size_t)wave_max / (ghi - glo));
 		for (uint32_t lo = 0;; lo += width) {
-			// ---- stage 1: positions [lo, lo + width) of every chain still consuming, grouped by walk kernel and longest
-			// first, like decode_round
-			std::vector<Task> wave;
+			// ---- stage 1: positions [lo, lo + width) of every chain still consuming
+			std::vector<WaveItem> wave;
+			std::vector<int> wave_chain;  // the chain of each picture of the wave
 			for (size_t c = glo; c < ghi; c++) {
-				const Chain &ch = chains[c];
+				Chain &ch = chains[c];
 				if (ch.next > ch.last) continue;
 				const Stream &s = b->streams[ch.stream];
 				for (uint32_t p = ch.first + lo; p <= ch.last && p - ch.first < lo + width; p++) {
 					const uint32_t end = p + 1 < s.pics.size() ? s.pics[p + 1] : s.bb.length;
-					wave.push_back({(int)c, p, walk_kind(b, s, p), end - s.pics[p]});
+					const int slot = b->free_slots.back();
+					b->free_slots.pop_back();
+					ch.slot[p - ch.first] = slot;
+					wave.push_back({ch.stream, p, slot, walk_kind(b, s, p), end - s.pics[p]});
+					wave_chain.push_back((int)c);
 				}
 			}
 			if (wave.empty()) break;
-			std::stable_sort(wave.begin(), wave.end(), [](const Task &x, const Task &y) {
-				return x.kind != y.kind ? x.kind < y.kind : x.bytes > y.bytes;
-			});
-			const int m = (int)wave.size();
-			int cnt[3] = {0, 0, 0};
-			for (int t = 0; t < m; t++) {
-				Chain &ch = chains[wave[t].chain];
-				const int slot = b->free_slots.back();
-				b->free_slots.pop_back();
-				ch.slot[wave[t].pic - ch.first] = slot;
-				b->h_ptasks[t] = parse_task(b, ch.stream, wave[t].pic, slot, t);
-				cnt[wave[t].kind]++;
-			}
-			if (b->recon_pending) {  // reconstruct launches of an earlier round or wave may still read these slots
-				CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_round, 0));
-				b->recon_pending = false;
-			}
-			CUDA_CHECK(cudaMemcpyAsync(b->d_ptasks, b->h_ptasks, m * sizeof(ParseTask), cudaMemcpyHostToDevice, b->st_main));
-			if (cnt[0]) launch_parse_pictures(b->d_ptasks, cnt[0], b->slot_mb, b->st_main, nullptr, &b->fork);
-			if (cnt[1]) launch_parse_pictures_slices(b->d_ptasks + cnt[0], cnt[1], b->slot_mb, b->st_main);
-			if (cnt[2]) launch_parse_pictures_b(b->d_ptasks + cnt[0] + cnt[1], cnt[2], b->slot_mb, b->st_main);
-			CUDA_CHECK(cudaMemcpyAsync(b->h_info, b->d_info, m * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
-			CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-			for (int t = 0; t < m; t++) {
-				Chain &ch = chains[wave[t].chain];
+			parse_wave(b, wave);
+			for (size_t t = 0; t < wave.size(); t++) {
+				Chain &ch = chains[wave_chain[t]];
 				ch.info[wave[t].pic - ch.first] = b->h_info[t];
 			}
 			// ---- decode()'s consumption rule over the infos (decode_round): which pictures reconstruct, at which depth
-			std::vector<Depth> depths;
+			std::vector<ReconStep> depths;
 			for (size_t c = glo; c < ghi; c++) {
 				Chain &ch = chains[c];
 				const Stream &s = b->streams[ch.stream];
@@ -1301,43 +1161,21 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 					const bool is_b = e.picture_type == 3;  // (only the B walk answers PIC_DECODED for one)
 					if (e.status == PIC_DECODED && (!is_b || k < ch.b_end)) {
 						const int slot = ch.slot[k - ch.first];
-						ReconTask t{};
-						t.hdr = b->d_hdr + (size_t)slot * b->slot_mb;
-						t.coef = b->d_coef + (size_t)slot * b->slot_mb * MB_COEF_INT16;
 						const bool leaf = ch.n_sets == 0;
-						if (is_b) {  // the two I/P sets: `cur` the older (forward), `1 - cur` the newer (backward) reference
-							t.cur = plane_set(s, ch.set[2 + ch.b_cur]);
-							t.fwd = plane_set(s, ch.set[ch.cur]);
-							t.bwd = plane_set(s, ch.set[1 - ch.cur]);
-						} else if (leaf) {  // into the destination, predicted (skipped macroblocks) from the zeroed scratch set
-							t.cur = plane_set(s, static_cast<uint8_t *>(planes_dst[order[q_lo]]));
-							t.fwd = plane_set(s, b->d_intra_fwd);
-						} else {
-							t.cur = plane_set(s, ch.set[ch.cur]);
-							t.fwd = plane_set(s, ch.set[1 - ch.cur]);
-						}
-						t.mb_width = s.seq.mb_width;
-						t.mb_size = s.seq.mb_size;
-						t.coded_width = s.seq.coded_width;
-						t.coded_height = s.seq.coded_height;
-						t.width = s.width;
-						t.height = s.height;
-						const bool out = q_hi > q_lo;
-						t.rgba = rgba && out ? static_cast<uint8_t *>(rgba_dst[order[q_lo]]) : nullptr;
+						uint8_t *out_rgba = rgba && q_hi > q_lo ? static_cast<uint8_t *>(rgba_dst[order[q_lo]]) : nullptr;
+						ReconTask t;
+						if (is_b)  // the two I/P sets: `cur` the older (forward), `1 - cur` the newer (backward) reference
+							t = recon_task(b, s, slot, ch.set[2 + ch.b_cur], ch.set[ch.cur], ch.set[1 - ch.cur], out_rgba);
+						else if (leaf)  // into the destination, predicted (skipped macroblocks) from the zeroed scratch set
+							t = recon_task(b, s, slot, static_cast<uint8_t *>(planes_dst[order[q_lo]]), b->d_intra_fwd, nullptr, out_rgba);
+						else
+							t = recon_task(b, s, slot, ch.set[ch.cur], ch.set[1 - ch.cur], nullptr, out_rgba);
 						if (depths.size() <= d) depths.emplace_back();
-						Depth &dp = depths[d++];
-						(is_b ? (t.rgba ? dp.bi_rgba : dp.bi) : (t.rgba ? dp.ip_rgba : dp.ip)).push_back(t);
+						ReconStep &dp = depths[d++];
+						dp.add(t);
 						for (int q = q_lo; q < q_hi; q++) {  // the first request gets the picture, duplicates a copy of it
-							if (!leaf || q > q_lo) {
-								dp.dst.push_back(planes_dst[order[q]]);
-								dp.src.push_back(t.cur.y);
-								dp.size.push_back((size_t)s.coded_size * 3 / 2);
-							}
-							if (rgba && q > q_lo) {
-								dp.dst.push_back(rgba_dst[order[q]]);
-								dp.src.push_back(t.rgba);
-								dp.size.push_back((size_t)s.width * s.height * 4);
-							}
+							if (!leaf || q > q_lo) dp.copy(planes_dst[order[q]], t.cur.y, (size_t)s.coded_size * 3 / 2);
+							if (rgba && q > q_lo) dp.copy(rgba_dst[order[q]], t.rgba, (size_t)s.width * s.height * 4);
 						}
 						if (is_b) ch.b_cur ^= 1;
 						else ch.cur ^= 1;
@@ -1348,24 +1186,13 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 			}
 			// ---- stage 2: one depth after the other on the reconstruct stream, each followed by its copies (a set is
 			// overwritten two references later, by a later launch on the same stream)
-			for (Depth &dp : depths) {
-				if (!dp.ip.empty()) launch_reconstruct(dp.ip.data(), (int)dp.ip.size(), b->st_recon);
-				if (!dp.ip_rgba.empty()) launch_reconstruct_rgba(dp.ip_rgba.data(), (int)dp.ip_rgba.size(), b->st_recon);
-				if (!dp.bi.empty()) launch_reconstruct_b(dp.bi.data(), (int)dp.bi.size(), false, b->st_recon);
-				if (!dp.bi_rgba.empty()) launch_reconstruct_b(dp.bi_rgba.data(), (int)dp.bi_rgba.size(), true, b->st_recon);
-				if (!dp.dst.empty()) {
-					b->copy_dst.swap(dp.dst);
-					b->copy_src.swap(dp.src);
-					b->copy_size.swap(dp.size);
-					copy_batch(b, b->st_recon);
-				}
+			for (ReconStep &dp : depths) {
+				launch_step(dp, b->st_recon);
+				if (!dp.dst.empty()) copy_batch(b, dp.dst, dp.src, dp.size, b->st_recon);
 			}
 			CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
 			b->recon_pending = true;
-			for (int t = 0; t < m; t++) {  // reused by the next wave's parse, which waits for ev_round
-				const Chain &ch = chains[wave[t].chain];
-				release_slot(b, ch.slot[wave[t].pic - ch.first]);
-			}
+			for (const WaveItem &w : wave) release_slot(b, w.slot);  // reused by the next wave's parse, which waits for ev_round
 		}
 		for (size_t c = glo; c < ghi; c++)  // never consumed: planes 0 (a copied destination was not zeroed)
 			if (chains[c].n_sets)
@@ -1391,30 +1218,9 @@ bool request_valid(const Batch *b, int si, void *planes, void *image, bool rgba)
 	return !rgba || (image && aligned(image));
 }
 
-long batch_decode_intra(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *planes_dst,
-                        void *const *rgba_dst, int flags, int32_t *n_present_out, int32_t *error_out) {
-	use_device(b);
-	const bool rgba = (flags & JSMPEG_B200_OUT_RGBA) != 0;
-	if (n < 0 || (n > 0 && (!streams || !pictures || !planes_dst || (rgba && !rgba_dst)))) return -2;
-	upload_all(b);
-	// ---- every request is checked before anything changes
-	std::vector<std::vector<uint32_t>> listed(b->streams.size());
-	std::vector<char> indexed(b->streams.size(), 0);
-	std::vector<PictureRequest> req(n);
-	for (int i = 0; i < n; i++) {
-		const int si = streams[i];
-		if (!request_valid(b, si, planes_dst[i], rgba ? rgba_dst[i] : nullptr, rgba)) return -2;
-		if (!indexed[si]) { listed[si] = intra_index(b->streams[si]); indexed[si] = 1; }
-		if (!std::binary_search(listed[si].begin(), listed[si].end(), pictures[i])) return -2;
-		req[i] = {si, pictures[i], pictures[i]};  // an I picture is its own chain start
-	}
-	if (n == 0) return 0;
-	decode_chains(b, req, planes_dst, rgba_dst, rgba, nullptr, n_present_out, error_out);
-	return n;
-}
-
-long batch_decode_pictures(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *planes_dst,
-                           void *const *rgba_dst, int flags, int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
+// decode_intra (`intra`: requests are looked up in the intra index) and decode_pictures (in the picture index)
+long batch_decode_chosen(Batch *b, bool intra, int n, const int *streams, const uint32_t *pictures, void *const *planes_dst,
+                         void *const *rgba_dst, int flags, int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
 	use_device(b);
 	const bool rgba = (flags & JSMPEG_B200_OUT_RGBA) != 0;
 	if (n < 0 || (n > 0 && (!streams || !pictures || !planes_dst || (rgba && !rgba_dst)))) return -2;
@@ -1426,7 +1232,10 @@ long batch_decode_pictures(Batch *b, int n, const int *streams, const uint32_t *
 	for (int i = 0; i < n; i++) {
 		const int si = streams[i];
 		if (!request_valid(b, si, planes_dst[i], rgba ? rgba_dst[i] : nullptr, rgba)) return -2;
-		if (!indexed[si]) { listed[si] = picture_index(b, b->streams[si]); indexed[si] = 1; }
+		if (!indexed[si]) {
+			listed[si] = intra ? intra_index(b->streams[si]) : picture_index(b, b->streams[si]);
+			indexed[si] = 1;
+		}
 		auto e = std::lower_bound(listed[si].begin(), listed[si].end(), pictures[i],
 		                          [](const IndexEntry &x, uint32_t k) { return x.pic < k; });
 		if (e == listed[si].end() || e->pic != pictures[i]) return -2;
@@ -1488,9 +1297,6 @@ jsmpeg_b200_batch_t *jsmpeg_b200_batch_create(int n_streams, int device, unsigne
 	b->device = device;
 	b->streams.resize(std::max(n_streams, 1));
 	b->max_slots_req = max_slots;
-	b->chunk_pictures = std::max(0, env_int("JSMPEG_B200_CHUNK", 0));
-	b->chunk_min_wave = std::max(1, env_int("JSMPEG_B200_CHUNK_MIN_WAVE", 256));
-	b->chunk_streams = std::min(std::max(1, env_int("JSMPEG_B200_CHUNK_STREAMS", 3)), 4);
 	b->decode_b = env_int("JSMPEG_B200_DECODE_B", 0) != 0;
 	b->slice_walk = env_int("JSMPEG_B200_SLICE_WALK", 0) != 0;
 	try {
@@ -1498,11 +1304,11 @@ jsmpeg_b200_batch_t *jsmpeg_b200_batch_create(int n_streams, int device, unsigne
 		CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_main, cudaStreamNonBlocking));
 		CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_recon, cudaStreamNonBlocking));
 		CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_copy, cudaStreamNonBlocking));
-		cudaEvent_t *evs[] = {&b->ev_a, &b->ev_b, &b->ev_mid};
-		for (auto e : evs) CUDA_CHECK(cudaEventCreate(e));
-		CUDA_CHECK(cudaEventCreateWithFlags(&b->ev_step, cudaEventDisableTiming));
-		CUDA_CHECK(cudaEventCreateWithFlags(&b->ev_round, cudaEventDisableTiming));
-		for (auto &e : b->ev_copied) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+		for (auto &st : b->st_side) CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+		cudaEvent_t *timed[] = {&b->ev_a, &b->ev_b, &b->ev_mid, &b->ev_recon[0], &b->ev_recon[1]};
+		for (auto e : timed) CUDA_CHECK(cudaEventCreate(e));
+		cudaEvent_t *untimed[] = {&b->ev_step, &b->ev_round, &b->ev_copied[0], &b->ev_copied[1], &b->ev_sfork, &b->ev_sjoin[0], &b->ev_sjoin[1]};
+		for (auto e : untimed) CUDA_CHECK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
 		CUDA_CHECK(cudaEventCreateWithFlags(&b->fork.fork, cudaEventDisableTiming));
 		for (int i = 0; i < PARSE_GROUPS; i++) {
 			CUDA_CHECK(cudaStreamCreateWithFlags(&b->fork.side[i], cudaStreamNonBlocking));
@@ -1544,21 +1350,17 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b) {
 	if (b->h_info) cudaFreeHost(b->h_info);
 	if (b->h_ptasks) cudaFreeHost(b->h_ptasks);
 	if (b->d_ptasks) cudaFree(b->d_ptasks);
-	if (b->h_rtasks) cudaFreeHost(b->h_rtasks);
-	if (b->d_rtasks) cudaFree(b->d_rtasks);
 	if (b->d_intra_fwd) cudaFree(b->d_intra_fwd);
 	if (b->d_chain_sets) cudaFree(b->d_chain_sets);
 	ts_scratch_destroy(b->ts);
 	ps_scratch_destroy(b->ps);
-	cudaEvent_t evs[] = {b->ev_a, b->ev_b, b->ev_mid, b->ev_step, b->ev_round, b->ev_copied[0], b->ev_copied[1], b->fork.fork};
-	for (auto e : evs) if (e) cudaEventDestroy(e);
-	for (auto v : {&b->ev_info, &b->ev_rec0, &b->ev_rec1}) for (auto e : *v) if (e) cudaEventDestroy(e);
+	for (auto e : {b->ev_a, b->ev_b, b->ev_mid, b->ev_recon[0], b->ev_recon[1], b->ev_step, b->ev_round, b->ev_copied[0],
+	               b->ev_copied[1], b->ev_sfork, b->ev_sjoin[0], b->ev_sjoin[1], b->fork.fork}) if (e) cudaEventDestroy(e);
 	for (int i = 0; i < PARSE_GROUPS; i++) {
 		if (b->fork.join[i]) cudaEventDestroy(b->fork.join[i]);
 		if (b->fork.side[i]) cudaStreamDestroy(b->fork.side[i]);
 	}
-	for (auto st : {b->st_main, b->st_recon, b->st_copy, b->st_side[0], b->st_side[1], b->st_chunk[0], b->st_chunk[1], b->st_chunk[2], b->st_chunk[3]}) if (st) cudaStreamDestroy(st);
-	for (auto e : {b->ev_fed, b->ev_sfork, b->ev_sjoin[0], b->ev_sjoin[1], b->ev_chunk_done[0], b->ev_chunk_done[1], b->ev_chunk_done[2], b->ev_chunk_done[3]}) if (e) cudaEventDestroy(e);
+	for (auto st : {b->st_main, b->st_recon, b->st_copy, b->st_side[0], b->st_side[1]}) if (st) cudaStreamDestroy(st);
 	(void)cudaGetLastError();
 	delete b;
 }
@@ -1567,9 +1369,6 @@ const char *jsmpeg_b200_batch_last_error(jsmpeg_b200_batch_t *b) { return (b && 
 
 int jsmpeg_b200_batch_set_option(jsmpeg_b200_batch_t *b, const char *name, int value) {
 	if (!b || !name) return -1;
-	if (!strcmp(name, "chunk_pictures")) { b->chunk_pictures = std::max(0, value); return 0; }
-	if (!strcmp(name, "chunk_min_wave")) { b->chunk_min_wave = std::max(1, value); return 0; }
-	if (!strcmp(name, "chunk_streams")) { b->chunk_streams = std::min(std::max(1, value), 4); return 0; }
 	if (!strcmp(name, "lookahead")) { b->lookahead = std::max(1, value); return 0; }
 	if (!strcmp(name, "slice_walk")) { b->slice_walk = value != 0; return 0; }  // (same records either way: nothing to flush)
 	if (!strcmp(name, "decode_b")) {
@@ -1668,10 +1467,10 @@ long jsmpeg_b200_batch_intra_index(jsmpeg_b200_batch_t *b, int stream, uint32_t 
 		use_device(b);
 		upload_all(b);
 		const Stream &s = b->streams[stream];
-		const std::vector<uint32_t> listed = intra_index(s);
+		const std::vector<IndexEntry> listed = intra_index(s);
 		for (long i = 0; i < std::min<long>((long)listed.size(), n_max); i++) {
-			const uint32_t pos = s.pics[listed[i]];
-			if (picture_out) picture_out[i] = listed[i];
+			const uint32_t pos = s.pics[listed[i].pic];
+			if (picture_out) picture_out[i] = listed[i].pic;
 			if (byte_pos_out) byte_pos_out[i] = pos;
 			if (temporal_reference_out) temporal_reference_out[i] = s.bb.bytes[pos + 4] << 2 | s.bb.bytes[pos + 5] >> 6;
 		}
@@ -1683,7 +1482,7 @@ long jsmpeg_b200_batch_decode_intra(jsmpeg_b200_batch_t *b, int n, const int *st
                                     void *const *planes_dst, void *const *rgba_dst, int flags, int32_t *n_present_out,
                                     int32_t *error_out) {
 	return guarded<long>(b, -1, [&] {
-		return batch_decode_intra(b, n, streams, pictures, planes_dst, rgba_dst, flags, n_present_out, error_out);
+		return batch_decode_chosen(b, true, n, streams, pictures, planes_dst, rgba_dst, flags, nullptr, n_present_out, error_out);
 	});
 }
 
@@ -1712,7 +1511,7 @@ long jsmpeg_b200_batch_decode_pictures(jsmpeg_b200_batch_t *b, int n, const int 
                                        void *const *planes_dst, void *const *rgba_dst, int flags, int32_t *status_out,
                                        int32_t *n_present_out, int32_t *error_out) {
 	return guarded<long>(b, -1, [&] {
-		return batch_decode_pictures(b, n, streams, pictures, planes_dst, rgba_dst, flags, status_out, n_present_out, error_out);
+		return batch_decode_chosen(b, false, n, streams, pictures, planes_dst, rgba_dst, flags, status_out, n_present_out, error_out);
 	});
 }
 

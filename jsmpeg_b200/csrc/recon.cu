@@ -96,8 +96,9 @@ void fill_task(CompactTask &c, const ReconTask &t) {
 
 }  // namespace
 
-void launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream) {
-	for (int first = 0; first < n_tasks; first += MAX_TASKS) {
+int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream) {
+	int launches = 0;
+	for (int first = 0; first < n_tasks; first += MAX_TASKS, launches++) {
 		const int n = n_tasks - first < MAX_TASKS ? n_tasks - first : MAX_TASKS;
 		ReconParams p;
 		int max_slots = 0;
@@ -110,10 +111,12 @@ void launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t s
 		dim3 grid((max_slots + THREADS - 1) / THREADS, n);
 		reconstruct_kernel<<<grid, THREADS, 0, stream>>>(p);
 	}
+	return launches;
 }
 
-void launch_reconstruct_rgba(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream) {
-	for (int first = 0; first < n_tasks; first += MAX_TASKS_RGBA) {
+int launch_reconstruct_rgba(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream) {
+	int launches = 0;
+	for (int first = 0; first < n_tasks; first += MAX_TASKS_RGBA, launches++) {
 		const int n = n_tasks - first < MAX_TASKS_RGBA ? n_tasks - first : MAX_TASKS_RGBA;
 		ReconRgbaParams p;
 		int max_w = 0, max_h = 0;
@@ -129,6 +132,7 @@ void launch_reconstruct_rgba(const ReconTask *tasks_host, int n_tasks, cudaStrea
 		dim3 grid((max_w + RGBA_MBS - 1) / RGBA_MBS, max_h, n);
 		reconstruct_rgba_kernel<<<grid, RGBA_THREADS, 0, stream>>>(p);
 	}
+	return launches;
 }
 
 int launch_reconstruct_b(const ReconTask *tasks_host, int n_tasks, bool rgba, cudaStream_t stream) {

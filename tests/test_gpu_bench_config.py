@@ -62,13 +62,6 @@ def test_one_wave_of_64_streams_device_output(workload):
     assert st["lane_walk_pictures"] == STREAMS * PICTURES and st["parse_errors"] == 0
     bad = [i for i in range(STREAMS) if _hash(bench, bd.read_planes(i)) != int(want[i, PICTURES - 1])]
     assert not bad, f"last picture differs from the reference in streams {bad}"
-    # the same wave with the parse/reconstruct pipeline cut into chunks of 6 pictures
-    bd.set_option("chunk_pictures", 6)
-    bd.rewind()
-    assert bd.decode(PICTURES, OUT_DEVICE) == STREAMS * PICTURES
-    bad = [i for i in range(STREAMS) if _hash(bench, bd.read_planes(i)) != int(want[i, PICTURES - 1])]
-    assert not bad, f"chunked pipeline: last picture differs in streams {bad}"
-    bd.set_option("chunk_pictures", 0)
     # in calls of 5 pictures: pictures 4, 9, 14, 19, 24 of every stream
     bd.rewind()
     for k in range(PICTURES // 5):
