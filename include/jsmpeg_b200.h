@@ -239,6 +239,47 @@ long jsmpeg_b200_batch_decode_pictures(jsmpeg_b200_batch_t *b, int n, const int 
                                        void *const *planes_dst, void *const *rgba_dst, int flags,
                                        int32_t *status_out, int32_t *n_present_out, int32_t *error_out);
 
+/* MACROBLOCK DATA (motion detection, shot-cut cues, compressed-domain analytics): each macroblock's coding mode and
+ * motion vectors of chosen pictures of any streams, read by the picture walks alone -- no coefficients, no pixels, no
+ * reference pictures, so every request of a call is one wave.  One entry per macroblock, raster order (= macroblock
+ * address), mb_height * mb_width entries per picture. */
+typedef struct jsmpeg_b200_macroblock_t {
+	int16_t fwd_x, fwd_y;  /* forward vector, luma half-pel units as used for prediction (full_pel already doubled) */
+	int16_t bwd_x, bwd_y;  /* backward vector (B pictures), same units */
+	uint8_t flags;         /* JSMPEG_B200_MB_* */
+	uint8_t cbp;           /* bit (5 - block) set <=> block coded; blocks 0-3 luma, 4 Cb, 5 Cr */
+	uint8_t qscale;        /* quantiser_scale in force */
+	uint8_t reserved[5];   /* 0 */
+} jsmpeg_b200_macroblock_t;   /* 16 bytes */
+#define JSMPEG_B200_MB_PRESENT  0x01  /* decoded (coded or skipped); all other fields are 0 when clear */
+#define JSMPEG_B200_MB_INTRA    0x02
+#define JSMPEG_B200_MB_SKIPPED  0x04  /* made by a macroblock-address increment > 1 */
+#define JSMPEG_B200_MB_BACKWARD 0x08  /* predicted from the backward reference (bwd_*) */
+#define JSMPEG_B200_MB_FORWARD  0x10  /* predicted from the forward reference (fwd_*) */
+/* FORWARD is set on every present non-intra macroblock of an I or P picture (skipped ones and P macroblocks without
+ * motion predict from the forward picture with the zero vector); in a B picture the two direction flags say which
+ * references a non-intra macroblock is predicted from (both: their average).  A vector whose flag is clear is 0.
+ * Chroma vectors follow from the luma vector and are not exported. */
+
+/* Pictures of `stream` that decode_macroblocks can describe now; returns how many there are (-1 dead, -2 stream out
+ * of range); the first min(count, n_max) go to the arrays, any of which may be NULL.  Picture k (numbered as above) is
+ * listed when it starts after the first sequence header, is closed (as above), and is one the walks decode: an I
+ * picture, a P picture with forward_f_code != 0, or a B picture with both f_codes != 0 -- B pictures whatever the
+ * "decode_b" option says, and with no chain start needed (a B picture's macroblock layer depends on its own bits). */
+long jsmpeg_b200_batch_macroblock_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out,
+                                        uint32_t *byte_pos_out, int32_t *type_out, int32_t *temporal_reference_out,
+                                        long n_max);
+/* Describe n listed pictures, of any streams.  Request i = picture pictures[i] of stream streams[i] into mb_dst[i]:
+ * DEVICE memory of mb_height * mb_width jsmpeg_b200_macroblock_t, 16-byte aligned.  Each picture is what the walk
+ * gives when it starts at the picture's own start code: for a clean stream, what a fresh decoder (B pictures on) gives
+ * for the first sequence header + the picture + its closing code, and the macroblocks decode() uses for picture k
+ * whenever it consumes it.  Synchronous; duplicates each get the entries.  n_present_out / error_out (may be NULL) get
+ * picture_info_t.n_present / .error per request.  Returns n; -1 dead; -2 a request is invalid (stream out of range or
+ * without sequence header, picture not in the macroblock index, NULL or misaligned destination) -- checked before any
+ * work, and then nothing changed.  Changes nothing decode() observes, as decode_intra. */
+long jsmpeg_b200_batch_decode_macroblocks(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                          void *const *mb_dst, int32_t *n_present_out, int32_t *error_out);
+
 void jsmpeg_b200_batch_get_stats(jsmpeg_b200_batch_t *b, jsmpeg_b200_stats_t *out);
 void jsmpeg_b200_batch_reset_stats(jsmpeg_b200_batch_t *b);
 

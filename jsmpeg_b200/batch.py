@@ -57,6 +57,8 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
     "jsmpeg_b200_batch_picture_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_pictures": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP, _VP]),
+    "jsmpeg_b200_batch_macroblock_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_long]),
+    "jsmpeg_b200_batch_decode_macroblocks": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_get_stats": (None, [_VP, ctypes.POINTER(Stats)]),
     "jsmpeg_b200_batch_reset_stats": (None, [_VP]),
     "jsmpeg_b200_debug_parse_picture": (ctypes.c_int, [_VP, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int, ctypes.c_int,
@@ -82,6 +84,19 @@ def planes_view(t, info):
     return t[:n].view(ch, cw), t[n:n + n // 4].view(ch // 2, cw // 2), t[n + n // 4:n + n // 2].view(ch // 2, cw // 2)
 
 
+MACROBLOCK_BYTES = 16  # sizeof(jsmpeg_b200_macroblock_t)
+MB_PRESENT, MB_INTRA, MB_SKIPPED, MB_BACKWARD, MB_FORWARD = 0x01, 0x02, 0x04, 0x08, 0x10  # JSMPEG_B200_MB_*
+
+
+def macroblocks_view(t):
+    """Named views of a decode_macroblocks tensor [mb_height, mb_width, 16]: "forward" and "backward" int16 [h, w, 2]
+    (x, y in luma half-pel units), "flags" (MB_*), "cbp" and "qscale" uint8 [h, w]."""
+    import torch
+    as16 = t.view(torch.int16)  # [h, w, 8]: fwd_x, fwd_y, bwd_x, bwd_y, ...
+    return {"forward": as16[..., 0:2], "backward": as16[..., 2:4], "flags": t[..., 8], "cbp": t[..., 9],
+            "qscale": t[..., 10]}
+
+
 def bind_batch_abi(lib):
     for name, (res, args) in _BATCH_ABI.items():
         fn = getattr(lib, name)
@@ -101,6 +116,7 @@ class BatchDecoder:
         self._pes = [[] for _ in range(n_streams)]  # per stream: every (payload byte offset, pts seconds) write_ts/write_ps returned
         self.last_intra_info = []  # per request of the last decode_intra: {"n_present", "error"} (picture_info_t)
         self.last_pictures_info = []  # per request of the last decode_pictures: {"status", "n_present", "error"}
+        self.last_macroblocks_info = []  # per request of the last decode_macroblocks: {"n_present", "error"}
         self.handle = self.lib.jsmpeg_b200_batch_create(n_streams, device, max_slots)
         err = self.lib.jsmpeg_b200_batch_last_error(self.handle)
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
@@ -296,6 +312,63 @@ class BatchDecoder:
         out, n_present, errors = self._decode_requests(self.lib.jsmpeg_b200_batch_decode_intra, reqs, rgba, [],
                                                        "a request names a picture that is not in the stream's intra index")
         self.last_intra_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(len(reqs))]
+        return out
+
+    def macroblock_index(self, stream):
+        """The pictures of `stream` that decode_macroblocks can describe now (include/jsmpeg_b200.h): one dict per
+        picture, {"picture": k, "byte_pos", "type" (picture_coding_type), "temporal_reference", "pts"}; `pts` as in
+        intra_index.  B pictures are listed whatever the decode_b option says."""
+        n = self.lib.jsmpeg_b200_batch_macroblock_index(self.handle, stream, None, None, None, None, 0)
+        if n == -2:
+            raise ValueError(f"stream {stream} out of range")
+        if n < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_macroblock_index failed")
+        pic, pos, kind, tr = np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.int32), np.zeros(n, np.int32)
+        n = self.lib.jsmpeg_b200_batch_macroblock_index(self.handle, stream, pic.ctypes.data, pos.ctypes.data,
+                                                        kind.ctypes.data, tr.ctypes.data, n)
+        return [{"picture": int(pic[i]), "byte_pos": int(pos[i]), "type": int(kind[i]), "temporal_reference": int(tr[i]),
+                 "pts": self._pts(stream, int(pos[i]))} for i in range(min(n, len(pic)))]
+
+    def decode_macroblocks(self, requests):
+        """Macroblock types and motion vectors of pictures listed by macroblock_index, of any streams, in one call:
+        `requests` is an iterable of (stream, picture).  Returns per request a torch.uint8 CUDA tensor [mb_height,
+        mb_width, 16] of jsmpeg_b200_macroblock_t entries (see macroblocks_view); last_macroblocks_info gets
+        {"n_present", "error"} per request.  The tensors are views of one allocation per picture size (thousands of
+        requests cost a few allocations, not thousands)."""
+        import torch
+        reqs = [(int(s), int(p)) for s, p in requests]
+        n = len(reqs)
+        shapes = {}  # per stream: (mb_height, mb_width)
+        for s, _ in reqs:
+            if s in shapes:
+                continue
+            if not 0 <= s < self.n_streams:
+                raise ValueError(f"stream {s} out of range")
+            info = self.stream_info(s)
+            if not info["has_sequence_header"]:
+                raise ValueError(f"stream {s} has no sequence header yet")
+            shapes[s] = ((info["height"] + 15) // 16, (info["width"] + 15) // 16)
+        dev = torch.device("cuda", self.device)
+        by_shape = {}  # per picture size: the requests of that size
+        for i, (s, _) in enumerate(reqs):
+            by_shape.setdefault(shapes[s], []).append(i)
+        out = [None] * n
+        for shape, idx in by_shape.items():  # (entries are 16 bytes: every view is 16-byte aligned)
+            views = torch.empty((len(idx), *shape, MACROBLOCK_BYTES), dtype=torch.uint8, device=dev).unbind(0)
+            for i, t in zip(idx, views):
+                out[i] = t
+        streams = (ctypes.c_int * max(n, 1))(*[s for s, _ in reqs])
+        pictures = (ctypes.c_uint32 * max(n, 1))(*[p for _, p in reqs])
+        dst = (_VP * max(n, 1))(*[t.data_ptr() for t in out])
+        n_present = (ctypes.c_int32 * max(n, 1))()
+        errors = (ctypes.c_int32 * max(n, 1))()
+        torch.cuda.current_stream(dev).synchronize()  # the allocations are the caller's stream's; the call uses its own
+        got = self.lib.jsmpeg_b200_batch_decode_macroblocks(self.handle, n, streams, pictures, dst, n_present, errors)
+        if got == -2:
+            raise ValueError("a request names a picture that is not in the stream's macroblock index")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_macroblocks failed")
+        self.last_macroblocks_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
         return out
 
     def _decode_requests(self, fn, reqs, rgba, extra_out, refused):

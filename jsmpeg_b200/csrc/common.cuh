@@ -114,8 +114,9 @@ struct ParseFork {
 	cudaEvent_t fork, join[PARSE_GROUPS];
 };
 // Stage 1 of I/P pictures: a walk + an expand launch per size group (one group without `fork`); walk_done, unless
-// nullptr, is recorded behind the first group's walk.  Returns the number of kernels launched.
-int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream,
+// nullptr, is recorded behind the first group's walk.  expand = false: the walk alone (macroblock records without
+// coefficients), in one group.  Returns the number of kernels launched.
+int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream,
                           cudaEvent_t walk_done = nullptr, const ParseFork *fork = nullptr);
 // Stage 2.  `tasks_host` is read on the host at launch time: the table travels in the kernel parameters.  Each
 // launcher returns the number of kernels it launched.
@@ -124,12 +125,27 @@ int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t st
 int launch_reconstruct_rgba(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
 // B pictures (every task has `bwd`): prediction from two references; `rgba` = with the fused conversion
 int launch_reconstruct_b(const ReconTask *tasks_host, int n_tasks, bool rgba, cudaStream_t stream);
-// stage 1 for B pictures: the serial walk with the B-picture macroblock layer (walk_b.cuh) + the same expand
-void launch_parse_pictures_b(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream);
-// stage 1 for I/P pictures of many slices (opt-in, walk_slices.cuh): a lane per slice + the same expand
-void launch_parse_pictures_slices(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream);
+// stage 1 for B pictures: the serial walk with the B-picture macroblock layer (walk_b.cuh) + the same expand unless
+// `expand` is false; returns the number of kernels launched
+int launch_parse_pictures_b(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream);
+// stage 1 for I/P pictures of many slices (opt-in, walk_slices.cuh): a lane per slice + the same expand unless
+// `expand` is false; returns the number of kernels launched
+int launch_parse_pictures_slices(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream);
 // the host routes an I/P picture to it when it has at least this many slices
 constexpr int SLICE_WALK_MIN_SLICES = 4;
+
+// Macroblock export (macroblocks.cu): request i converts the records of one picture (`mb_size` of them at `src`, a
+// picture of picture_coding_type `picture_type`) into the public jsmpeg_b200_macroblock_t layout at `dst`; `first` is
+// the number of macroblocks of requests 0 .. i-1.  One thread per macroblock of all requests, one launch.
+struct MbExportTask {
+	const mb_record_t *src;
+	void *dst;
+	uint32_t first;
+	int32_t mb_size;
+	int32_t picture_type;
+	int32_t pad;
+};
+void launch_export_macroblocks(const MbExportTask *tasks, int n_tasks, uint32_t total_mb, cudaStream_t stream);
 
 // device MPEG-TS demux (tsdemux.cu)
 struct TsScratch;

@@ -25,6 +25,7 @@
 // side streams) and waits for the picture infos; the host then consumes them in decode() order and
 // queues one reconstruct step per picture depth (ReconStep, launch_step) on the reconstruct stream.
 // Cutting the wave into chunks to overlap stage 1 with stage 2 was measured not to pay (DESIGN 8).
+// decode_macroblocks runs the same waves walk-only (no expand, no reconstruct) and exports the records (DESIGN 3.8).
 #include <sched.h>
 
 #include <algorithm>
@@ -155,6 +156,9 @@ struct jsmpeg_b200_batch_t {
 	size_t intra_fwd_bytes = 0;
 	uint8_t *d_chain_sets = nullptr;
 	size_t chain_sets_bytes = 0;
+	// decode_macroblocks: the export tasks of a wave (DESIGN 3.8)
+	MbExportTask *h_xtasks = nullptr, *d_xtasks = nullptr;
+	int xtask_cap = 0;
 	jsmpeg_b200_stats_t stats{};
 };
 
@@ -605,11 +609,12 @@ int picture_type_of(const Stream &s, uint32_t pic) {
 	return (uint64_t)pos + 5 < s.bb.length ? (s.bb.bytes[pos + 5] >> 3) & 7 : 0;
 }
 
-// Which walk kernel takes picture `pic` of a stream: 0 the lane-parallel walk, 1 the slice walk, 2 the B-picture walk
-int walk_kind(const Batch *b, const Stream &s, uint32_t pic) {
-	// the extension: a type 3 picture goes to the B-picture walk; everything else, and everything without it, to the I/P walk
+// Which walk kernel takes picture `pic` of a stream: 0 the lane-parallel walk, 1 the slice walk, 2 the B-picture walk.
+// b_walk: a type 3 picture goes to the B-picture walk (decode() and decode_pictures: the decode_b option); everything
+// else, and everything without it, to the I/P walk
+int walk_kind(const Batch *b, const Stream &s, uint32_t pic, bool b_walk) {
 	const int type = picture_type_of(s, pic);
-	int kind = (b->decode_b && type == 3) ? 2 : 0;
+	int kind = (b_walk && type == 3) ? 2 : 0;
 	if (b->slice_walk && (type == 1 || type == 2)) {  // enough slice start codes between this picture's and the next one's?
 		const uint32_t hi = pic + 1 < s.pic_code.size() ? s.pic_code[pic + 1] : (uint32_t)s.codes.size();
 		int n_slices = 0;
@@ -654,14 +659,15 @@ struct WaveItem {
 	uint32_t bytes;
 };
 
-// Stage 1 of `wave` as one wave, for decode() and decode_chains alike.  The tasks are grouped by walk kernel and,
+// Stage 1 of `wave` as one wave, for decode(), decode_chains and decode_macroblocks alike; expand = false runs the walks
+// alone (records without coefficients: decode_macroblocks).  The tasks are grouped by walk kernel and,
 // within a kernel, longest first: a CTA's warps, and consecutive CTAs (which land on different SMs), then carry
 // similar amounts of work and the walk ends without a long tail.  The first kernel present runs on the main stream;
 // the others have walk kernels of their own (one warp per picture, latency-bound like every walk) and run beside it on
 // side streams, forked after the upload and joined before the infos are read.  On return the infos are on the host,
 // b->h_info[i] that of wave[i], and ev_a / ev_mid / ev_b bracket the wave and its lane-parallel walk.  Returns the
 // number of kernels launched.
-int parse_wave(Batch *b, const std::vector<WaveItem> &wave) {
+int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 	const int n = (int)wave.size();
 	std::vector<int> order(n);
 	for (int i = 0; i < n; i++) order[i] = i;
@@ -694,13 +700,9 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave) {
 			st = b->st_side[n_side];
 			CUDA_CHECK(cudaStreamWaitEvent(st, b->ev_sfork, 0));
 		}
-		if (kind == 0) {
-			launches += launch_parse_pictures(b->d_ptasks, cnt[0], b->slot_mb, st, b->ev_mid, &b->fork);
-		} else {
-			if (kind == 1) launch_parse_pictures_slices(b->d_ptasks + off[1], cnt[1], b->slot_mb, st);
-			else launch_parse_pictures_b(b->d_ptasks + off[2], cnt[2], b->slot_mb, st);
-			launches += 2;  // walk + expand
-		}
+		if (kind == 0) launches += launch_parse_pictures(b->d_ptasks, cnt[0], b->slot_mb, expand, st, b->ev_mid, &b->fork);
+		else if (kind == 1) launches += launch_parse_pictures_slices(b->d_ptasks + off[1], cnt[1], b->slot_mb, expand, st);
+		else launches += launch_parse_pictures_b(b->d_ptasks + off[2], cnt[2], b->slot_mb, expand, st);
 		if (kind != primary) {
 			CUDA_CHECK(cudaEventRecord(b->ev_sjoin[n_side], st));
 			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_sjoin[n_side], 0));
@@ -769,12 +771,12 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			s.cache.push_back(p);
 			++next;
 			const uint32_t pic = (uint32_t)(next - 1 - s.pics.begin());
-			wave.push_back({si, pic, p.slot, walk_kind(b, s, pic), (next < s.pics.end() ? *next : s.bb.length) - p.pos});
+			wave.push_back({si, pic, p.slot, walk_kind(b, s, pic, b->decode_b), (next < s.pics.end() ? *next : s.bb.length) - p.pos});
 		}
 	}
 	// ---- 2. stage 1: the wave, every picture's info on the host before consumption starts
 	if (!wave.empty()) {
-		b->stats.kernel_launches += parse_wave(b, wave);
+		b->stats.kernel_launches += parse_wave(b, wave, true);
 		for (size_t i = 0; i < wave.size(); i++) {  // a stream's pictures are in the wave in cache order
 			const int si = wave[i].stream;
 			Parsed &p = b->streams[si].cache[fresh[si]++];
@@ -964,13 +966,13 @@ uint32_t picture_header_bits(const Stream &s, uint32_t pic, int bit, int n) {
 	return v;
 }
 
-// Whether decode() reconstructs picture k (PIC_DECODED), by the walks' rule (walk.cuh, walk_b.cuh): an I picture, a
-// P picture with forward_f_code != 0, and with decode_b a B picture with both f_codes != 0
-bool picture_decoded(const Batch *b, const Stream &s, uint32_t k) {
+// Whether the walks decode picture k (PIC_DECODED), by their rule (walk.cuh, walk_b.cuh): an I picture, a P picture with
+// forward_f_code != 0, and when B pictures go to the B walk (decode_b) a B picture with both f_codes != 0
+bool picture_decoded(const Stream &s, uint32_t k, bool decode_b) {
 	const int type = picture_type_of(s, k);
 	if (type == 1) return true;
 	if (type == 2) return picture_header_bits(s, k, 30, 3) != 0;
-	return type == 3 && b->decode_b && picture_header_bits(s, k, 30, 3) != 0 && picture_header_bits(s, k, 34, 3) != 0;
+	return type == 3 && decode_b && picture_header_bits(s, k, 30, 3) != 0 && picture_header_bits(s, k, 34, 3) != 0;
 }
 
 // The pictures decode_pictures can decode now: after the first sequence header, closed, reconstructed by decode(),
@@ -988,7 +990,7 @@ std::vector<IndexEntry> picture_index(const Batch *b, const Stream &s) {
 		const bool after = s.pics[k] >= s.seq_floor;
 		if (after && type == 1) keys.push_back(k);
 		refs += type == 1 || (type == 2 && picture_header_bits(s, k, 30, 3) != 0);
-		if (!after || !picture_decoded(b, s, k) || !picture_closed(s, k)) continue;
+		if (!after || !picture_decoded(s, k, b->decode_b) || !picture_closed(s, k)) continue;
 		const uint32_t need = type == 1 ? 0 : type - 1;
 		// (every key is a reference: this looks at most three keys back)
 		for (auto j = keys.rbegin(); j != keys.rend(); ++j)
@@ -1129,12 +1131,12 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 					const int slot = b->free_slots.back();
 					b->free_slots.pop_back();
 					ch.slot[p - ch.first] = slot;
-					wave.push_back({ch.stream, p, slot, walk_kind(b, s, p), end - s.pics[p]});
+					wave.push_back({ch.stream, p, slot, walk_kind(b, s, p, b->decode_b), end - s.pics[p]});
 					wave_chain.push_back((int)c);
 				}
 			}
 			if (wave.empty()) break;
-			parse_wave(b, wave);
+			parse_wave(b, wave, true);
 			for (size_t t = 0; t < wave.size(); t++) {
 				Chain &ch = chains[wave_chain[t]];
 				ch.info[wave[t].pic - ch.first] = b->h_info[t];
@@ -1246,6 +1248,104 @@ long batch_decode_chosen(Batch *b, bool intra, int n, const int *streams, const 
 	return n;
 }
 
+// ---- decode_macroblocks: the walks' records of chosen pictures of any streams, in the public layout (DESIGN 3.8) ----
+
+// The pictures decode_macroblocks can describe now: after the first sequence header, closed, and decoded by the walks
+// with B pictures going to the B walk whatever decode_b says.  No chain start: a picture's macroblock layer depends on
+// its own bits only.
+std::vector<uint32_t> macroblock_index(const Stream &s) {
+	std::vector<uint32_t> out;
+	if (!s.has_seq) return out;
+	for (uint32_t k = 0; k < s.pics.size(); k++)
+		if (s.pics[k] >= s.seq_floor && picture_decoded(s, k, true) && picture_closed(s, k)) out.push_back(k);
+	return out;
+}
+
+// Each unique (stream, picture) of the requests takes a record slot; waves of as many as there are free slots (after
+// flushing the look-ahead when they do not cover the call) run the walks alone, and one export launch per wave, on the
+// main stream behind the walks and before the slots are released, writes every request of the wave to its
+// destination.  The next wave's walks are queued behind it.  The requests are valid (the caller checked them).
+void decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *dst,
+                        int32_t *n_present_out, int32_t *error_out) {
+	ensure_pool(b);
+	std::vector<std::pair<int, uint32_t>> uniq(n);
+	for (int i = 0; i < n; i++) uniq[i] = {streams[i], pictures[i]};
+	std::sort(uniq.begin(), uniq.end());
+	uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
+	std::vector<size_t> uniq_of(n);  // request i describes picture uniq[uniq_of[i]]
+	for (int i = 0; i < n; i++)
+		uniq_of[i] = std::lower_bound(uniq.begin(), uniq.end(), std::make_pair(streams[i], pictures[i])) - uniq.begin();
+	if (b->free_slots.size() < uniq.size())  // decode() parses the look-ahead again
+		for (auto &s : b->streams) flush_cache(b, s);
+	if (n > b->xtask_cap) {
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		if (b->h_xtasks) { CUDA_CHECK(cudaFreeHost(b->h_xtasks)); b->h_xtasks = nullptr; }
+		if (b->d_xtasks) { CUDA_CHECK(cudaFree(b->d_xtasks)); b->d_xtasks = nullptr; }
+		b->xtask_cap = 0;
+		b->h_xtasks = pinned_alloc<MbExportTask>(n);
+		b->d_xtasks = dev_alloc<MbExportTask>(n);
+		b->xtask_cap = n;
+	}
+	const size_t wave_max = b->free_slots.size();
+	std::vector<int32_t> n_present(n, 0), error(n, 0);
+	for (size_t lo = 0; lo < uniq.size(); lo += wave_max) {
+		const size_t hi = std::min(uniq.size(), lo + wave_max);
+		std::vector<WaveItem> wave;
+		for (size_t u = lo; u < hi; u++) {
+			const Stream &s = b->streams[uniq[u].first];
+			const uint32_t p = uniq[u].second;
+			const uint32_t end = p + 1 < s.pics.size() ? s.pics[p + 1] : s.bb.length;
+			const int slot = b->free_slots.back();
+			b->free_slots.pop_back();
+			wave.push_back({uniq[u].first, p, slot, walk_kind(b, s, p, true), end - s.pics[p]});
+		}
+		// (parse_wave waits for the infos, which also means the previous wave's task upload has read h_xtasks)
+		parse_wave(b, wave, false);
+		int m = 0;
+		uint32_t total = 0;
+		for (int i = 0; i < n; i++) {
+			if (uniq_of[i] < lo || uniq_of[i] >= hi) continue;
+			const WaveItem &w = wave[uniq_of[i] - lo];
+			const picture_info_t &info = b->h_info[uniq_of[i] - lo];
+			n_present[i] = info.n_present;
+			error[i] = info.error;
+			const int mb_size = b->streams[w.stream].seq.mb_size;
+			b->h_xtasks[m++] = MbExportTask{b->d_hdr + (size_t)w.slot * b->slot_mb, dst[i], total, mb_size, info.picture_type, 0};
+			total += (uint32_t)mb_size;
+		}
+		CUDA_CHECK(cudaMemcpyAsync(b->d_xtasks, b->h_xtasks, m * sizeof(MbExportTask), cudaMemcpyHostToDevice, b->st_main));
+		launch_export_macroblocks(b->d_xtasks, m, total, b->st_main);
+		for (const WaveItem &w : wave) release_slot(b, w.slot);  // the next wave's walks queue behind the export
+	}
+	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+	for (int i = 0; i < n; i++) {
+		if (n_present_out) n_present_out[i] = n_present[i];
+		if (error_out) error_out[i] = error[i];
+	}
+}
+
+long batch_decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *mb_dst,
+                              int32_t *n_present_out, int32_t *error_out) {
+	use_device(b);
+	if (n < 0 || (n > 0 && (!streams || !pictures || !mb_dst))) return -2;
+	upload_all(b);
+	// ---- every request is checked before anything changes
+	std::vector<std::vector<uint32_t>> listed(b->streams.size());
+	std::vector<char> indexed(b->streams.size(), 0);
+	for (int i = 0; i < n; i++) {
+		const int si = streams[i];
+		if (!request_valid(b, si, mb_dst[i], nullptr, false)) return -2;
+		if (!indexed[si]) {
+			listed[si] = macroblock_index(b->streams[si]);
+			indexed[si] = 1;
+		}
+		if (!std::binary_search(listed[si].begin(), listed[si].end(), pictures[i])) return -2;
+	}
+	if (n == 0) return 0;
+	decode_macroblocks(b, n, streams, pictures, mb_dst, n_present_out, error_out);
+	return n;
+}
+
 int env_int(const char *name, int fallback) {
 	const char *e = getenv(name);
 	return e && *e ? atoi(e) : fallback;
@@ -1352,6 +1452,8 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b) {
 	if (b->d_ptasks) cudaFree(b->d_ptasks);
 	if (b->d_intra_fwd) cudaFree(b->d_intra_fwd);
 	if (b->d_chain_sets) cudaFree(b->d_chain_sets);
+	if (b->h_xtasks) cudaFreeHost(b->h_xtasks);
+	if (b->d_xtasks) cudaFree(b->d_xtasks);
 	ts_scratch_destroy(b->ts);
 	ps_scratch_destroy(b->ps);
 	for (auto e : {b->ev_a, b->ev_b, b->ev_mid, b->ev_recon[0], b->ev_recon[1], b->ev_step, b->ev_round, b->ev_copied[0],
@@ -1513,6 +1615,30 @@ long jsmpeg_b200_batch_decode_pictures(jsmpeg_b200_batch_t *b, int n, const int 
 	return guarded<long>(b, -1, [&] {
 		return batch_decode_chosen(b, false, n, streams, pictures, planes_dst, rgba_dst, flags, status_out, n_present_out, error_out);
 	});
+}
+
+long jsmpeg_b200_batch_macroblock_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out, uint32_t *byte_pos_out,
+                                        int32_t *type_out, int32_t *temporal_reference_out, long n_max) {
+	return guarded<long>(b, -1, [&]() -> long {
+		if (stream < 0 || stream >= (int)b->streams.size()) return -2;
+		use_device(b);
+		upload_all(b);
+		const Stream &s = b->streams[stream];
+		const std::vector<uint32_t> listed = macroblock_index(s);
+		for (long i = 0; i < std::min<long>((long)listed.size(), n_max); i++) {
+			const uint32_t k = listed[i];
+			if (picture_out) picture_out[i] = k;
+			if (byte_pos_out) byte_pos_out[i] = s.pics[k];
+			if (type_out) type_out[i] = picture_type_of(s, k);
+			if (temporal_reference_out) temporal_reference_out[i] = (int32_t)picture_header_bits(s, k, 0, 10);
+		}
+		return (long)listed.size();
+	});
+}
+
+long jsmpeg_b200_batch_decode_macroblocks(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                          void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
+	return guarded<long>(b, -1, [&] { return batch_decode_macroblocks(b, n, streams, pictures, mb_dst, n_present_out, error_out); });
 }
 
 int jsmpeg_b200_batch_get_planes(jsmpeg_b200_batch_t *b, int stream, void **y, void **cr, void **cb) {
@@ -1783,7 +1909,7 @@ int jsmpeg_b200_debug_parse_picture(const uint8_t *es, uint32_t es_len, uint32_t
 		t.stage = d_stage; t.stage_entries = stage_entries_for(sp.mb_size);
 		t.codes = nullptr; t.n_codes = 0; t.code_hint = 0;  // this hook lets the walk search the slice end itself
 		CUDA_CHECK(cudaMemcpy(d_task, &t, sizeof(t), cudaMemcpyHostToDevice));
-		launch_parse_pictures(d_task, 1, sp.mb_size, 0);
+		launch_parse_pictures(d_task, 1, sp.mb_size, true, 0);
 		CUDA_CHECK(cudaGetLastError());
 		CUDA_CHECK(cudaDeviceSynchronize());
 		CUDA_CHECK(cudaMemcpy(info_out, d_info, sizeof(picture_info_t), cudaMemcpyDeviceToHost));

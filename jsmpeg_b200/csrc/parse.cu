@@ -159,6 +159,12 @@ expand_blocks_kernel(const ParseTask *__restrict__ tasks) {
 	}
 }
 
+// Stage 1b of n_tasks pictures of up to max_mb_size macroblocks on `stream`
+void launch_expand(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream) {
+	dim3 grid((max_mb_size * 6 + CTA_THREADS * EXPAND_GROUPS - 1) / (CTA_THREADS * EXPAND_GROUPS), n_tasks);
+	expand_blocks_kernel<<<grid, CTA_THREADS, EXPAND_SMEM, stream>>>(tasks);
+}
+
 }  // namespace
 
 // The multi-symbol walk table (walk.cuh: build_ms_table), built once per device from the generated DCT table.
@@ -188,7 +194,7 @@ static const uint16_t *ms_table_for_current_device() {
 	return d;
 }
 
-int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream,
+int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream,
                           cudaEvent_t walk_done, const ParseFork *fork) {
 	if (n_tasks <= 0) return 0;
 	const uint16_t *ms = ms_table_for_current_device();
@@ -202,8 +208,9 @@ int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, 
 	// The wave arrives sorted by picture size, largest first.  A wave of at least 64 pictures per group is cut into
 	// PARSE_GROUPS equal groups: group 0 (largest pictures) stays on `stream`, the others go to side streams, each walk
 	// followed by its own expand, so that the expand of the smaller pictures runs while the walk of the bigger ones is
-	// still going.  On an H100 this takes 3 ms off stage 1 of a 3840-picture 1080p wave (DESIGN 8).
-	const int groups = (fork && n_tasks >= 64 * PARSE_GROUPS) ? PARSE_GROUPS : 1;
+	// still going.  On an H100 this takes 3 ms off stage 1 of a 3840-picture 1080p wave (DESIGN 8).  A walk-only wave
+	// has no expand to overlap: one group.
+	const int groups = (expand && fork && n_tasks >= 64 * PARSE_GROUPS) ? PARSE_GROUPS : 1;
 	if (groups > 1) CUDA_CHECK(cudaEventRecord(fork->fork, stream));
 	for (int g = 0; g < groups; g++) {
 		const int lo = (int)((long)n_tasks * g / groups), hi = (int)((long)n_tasks * (g + 1) / groups);
@@ -217,34 +224,33 @@ int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, 
 			walk_pictures_kernel<<<(n + per_cta - 1) / per_cta, WALK_THREADS, walk_smem, st>>>(
 			    tasks + lo, n, reinterpret_cast<const uint4 *>(ms));
 		if (g == 0 && walk_done) CUDA_CHECK(cudaEventRecord(walk_done, st));
-		dim3 grid((max_mb_size * 6 + CTA_THREADS * EXPAND_GROUPS - 1) / (CTA_THREADS * EXPAND_GROUPS), n);
-		expand_blocks_kernel<<<grid, CTA_THREADS, EXPAND_SMEM, st>>>(tasks + lo);
+		if (expand) launch_expand(tasks + lo, n, max_mb_size, st);
 		if (g > 0) {
 			CUDA_CHECK(cudaEventRecord(fork->join[g], st));
 			CUDA_CHECK(cudaStreamWaitEvent(stream, fork->join[g], 0));
 		}
 	}
-	return 2 * groups;
+	return (expand ? 2 : 1) * groups;
 }
 
-// B pictures: one walk + one expand launch on `stream` (no size groups: B pictures are the small ones of a stream)
-void launch_parse_pictures_b(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream) {
-	if (n_tasks <= 0) return;
+// B pictures: one walk (+ one expand) launch on `stream` (no size groups: B pictures are the small ones of a stream)
+int launch_parse_pictures_b(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream) {
+	if (n_tasks <= 0) return 0;
 	const uint16_t *ms = ms_table_for_current_device();
 	const int per_cta = WALK_THREADS / 32;
 	walk_pictures_b_kernel<<<(n_tasks + per_cta - 1) / per_cta, WALK_THREADS, WALK_SMEM_SERIAL, stream>>>(
 	    tasks, n_tasks, reinterpret_cast<const uint4 *>(ms));
-	dim3 grid((max_mb_size * 6 + CTA_THREADS * EXPAND_GROUPS - 1) / (CTA_THREADS * EXPAND_GROUPS), n_tasks);
-	expand_blocks_kernel<<<grid, CTA_THREADS, EXPAND_SMEM, stream>>>(tasks);
+	if (expand) launch_expand(tasks, n_tasks, max_mb_size, stream);
+	return expand ? 2 : 1;
 }
 
-// Pictures of many slices (opt-in): one walk (a lane per slice) + one expand launch on `stream`
-void launch_parse_pictures_slices(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStream_t stream) {
-	if (n_tasks <= 0) return;
+// Pictures of many slices (opt-in): one walk (a lane per slice) (+ one expand) launch on `stream`
+int launch_parse_pictures_slices(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream) {
+	if (n_tasks <= 0) return 0;
 	const uint16_t *ms = ms_table_for_current_device();
 	const int per_cta = WALK_THREADS / 32;
 	walk_pictures_slices_kernel<<<(n_tasks + per_cta - 1) / per_cta, WALK_THREADS, WALK_SMEM_LANES, stream>>>(
 	    tasks, n_tasks, reinterpret_cast<const uint4 *>(ms));
-	dim3 grid((max_mb_size * 6 + CTA_THREADS * EXPAND_GROUPS - 1) / (CTA_THREADS * EXPAND_GROUPS), n_tasks);
-	expand_blocks_kernel<<<grid, CTA_THREADS, EXPAND_SMEM, stream>>>(tasks);
+	if (expand) launch_expand(tasks, n_tasks, max_mb_size, stream);
+	return expand ? 2 : 1;
 }

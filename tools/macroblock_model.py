@@ -1,0 +1,77 @@
+"""Serial model of the macroblock index (jsmpeg_b200_batch_macroblock_index) and of what decode_macroblocks must give.
+
+Picture k of a stream is the k-th picture start code (00 00 01 00) in its buffer.  The index lists picture k when
+  1. it starts at or after the end of the stream's first sequence header,
+  2. it is closed (tools/intra_model.py), and
+  3. the walks decode it with B pictures on: picture_coding_type 1; 2 with forward_f_code != 0; 3 with both f_codes
+     != 0 (tools/chain_model.py: is_decoded) -- whatever the decode_b option says, and with no chain start.
+A listed picture's entries are export() of the records a fresh decoder with B pictures on gives for fresh_bytes(): the
+first sequence header, the picture's bytes up to its closing code, and the closing code itself.
+"""
+from __future__ import annotations
+
+import numpy as np
+
+import chain_model
+import intra_model
+
+# jsmpeg_b200_macroblock_t flags (include/jsmpeg_b200.h) and mb_record_t flags (jsmpeg_b200/csrc/records.h)
+MB_PRESENT, MB_INTRA, MB_SKIPPED, MB_BACKWARD, MB_FORWARD = 0x01, 0x02, 0x04, 0x08, 0x10
+MBF_PRESENT, MBF_INTRA, MBF_SKIPPED, MBF_MOTION_BWD, MBF_MOTION_FWD = 0x01, 0x02, 0x04, 0x08, 0x10
+
+RECORD = np.dtype([("mv_h", "<i2"), ("mv_v", "<i2"), ("flags", "u1"), ("cbp", "u1"), ("dc_only", "u1"), ("qscale", "u1"),
+                   ("bit_pos", "<u4"), ("bwd_x", "<i2"), ("bwd_y", "<i2")])  # mb_record_t, mv_bwd split into its halves
+ENTRY = np.dtype([("fwd_x", "<i2"), ("fwd_y", "<i2"), ("bwd_x", "<i2"), ("bwd_y", "<i2"), ("flags", "u1"), ("cbp", "u1"),
+                  ("qscale", "u1"), ("reserved", "u1", 5)])  # jsmpeg_b200_macroblock_t
+assert RECORD.itemsize == ENTRY.itemsize == 16
+
+
+def macroblock_index(es):
+    """[{"picture", "byte_pos", "type", "temporal_reference", "close"}] of the pictures the index lists for `es`."""
+    seq = intra_model.first_sequence_header(es)
+    if seq is None:
+        return []
+    floor = (seq[1] + 7) >> 3
+    codes = [p for p in intra_model.prefixes(es) if p + 3 < len(es)]
+    out, k = [], -1
+    for j, p in enumerate(codes):
+        if es[p + 3] != 0:
+            continue
+        k += 1
+        if p < floor or not chain_model.is_decoded(es, p, True):
+            continue
+        close = next((q for q in codes[j + 1:] if intra_model._closes(es[q + 3])), None)
+        if close is not None:
+            out.append({"picture": k, "byte_pos": p, "type": chain_model.picture_type(es, p),
+                        "temporal_reference": chain_model.header_bits(es, p, 0, 10), "close": close})
+    return out
+
+
+def fresh_bytes(es, entry):
+    """What a fresh decoder is fed for a listed picture: first sequence header + the picture + its closing code."""
+    return intra_model.fresh_bytes(es, entry)
+
+
+def export(records, picture_type):
+    """The public entries (uint8 [n, 16]) of n mb_record_t (any 16-byte-per-record buffer) of a picture of
+    picture_coding_type `picture_type` -- the rule of jsmpeg_b200/csrc/macroblocks.cuh."""
+    r = np.frombuffer(np.ascontiguousarray(records).tobytes(), RECORD)
+    present = (r["flags"] & MBF_PRESENT) != 0
+    intra = (r["flags"] & MBF_INTRA) != 0
+    if picture_type == 3:
+        fwd = present & ~intra & ((r["flags"] & MBF_MOTION_FWD) != 0)
+        bwd = present & ~intra & ((r["flags"] & MBF_MOTION_BWD) != 0)
+    else:
+        fwd = present & ~intra
+        bwd = np.zeros_like(present)
+    e = np.zeros(len(r), ENTRY)
+    e["flags"] = np.where(present, MB_PRESENT, 0) | np.where(present & intra, MB_INTRA, 0) | \
+        np.where(present & ((r["flags"] & MBF_SKIPPED) != 0), MB_SKIPPED, 0) | \
+        np.where(fwd, MB_FORWARD, 0) | np.where(bwd, MB_BACKWARD, 0)
+    e["fwd_x"] = np.where(fwd, r["mv_h"], 0)
+    e["fwd_y"] = np.where(fwd, r["mv_v"], 0)
+    e["bwd_x"] = np.where(bwd, r["bwd_x"], 0)
+    e["bwd_y"] = np.where(bwd, r["bwd_y"], 0)
+    e["cbp"] = np.where(present, r["cbp"], 0)
+    e["qscale"] = np.where(present, r["qscale"], 0)
+    return e.view(np.uint8).reshape(len(r), 16)
