@@ -8,6 +8,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "coef_records.h"
 #include "records.h"
 
 // A failed CUDA call never takes the host process down (the reference "never fails": a decoder that
@@ -64,7 +65,8 @@ struct ParseTask {
 	int32_t mb_width, mb_size;  // copies of the sequence parameters (no dependent load in front of the walk)
 	// lane-parallel walk: staging area for relative macroblock records (walk.cuh, WALK_STAGE): stage_entries
 	// entries of 64 bytes, shared out among the lanes; nullptr = no staging (the walk then makes a second,
-	// storing pass over the bits)
+	// storing pass over the bits).  Once the picture's walk has finished the area is dead, and stage 1b reuses it
+	// as the picture's compact coefficient plane (compact_plane); nullptr = stage 1b writes dense records only.
 	uint4 *stage;
 	int32_t stage_entries;
 	// the stream's start-code prefixes (byte positions of 00 00 01, sorted, all of them up to es_len) and the
@@ -79,6 +81,14 @@ struct ParseTask {
 // second pass) + one per lane for rounding
 constexpr int stage_entries_for(int mb_size) { return 3 * mb_size + 64; }
 
+// The compact coefficient plane of a picture (coef_records.h): one 32-byte record per block slot mb * 6 + b, in the
+// picture's staging area.  6 * 32 * mb_size bytes fit the stage_entries_for(mb_size) * 64 = 192 * mb_size + 4096
+// bytes of the area; the walk is done with it before stage 1b of the same picture runs (same stream), and a slot is
+// walked again only after the reconstruction of its last picture (ev_round, engine.cu), the rule that already
+// guards the dense coefficient plane.
+static_assert(6 * sizeof(coef_record_t) <= 3 * 64, "the compact plane fits the staging area");
+__host__ __device__ inline coef_record_t *compact_plane(uint4 *stage) { return reinterpret_cast<coef_record_t *>(stage); }
+
 struct PlaneSet {
 	uint8_t *y, *cr, *cb;
 };
@@ -86,7 +96,8 @@ struct PlaneSet {
 // Stage 2: one task per (stream, picture); blockIdx.y selects the task.
 struct ReconTask {
 	const mb_record_t *hdr;
-	const int16_t *coef;
+	const int16_t *coef;            // dense records: the blocks the compact plane marks COEF_RECORD_DENSE
+	const coef_record_t *compact;   // compact records (coef_records.h), or nullptr: every coded block is dense
 	PlaneSet cur;   // written
 	PlaneSet fwd;   // read (previous I/P picture; B picture: the older of the two most recent I/P pictures)
 	int32_t mb_width, mb_size;

@@ -722,6 +722,7 @@ ReconTask recon_task(const Batch *b, const Stream &s, int slot, uint8_t *cur, ui
 	ReconTask t{};
 	t.hdr = b->d_hdr + (size_t)slot * b->slot_mb;
 	t.coef = b->d_coef + (size_t)slot * b->slot_mb * MB_COEF_INT16;
+	t.compact = compact_plane(b->d_stage + (size_t)slot * stage_entries_for(b->slot_mb) * 4);  // (stage 1b wrote it: parse_task)
 	t.cur = plane_set(s, cur);
 	t.fwd = plane_set(s, fwd);
 	if (bwd) t.bwd = plane_set(s, bwd);
@@ -861,7 +862,7 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 				b->stats.coded_blocks += e.info.n_coded_blocks;
 				b->stats.macroblocks += e.info.n_present;
 				b->stats.algorithmic_bytes += planes + (e.info.picture_type == 2 ? planes : (is_b ? 2 * planes : 0)) +
-				                              (uint64_t)s.seq.mb_size * sizeof(mb_record_t) + (uint64_t)e.info.n_coded_blocks * 128;
+				                              (uint64_t)s.seq.mb_size * sizeof(mb_record_t) + (uint64_t)e.info.n_coded_blocks * sizeof(coef_record_t);
 			}
 			release_slot(b, e.slot);  // reused by the NEXT round's parse, which waits for this round's reconstruction (ev_round)
 		}
@@ -1915,6 +1916,15 @@ int jsmpeg_b200_debug_parse_picture(const uint8_t *es, uint32_t es_len, uint32_t
 		CUDA_CHECK(cudaMemcpy(info_out, d_info, sizeof(picture_info_t), cudaMemcpyDeviceToHost));
 		CUDA_CHECK(cudaMemcpy(hdr_out, d_hdr, n_mb * sizeof(mb_record_t), cudaMemcpyDeviceToHost));
 		CUDA_CHECK(cudaMemcpy(coef_out, d_coef, n_mb * MB_COEF_INT16 * sizeof(int16_t), cudaMemcpyDeviceToHost));
+		// stage 1b left most blocks as compact records in the staging area: the caller gets them dense
+		std::vector<coef_record_t> compact(n_mb * 6);
+		CUDA_CHECK(cudaMemcpy(compact.data(), d_stage, compact.size() * sizeof(coef_record_t), cudaMemcpyDeviceToHost));
+		const mb_record_t *hdr = static_cast<const mb_record_t *>(hdr_out);
+		for (size_t slot = 0; slot < n_mb * 6; slot++) {
+			const mb_record_t &r = hdr[slot / 6];
+			if ((r.flags & MBF_PRESENT) && (r.cbp & (0x20 >> (slot % 6))) && compact[slot].mask != COEF_RECORD_DENSE)
+				coef_record_unpack(compact[slot], static_cast<int16_t *>(coef_out) + slot * 64);
+		}
 		cudaFree(d_es); cudaFree(d_seq); cudaFree(d_hdr); cudaFree(d_coef); cudaFree(d_park); cudaFree(d_stage); cudaFree(d_info); cudaFree(d_task);
 		return 0;
 	} catch (const std::exception &e) {
@@ -1931,6 +1941,16 @@ int jsmpeg_b200_debug_reconstruct(int mb_width, int mb_height, const void *hdr, 
 		const size_t ysz = n_mb * 256, csz = ysz / 4, total = ysz + 2 * csz;
 		mb_record_t *d_hdr = dev_alloc<mb_record_t>(n_mb);
 		int16_t *d_coef = dev_alloc<int16_t>(n_mb * MB_COEF_INT16);
+		// the caller's dense blocks as stage 1b would hand them over: compact records where they fit
+		std::vector<coef_record_t> compact(n_mb * 6);
+		for (size_t slot = 0; slot < n_mb * 6; slot++) {
+			const int16_t *blk = static_cast<const int16_t *>(coef) + slot * 64;
+			const uint64_t pos = coef_nonzero_positions(blk);
+			if (coef_record_fits(pos)) compact[slot] = coef_record_pack(pos, blk);
+			else compact[slot].mask = COEF_RECORD_DENSE;
+		}
+		coef_record_t *d_compact = dev_alloc<coef_record_t>(n_mb * 6);
+		CUDA_CHECK(cudaMemcpy(d_compact, compact.data(), compact.size() * sizeof(coef_record_t), cudaMemcpyHostToDevice));
 		const size_t pad = (size_t)mb_width * 16 + 64;
 		uint8_t *d_fwd = dev_alloc<uint8_t>(total + pad), *d_cur = dev_alloc<uint8_t>(total + pad);
 		CUDA_CHECK(cudaMemset(d_fwd + total, 0, pad));
@@ -1943,7 +1963,7 @@ int jsmpeg_b200_debug_reconstruct(int mb_width, int mb_height, const void *hdr, 
 		CUDA_CHECK(cudaMemcpy(d_cur + ysz, cur_cr, csz, cudaMemcpyHostToDevice));
 		CUDA_CHECK(cudaMemcpy(d_cur + ysz + csz, cur_cb, csz, cudaMemcpyHostToDevice));
 		ReconTask t{};
-		t.hdr = d_hdr; t.coef = d_coef;
+		t.hdr = d_hdr; t.coef = d_coef; t.compact = d_compact;
 		t.cur = PlaneSet{d_cur, d_cur + ysz, d_cur + ysz + csz};
 		t.fwd = PlaneSet{d_fwd, d_fwd + ysz, d_fwd + ysz + csz};
 		t.mb_width = mb_width; t.mb_size = (int)n_mb;
@@ -1954,7 +1974,7 @@ int jsmpeg_b200_debug_reconstruct(int mb_width, int mb_height, const void *hdr, 
 		CUDA_CHECK(cudaMemcpy(cur_y, d_cur, ysz, cudaMemcpyDeviceToHost));
 		CUDA_CHECK(cudaMemcpy(cur_cr, d_cur + ysz, csz, cudaMemcpyDeviceToHost));
 		CUDA_CHECK(cudaMemcpy(cur_cb, d_cur + ysz + csz, csz, cudaMemcpyDeviceToHost));
-		cudaFree(d_hdr); cudaFree(d_coef); cudaFree(d_fwd); cudaFree(d_cur);
+		cudaFree(d_hdr); cudaFree(d_coef); cudaFree(d_compact); cudaFree(d_fwd); cudaFree(d_cur);
 		return 0;
 	} catch (const std::exception &e) {
 		fprintf(stderr, "%s\n", e.what());

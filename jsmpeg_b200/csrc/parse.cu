@@ -21,8 +21,9 @@
 //       chain) is its in-kernel fall-back and, with JSMPEG_B200_WALK=serial, a kernel of its own.
 //   1b  expand_blocks_kernel    one thread per coded BLOCK, all blocks of all pictures at once:
 //       re-reads the block's codes from its bit offset, does run/level -> zig-zag -> dequantise ->
-//       oddify -> clip (src/mpeg1.js:757-811) into a shared-memory tile; the 64 x int16 block record
-//       leaves as one 128-byte TMA bulk store.
+//       oddify -> clip (src/mpeg1.js:757-811) into a shared-memory tile; the block leaves as its 32-byte
+//       compact record (coef_records.h) or, with more than 12 values, as the 64 x int16 dense record,
+//       each as one TMA bulk store.
 //
 // VLCs are decoded with clz-indexed look-up tables in shared memory (tools/gen_tables.py; pinned
 // to the reference's trees by tests/test_vlc_tables.py) instead of the reference's one-bit-per-step
@@ -155,7 +156,7 @@ expand_blocks_kernel(const ParseTask *__restrict__ tasks) {
 #pragma unroll
 		for (int i = 0; i < 8; i++) tile[i] = make_uint4(0u, 0u, 0u, 0u);  // (the last bulk store has read the tile: expand_block waits)
 		expand_block(t, rec_now, parked_now, reinterpret_cast<uint4 *>(t.coef) + (size_t)slot_now * 8, sbase,
-		             sbase + EXP_OFF_TILES + threadIdx.x * TILE_PITCH);
+		             sbase + EXP_OFF_TILES + threadIdx.x * TILE_PITCH, t.stage ? compact_plane(t.stage) + slot_now : nullptr);
 	}
 }
 

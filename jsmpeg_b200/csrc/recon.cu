@@ -6,11 +6,14 @@
 // 16x16 / 8x8 / 8x8 pixels, so all blocks of a picture (and of all streams) are independent.
 //
 // Mapping: ONE THREAD PER 8x8 BLOCK, the whole block in registers.
-//   * the block's 128-byte coefficient record is fetched by ONE instruction per lane: a TMA 1-D
-//     bulk copy (cp.async.bulk global -> shared, SASS UBLKCP) into a 144-byte-pitched row of
-//     the warp's staging area, completion counted on a per-warp mbarrier; the lane then reads
-//     its row back with eight conflict-free LDS.128.  (Eight per-lane LDG.128 at a 128-byte
-//     stride cost 32 L1 wavefronts per instruction and made the kernel L1TEX-bound.)
+//   * the block's 32-byte compact coefficient record (coef_records.h: position mask + at most 12
+//     values) is loaded with two LDG.128; the lane zeroes its 144-byte-pitched row of the warp's
+//     staging area and scatters the values into it.  A block with more values has a dense
+//     128-byte record: it is fetched by ONE instruction per lane, a TMA 1-D bulk copy
+//     (cp.async.bulk global -> shared, SASS UBLKCP) into the row, completion counted on a
+//     per-warp mbarrier.  Either way the lane then reads its row back with eight conflict-free
+//     LDS.128.  (Eight per-lane LDG.128 at a 128-byte stride cost 32 L1 wavefronts per
+//     instruction and made the kernel L1TEX-bound.)
 //     The coefficients are multiplied by PREMULTIPLIER (src/mpeg1.js:810, 1026-1035) -- compile-time immediates,
 //     the loops are fully unrolled -- and go through the 8 column passes (mpeg1.js:925-947) and
 //     the 8 row passes with (v+128)>>8 (mpeg1.js:952-981) without leaving the register file:
@@ -31,8 +34,9 @@
 // A vector whose footprint leaves the plane (non-conforming, SURVEY Q11) takes a per-tap
 // bounds-checked path.
 //
-// HBM roofline accounting (DESIGN.md): per macroblock 16 B header + 128 B per coded block +
-// 384 B written + 384 B of forward-plane samples (P pictures), each counted once.
+// HBM roofline accounting (DESIGN.md): per macroblock 16 B header + 32 B per coded block (its
+// compact record; the about 0.5 % of blocks with a dense record are not counted) + 384 B written +
+// 384 B of forward-plane samples (P pictures), each counted once.
 #include "recon.cuh"
 
 namespace {
@@ -86,6 +90,7 @@ reconstruct_rgba_b_kernel(const __grid_constant__ ReconRgbaParamsB params) {
 void fill_task(CompactTask &c, const ReconTask &t) {
 	c.hdr = t.hdr;
 	c.coef = t.coef;
+	c.compact = t.compact;
 	c.cur = t.cur.y;   // planes are contiguous: Y | Cr | Cb (engine.cu plane_set)
 	c.fwd = t.fwd.y;
 	c.mb_width = t.mb_width;

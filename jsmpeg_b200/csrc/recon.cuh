@@ -12,20 +12,25 @@ namespace {
 
 constexpr int THREADS = 128;
 constexpr int ROW_PITCH = 144;                       // bytes per staged block: 128 + 16 (bank spread)
-constexpr int WARP_STAGE = 32 * ROW_PITCH + 16;      // + the warp's mbarrier
+constexpr int WARP_ZZ = 32 * ROW_PITCH + 16;         // the warp's zig-zag -> raster table (64 bytes, compact records)
+constexpr int WARP_STAGE = WARP_ZZ + 64;             // + the warp's mbarrier (at 32 * ROW_PITCH) and the table
 constexpr int MAX_TASKS = 80;       // per launch; (80 * 48 B) + 16 < 4 KB of kernel parameters
 constexpr int MAX_TASKS_RGBA = 60;  // the RGBA variant's parameters: (60 * (48 + 16) B) + 16 < 4 KB
 
 
 struct CompactTask {
 	const mb_record_t *hdr;
-	const int16_t *coef;
+	const int16_t *coef;             // dense coefficient records
+	const coef_record_t *compact;    // compact coefficient records (coef_records.h), or nullptr: every coded block is dense
 	uint8_t *cur;        // Y at 0, Cr at coded_size, Cb at coded_size * 5 / 4; readable for coded_width + 64 bytes past the end
 	const uint8_t *fwd;
-	int32_t mb_width, mb_height;
+	// (bit fields: the task stays 48 bytes, so that a launch still carries 80 of them in 4 KB of parameters; MPEG-1
+	// pictures are at most 4095 x 4095 samples, 256 x 256 macroblocks)
+	int32_t mb_width : 12, mb_height : 12;
+	uint32_t flags : 8;  // (none defined)
 	uint32_t row_magic;  // floor(2^32 / (6 mb_width)) + 1: slot / (6 mb_width) == umulhi(slot, row_magic) for every slot of a picture
-	uint32_t flags;      // (none defined)
 };
+static_assert(sizeof(CompactTask) == 48, "kernel parameter budget");
 
 template <int N>
 struct ReconParamsT {
@@ -297,11 +302,13 @@ static inline uint32_t smem_u32(const void *) { return 0; }
 // Latency plan (the kernel was stalled on memory it asked for too late):
 //   t0  the header load starts;  the header and the coefficient record of the CTA that will run here two
 //       pictures of the launch later are pulled into L2
-//   t0' header there: the records of the coded blocks are requested (TMA).  (Requesting every slot's record
-//       before the header is known, for pictures with most blocks coded, gained nothing for more DRAM
-//       traffic; removed.)
+//   t0' header there: the 32-byte compact records of the coded blocks are loaded (coef_records.h).  (Requesting
+//       every slot's record before the header is known, for pictures with most blocks coded, gained nothing for
+//       more DRAM traffic; removed.)
 //   t1  header there: the nine reference rows of a predicted block are pulled into L2 (no registers)
-//   t2  records there: IDCT (some 700 instructions) -- the reference rows arrive meanwhile
+//   t1' compact records there: the lanes whose record is marked dense request their 128-byte dense record (TMA);
+//       the others build their staging row from the record: zeros + at most 12 values
+//   t2  rows staged: IDCT (some 700 instructions) -- the reference rows arrive meanwhile
 //   t3  prediction reads hit L2, + residual, store
 // block (mb_row, mb_col, b) of picture `ty`; the 32 lanes of the warp call it together, wstage = the warp's staging
 // area.  KEEP: the block's eight packed output rows come back in `rows` (also for a macroblock that is not present:
@@ -318,6 +325,12 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 	const uint32_t mbar = smem_u32(wstage + 32 * ROW_PITCH);
 	const uint32_t my_row = smem_u32(wstage + lane * ROW_PITCH);
 	const int16_t *cblk = t.coef + ((size_t)mb * 6 + b) * 64;
+	const bool compact = t.compact != nullptr;  // warp-uniform: the warp's blocks belong to one task
+	if (compact) {  // the zig-zag -> raster table of the warp's scatters
+		wstage[WARP_ZZ + lane] = (uint8_t)coef_zigzag_raster(lane);
+		wstage[WARP_ZZ + 32 + lane] = (uint8_t)coef_zigzag_raster(32 + lane);
+		__syncwarp();
+	}
 
 	// ---- coefficient records of the warp's blocks: one TMA bulk copy per lane
 	// `want` = this lane's record is copied; warp-uniform `copy_mask` = which lanes' are
@@ -355,7 +368,8 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		const auto &t2 = params.t[ty + 2];
 		if (in_picture && mb < t2.mb_width * t2.mb_height) {
 			prefetch_l2(t2.hdr + mb);
-			prefetch_l2(t2.coef + ((size_t)mb * 6 + b) * 64);
+			if (t2.compact) prefetch_l2(t2.compact + ((size_t)mb * 6 + b));
+			else prefetch_l2(t2.coef + ((size_t)mb * 6 + b) * 64);
 		}
 	}
 	const int flags = rec.y & 0xff;
@@ -366,10 +380,12 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 	const bool dc_only = coded && ((rec.y >> 16) & bit);
 	const bool full = coded && !dc_only;
 	const bool warp_full = __any_sync(0xffffffffu, full);  // warp-uniform: some lane needs the transform
-
-	const unsigned coded_mask = __ballot_sync(0xffffffffu, coded);
-	if (coded_mask) request_records(coded, coded_mask);  // only what is coded (the DC-only blocks' value too)
-	const bool copying = coded_mask != 0;                 // warp-uniform
+	// the compact record of a coded block: c0 = {mask lo, mask hi, levels 0-1, levels 2-3}, c1 = levels 4-11
+	uint4 c0 = make_uint4(0u, 0u, 0u, 0u), c1 = c0;
+	if (compact && coded) {
+		c0 = __ldg(reinterpret_cast<const uint4 *>(t.compact + ((size_t)mb * 6 + b)));
+		c1 = __ldg(reinterpret_cast<const uint4 *>(t.compact + ((size_t)mb * 6 + b)) + 1);
+	}
 
 	const int stride_y = W * 16;
 	const int ysize = stride_y * t.mb_height * 16;
@@ -419,6 +435,13 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		for (int r = 0; r < 9; r++) prefetch_l2(splane + src + r * stride + 4);
 	}
 
+	// only the blocks without a compact record come as a dense record (the DC-only blocks' value too)
+	const bool dense = coded && (!compact || (c0.x & c0.y) == 0xffffffffu);
+	static_assert(COEF_RECORD_DENSE == ~(uint64_t)0, "the dense marker is a mask of all ones");
+	const unsigned dense_mask = __ballot_sync(0xffffffffu, dense);
+	if (dense_mask) request_records(dense, dense_mask);
+	const bool copying = dense_mask != 0;  // warp-uniform
+
 	if (copying) {  // t2: wait for the warp's copies (phase 0 of a barrier used once)
 #ifndef JSMPEG_WALK_EMU
 		uint32_t done = 0;
@@ -445,15 +468,26 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 	// with at least one block that needs the transform, every lane runs it -- the DC-only lanes on their staged
 	// record (zeros behind coefficient 0, the expand kernel writes whole records), the uncoded lanes on a row
 	// they zero themselves -- instead of the warp running the transform AND the 64-register fill one after the other.
+	// A lane with a compact record zeroes its row too and scatters the record's values into it.
 	int v[64];
 	if (warp_full) {
-		if (!coded) {  // present, nothing coded: a residual of zeros
+		if (!dense) {  // uncoded (a residual of zeros) or a compact record
 #ifndef JSMPEG_WALK_EMU
 #pragma unroll
 			for (int i = 0; i < 8; i++) asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(my_row + i * 16), "r"(0u) : "memory");
 #else
 			memset(wstage + lane * ROW_PITCH, 0, 128);
 #endif
+			const uint32_t lv[COEF_RECORD_LEVELS / 2] = {c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+			uint64_t m = (uint64_t)c0.y << 32 | c0.x;  // 0 for an uncoded block
+#pragma unroll
+			for (int k = 0; k < COEF_RECORD_LEVELS; k++) {
+				if (m) {
+					const int raster = wstage[WARP_ZZ + coef_lowest64(m)];
+					m &= m - 1;
+					*reinterpret_cast<int16_t *>(wstage + lane * ROW_PITCH + raster * 2) = (int16_t)(lv[k >> 1] >> (16 * (k & 1)));
+				}
+			}
 		}
 #pragma unroll
 		for (int i = 0; i < 8; i++) {
@@ -474,14 +508,16 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		idct_rows<0>(v);
 	} else {
 		int dc = 0;
-		if (coded) {  // mpeg1.js:838-841, 850-853: the staged record's first value
-			int16_t c0;
+		if (dense) {  // mpeg1.js:838-841, 850-853: the staged record's first value
+			int16_t d0;
 #ifndef JSMPEG_WALK_EMU
-			asm volatile("ld.shared.s16 %0, [%1];" : "=h"(c0) : "r"(my_row));
+			asm volatile("ld.shared.s16 %0, [%1];" : "=h"(d0) : "r"(my_row));
 #else
-			memcpy(&c0, wstage + lane * ROW_PITCH, 2);
+			memcpy(&d0, wstage + lane * ROW_PITCH, 2);
 #endif
-			dc = ((int)c0 * PM[0] + 128) >> 8;
+			dc = ((int)d0 * PM[0] + 128) >> 8;
+		} else if (c0.x & 1u) {  // a compact record's first value is coefficient 0 when zig-zag position 0 is written
+			dc = ((int)(int16_t)(c0.z & 0xffffu) * PM[0] + 128) >> 8;
 		}
 #pragma unroll
 		for (int i = 0; i < 64; i++) v[i] = dc;
@@ -645,7 +681,9 @@ __device__ __forceinline__ void reconstruct_rgba_block(const PARAMS &params, con
 	if (warp < 2) { b = warp * 2 + (lane & 1); local = lane >> 1; }
 	else { b = 4 + (lane >> 4); local = lane & 15; }
 	const int mb_col = first_mb_col + local;
-	const bool in_picture = mb_col < t.mb_width;
+	// (the launch's grid covers its tallest picture: rows below a shorter one are outside it, and the slot's records
+	// there are stale ones of an earlier, bigger picture)
+	const bool in_picture = mb_col < t.mb_width && mb_row < t.mb_height;
 	uint2 rows[8];
 #pragma unroll
 	for (int r = 0; r < 8; r++) rows[r] = make_uint2(0u, 0u);

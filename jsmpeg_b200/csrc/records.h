@@ -11,7 +11,13 @@
  *     mb_record_t hdr [mb_size]                    16 B each, indexed by macroblock address
  *     int16_t     coef[mb_size][6][64]            128 B per block, de-zigzagged (raster) order,
  *                                                 only blocks whose cbp bit is set are written/read
+ *     uint2       park[mb_size][6]                the walk's hand-over to stage 1b (common.cuh: ParseTask)
+ *     staging area                                the lane-parallel walk's relative records; once the walk is done,
+ *                                                 the compact coefficient plane: 32 B per block (coef_records.h)
  * Fixed slots (no allocation, no offsets): any slice / picture can be parsed independently.
+ * Stage 1b hands a coded block over as its 32-byte compact record (a position mask + at most 12 values,
+ * coef_records.h); only a block with more values is written here, as the 128-byte dense record below, and
+ * its compact record says so.
  *
  * Coefficient values: the reference keeps `level * PREMULTIPLIER_MATRIX[i]` in int32
  * (src/mpeg1.js:810); that does not fit int16 (2047*62), so the record holds the dequantised,

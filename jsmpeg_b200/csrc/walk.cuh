@@ -1196,7 +1196,10 @@ __device__ void walk_picture(const ParseTask &t, uint32_t sbase, int lane, uint3
 // 1b: one coded block, from the offset the walk parked to the finished 64 x int16 record.
 // rec = the macroblock record's second word (flags | cbp << 8 | dc_only << 16 | quantiser scale << 24),
 // parked = {bit offset of the block's first coefficient code, intra dc * 8} from the walk's dense side
-// array, stile = the shared-memory address of this thread's (zeroed) 128-byte tile.
+// array, stile = the shared-memory address of this thread's (zeroed) 128-byte tile.  crec = the block's compact
+// record (coef_records.h), or nullptr: the block leaves as a dense record at `slot`.  With crec, a block of at most
+// COEF_RECORD_LEVELS positions leaves as its 32-byte compact record alone; a bigger one marks crec dense and leaves
+// as the dense record at `slot`.
 //
 // The kernel is bound by the integer ALU pipe, so the loop is built to need
 // few ALU instructions per code:
@@ -1223,7 +1226,7 @@ __device__ __forceinline__ int dequant_sm(int mag2_plus, int neg, int qs, uint32
 	return (neg && t != 0) ? -r : r;
 }
 __device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, uint2 parked, uint4 *__restrict__ slot,
-                                             uint32_t sbase, uint32_t stile) {
+                                             uint32_t sbase, uint32_t stile, coef_record_t *__restrict__ crec = nullptr) {
 	const bool intra = rec & MBF_INTRA;
 	const int ni = intra ? 0 : 1;
 	const int qs = (int)(rec >> 24);
@@ -1242,9 +1245,11 @@ __device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, u
 	uint32_t w = window(pos);
 
 	int n = 0;
+	uint64_t written = 0;  // zig-zag positions stored (the compact record's mask)
 	if (intra) {
 		sts_s16(stile, (int)(int16_t)(parked.y & 0xffffu));  // coefficient 0
 		n = 1;
+		written = 1;
 	} else if (w >> 31) {
 		// dct_coeff_first of a non-intra block: a leading '1' is (run 0, level +-1) with its sign bit, never
 		// end_of_block (mpeg1.js:757-760, 781-787) -- handled here, once, instead of in every trip of the loop
@@ -1253,6 +1258,7 @@ __device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, u
 		pos += 2u;
 		w = window(pos);
 		n = 1;
+		written = 1;
 	}
 	for (;;) {  // mpeg1.js:757-811; the walk has already validated every code of this block
 		uint32_t x = lds_u32(sbase + EXP_OFF_TOP8 + ((w >> 24) << 2));
@@ -1291,7 +1297,43 @@ __device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, u
 		}
 		const uint32_t q = lds_u16(xq + (uint32_t)(n - 1) * 2u);
 		sts_s16(stile + (q & 0xffu), dequant_sm(mag2 + ni, neg, qs, q));
+		written |= (uint64_t)1 << (n - 1);
 	}
+	if (crec && coef_record_fits(written)) {
+		// the compact record: the written values in zig-zag order, read back from the tile (its raster offsets come
+		// from the quantiser table's low byte), then written over the tile's first 32 bytes, which leave as one
+		// 32-byte bulk store -- whole sectors, like the dense record's
+		uint32_t lv[COEF_RECORD_LEVELS / 2] = {};
+		uint64_t m = written;
+#pragma unroll
+		for (int k = 0; k < COEF_RECORD_LEVELS; k++) {
+			if (m) {
+				const uint32_t q = lds_u16(xq + (uint32_t)coef_lowest64(m) * 2u);
+				m &= m - 1;
+				uint32_t v;
+#ifndef JSMPEG_WALK_EMU
+				asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(stile + (q & 0xffu)) : "memory");
+#else
+				v = lds_u16(stile + (q & 0xffu));
+#endif
+				lv[k >> 1] |= v << (16 * (k & 1));
+			}
+		}
+#ifndef JSMPEG_WALK_EMU
+		asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(stile), "r"((uint32_t)written), "r"((uint32_t)(written >> 32)),
+		             "r"(lv[0]), "r"(lv[1]) : "memory");
+		asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(stile + 16u), "r"(lv[2]), "r"(lv[3]), "r"(lv[4]), "r"(lv[5]) : "memory");
+		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+		asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], 32;" ::"l"(crec), "r"(stile) : "memory");
+		asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+		asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+#else
+		memcpy(crec, &written, 8);
+		memcpy(reinterpret_cast<uint8_t *>(crec) + 8, lv, sizeof lv);
+#endif
+		return;
+	}
+	if (crec) crec->mask = COEF_RECORD_DENSE;  // (rare: more positions than the compact record holds)
 	// The finished block leaves as ONE 128-byte TMA bulk store (shared -> global, SASS UBLKCP): whole
 	// lines reach L2, whereas eight 16-byte stores per thread half-fill 32-byte sectors and made L2
 	// read every sector back before merging (about as many bytes read as written).
