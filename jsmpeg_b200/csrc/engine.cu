@@ -31,10 +31,12 @@
 #include <algorithm>
 #include <cstring>
 #include <deque>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "bitbuffer.h"
+#include "buffers.h"
 #include "common.cuh"
 #include "../../include/jsmpeg_b200.h"
 
@@ -43,22 +45,10 @@ namespace {
 constexpr int HOST_RING = 4;
 constexpr uint32_t ES_PAD = 512;  // readable, zeroed slack after the ES mirror (the walk's ring prefetches 64 bytes ahead)
 
-template <typename T>
-T *dev_alloc(size_t n) {
-	T *p = nullptr;
-	CUDA_CHECK(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)));
-	return p;
-}
-template <typename T>
-T *pinned_alloc(size_t n) {
-	T *p = nullptr;
-	CUDA_CHECK(cudaHostAlloc(&p, std::max<size_t>(n, 1) * sizeof(T), cudaHostAllocDefault));
-	return p;
-}
-
-// the bit buffer lives in pinned host memory (H2D copies of new bytes run at PCIe speed)
-void *bb_pinned_alloc(size_t n, void *) { return pinned_alloc<uint8_t>(n); }
-void bb_pinned_release(void *p, void *) { (void)cudaFreeHost(p); }
+// the bit buffer lives in pinned host memory (H2D copies of new bytes run at PCIe speed); bitbuffer.h owns it
+// through these hooks
+void *bb_pinned_alloc(size_t n, void *) { return PinnedAlloc::alloc(std::max<size_t>(n, 1)); }
+void bb_pinned_release(void *p, void *) { PinnedAlloc::release(p); }
 const bitbuffer::Allocator kPinned = {bb_pinned_alloc, bb_pinned_release, nullptr};
 
 struct Parsed {
@@ -77,10 +67,10 @@ struct Stream {
 	uint32_t seq_end_index = 0;  // bit index right after the sequence header
 	uint32_t seq_floor = 0;      // byte position in the CURRENT buffer from which pictures follow the sequence header
 	SeqParams seq{};
-	SeqParams *d_seq = nullptr;
+	DeviceBuffer<SeqParams> d_seq;
 	// ES mirror in HBM + start-code index
-	uint8_t *d_es = nullptr;
-	uint32_t d_capacity = 0, d_valid = 0;
+	DeviceBuffer<uint8_t> d_es;
+	uint32_t d_valid = 0;
 	std::vector<uint32_t> pics;  // sorted byte positions of picture start codes (00 00 01 00)
 	std::vector<uint32_t> codes, pic_code;  // every start-code prefix (00 00 01), sorted; pics[k] == codes[pic_code[k]]
 	uint32_t codes_classified = 0;          // codes[0 .. codes_classified) have had their fourth byte looked at
@@ -88,23 +78,28 @@ struct Stream {
 	uint32_t scan_from = 0;      // the span a pending scan covers starts here
 	bool scan_pending = false;
 	// planes: two sets in HBM (ping-pong like mpeg1.js:221-246), a host ring for OUT_HOST
-	uint8_t *d_planes[2] = {nullptr, nullptr};
+	DeviceBuffer<uint8_t> d_planes[2];
 	int cur = 0;  // set written by the next I/P picture; forward = 1 - cur
-	uint8_t *h_planes[HOST_RING] = {};
+	PinnedBuffer<uint8_t> h_planes[HOST_RING];
 	int h_head = -1;
 	// B-picture extension ("decode_b"): two more sets in HBM, written in turn -- a B picture is no reference, the
 	// ping-pong above is untouched by it; d_last = the set holding the most recently decoded picture
-	uint8_t *d_planes_b[2] = {nullptr, nullptr};
+	DeviceBuffer<uint8_t> d_planes_b[2];
 	int b_cur = 0;
 	uint8_t *d_last = nullptr;
 	int last_type = 0, last_temporal = 0;  // picture_coding_type / temporal_reference of the last picture decode() consumed
-	uint8_t *d_rgba = nullptr;
+	DeviceBuffer<uint8_t> d_rgba;
 	std::vector<int16_t> ts_bound;     // device TS demux: the stream id every PID is bound to, 0 = none (ts.js pidsToStreamIds)
 	std::vector<uint8_t> ts_leftover;  // ... and the bytes the last write_ts left over (ts.js leftoverBytes)
 	std::vector<uint8_t> ps_leftover;  // device PS demux: the bytes the last write_ps left over
 	bool ps_in_sync = false;           // ... and whether they continue the item chain (else: look for a pack header)
 	// parsed-ahead pictures, consecutive, front = next picture decode() consumes
 	std::deque<Parsed> cache;
+};
+
+struct ScratchDeleter {
+	void operator()(TsScratch *s) const { ts_scratch_destroy(s); }
+	void operator()(PsScratch *s) const { ps_scratch_destroy(s); }
 };
 
 }  // namespace
@@ -117,22 +112,25 @@ struct jsmpeg_b200_batch_t {
 	std::vector<Stream> streams;
 	// start-code scan of all streams in one launch (scan.cu): span list, per-span hit counts and positions;
 	// and the device's copy of every stream's sorted prefix list (ParseTask::codes), one row per stream
-	ScanSpan *d_spans = nullptr, *h_spans = nullptr;
-	uint32_t *d_scan_counts = nullptr, *h_scan_counts = nullptr, *d_scan_pos = nullptr, *h_scan_pos = nullptr;
-	uint32_t scan_rows = 0, scan_seg = 0;       // room: spans, positions per span
-	uint32_t *d_codes = nullptr, *h_codes = nullptr;
-	uint32_t codes_rows = 0, codes_stride = 0;  // rows = streams, stride = entries per row
+	// (scan_seg(), codes_stride(): the row lengths)
+	DeviceBuffer<ScanSpan> d_spans;
+	PinnedBuffer<ScanSpan> h_spans;
+	DeviceBuffer<uint32_t> d_scan_counts, d_scan_pos;
+	PinnedBuffer<uint32_t> h_scan_counts, h_scan_pos;
+	DeviceBuffer<uint32_t> d_codes;  // empty until the first list is staged: the walks then search slice ends themselves
+	PinnedBuffer<uint32_t> h_codes;
 	cudaStream_t st_main = nullptr, st_recon = nullptr, st_copy = nullptr;  // uploads + scan + parse | reconstruct | copy-out
 	cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_mid = nullptr, ev_step = nullptr, ev_round = nullptr, ev_copied[2] = {nullptr, nullptr};
 	cudaEvent_t ev_recon[2] = {nullptr, nullptr};  // around a round's reconstruct launches (timing)
 	// record slots
 	unsigned max_slots_req = 0;
 	int slot_mb = 0, n_slots = 0;
-	mb_record_t *d_hdr = nullptr;
-	int16_t *d_coef = nullptr;
-	uint2 *d_park = nullptr;
-	uint4 *d_stage = nullptr;  // per slot: stage_entries_for(slot_mb) x 64 B (lane-parallel walk, relative records)
-	picture_info_t *d_info = nullptr, *h_info = nullptr;
+	DeviceBuffer<mb_record_t> d_hdr;
+	DeviceBuffer<int16_t> d_coef;
+	DeviceBuffer<uint2> d_park;
+	DeviceBuffer<uint4> d_stage;  // per slot: stage_entries_for(slot_mb) x 64 B (lane-parallel walk, relative records)
+	DeviceBuffer<picture_info_t> d_info;
+	PinnedBuffer<picture_info_t> h_info;
 	std::vector<int> free_slots;
 	int lookahead = 1;
 	bool decode_b = false;       // the B-picture extension: off = B pictures are skipped like the reference does (mpeg1.js:181-184)
@@ -143,22 +141,20 @@ struct jsmpeg_b200_batch_t {
 	cudaEvent_t ev_sfork = nullptr, ev_sjoin[2] = {nullptr, nullptr};
 	bool recon_pending = false;  // reconstruct launches of an earlier round may still read record slots
 	// parse task staging
-	ParseTask *h_ptasks = nullptr, *d_ptasks = nullptr;
-	int ptask_cap = 0;
+	PinnedBuffer<ParseTask> h_ptasks;
+	DeviceBuffer<ParseTask> d_ptasks;
 	uint64_t copy_steps = 0;  // reconstruct launches with a copy-out so far (event parity)
 	ParseFork fork{};
 	bool batch_copy_ok = true;
-	TsScratch *ts = nullptr;
-	PsScratch *ps = nullptr;
+	std::unique_ptr<TsScratch, ScratchDeleter> ts;
+	std::unique_ptr<PsScratch, ScratchDeleter> ps;
 	// decode_pictures / decode_intra: the forward plane set a chain of one picture names, zeroed and never written
 	// (DESIGN 3.6); and the pool of the other chains' plane sets, zeroed per chain group (DESIGN 3.7)
-	uint8_t *d_intra_fwd = nullptr;
-	size_t intra_fwd_bytes = 0;
-	uint8_t *d_chain_sets = nullptr;
-	size_t chain_sets_bytes = 0;
+	DeviceBuffer<uint8_t> d_intra_fwd;
+	DeviceBuffer<uint8_t> d_chain_sets;
 	// decode_macroblocks: the export tasks of a wave (DESIGN 3.8)
-	MbExportTask *h_xtasks = nullptr, *d_xtasks = nullptr;
-	int xtask_cap = 0;
+	PinnedBuffer<MbExportTask> h_xtasks;
+	DeviceBuffer<MbExportTask> d_xtasks;
 	jsmpeg_b200_stats_t stats{};
 };
 
@@ -273,16 +269,16 @@ void parse_sequence_header(Batch *b, Stream &s, uint32_t bit_index) {
 	s.has_seq = true;
 
 	const size_t plane_bytes = (size_t)s.coded_size * 3 / 2;
-	s.d_seq = dev_alloc<SeqParams>(1);
-	CUDA_CHECK(cudaMemcpyAsync(s.d_seq, &s.seq, sizeof(SeqParams), cudaMemcpyHostToDevice, b->st_main));
-	for (int i = 0; i < 2; i++) {
+	s.d_seq.reserve(1);
+	CUDA_CHECK(cudaMemcpyAsync(s.d_seq.data(), &s.seq, sizeof(SeqParams), cudaMemcpyHostToDevice, b->st_main));
+	for (auto &p : s.d_planes) {
 		// + coded_width + 64: stage 2's row loads may touch (never use) up to one row past a plane set's end
-		s.d_planes[i] = dev_alloc<uint8_t>(plane_bytes + s.seq.coded_width + 64);
-		CUDA_CHECK(cudaMemsetAsync(s.d_planes[i], 0, plane_bytes + s.seq.coded_width + 64, b->st_main));  // JS typed arrays start zeroed
+		p.reserve(plane_bytes + s.seq.coded_width + 64);
+		CUDA_CHECK(cudaMemsetAsync(p.data(), 0, plane_bytes + s.seq.coded_width + 64, b->st_main));  // JS typed arrays start zeroed
 	}
-	for (int i = 0; i < HOST_RING; i++) {
-		s.h_planes[i] = pinned_alloc<uint8_t>(plane_bytes);
-		memset(s.h_planes[i], 0, plane_bytes);
+	for (auto &p : s.h_planes) {
+		p.reserve(plane_bytes);
+		memset(p.data(), 0, plane_bytes);
 	}
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));  // s.seq is read by the async copy
 }
@@ -310,69 +306,55 @@ void stream_did_write(Batch *b, Stream &s, uint32_t n) {
 
 // Room for `need` ES bytes (+ pad) in the HBM mirror; what is already resident stays resident.
 void reserve_device_es(Batch *b, Stream &s, uint32_t need) {
-	if ((uint64_t)need + ES_PAD <= s.d_capacity) return;
-	uint64_t cap = std::max<uint64_t>((uint64_t)need + ES_PAD, (uint64_t)s.d_capacity * 2);
+	if ((uint64_t)need + ES_PAD <= s.d_es.size()) return;
+	uint64_t cap = std::max<uint64_t>((uint64_t)need + ES_PAD, (uint64_t)s.d_es.size() * 2);
 	cap = std::min<uint64_t>((cap + 255u) & ~255ull, 0xffffff00ull);
-	uint8_t *n = dev_alloc<uint8_t>(cap);
-	if (s.d_es) {
-		if (s.d_valid) CUDA_CHECK(cudaMemcpyAsync(n, s.d_es, s.d_valid, cudaMemcpyDeviceToDevice, b->st_main));
+	DeviceBuffer<uint8_t> n(cap);
+	if (s.d_es.data()) {
+		if (s.d_valid) CUDA_CHECK(cudaMemcpyAsync(n.data(), s.d_es.data(), s.d_valid, cudaMemcpyDeviceToDevice, b->st_main));
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-		CUDA_CHECK(cudaFree(s.d_es));
 	}
-	s.d_es = n;
-	s.d_capacity = (uint32_t)cap;
+	s.d_es = std::move(n);
 }
+
+// Positions per span of the scan buffers, entries per stream of the device's prefix lists
+uint32_t scan_seg(const Batch *b) { return b->d_spans.size() ? (uint32_t)(b->d_scan_pos.size() / b->d_spans.size()) : 0; }
+uint32_t codes_stride(const Batch *b) { return (uint32_t)(b->d_codes.size() / b->streams.size()); }
 
 // Room for `rows` spans with `seg` positions each (contents are per scan: nothing to keep).
 void reserve_scan(Batch *b, uint32_t rows, uint32_t seg) {
-	if (rows <= b->scan_rows && seg <= b->scan_seg) return;
-	rows = std::max(rows, b->scan_rows);
-	seg = std::max(seg, b->scan_seg);
-	if (b->d_spans) CUDA_CHECK(cudaFree(b->d_spans));
-	if (b->d_scan_counts) CUDA_CHECK(cudaFree(b->d_scan_counts));
-	if (b->d_scan_pos) CUDA_CHECK(cudaFree(b->d_scan_pos));
-	if (b->h_spans) CUDA_CHECK(cudaFreeHost(b->h_spans));
-	if (b->h_scan_counts) CUDA_CHECK(cudaFreeHost(b->h_scan_counts));
-	if (b->h_scan_pos) CUDA_CHECK(cudaFreeHost(b->h_scan_pos));
-	b->d_spans = nullptr; b->d_scan_counts = nullptr; b->d_scan_pos = nullptr;
-	b->h_spans = nullptr; b->h_scan_counts = nullptr; b->h_scan_pos = nullptr;
-	b->scan_rows = b->scan_seg = 0;
-	b->d_spans = dev_alloc<ScanSpan>(rows);
-	b->h_spans = pinned_alloc<ScanSpan>(rows);
-	b->d_scan_counts = dev_alloc<uint32_t>(rows);
-	b->h_scan_counts = pinned_alloc<uint32_t>(rows);
-	b->d_scan_pos = dev_alloc<uint32_t>((size_t)rows * seg);
-	b->h_scan_pos = pinned_alloc<uint32_t>((size_t)rows * seg);
-	b->scan_rows = rows;
-	b->scan_seg = seg;
+	const uint32_t have_rows = (uint32_t)b->d_spans.size(), have_seg = scan_seg(b);
+	if (rows <= have_rows && seg <= have_seg) return;
+	rows = std::max(rows, have_rows);
+	seg = std::max(seg, have_seg);
+	b->d_spans.reserve(rows);
+	b->h_spans.reserve(rows);
+	b->d_scan_counts.reserve(rows);
+	b->h_scan_counts.reserve(rows);
+	b->d_scan_pos.reserve((size_t)rows * seg);
+	b->h_scan_pos.reserve((size_t)rows * seg);
 }
 
 // One launch over the pending spans (h_spans[0 .. n)); the counts come back to h_scan_counts.
 void launch_scan(Batch *b, int n, uint32_t longest) {
-	CUDA_CHECK(cudaMemcpyAsync(b->d_spans, b->h_spans, n * sizeof(ScanSpan), cudaMemcpyHostToDevice, b->st_main));
-	CUDA_CHECK(cudaMemsetAsync(b->d_scan_counts, 0, n * sizeof(uint32_t), b->st_main));
-	launch_scan_start_codes(b->d_spans, n, longest, b->d_scan_pos, b->scan_seg, b->d_scan_counts, b->st_main);
+	CUDA_CHECK(cudaMemcpyAsync(b->d_spans.data(), b->h_spans.data(), n * sizeof(ScanSpan), cudaMemcpyHostToDevice, b->st_main));
+	CUDA_CHECK(cudaMemsetAsync(b->d_scan_counts.data(), 0, n * sizeof(uint32_t), b->st_main));
+	launch_scan_start_codes(b->d_spans.data(), n, longest, b->d_scan_pos.data(), scan_seg(b), b->d_scan_counts.data(), b->st_main);
 	b->stats.kernel_launches++;
-	CUDA_CHECK(cudaMemcpyAsync(b->h_scan_counts, b->d_scan_counts, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, b->st_main));
+	CUDA_CHECK(cudaMemcpyAsync(b->h_scan_counts.data(), b->d_scan_counts.data(), n * sizeof(uint32_t), cudaMemcpyDeviceToHost, b->st_main));
 }
 
 // The device's copy of every stream's prefix list: row si = streams[si].codes.  The host has them all, so a
 // change of geometry (more streams, a longer list) just stages everything again.  Returns true if rebuilt.
-bool reserve_codes(Batch *b, uint32_t rows, uint32_t entries) {
-	if (rows == b->codes_rows && entries <= b->codes_stride) return false;
-	const uint32_t stride = std::max<uint32_t>(std::max<uint32_t>(2 * b->codes_stride, entries + 256u), 1024u);
-	if (b->d_codes) {
+bool reserve_codes(Batch *b, uint32_t entries) {
+	if (b->d_codes.data() && entries <= codes_stride(b)) return false;
+	const uint32_t stride = std::max<uint32_t>(std::max<uint32_t>(2 * codes_stride(b), entries + 256u), 1024u);
+	if (b->d_codes.data()) {
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));  // (tasks of an earlier round may still name the old rows)
 		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-		CUDA_CHECK(cudaFree(b->d_codes));
 	}
-	if (b->h_codes) CUDA_CHECK(cudaFreeHost(b->h_codes));
-	b->d_codes = nullptr; b->h_codes = nullptr;
-	b->codes_rows = b->codes_stride = 0;
-	b->d_codes = dev_alloc<uint32_t>((size_t)rows * stride);
-	b->h_codes = pinned_alloc<uint32_t>((size_t)rows * stride);
-	b->codes_rows = rows;
-	b->codes_stride = stride;
+	b->d_codes.reserve(b->streams.size() * stride);
+	b->h_codes.reserve(b->streams.size() * stride);
 	return true;
 }
 
@@ -382,11 +364,11 @@ void begin_upload(Batch *b, Stream &s) {
 	reserve_device_es(b, s, s.bb.length);
 	if (s.d_valid < s.bb.length) {
 		uint32_t from = s.d_valid & ~15u;
-		CUDA_CHECK(cudaMemcpyAsync(s.d_es + from, s.bb.bytes + from, s.bb.length - from, cudaMemcpyHostToDevice, b->st_main));
+		CUDA_CHECK(cudaMemcpyAsync(s.d_es.data() + from, s.bb.bytes + from, s.bb.length - from, cudaMemcpyHostToDevice, b->st_main));
 		b->stats.h2d_bytes += s.bb.length - from;
 		s.d_valid = s.bb.length;
 		// the kernels rely on zeros right after the data (bytes past the end read as 0, like JS)
-		CUDA_CHECK(cudaMemsetAsync(s.d_es + s.bb.length, 0, ES_PAD, b->st_main));
+		CUDA_CHECK(cudaMemsetAsync(s.d_es.data() + s.bb.length, 0, ES_PAD, b->st_main));
 	}
 	if (s.scanned < s.bb.length) {
 		s.scan_from = s.scanned >= 2 ? s.scanned - 2 : 0;  // a prefix needs its three bytes: those from scanned - 2 on were not complete
@@ -416,7 +398,7 @@ long upload_all(Batch *b) {
 		reserve_scan(b, (uint32_t)n, seg);
 		for (int k = 0; k < n; k++) {
 			const Stream &s = b->streams[pending[k]];
-			b->h_spans[k] = ScanSpan{s.d_es, s.scan_from, s.bb.length};
+			b->h_spans[k] = ScanSpan{s.d_es.data(), s.scan_from, s.bb.length};
 		}
 		launch_scan(b, n, longest);
 		CUDA_CHECK(cudaEventRecord(b->ev_b, b->st_main));
@@ -424,23 +406,23 @@ long upload_all(Batch *b) {
 		float ms = 0;
 		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_a, b->ev_b));
 		b->stats.scan_ms += ms;
-		uint32_t most = *std::max_element(b->h_scan_counts, b->h_scan_counts + n);
-		if (most > b->scan_seg) {
+		uint32_t most = *std::max_element(b->h_scan_counts.data(), b->h_scan_counts.data() + n);
+		if (most > scan_seg(b)) {
 			// a list overflowed (hostile input: start codes cannot overlap, so at most length / 3 of them): once
 			// more, with room for the count the kernel reported
 			reserve_scan(b, (uint32_t)n, most + 16u);
-			for (int k = 0; k < n; k++) {  // (the pinned span list was reallocated)
+			for (int k = 0; k < n; k++) {  // (the pinned span list may have been reallocated)
 				const Stream &s = b->streams[pending[k]];
-				b->h_spans[k] = ScanSpan{s.d_es, s.scan_from, s.bb.length};
+				b->h_spans[k] = ScanSpan{s.d_es.data(), s.scan_from, s.bb.length};
 			}
 			launch_scan(b, n, longest);
 			CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-			most = *std::max_element(b->h_scan_counts, b->h_scan_counts + n);
-			if (most > b->scan_seg) throw std::runtime_error("jsmpeg_b200: start-code index overflow after a rescan");
+			most = *std::max_element(b->h_scan_counts.data(), b->h_scan_counts.data() + n);
+			if (most > scan_seg(b)) throw std::runtime_error("jsmpeg_b200: start-code index overflow after a rescan");
 		}
 		if (most) {  // the positions of all spans in one (strided) copy
-			CUDA_CHECK(cudaMemcpy2DAsync(b->h_scan_pos, (size_t)b->scan_seg * sizeof(uint32_t), b->d_scan_pos,
-			                             (size_t)b->scan_seg * sizeof(uint32_t), (size_t)most * sizeof(uint32_t), (size_t)n,
+			CUDA_CHECK(cudaMemcpy2DAsync(b->h_scan_pos.data(), (size_t)scan_seg(b) * sizeof(uint32_t), b->d_scan_pos.data(),
+			                             (size_t)scan_seg(b) * sizeof(uint32_t), (size_t)most * sizeof(uint32_t), (size_t)n,
 			                             cudaMemcpyDeviceToHost, b->st_main));
 			b->stats.d2h_bytes += (uint64_t)most * n * sizeof(uint32_t);
 			CUDA_CHECK(cudaStreamSynchronize(b->st_main));
@@ -448,7 +430,7 @@ long upload_all(Batch *b) {
 		bool grew = false;
 		for (int k = 0; k < n; k++) {
 			Stream &s = b->streams[pending[k]];
-			uint32_t *hits = b->h_scan_pos + (size_t)k * b->scan_seg;
+			uint32_t *hits = b->h_scan_pos.data() + (size_t)k * scan_seg(b);
 			const uint32_t cnt = b->h_scan_counts[k];
 			std::sort(hits, hits + cnt);
 			// the rescanned window starts 2 bytes before the old frontier, so nothing is reported twice
@@ -460,15 +442,16 @@ long upload_all(Batch *b) {
 		if (grew) {  // the device's copy, for the lane-parallel walk's slice ends: every row that changed, in one copy
 			size_t longest_list = 0;
 			for (auto &s : b->streams) longest_list = std::max(longest_list, s.codes.size());
-			const bool rebuilt = reserve_codes(b, (uint32_t)S, (uint32_t)longest_list);
+			const bool rebuilt = reserve_codes(b, (uint32_t)longest_list);
+			const uint32_t stride = codes_stride(b);
 			for (int si = 0; si < S; si++) {
 				const Stream &s = b->streams[si];
 				// (a rewound stream's list starts over: staging whole rows keeps this free of bookkeeping; they are short)
 				if (!s.codes.empty() && (rebuilt || std::find(pending.begin(), pending.end(), si) != pending.end()))
-					memcpy(b->h_codes + (size_t)si * b->codes_stride, s.codes.data(), s.codes.size() * sizeof(uint32_t));
+					memcpy(b->h_codes.data() + (size_t)si * stride, s.codes.data(), s.codes.size() * sizeof(uint32_t));
 			}
-			CUDA_CHECK(cudaMemcpy2DAsync(b->d_codes, (size_t)b->codes_stride * sizeof(uint32_t), b->h_codes,
-			                             (size_t)b->codes_stride * sizeof(uint32_t), longest_list * sizeof(uint32_t), (size_t)S,
+			CUDA_CHECK(cudaMemcpy2DAsync(b->d_codes.data(), (size_t)stride * sizeof(uint32_t), b->h_codes.data(),
+			                             (size_t)stride * sizeof(uint32_t), longest_list * sizeof(uint32_t), (size_t)S,
 			                             cudaMemcpyHostToDevice, b->st_main));
 			b->stats.h2d_bytes += (uint64_t)longest_list * S * sizeof(uint32_t);
 			CUDA_CHECK(cudaStreamSynchronize(b->st_main));  // the pinned staging is written again by the next scan
@@ -499,12 +482,8 @@ void ensure_pool(Batch *b) {
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
 	b->recon_pending = false;
-	if (b->d_hdr) { CUDA_CHECK(cudaFree(b->d_hdr)); b->d_hdr = nullptr; }
-	if (b->d_coef) { CUDA_CHECK(cudaFree(b->d_coef)); b->d_coef = nullptr; }
-	if (b->d_park) { CUDA_CHECK(cudaFree(b->d_park)); b->d_park = nullptr; }
-	if (b->d_stage) { CUDA_CHECK(cudaFree(b->d_stage)); b->d_stage = nullptr; }
-	if (b->d_info) { CUDA_CHECK(cudaFree(b->d_info)); b->d_info = nullptr; }
-	if (b->h_info) { CUDA_CHECK(cudaFreeHost(b->h_info)); b->h_info = nullptr; }
+	// the old pool goes before the free memory is measured
+	b->d_hdr.reset(); b->d_coef.reset(); b->d_park.reset(); b->d_stage.reset(); b->d_info.reset(); b->h_info.reset();
 	b->slot_mb = 0;
 	b->n_slots = 0;
 	b->free_slots.clear();
@@ -518,26 +497,22 @@ void ensure_pool(Batch *b) {
 	const size_t fit = (size_t)(0.9 * (double)free_b) / slot_bytes;  // a request beyond the device is cut, not fatal
 	if (n == 0) n = std::min<size_t>((size_t)(0.45 * (double)free_b) / slot_bytes, 4096);
 	n = std::max<size_t>(std::min(n, fit), 2);
-	b->d_hdr = dev_alloc<mb_record_t>(n * need_mb);
-	b->d_coef = dev_alloc<int16_t>(n * need_mb * MB_COEF_INT16);
-	b->d_park = dev_alloc<uint2>(n * need_mb * 6);
-	b->d_stage = dev_alloc<uint4>(n * (size_t)stage_entries_for(need_mb) * 4);
-	b->d_info = dev_alloc<picture_info_t>(n);
-	b->h_info = pinned_alloc<picture_info_t>(n);
+	b->d_hdr.reserve(n * need_mb);
+	b->d_coef.reserve(n * need_mb * MB_COEF_INT16);
+	b->d_park.reserve(n * need_mb * 6);
+	b->d_stage.reserve(n * (size_t)stage_entries_for(need_mb) * 4);
+	b->d_info.reserve(n);
+	b->h_info.reserve(n);
 	b->slot_mb = need_mb;
 	b->n_slots = (int)n;
 	for (int i = (int)n - 1; i >= 0; i--) b->free_slots.push_back(i);
 }
 
 void ensure_task_caps(Batch *b, int n_parse) {
-	if (n_parse <= b->ptask_cap) return;
-	if (b->h_ptasks) { CUDA_CHECK(cudaFreeHost(b->h_ptasks)); b->h_ptasks = nullptr; }
-	if (b->d_ptasks) { CUDA_CHECK(cudaFree(b->d_ptasks)); b->d_ptasks = nullptr; }
-	const int cap = std::max(n_parse, b->ptask_cap * 2);
-	b->ptask_cap = 0;
-	b->h_ptasks = pinned_alloc<ParseTask>(cap);
-	b->d_ptasks = dev_alloc<ParseTask>(cap);
-	b->ptask_cap = cap;
+	if ((size_t)n_parse <= b->d_ptasks.size()) return;
+	const size_t cap = std::max<size_t>(n_parse, b->d_ptasks.size() * 2);
+	b->h_ptasks.reserve(cap);
+	b->d_ptasks.reserve(cap);
 }
 
 PlaneSet plane_set(const Stream &s, uint8_t *base) {
@@ -631,19 +606,19 @@ int walk_kind(const Batch *b, const Stream &s, uint32_t pic, bool b_walk) {
 ParseTask parse_task(const Batch *b, int si, uint32_t pic, int slot, int info_idx) {
 	const Stream &s = b->streams[si];
 	ParseTask t{};
-	t.es = s.d_es;
+	t.es = s.d_es.data();
 	t.es_len = s.bb.length;
 	t.start_byte = s.pics[pic] + 4;
-	t.seq = s.d_seq;
-	t.hdr = b->d_hdr + (size_t)slot * b->slot_mb;
-	t.coef = b->d_coef + (size_t)slot * b->slot_mb * MB_COEF_INT16;
-	t.park = b->d_park + (size_t)slot * b->slot_mb * 6;
-	t.info = b->d_info + info_idx;
+	t.seq = s.d_seq.data();
+	t.hdr = b->d_hdr.data() + (size_t)slot * b->slot_mb;
+	t.coef = b->d_coef.data() + (size_t)slot * b->slot_mb * MB_COEF_INT16;
+	t.park = b->d_park.data() + (size_t)slot * b->slot_mb * 6;
+	t.info = b->d_info.data() + info_idx;
 	t.mb_width = s.seq.mb_width;
 	t.mb_size = s.seq.mb_size;
-	t.stage = b->d_stage + (size_t)slot * stage_entries_for(b->slot_mb) * 4;
+	t.stage = b->d_stage.data() + (size_t)slot * stage_entries_for(b->slot_mb) * 4;
 	t.stage_entries = stage_entries_for(b->slot_mb);
-	t.codes = b->d_codes ? b->d_codes + (size_t)si * b->codes_stride : nullptr;
+	t.codes = b->d_codes.data() ? b->d_codes.data() + (size_t)si * codes_stride(b) : nullptr;
 	t.n_codes = (uint32_t)s.codes.size();
 	t.code_hint = s.pic_code[pic];
 	return t;
@@ -685,7 +660,7 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 		CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_round, 0));
 		b->recon_pending = false;
 	}
-	CUDA_CHECK(cudaMemcpyAsync(b->d_ptasks, b->h_ptasks, n * sizeof(ParseTask), cudaMemcpyHostToDevice, b->st_main));
+	CUDA_CHECK(cudaMemcpyAsync(b->d_ptasks.data(), b->h_ptasks.data(), n * sizeof(ParseTask), cudaMemcpyHostToDevice, b->st_main));
 	CUDA_CHECK(cudaEventRecord(b->ev_a, b->st_main));
 	int primary = 0;
 	while (cnt[primary] == 0) primary++;
@@ -700,16 +675,16 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 			st = b->st_side[n_side];
 			CUDA_CHECK(cudaStreamWaitEvent(st, b->ev_sfork, 0));
 		}
-		if (kind == 0) launches += launch_parse_pictures(b->d_ptasks, cnt[0], b->slot_mb, expand, st, b->ev_mid, &b->fork);
-		else if (kind == 1) launches += launch_parse_pictures_slices(b->d_ptasks + off[1], cnt[1], b->slot_mb, expand, st);
-		else launches += launch_parse_pictures_b(b->d_ptasks + off[2], cnt[2], b->slot_mb, expand, st);
+		if (kind == 0) launches += launch_parse_pictures(b->d_ptasks.data(), cnt[0], b->slot_mb, expand, st, b->ev_mid, &b->fork);
+		else if (kind == 1) launches += launch_parse_pictures_slices(b->d_ptasks.data() + off[1], cnt[1], b->slot_mb, expand, st);
+		else launches += launch_parse_pictures_b(b->d_ptasks.data() + off[2], cnt[2], b->slot_mb, expand, st);
 		if (kind != primary) {
 			CUDA_CHECK(cudaEventRecord(b->ev_sjoin[n_side], st));
 			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_sjoin[n_side], 0));
 			n_side++;
 		}
 	}
-	CUDA_CHECK(cudaMemcpyAsync(b->h_info, b->d_info, n * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
+	CUDA_CHECK(cudaMemcpyAsync(b->h_info.data(), b->d_info.data(), n * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
 	if (cnt[0] == 0) CUDA_CHECK(cudaEventRecord(b->ev_mid, b->st_main));  // (a wave without the lane-parallel walk)
 	CUDA_CHECK(cudaEventRecord(b->ev_b, b->st_main));
 	CUDA_CHECK(cudaEventSynchronize(b->ev_b));
@@ -720,9 +695,9 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 // from `fwd` (and, for a B picture, `bwd`), with the fused RGBA conversion into `rgba` unless that is nullptr
 ReconTask recon_task(const Batch *b, const Stream &s, int slot, uint8_t *cur, uint8_t *fwd, uint8_t *bwd, uint8_t *rgba) {
 	ReconTask t{};
-	t.hdr = b->d_hdr + (size_t)slot * b->slot_mb;
-	t.coef = b->d_coef + (size_t)slot * b->slot_mb * MB_COEF_INT16;
-	t.compact = compact_plane(b->d_stage + (size_t)slot * stage_entries_for(b->slot_mb) * 4);  // (stage 1b wrote it: parse_task)
+	t.hdr = b->d_hdr.data() + (size_t)slot * b->slot_mb;
+	t.coef = b->d_coef.data() + (size_t)slot * b->slot_mb * MB_COEF_INT16;
+	t.compact = compact_plane(b->d_stage.data() + (size_t)slot * stage_entries_for(b->slot_mb) * 4);  // (stage 1b wrote it: parse_task)
 	t.cur = plane_set(s, cur);
 	t.fwd = plane_set(s, fwd);
 	if (bwd) t.bwd = plane_set(s, bwd);
@@ -825,27 +800,27 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 				const bool is_b = e.info.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
 				uint8_t *rgba = nullptr;
 				if (flags & JSMPEG_B200_OUT_RGBA) {
-					if (!s.d_rgba) {  // opaque white, like the canvas the reference creates (canvas2d.js:24-29): the odd edge keeps it
-						s.d_rgba = dev_alloc<uint8_t>((size_t)s.width * s.height * 4);
-						CUDA_CHECK(cudaMemsetAsync(s.d_rgba, 0xff, (size_t)s.width * s.height * 4, b->st_recon));
+					if (!s.d_rgba.data()) {  // opaque white, like the canvas the reference creates (canvas2d.js:24-29): the odd edge keeps it
+						s.d_rgba.reserve((size_t)s.width * s.height * 4);
+						CUDA_CHECK(cudaMemsetAsync(s.d_rgba.data(), 0xff, (size_t)s.width * s.height * 4, b->st_recon));
 					}
-					rgba = s.d_rgba;
+					rgba = s.d_rgba.data();
 				}
 				ReconTask t;
 				if (is_b) {
 					// after the swaps `cur` holds the older and `1 - cur` the newer of the two most recent I/P pictures:
 					// the B picture's forward (past) and backward (future) reference.  It goes to a set of its own.
-					if (!s.d_planes_b[0]) {
+					if (!s.d_planes_b[0].data()) {
 						const size_t bytes = (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64;
 						for (auto &pb : s.d_planes_b) {
-							pb = dev_alloc<uint8_t>(bytes);
-							CUDA_CHECK(cudaMemsetAsync(pb, 0, bytes, b->st_recon));
+							pb.reserve(bytes);
+							CUDA_CHECK(cudaMemsetAsync(pb.data(), 0, bytes, b->st_recon));
 						}
 					}
-					t = recon_task(b, s, e.slot, s.d_planes_b[s.b_cur], s.d_planes[s.cur], s.d_planes[1 - s.cur], rgba);
+					t = recon_task(b, s, e.slot, s.d_planes_b[s.b_cur].data(), s.d_planes[s.cur].data(), s.d_planes[1 - s.cur].data(), rgba);
 					s.b_cur ^= 1;  // no reference: the I/P ping-pong stays as it is
 				} else {
-					t = recon_task(b, s, e.slot, s.d_planes[s.cur], s.d_planes[1 - s.cur], nullptr, rgba);
+					t = recon_task(b, s, e.slot, s.d_planes[s.cur].data(), s.d_planes[1 - s.cur].data(), nullptr, rgba);
 					s.cur ^= 1;  // mpeg1.js:221-246: the picture just decoded becomes `forward`
 				}
 				s.d_last = t.cur.y;
@@ -854,7 +829,7 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 				steps[step].add(t);
 				if (flags & JSMPEG_B200_OUT_HOST) {  // into the next slot of the stream's host ring
 					s.h_head = (s.h_head + 1) % HOST_RING;
-					steps[step].copy(s.h_planes[s.h_head], t.cur.y, planes);
+					steps[step].copy(s.h_planes[s.h_head].data(), t.cur.y, planes);
 					b->stats.d2h_bytes += planes;
 				}
 				step++;
@@ -1063,16 +1038,10 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 		chains.push_back(std::move(c));
 		lo = hi;
 	}
-	if (leaves && set_bytes > b->intra_fwd_bytes) {
-		if (b->d_intra_fwd) {
-			CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-			CUDA_CHECK(cudaFree(b->d_intra_fwd));
-			b->d_intra_fwd = nullptr;
-			b->intra_fwd_bytes = 0;
-		}
-		b->d_intra_fwd = dev_alloc<uint8_t>(set_bytes);
-		CUDA_CHECK(cudaMemsetAsync(b->d_intra_fwd, 0, set_bytes, b->st_recon));
-		b->intra_fwd_bytes = set_bytes;
+	if (leaves && set_bytes > b->d_intra_fwd.size()) {
+		if (b->d_intra_fwd.data()) CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+		b->d_intra_fwd.reserve(set_bytes);
+		CUDA_CHECK(cudaMemsetAsync(b->d_intra_fwd.data(), 0, set_bytes, b->st_recon));
 	}
 	// what a request that is never consumed keeps: planes 0, RGBA opaque white.  A leaf is reconstructed into its
 	// destination, whose absent macroblocks keep that 0; every other destination is written whole by a copy.
@@ -1092,7 +1061,7 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 	// of the free device memory -- a request beyond the device is cut into groups, not refused
 	size_t free_b = 0, total_b = 0;
 	CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-	const size_t max_sets = std::max<size_t>(4, ((size_t)(0.5 * (double)free_b) + b->chain_sets_bytes) / set_bytes);
+	const size_t max_sets = std::max<size_t>(4, ((size_t)(0.5 * (double)free_b) + b->d_chain_sets.size()) / set_bytes);
 	std::vector<std::pair<size_t, size_t>> groups;
 	size_t most_sets = 0;
 	for (size_t lo = 0; lo < chains.size();) {
@@ -1102,22 +1071,16 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 		most_sets = std::max(most_sets, sets);
 		lo = hi;
 	}
-	if (most_sets * set_bytes > b->chain_sets_bytes) {
-		if (b->d_chain_sets) {
-			CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-			CUDA_CHECK(cudaFree(b->d_chain_sets));
-			b->d_chain_sets = nullptr;
-			b->chain_sets_bytes = 0;
-		}
-		b->d_chain_sets = dev_alloc<uint8_t>(most_sets * set_bytes);
-		b->chain_sets_bytes = most_sets * set_bytes;
+	if (most_sets * set_bytes > b->d_chain_sets.size()) {
+		if (b->d_chain_sets.data()) CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+		b->d_chain_sets.reserve(most_sets * set_bytes);
 	}
 	for (const auto &[glo, ghi] : groups) {
 		size_t sets = 0;
 		for (size_t c = glo; c < ghi; c++)
-			for (int k = 0; k < chains[c].n_sets; k++) chains[c].set[k] = b->d_chain_sets + set_bytes * sets++;
+			for (int k = 0; k < chains[c].n_sets; k++) chains[c].set[k] = b->d_chain_sets.data() + set_bytes * sets++;
 		if (sets)  // a fresh decoder's planes start zeroed, the B sets too (the previous group's copies are queued before)
-			CUDA_CHECK(cudaMemsetAsync(b->d_chain_sets, 0, set_bytes * sets, b->st_recon));
+			CUDA_CHECK(cudaMemsetAsync(b->d_chain_sets.data(), 0, set_bytes * sets, b->st_recon));
 		const uint32_t width = (uint32_t)std::max<size_t>(1, (size_t)wave_max / (ghi - glo));
 		for (uint32_t lo = 0;; lo += width) {
 			// ---- stage 1: positions [lo, lo + width) of every chain still consuming
@@ -1170,7 +1133,7 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 						if (is_b)  // the two I/P sets: `cur` the older (forward), `1 - cur` the newer (backward) reference
 							t = recon_task(b, s, slot, ch.set[2 + ch.b_cur], ch.set[ch.cur], ch.set[1 - ch.cur], out_rgba);
 						else if (leaf)  // into the destination, predicted (skipped macroblocks) from the zeroed scratch set
-							t = recon_task(b, s, slot, static_cast<uint8_t *>(planes_dst[order[q_lo]]), b->d_intra_fwd, nullptr, out_rgba);
+							t = recon_task(b, s, slot, static_cast<uint8_t *>(planes_dst[order[q_lo]]), b->d_intra_fwd.data(), nullptr, out_rgba);
 						else
 							t = recon_task(b, s, slot, ch.set[ch.cur], ch.set[1 - ch.cur], nullptr, out_rgba);
 						if (depths.size() <= d) depths.emplace_back();
@@ -1278,14 +1241,10 @@ void decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pic
 		uniq_of[i] = std::lower_bound(uniq.begin(), uniq.end(), std::make_pair(streams[i], pictures[i])) - uniq.begin();
 	if (b->free_slots.size() < uniq.size())  // decode() parses the look-ahead again
 		for (auto &s : b->streams) flush_cache(b, s);
-	if (n > b->xtask_cap) {
+	if ((size_t)n > b->d_xtasks.size()) {
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-		if (b->h_xtasks) { CUDA_CHECK(cudaFreeHost(b->h_xtasks)); b->h_xtasks = nullptr; }
-		if (b->d_xtasks) { CUDA_CHECK(cudaFree(b->d_xtasks)); b->d_xtasks = nullptr; }
-		b->xtask_cap = 0;
-		b->h_xtasks = pinned_alloc<MbExportTask>(n);
-		b->d_xtasks = dev_alloc<MbExportTask>(n);
-		b->xtask_cap = n;
+		b->h_xtasks.reserve(n);
+		b->d_xtasks.reserve(n);
 	}
 	const size_t wave_max = b->free_slots.size();
 	std::vector<int32_t> n_present(n, 0), error(n, 0);
@@ -1311,11 +1270,11 @@ void decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pic
 			n_present[i] = info.n_present;
 			error[i] = info.error;
 			const int mb_size = b->streams[w.stream].seq.mb_size;
-			b->h_xtasks[m++] = MbExportTask{b->d_hdr + (size_t)w.slot * b->slot_mb, dst[i], total, mb_size, info.picture_type, 0};
+			b->h_xtasks[m++] = MbExportTask{b->d_hdr.data() + (size_t)w.slot * b->slot_mb, dst[i], total, mb_size, info.picture_type, 0};
 			total += (uint32_t)mb_size;
 		}
-		CUDA_CHECK(cudaMemcpyAsync(b->d_xtasks, b->h_xtasks, m * sizeof(MbExportTask), cudaMemcpyHostToDevice, b->st_main));
-		launch_export_macroblocks(b->d_xtasks, m, total, b->st_main);
+		CUDA_CHECK(cudaMemcpyAsync(b->d_xtasks.data(), b->h_xtasks.data(), m * sizeof(MbExportTask), cudaMemcpyHostToDevice, b->st_main));
+		launch_export_macroblocks(b->d_xtasks.data(), m, total, b->st_main);
 		for (const WaveItem &w : wave) release_slot(b, w.slot);  // the next wave's walks queue behind the export
 	}
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
@@ -1361,14 +1320,14 @@ long append_demuxed(Batch *b, Stream &s, uint32_t total, F &&gather, uint64_t *p
 	uint8_t *hdst = static_cast<uint8_t *>(stream_get_write_ptr(b, s, total));
 	reserve_device_es(b, s, s.bb.length + total);
 	if (s.d_valid < s.bb.length) {  // bytes written the ordinary way that are not resident yet
-		CUDA_CHECK(cudaMemcpyAsync(s.d_es + s.d_valid, s.bb.bytes + s.d_valid, s.bb.length - s.d_valid, cudaMemcpyHostToDevice, b->st_main));
+		CUDA_CHECK(cudaMemcpyAsync(s.d_es.data() + s.d_valid, s.bb.bytes + s.d_valid, s.bb.length - s.d_valid, cudaMemcpyHostToDevice, b->st_main));
 		b->stats.h2d_bytes += s.bb.length - s.d_valid;
 		s.d_valid = s.bb.length;
 	}
 	const int count = gather(s.bb.length);
 	// the host keeps a mirror of the ES (sequence header parse, EVICT bookkeeping): copy the new bytes back
-	CUDA_CHECK(cudaMemcpyAsync(hdst, s.d_es + s.bb.length, (size_t)total, cudaMemcpyDeviceToHost, b->st_main));
-	CUDA_CHECK(cudaMemsetAsync(s.d_es + s.bb.length + total, 0, ES_PAD, b->st_main));
+	CUDA_CHECK(cudaMemcpyAsync(hdst, s.d_es.data() + s.bb.length, (size_t)total, cudaMemcpyDeviceToHost, b->st_main));
+	CUDA_CHECK(cudaMemsetAsync(s.d_es.data() + s.bb.length + total, 0, ES_PAD, b->st_main));
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 	b->stats.d2h_bytes += (uint64_t)total;
 	stream_did_write(b, s, total);
@@ -1426,37 +1385,7 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b) {
 	// best effort, nothing here may throw: the context may be the very thing that failed
 	(void)cudaSetDevice(b->device);
 	(void)cudaDeviceSynchronize();
-	for (auto &s : b->streams) {
-		if (s.bb.bytes) cudaFreeHost(s.bb.bytes);
-		if (s.d_seq) cudaFree(s.d_seq);
-		if (s.d_es) cudaFree(s.d_es);
-		if (s.d_rgba) cudaFree(s.d_rgba);
-		for (auto p : s.d_planes) if (p) cudaFree(p);
-		for (auto p : s.d_planes_b) if (p) cudaFree(p);
-		for (auto p : s.h_planes) if (p) cudaFreeHost(p);
-	}
-	if (b->d_spans) cudaFree(b->d_spans);
-	if (b->h_spans) cudaFreeHost(b->h_spans);
-	if (b->d_scan_counts) cudaFree(b->d_scan_counts);
-	if (b->h_scan_counts) cudaFreeHost(b->h_scan_counts);
-	if (b->d_scan_pos) cudaFree(b->d_scan_pos);
-	if (b->h_scan_pos) cudaFreeHost(b->h_scan_pos);
-	if (b->d_codes) cudaFree(b->d_codes);
-	if (b->h_codes) cudaFreeHost(b->h_codes);
-	if (b->d_hdr) cudaFree(b->d_hdr);
-	if (b->d_coef) cudaFree(b->d_coef);
-	if (b->d_park) cudaFree(b->d_park);
-	if (b->d_stage) cudaFree(b->d_stage);
-	if (b->d_info) cudaFree(b->d_info);
-	if (b->h_info) cudaFreeHost(b->h_info);
-	if (b->h_ptasks) cudaFreeHost(b->h_ptasks);
-	if (b->d_ptasks) cudaFree(b->d_ptasks);
-	if (b->d_intra_fwd) cudaFree(b->d_intra_fwd);
-	if (b->d_chain_sets) cudaFree(b->d_chain_sets);
-	if (b->h_xtasks) cudaFreeHost(b->h_xtasks);
-	if (b->d_xtasks) cudaFree(b->d_xtasks);
-	ts_scratch_destroy(b->ts);
-	ps_scratch_destroy(b->ps);
+	for (auto &s : b->streams) if (s.bb.bytes) kPinned.release(s.bb.bytes, kPinned.ctx);
 	for (auto e : {b->ev_a, b->ev_b, b->ev_mid, b->ev_recon[0], b->ev_recon[1], b->ev_step, b->ev_round, b->ev_copied[0],
 	               b->ev_copied[1], b->ev_sfork, b->ev_sjoin[0], b->ev_sjoin[1], b->fork.fork}) if (e) cudaEventDestroy(e);
 	for (int i = 0; i < PARSE_GROUPS; i++) {
@@ -1464,8 +1393,8 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b) {
 		if (b->fork.side[i]) cudaStreamDestroy(b->fork.side[i]);
 	}
 	for (auto st : {b->st_main, b->st_recon, b->st_copy, b->st_side[0], b->st_side[1]}) if (st) cudaStreamDestroy(st);
+	delete b;  // the buffers free themselves, after the synchronize above
 	(void)cudaGetLastError();
-	delete b;
 }
 
 const char *jsmpeg_b200_batch_last_error(jsmpeg_b200_batch_t *b) { return (b && b->dead) ? b->error.c_str() : nullptr; }
@@ -1551,8 +1480,8 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 			s.h_head = -1;
 			s.seq_floor = 0;
 			if (s.has_seq) {
-				for (auto p : s.d_planes) CUDA_CHECK(cudaMemsetAsync(p, 0, (size_t)s.coded_size * 3 / 2, b->st_main));
-				for (auto p : s.d_planes_b) if (p) CUDA_CHECK(cudaMemsetAsync(p, 0, (size_t)s.coded_size * 3 / 2, b->st_main));
+				for (auto &p : s.d_planes) CUDA_CHECK(cudaMemsetAsync(p.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_main));
+				for (auto &p : s.d_planes_b) if (p.data()) CUDA_CHECK(cudaMemsetAsync(p.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_main));
 			}
 		}
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
@@ -1646,7 +1575,7 @@ int jsmpeg_b200_batch_get_planes(jsmpeg_b200_batch_t *b, int stream, void **y, v
 	const Stream &s = b->streams[stream];
 	if (!s.has_seq) return -1;
 	// most recent picture = forward (mpeg1.c:841-851); with the B-picture extension it may be a B picture's own set
-	PlaneSet p = plane_set(s, s.d_last ? s.d_last : s.d_planes[1 - s.cur]);
+	PlaneSet p = plane_set(s, s.d_last ? s.d_last : s.d_planes[1 - s.cur].data());
 	if (y) *y = p.y;
 	if (cr) *cr = p.cr;
 	if (cb) *cb = p.cb;
@@ -1656,7 +1585,7 @@ int jsmpeg_b200_batch_get_planes(jsmpeg_b200_batch_t *b, int stream, void **y, v
 int jsmpeg_b200_batch_get_host_planes(jsmpeg_b200_batch_t *b, int stream, void **y, void **cr, void **cb) {
 	const Stream &s = b->streams[stream];
 	if (!s.has_seq) return -1;
-	PlaneSet p = plane_set(s, s.h_planes[s.h_head < 0 ? 0 : s.h_head]);
+	PlaneSet p = plane_set(s, s.h_planes[s.h_head < 0 ? 0 : s.h_head].data());
 	if (y) *y = p.y;
 	if (cr) *cr = p.cr;
 	if (cb) *cb = p.cb;
@@ -1665,8 +1594,8 @@ int jsmpeg_b200_batch_get_host_planes(jsmpeg_b200_batch_t *b, int stream, void *
 
 int jsmpeg_b200_batch_get_rgba(jsmpeg_b200_batch_t *b, int stream, void **rgba) {
 	const Stream &s = b->streams[stream];
-	if (!s.has_seq || !s.d_rgba) return -1;
-	*rgba = s.d_rgba;
+	if (!s.has_seq || !s.d_rgba.data()) return -1;
+	*rgba = s.d_rgba.data();
 	return 0;
 }
 
@@ -1675,7 +1604,7 @@ int jsmpeg_b200_batch_read_planes(jsmpeg_b200_batch_t *b, int stream, void *y, v
 		use_device(b);
 		const Stream &s = b->streams[stream];
 		if (!s.has_seq) return -1;
-		PlaneSet p = plane_set(s, s.d_last ? s.d_last : s.d_planes[1 - s.cur]);
+		PlaneSet p = plane_set(s, s.d_last ? s.d_last : s.d_planes[1 - s.cur].data());
 		if (y) CUDA_CHECK(cudaMemcpy(y, p.y, s.coded_size, cudaMemcpyDeviceToHost));
 		if (cr) CUDA_CHECK(cudaMemcpy(cr, p.cr, s.coded_size >> 2, cudaMemcpyDeviceToHost));
 		if (cb) CUDA_CHECK(cudaMemcpy(cb, p.cb, s.coded_size >> 2, cudaMemcpyDeviceToHost));
@@ -1689,7 +1618,7 @@ long jsmpeg_b200_batch_write_ts(jsmpeg_b200_batch_t *b, int stream, const uint8_
 	return guarded<long>(b, -1, [&]() -> long {
 		use_device(b);
 		Stream &s = b->streams[stream];
-		if (!b->ts) b->ts = ts_scratch_create();
+		if (!b->ts) b->ts.reset(ts_scratch_create());
 		if (s.ts_bound.empty()) s.ts_bound.assign(8192, 0);
 		// what the previous call left over comes first (a partial packet, a resync that wanted more data: ts.js:25-41)
 		const uint8_t *data = ts;
@@ -1700,14 +1629,14 @@ long jsmpeg_b200_batch_write_ts(jsmpeg_b200_batch_t *b, int stream, const uint8_
 			n_data = s.ts_leftover.size();
 		}
 		size_t consumed = 0;
-		const long total = ts_demux_measure(b->ts, data, n_data, stream_id, s.ts_bound.data(), &consumed, b->st_main);
+		const long total = ts_demux_measure(b->ts.get(), data, n_data, stream_id, s.ts_bound.data(), &consumed, b->st_main);
 		std::vector<uint8_t> rest(data + consumed, data + n_data);  // (data may alias ts_leftover)
 		s.ts_leftover.swap(rest);
 		if (total <= 0) return total;
 		b->stats.kernel_launches += 7;
 		b->stats.h2d_bytes += n_data;
 		return append_demuxed(b, s, (uint32_t)total, [&](uint32_t es_base) {
-			return ts_demux_gather(b->ts, s.d_es, es_base, pts_out, offset_out, n_max, b->st_main);
+			return ts_demux_gather(b->ts.get(), s.d_es.data(), es_base, pts_out, offset_out, n_max, b->st_main);
 		}, pts_out, offset_out, n_max, n_pes);
 	});
 }
@@ -1719,7 +1648,7 @@ long jsmpeg_b200_batch_write_ps(jsmpeg_b200_batch_t *b, int stream, const uint8_
 		if (stream_id < 0xE0 || stream_id > 0xEF) return -2;  // not a video stream id: the caller's mistake, nothing changes
 		use_device(b);
 		Stream &s = b->streams[stream];
-		if (!b->ps) b->ps = ps_scratch_create();
+		if (!b->ps) b->ps.reset(ps_scratch_create());
 		// what the previous call left over comes first: an unfinished item, or the tail that may begin a pack header
 		const uint8_t *data = ps;
 		size_t n_data = n_bytes;
@@ -1729,16 +1658,16 @@ long jsmpeg_b200_batch_write_ps(jsmpeg_b200_batch_t *b, int stream, const uint8_
 			n_data = s.ps_leftover.size();
 		}
 		size_t consumed = 0;
-		const long total = ps_demux_measure(b->ps, data, n_data, stream_id, &s.ps_in_sync, &consumed, b->st_main);
+		const long total = ps_demux_measure(b->ps.get(), data, n_data, stream_id, &s.ps_in_sync, &consumed, b->st_main);
 		std::vector<uint8_t> rest(data + consumed, data + n_data);  // (data may alias ps_leftover)
 		s.ps_leftover.swap(rest);
 		b->stats.h2d_bytes += n_data;
 		long r = total;
 		if (total > 0)
 			r = append_demuxed(b, s, (uint32_t)total, [&](uint32_t es_base) {
-				return ps_demux_gather(b->ps, s.d_es, es_base, pts_out, offset_out, n_max, b->st_main);
+				return ps_demux_gather(b->ps.get(), s.d_es.data(), es_base, pts_out, offset_out, n_max, b->st_main);
 			}, pts_out, offset_out, n_max, n_pes);
-		b->stats.kernel_launches += ps_demux_launches(b->ps);
+		b->stats.kernel_launches += ps_demux_launches(b->ps.get());
 		return r;
 	});
 }
@@ -1747,8 +1676,8 @@ int jsmpeg_b200_batch_read_rgba(jsmpeg_b200_batch_t *b, int stream, void *rgba) 
 	return guarded<int>(b, -1, [&] {
 		use_device(b);
 		const Stream &s = b->streams[stream];
-		if (!s.has_seq || !s.d_rgba) return -1;
-		CUDA_CHECK(cudaMemcpy(rgba, s.d_rgba, (size_t)s.width * s.height * 4, cudaMemcpyDeviceToHost));
+		if (!s.has_seq || !s.d_rgba.data()) return -1;
+		CUDA_CHECK(cudaMemcpy(rgba, s.d_rgba.data(), (size_t)s.width * s.height * 4, cudaMemcpyDeviceToHost));
 		return 0;
 	});
 }
@@ -1876,7 +1805,7 @@ long jsmpeg_b200_debug_read_es(jsmpeg_b200_batch_t *b, int stream, void *dst, si
 		use_device(b);
 		const Stream &s = b->streams[stream];
 		const size_t n = std::min<size_t>(cap, s.d_valid);
-		if (n) CUDA_CHECK(cudaMemcpy(dst, s.d_es, n, cudaMemcpyDeviceToHost));
+		if (n) CUDA_CHECK(cudaMemcpy(dst, s.d_es.data(), n, cudaMemcpyDeviceToHost));
 		return (long)s.d_valid;
 	});
 }
@@ -1892,40 +1821,39 @@ int jsmpeg_b200_debug_parse_picture(const uint8_t *es, uint32_t es_len, uint32_t
 		memcpy(sp.non_intra_q, non_intra_q, 64);
 		seq_fill_xq(sp);
 		const size_t n_mb = sp.mb_size;
-		uint8_t *d_es = dev_alloc<uint8_t>(es_len + ES_PAD);
-		SeqParams *d_seq = dev_alloc<SeqParams>(1);
-		mb_record_t *d_hdr = dev_alloc<mb_record_t>(n_mb);
-		int16_t *d_coef = dev_alloc<int16_t>(n_mb * MB_COEF_INT16);
-		uint2 *d_park = dev_alloc<uint2>(n_mb * 6);
-		uint4 *d_stage = dev_alloc<uint4>((size_t)stage_entries_for(sp.mb_size) * 4);
-		picture_info_t *d_info = dev_alloc<picture_info_t>(1);
-		ParseTask *d_task = dev_alloc<ParseTask>(1);
-		CUDA_CHECK(cudaMemcpy(d_es, es, es_len, cudaMemcpyHostToDevice));
-		CUDA_CHECK(cudaMemset(d_es + es_len, 0, ES_PAD));
-		CUDA_CHECK(cudaMemcpy(d_seq, &sp, sizeof(sp), cudaMemcpyHostToDevice));
-		CUDA_CHECK(cudaMemset(d_coef, 0, n_mb * MB_COEF_INT16 * sizeof(int16_t)));
+		DeviceBuffer<uint8_t> d_es(es_len + ES_PAD);
+		DeviceBuffer<SeqParams> d_seq(1);
+		DeviceBuffer<mb_record_t> d_hdr(n_mb);
+		DeviceBuffer<int16_t> d_coef(n_mb * MB_COEF_INT16);
+		DeviceBuffer<uint2> d_park(n_mb * 6);
+		DeviceBuffer<uint4> d_stage((size_t)stage_entries_for(sp.mb_size) * 4);
+		DeviceBuffer<picture_info_t> d_info(1);
+		DeviceBuffer<ParseTask> d_task(1);
+		CUDA_CHECK(cudaMemcpy(d_es.data(), es, es_len, cudaMemcpyHostToDevice));
+		CUDA_CHECK(cudaMemset(d_es.data() + es_len, 0, ES_PAD));
+		CUDA_CHECK(cudaMemcpy(d_seq.data(), &sp, sizeof(sp), cudaMemcpyHostToDevice));
+		CUDA_CHECK(cudaMemset(d_coef.data(), 0, n_mb * MB_COEF_INT16 * sizeof(int16_t)));
 		ParseTask t{};
-		t.es = d_es; t.es_len = es_len; t.start_byte = start_byte; t.seq = d_seq; t.hdr = d_hdr; t.coef = d_coef; t.info = d_info;
-		t.park = d_park; t.mb_width = mb_width; t.mb_size = sp.mb_size;
-		t.stage = d_stage; t.stage_entries = stage_entries_for(sp.mb_size);
+		t.es = d_es.data(); t.es_len = es_len; t.start_byte = start_byte; t.seq = d_seq.data(); t.hdr = d_hdr.data();
+		t.coef = d_coef.data(); t.info = d_info.data(); t.park = d_park.data(); t.mb_width = mb_width; t.mb_size = sp.mb_size;
+		t.stage = d_stage.data(); t.stage_entries = stage_entries_for(sp.mb_size);
 		t.codes = nullptr; t.n_codes = 0; t.code_hint = 0;  // this hook lets the walk search the slice end itself
-		CUDA_CHECK(cudaMemcpy(d_task, &t, sizeof(t), cudaMemcpyHostToDevice));
-		launch_parse_pictures(d_task, 1, sp.mb_size, true, 0);
+		CUDA_CHECK(cudaMemcpy(d_task.data(), &t, sizeof(t), cudaMemcpyHostToDevice));
+		launch_parse_pictures(d_task.data(), 1, sp.mb_size, true, 0);
 		CUDA_CHECK(cudaGetLastError());
 		CUDA_CHECK(cudaDeviceSynchronize());
-		CUDA_CHECK(cudaMemcpy(info_out, d_info, sizeof(picture_info_t), cudaMemcpyDeviceToHost));
-		CUDA_CHECK(cudaMemcpy(hdr_out, d_hdr, n_mb * sizeof(mb_record_t), cudaMemcpyDeviceToHost));
-		CUDA_CHECK(cudaMemcpy(coef_out, d_coef, n_mb * MB_COEF_INT16 * sizeof(int16_t), cudaMemcpyDeviceToHost));
+		CUDA_CHECK(cudaMemcpy(info_out, d_info.data(), sizeof(picture_info_t), cudaMemcpyDeviceToHost));
+		CUDA_CHECK(cudaMemcpy(hdr_out, d_hdr.data(), n_mb * sizeof(mb_record_t), cudaMemcpyDeviceToHost));
+		CUDA_CHECK(cudaMemcpy(coef_out, d_coef.data(), n_mb * MB_COEF_INT16 * sizeof(int16_t), cudaMemcpyDeviceToHost));
 		// stage 1b left most blocks as compact records in the staging area: the caller gets them dense
 		std::vector<coef_record_t> compact(n_mb * 6);
-		CUDA_CHECK(cudaMemcpy(compact.data(), d_stage, compact.size() * sizeof(coef_record_t), cudaMemcpyDeviceToHost));
+		CUDA_CHECK(cudaMemcpy(compact.data(), d_stage.data(), compact.size() * sizeof(coef_record_t), cudaMemcpyDeviceToHost));
 		const mb_record_t *hdr = static_cast<const mb_record_t *>(hdr_out);
 		for (size_t slot = 0; slot < n_mb * 6; slot++) {
 			const mb_record_t &r = hdr[slot / 6];
 			if ((r.flags & MBF_PRESENT) && (r.cbp & (0x20 >> (slot % 6))) && compact[slot].mask != COEF_RECORD_DENSE)
 				coef_record_unpack(compact[slot], static_cast<int16_t *>(coef_out) + slot * 64);
 		}
-		cudaFree(d_es); cudaFree(d_seq); cudaFree(d_hdr); cudaFree(d_coef); cudaFree(d_park); cudaFree(d_stage); cudaFree(d_info); cudaFree(d_task);
 		return 0;
 	} catch (const std::exception &e) {
 		fprintf(stderr, "%s\n", e.what());
@@ -1939,8 +1867,8 @@ int jsmpeg_b200_debug_reconstruct(int mb_width, int mb_height, const void *hdr, 
 	try {
 		const size_t n_mb = (size_t)mb_width * mb_height;
 		const size_t ysz = n_mb * 256, csz = ysz / 4, total = ysz + 2 * csz;
-		mb_record_t *d_hdr = dev_alloc<mb_record_t>(n_mb);
-		int16_t *d_coef = dev_alloc<int16_t>(n_mb * MB_COEF_INT16);
+		DeviceBuffer<mb_record_t> d_hdr(n_mb);
+		DeviceBuffer<int16_t> d_coef(n_mb * MB_COEF_INT16);
 		// the caller's dense blocks as stage 1b would hand them over: compact records where they fit
 		std::vector<coef_record_t> compact(n_mb * 6);
 		for (size_t slot = 0; slot < n_mb * 6; slot++) {
@@ -1949,13 +1877,14 @@ int jsmpeg_b200_debug_reconstruct(int mb_width, int mb_height, const void *hdr, 
 			if (coef_record_fits(pos)) compact[slot] = coef_record_pack(pos, blk);
 			else compact[slot].mask = COEF_RECORD_DENSE;
 		}
-		coef_record_t *d_compact = dev_alloc<coef_record_t>(n_mb * 6);
-		CUDA_CHECK(cudaMemcpy(d_compact, compact.data(), compact.size() * sizeof(coef_record_t), cudaMemcpyHostToDevice));
+		DeviceBuffer<coef_record_t> d_compact(n_mb * 6);
+		CUDA_CHECK(cudaMemcpy(d_compact.data(), compact.data(), compact.size() * sizeof(coef_record_t), cudaMemcpyHostToDevice));
 		const size_t pad = (size_t)mb_width * 16 + 64;
-		uint8_t *d_fwd = dev_alloc<uint8_t>(total + pad), *d_cur = dev_alloc<uint8_t>(total + pad);
+		DeviceBuffer<uint8_t> fwd_buf(total + pad), cur_buf(total + pad);
+		uint8_t *d_fwd = fwd_buf.data(), *d_cur = cur_buf.data();
 		CUDA_CHECK(cudaMemset(d_fwd + total, 0, pad));
-		CUDA_CHECK(cudaMemcpy(d_hdr, hdr, n_mb * sizeof(mb_record_t), cudaMemcpyHostToDevice));
-		CUDA_CHECK(cudaMemcpy(d_coef, coef, n_mb * MB_COEF_INT16 * sizeof(int16_t), cudaMemcpyHostToDevice));
+		CUDA_CHECK(cudaMemcpy(d_hdr.data(), hdr, n_mb * sizeof(mb_record_t), cudaMemcpyHostToDevice));
+		CUDA_CHECK(cudaMemcpy(d_coef.data(), coef, n_mb * MB_COEF_INT16 * sizeof(int16_t), cudaMemcpyHostToDevice));
 		CUDA_CHECK(cudaMemcpy(d_fwd, fwd_y, ysz, cudaMemcpyHostToDevice));
 		CUDA_CHECK(cudaMemcpy(d_fwd + ysz, fwd_cr, csz, cudaMemcpyHostToDevice));
 		CUDA_CHECK(cudaMemcpy(d_fwd + ysz + csz, fwd_cb, csz, cudaMemcpyHostToDevice));
@@ -1963,7 +1892,7 @@ int jsmpeg_b200_debug_reconstruct(int mb_width, int mb_height, const void *hdr, 
 		CUDA_CHECK(cudaMemcpy(d_cur + ysz, cur_cr, csz, cudaMemcpyHostToDevice));
 		CUDA_CHECK(cudaMemcpy(d_cur + ysz + csz, cur_cb, csz, cudaMemcpyHostToDevice));
 		ReconTask t{};
-		t.hdr = d_hdr; t.coef = d_coef; t.compact = d_compact;
+		t.hdr = d_hdr.data(); t.coef = d_coef.data(); t.compact = d_compact.data();
 		t.cur = PlaneSet{d_cur, d_cur + ysz, d_cur + ysz + csz};
 		t.fwd = PlaneSet{d_fwd, d_fwd + ysz, d_fwd + ysz + csz};
 		t.mb_width = mb_width; t.mb_size = (int)n_mb;
@@ -1974,7 +1903,6 @@ int jsmpeg_b200_debug_reconstruct(int mb_width, int mb_height, const void *hdr, 
 		CUDA_CHECK(cudaMemcpy(cur_y, d_cur, ysz, cudaMemcpyDeviceToHost));
 		CUDA_CHECK(cudaMemcpy(cur_cr, d_cur + ysz, csz, cudaMemcpyDeviceToHost));
 		CUDA_CHECK(cudaMemcpy(cur_cb, d_cur + ysz + csz, csz, cudaMemcpyDeviceToHost));
-		cudaFree(d_hdr); cudaFree(d_coef); cudaFree(d_compact); cudaFree(d_fwd); cudaFree(d_cur);
 		return 0;
 	} catch (const std::exception &e) {
 		fprintf(stderr, "%s\n", e.what());

@@ -22,6 +22,7 @@
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
+#include "buffers.h"
 #include "common.cuh"
 #include "psdemux.cuh"
 
@@ -163,46 +164,33 @@ __global__ void ps_gather_kernel(const uint8_t *__restrict__ buf, uint32_t m, co
 }  // namespace
 
 struct PsScratch {
-	uint8_t *buf = nullptr, *marked = nullptr;
-	size_t buf_cap = 0;
-	uint32_t *scan_pos = nullptr, *scan_count = nullptr, *sel = nullptr, *sel_count = nullptr, *pos = nullptr;
-	uint32_t scan_cap = 0;
-	ScanSpan *span = nullptr;
-	uint32_t *jump = nullptr;  // (levels + 1) x cap
-	uint2 *term = nullptr;
-	uint32_t *rev = nullptr, *next_pack_rev = nullptr, *ctl = nullptr;
-	uint32_t *src = nullptr, *lens = nullptr, *offsets = nullptr;
-	uint64_t *pts = nullptr;
-	uint32_t *pes_count = nullptr, *pes_offset = nullptr;
-	uint64_t *pes_pts = nullptr;
-	uint8_t *temp = nullptr;  // cub's temporary storage
-	size_t temp_bytes = 0, cap = 0;
+	DeviceBuffer<uint8_t> buf, marked;
+	DeviceBuffer<uint32_t> scan_pos, scan_count, sel, sel_count, pos;
+	DeviceBuffer<ScanSpan> span;
+	DeviceBuffer<uint32_t> jump;  // (levels + 1) x cap
+	DeviceBuffer<uint2> term;
+	DeviceBuffer<uint32_t> rev, next_pack_rev, ctl;
+	DeviceBuffer<uint32_t> src, lens, offsets;
+	DeviceBuffer<uint64_t> pts;
+	DeviceBuffer<uint32_t> pes_count, pes_offset;
+	DeviceBuffer<uint64_t> pes_pts;
+	DeviceBuffer<uint8_t> temp;  // cub's temporary storage
+	size_t cap = 0;  // candidates the per-candidate arrays have room for
 	int levels = 0;
 	uint32_t m = 0, launches = 0;
 };
 
-template <typename T>
-static void ps_realloc(T *&p, size_t n) {
-	if (p) CUDA_CHECK(cudaFree(p));
-	p = nullptr;
-	CUDA_CHECK(cudaMalloc(&p, (n ? n : 1) * sizeof(T)));
-}
-
 // room for `need` bytes of cub's temporary storage
 static void *ps_temp(PsScratch &s, size_t need) {
-	if (need > s.temp_bytes) {
-		ps_realloc(s.temp, need);
-		s.temp_bytes = need;
-	}
-	return s.temp;
+	s.temp.reserve(need);
+	return s.temp.data();
 }
 
 static void ps_reserve_scan(PsScratch &s, uint32_t n) {
-	if (n <= s.scan_cap) return;
+	if (n <= s.scan_pos.size()) return;
 	const uint32_t cap = n + n / 4 + 64;
-	ps_realloc(s.scan_pos, cap);
-	ps_realloc(s.sel, cap);
-	s.scan_cap = cap;
+	s.scan_pos.reserve(cap);
+	s.sel.reserve(cap);
 }
 
 static void ps_reserve(PsScratch &s, size_t m) {
@@ -211,30 +199,24 @@ static void ps_reserve(PsScratch &s, size_t m) {
 	if (m <= s.cap && levels <= s.levels) return;
 	const size_t cap = m + m / 4 + 64;
 	while ((size_t(1) << levels) < cap) levels++;
-	ps_realloc(s.pos, cap);
-	ps_realloc(s.jump, (size_t)(levels + 1) * cap);
-	ps_realloc(s.term, cap);
-	ps_realloc(s.rev, cap);
-	ps_realloc(s.next_pack_rev, cap);
-	ps_realloc(s.marked, cap);
-	ps_realloc(s.src, cap);
-	ps_realloc(s.lens, cap + 1);
-	ps_realloc(s.offsets, cap + 1);
-	ps_realloc(s.pts, cap);
-	ps_realloc(s.pes_offset, cap);
-	ps_realloc(s.pes_pts, cap);
+	s.pos.reserve(cap);
+	s.jump.reserve((size_t)(levels + 1) * cap);
+	s.term.reserve(cap);
+	s.rev.reserve(cap);
+	s.next_pack_rev.reserve(cap);
+	s.marked.reserve(cap);
+	s.src.reserve(cap);
+	s.lens.reserve(cap + 1);
+	s.offsets.reserve(cap + 1);
+	s.pts.reserve(cap);
+	s.pes_offset.reserve(cap);
+	s.pes_pts.reserve(cap);
 	s.cap = cap;
 	s.levels = levels;
 }
 
 PsScratch *ps_scratch_create() { return new PsScratch(); }
-void ps_scratch_destroy(PsScratch *s) {
-	if (!s) return;
-	void *all[] = {s->buf, s->marked, s->scan_pos, s->scan_count, s->sel, s->sel_count, s->pos, s->span, s->jump, s->term, s->rev,
-	               s->next_pack_rev, s->ctl, s->src, s->lens, s->offsets, s->pts, s->pes_count, s->pes_offset, s->pes_pts, s->temp};
-	for (void *p : all) if (p) cudaFree(p);
-	delete s;
-}
+void ps_scratch_destroy(PsScratch *s) { delete s; }
 
 // Phase 1: upload, candidates, chain, classify, scan.  *in_sync in/out: does the buffer continue the chain of
 // the previous call at its first byte?  Returns the ES byte count; *consumed = the bytes of the buffer the
@@ -246,42 +228,37 @@ long ps_demux_measure(PsScratch *s, const uint8_t *host, size_t n_bytes, int str
 	if (n_bytes == 0) return 0;
 	if (n_bytes > 0xfffff000ull) throw std::runtime_error("jsmpeg_b200: program stream buffer of 4 GiB or more");
 	const uint32_t n = (uint32_t)n_bytes;
-	if (n_bytes + 32 > s->buf_cap) {  // the scan reads 16-byte vectors and a look-ahead word
-		const size_t cap = n_bytes + n_bytes / 4 + 32;
-		ps_realloc(s->buf, cap);
-		s->buf_cap = cap;
-	}
-	if (!s->span) {
-		ps_realloc(s->span, 1);
-		ps_realloc(s->scan_count, 1);
-		ps_realloc(s->sel_count, 1);
-		ps_realloc(s->ctl, 3);
-		ps_realloc(s->pes_count, 1);
-	}
-	CUDA_CHECK(cudaMemcpyAsync(s->buf, host, n_bytes, cudaMemcpyHostToDevice, st));
-	CUDA_CHECK(cudaMemsetAsync(s->buf + n_bytes, 0, 32, st));
-	const ScanSpan span{s->buf, 0, n};
-	CUDA_CHECK(cudaMemcpyAsync(s->span, &span, sizeof(span), cudaMemcpyHostToDevice, st));
+	// the scan reads 16-byte vectors and a look-ahead word
+	if (n_bytes + 32 > s->buf.size()) s->buf.reserve(n_bytes + n_bytes / 4 + 32);
+	s->span.reserve(1);
+	s->scan_count.reserve(1);
+	s->sel_count.reserve(1);
+	s->ctl.reserve(3);
+	s->pes_count.reserve(1);
+	CUDA_CHECK(cudaMemcpyAsync(s->buf.data(), host, n_bytes, cudaMemcpyHostToDevice, st));
+	CUDA_CHECK(cudaMemsetAsync(s->buf.data() + n_bytes, 0, 32, st));
+	const ScanSpan span{s->buf.data(), 0, n};
+	CUDA_CHECK(cudaMemcpyAsync(s->span.data(), &span, sizeof(span), cudaMemcpyHostToDevice, st));
 	// candidates: every 00 00 01 (a scan that ran out of room counts on: rescan with room for all)
 	ps_reserve_scan(*s, n / 256 + 1024);
 	uint32_t hits = 0;
 	for (;;) {
-		CUDA_CHECK(cudaMemsetAsync(s->scan_count, 0, sizeof(uint32_t), st));
-		launch_scan_start_codes(s->span, 1, n, s->scan_pos, s->scan_cap, s->scan_count, st);
+		CUDA_CHECK(cudaMemsetAsync(s->scan_count.data(), 0, sizeof(uint32_t), st));
+		launch_scan_start_codes(s->span.data(), 1, n, s->scan_pos.data(), (uint32_t)s->scan_pos.size(), s->scan_count.data(), st);
 		s->launches++;
-		CUDA_CHECK(cudaMemcpyAsync(&hits, s->scan_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+		CUDA_CHECK(cudaMemcpyAsync(&hits, s->scan_count.data(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 		CUDA_CHECK(cudaStreamSynchronize(st));
-		if (hits <= s->scan_cap) break;
+		if (hits <= s->scan_pos.size()) break;
 		ps_reserve_scan(*s, hits);
 	}
 	ps_reserve(*s, hits);
 	uint32_t m = 0;
 	if (hits) {
-		const KeepCode keep{s->buf, n};
+		const KeepCode keep{s->buf.data(), n};
 		size_t bytes = 0;
-		cub::DeviceSelect::If(nullptr, bytes, s->scan_pos, s->sel, s->sel_count, (int)hits, keep, st);
-		cub::DeviceSelect::If(ps_temp(*s, bytes), bytes, s->scan_pos, s->sel, s->sel_count, (int)hits, keep, st);
-		CUDA_CHECK(cudaMemcpyAsync(&m, s->sel_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+		cub::DeviceSelect::If(nullptr, bytes, s->scan_pos.data(), s->sel.data(), s->sel_count.data(), (int)hits, keep, st);
+		cub::DeviceSelect::If(ps_temp(*s, bytes), bytes, s->scan_pos.data(), s->sel.data(), s->sel_count.data(), (int)hits, keep, st);
+		CUDA_CHECK(cudaMemcpyAsync(&m, s->sel_count.data(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 		CUDA_CHECK(cudaStreamSynchronize(st));
 		s->launches++;
 	}
@@ -289,37 +266,37 @@ long ps_demux_measure(PsScratch *s, const uint8_t *host, size_t n_bytes, int str
 		int bits = 1;
 		while (bits < 32 && (1ull << bits) <= n) bits++;
 		size_t bytes = 0;
-		cub::DeviceRadixSort::SortKeys(nullptr, bytes, s->sel, s->pos, (int)m, 0, bits, st);
-		cub::DeviceRadixSort::SortKeys(ps_temp(*s, bytes), bytes, s->sel, s->pos, (int)m, 0, bits, st);
+		cub::DeviceRadixSort::SortKeys(nullptr, bytes, s->sel.data(), s->pos.data(), (int)m, 0, bits, st);
+		cub::DeviceRadixSort::SortKeys(ps_temp(*s, bytes), bytes, s->sel.data(), s->pos.data(), (int)m, 0, bits, st);
 		s->launches++;
 	}
 	const int block = 256;
 	const int grid = (int)((m + block - 1) / block);
 	int levels = 1;
 	while ((1u << levels) < m) levels++;
-	uint32_t *jtop = s->jump + (size_t)levels * s->cap;
+	uint32_t *jtop = s->jump.data() + (size_t)levels * s->cap;
 	if (m) {
-		ps_link_kernel<<<grid, block, 0, st>>>(s->buf, n, s->pos, m, s->jump, s->term, s->rev);
+		ps_link_kernel<<<grid, block, 0, st>>>(s->buf.data(), n, s->pos.data(), m, s->jump.data(), s->term.data(), s->rev.data());
 		size_t bytes = 0;
-		cub::DeviceScan::InclusiveScan(nullptr, bytes, s->rev, s->next_pack_rev, MinOp(), (int)m, st);
-		cub::DeviceScan::InclusiveScan(ps_temp(*s, bytes), bytes, s->rev, s->next_pack_rev, MinOp(), (int)m, st);
+		cub::DeviceScan::InclusiveScan(nullptr, bytes, s->rev.data(), s->next_pack_rev.data(), MinOp(), (int)m, st);
+		cub::DeviceScan::InclusiveScan(ps_temp(*s, bytes), bytes, s->rev.data(), s->next_pack_rev.data(), MinOp(), (int)m, st);
 		for (int k = 0; k < levels; k++)
-			ps_double_kernel<<<grid, block, 0, st>>>(s->jump + (size_t)k * s->cap, s->jump + (size_t)(k + 1) * s->cap, m);
-		CUDA_CHECK(cudaMemsetAsync(s->marked, 0, m, st));
+			ps_double_kernel<<<grid, block, 0, st>>>(s->jump.data() + (size_t)k * s->cap, s->jump.data() + (size_t)(k + 1) * s->cap, m);
+		CUDA_CHECK(cudaMemsetAsync(s->marked.data(), 0, m, st));
 		s->launches += 2 + levels;
 	}
 	// the chain, one round per break
 	uint32_t from = *in_sync ? NONE : 0;
 	uint32_t ctl[3] = {NONE, T_NOHEAD, 0};
 	for (;;) {
-		ps_head_kernel<<<1, 1, 0, st>>>(s->buf, n, s->pos, m, s->next_pack_rev, from, s->ctl, s->marked);
+		ps_head_kernel<<<1, 1, 0, st>>>(s->buf.data(), n, s->pos.data(), m, s->next_pack_rev.data(), from, s->ctl.data(), s->marked.data());
 		if (m) {
-			for (int k = levels; k >= 0; k--) ps_mark_kernel<<<grid, block, 0, st>>>(s->jump + (size_t)k * s->cap, m, s->marked);
-			ps_end_kernel<<<1, 1, 0, st>>>(jtop, s->term, s->ctl);
+			for (int k = levels; k >= 0; k--) ps_mark_kernel<<<grid, block, 0, st>>>(s->jump.data() + (size_t)k * s->cap, m, s->marked.data());
+			ps_end_kernel<<<1, 1, 0, st>>>(jtop, s->term.data(), s->ctl.data());
 			s->launches += levels + 2;
 		}
 		s->launches++;
-		CUDA_CHECK(cudaMemcpyAsync(ctl, s->ctl, sizeof(ctl), cudaMemcpyDeviceToHost, st));
+		CUDA_CHECK(cudaMemcpyAsync(ctl, s->ctl.data(), sizeof(ctl), cudaMemcpyDeviceToHost, st));
 		CUDA_CHECK(cudaStreamSynchronize(st));
 		if (ctl[1] != T_BREAK) break;
 		from = ctl[2] + 1;
@@ -332,14 +309,14 @@ long ps_demux_measure(PsScratch *s, const uint8_t *host, size_t n_bytes, int str
 			*in_sync = false;
 	}
 	if (m == 0) return 0;
-	ps_classify_kernel<<<grid, block, 0, st>>>(s->buf, n, s->pos, m, s->marked, stream_id, s->src, s->lens, s->pts);
-	CUDA_CHECK(cudaMemsetAsync(s->lens + m, 0, sizeof(uint32_t), st));
+	ps_classify_kernel<<<grid, block, 0, st>>>(s->buf.data(), n, s->pos.data(), m, s->marked.data(), stream_id, s->src.data(), s->lens.data(), s->pts.data());
+	CUDA_CHECK(cudaMemsetAsync(s->lens.data() + m, 0, sizeof(uint32_t), st));
 	size_t bytes = 0;
-	cub::DeviceScan::ExclusiveSum(nullptr, bytes, s->lens, s->offsets, (int)(m + 1), st);
-	cub::DeviceScan::ExclusiveSum(ps_temp(*s, bytes), bytes, s->lens, s->offsets, (int)(m + 1), st);
+	cub::DeviceScan::ExclusiveSum(nullptr, bytes, s->lens.data(), s->offsets.data(), (int)(m + 1), st);
+	cub::DeviceScan::ExclusiveSum(ps_temp(*s, bytes), bytes, s->lens.data(), s->offsets.data(), (int)(m + 1), st);
 	s->launches += 2;
 	uint32_t total = 0;
-	CUDA_CHECK(cudaMemcpyAsync(&total, s->offsets + m, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+	CUDA_CHECK(cudaMemcpyAsync(&total, s->offsets.data() + m, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 	CUDA_CHECK(cudaStreamSynchronize(st));
 	s->m = m;
 	return (long)total;
@@ -348,17 +325,17 @@ long ps_demux_measure(PsScratch *s, const uint8_t *host, size_t n_bytes, int str
 // Phase 2: gather into es[es_base ...]; returns the PES count, lists copied to the host arrays.
 int ps_demux_gather(PsScratch *s, uint8_t *es, uint32_t es_base, uint64_t *pts_out, uint32_t *offset_out, int n_max, cudaStream_t st) {
 	if (s->m == 0) return 0;
-	CUDA_CHECK(cudaMemsetAsync(s->pes_count, 0, sizeof(uint32_t), st));
-	ps_gather_kernel<<<s->m, 128, 0, st>>>(s->buf, s->m, s->src, s->lens, s->offsets, s->pts, es, es_base, s->pes_count,
-	                                       s->pes_offset, s->pes_pts);
+	CUDA_CHECK(cudaMemsetAsync(s->pes_count.data(), 0, sizeof(uint32_t), st));
+	ps_gather_kernel<<<s->m, 128, 0, st>>>(s->buf.data(), s->m, s->src.data(), s->lens.data(), s->offsets.data(), s->pts.data(), es, es_base, s->pes_count.data(),
+	                                       s->pes_offset.data(), s->pes_pts.data());
 	s->launches++;
 	uint32_t count = 0;
-	CUDA_CHECK(cudaMemcpyAsync(&count, s->pes_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+	CUDA_CHECK(cudaMemcpyAsync(&count, s->pes_count.data(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 	CUDA_CHECK(cudaStreamSynchronize(st));
 	if (pts_out && offset_out && n_max > 0) {
 		const uint32_t k = count < (uint32_t)n_max ? count : (uint32_t)n_max;
-		CUDA_CHECK(cudaMemcpyAsync(pts_out, s->pes_pts, k * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-		CUDA_CHECK(cudaMemcpyAsync(offset_out, s->pes_offset, k * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+		CUDA_CHECK(cudaMemcpyAsync(pts_out, s->pes_pts.data(), k * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+		CUDA_CHECK(cudaMemcpyAsync(offset_out, s->pes_offset.data(), k * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 		CUDA_CHECK(cudaStreamSynchronize(st));
 	}
 	return (int)count;

@@ -29,6 +29,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
+#include "buffers.h"
 #include "common.cuh"
 
 namespace {
@@ -195,82 +196,61 @@ __global__ void ts_gather_kernel(const uint8_t *__restrict__ ts, const uint32_t 
 }  // namespace
 
 struct TsScratch {
-	uint8_t *ts = nullptr;
-	size_t ts_cap = 0;
-	uint32_t *grid = nullptr, *grid_out = nullptr;
-	PacketInfo *info = nullptr;
-	PacketUse *use = nullptr;
-	uint32_t *lens = nullptr, *offsets = nullptr;
-	uint8_t *is_pes = nullptr;
-	uint64_t *pts = nullptr;
-	uint64_t *ev_key = nullptr, *ev_key2 = nullptr;
-	uint32_t *ev_val = nullptr, *ev_val2 = nullptr, *ev_count = nullptr;
-	int16_t *bound = nullptr;
-	uint32_t *pes_count = nullptr, *pes_offset = nullptr;
-	uint64_t *pes_pts = nullptr;
-	int *misaligned = nullptr;
-	void *scan_temp = nullptr, *sort_temp = nullptr;
-	size_t scan_bytes = 0, sort_bytes = 0, n_cap = 0;
+	DeviceBuffer<uint8_t> ts;  // 16 bytes of slack past the packets
+	DeviceBuffer<uint32_t> grid, grid_out;
+	DeviceBuffer<PacketInfo> info;
+	DeviceBuffer<PacketUse> use;
+	DeviceBuffer<uint32_t> lens, offsets;
+	DeviceBuffer<uint8_t> is_pes;
+	DeviceBuffer<uint64_t> pts;
+	DeviceBuffer<uint64_t> ev_key, ev_key2;
+	DeviceBuffer<uint32_t> ev_val, ev_val2, ev_count;
+	DeviceBuffer<int16_t> bound;
+	DeviceBuffer<uint32_t> pes_count, pes_offset;
+	DeviceBuffer<uint64_t> pes_pts;
+	DeviceBuffer<int> misaligned;
+	DeviceBuffer<uint8_t> scan_temp, sort_temp;  // cub's temporary storage
+	size_t n_cap = 0;  // packets the per-packet arrays have room for
 	bool grid_in_use = false;
 	uint32_t n_packets = 0;
 };
 
 static void ts_reserve(TsScratch &s, size_t ts_bytes, size_t n) {
-	if (ts_bytes > s.ts_cap) {
-		if (s.ts) CUDA_CHECK(cudaFree(s.ts));
-		s.ts = nullptr;
-		s.ts_cap = 0;
-		CUDA_CHECK(cudaMalloc(&s.ts, ts_bytes + ts_bytes / 4 + 16));
-		s.ts_cap = ts_bytes + ts_bytes / 4;
-	}
-	if (!s.bound) {
-		CUDA_CHECK(cudaMalloc(&s.bound, 8192 * sizeof(int16_t)));
-		CUDA_CHECK(cudaMalloc(&s.misaligned, sizeof(int)));
-		CUDA_CHECK(cudaMalloc(&s.pes_count, sizeof(uint32_t)));
-		CUDA_CHECK(cudaMalloc(&s.ev_count, sizeof(uint32_t)));
-		CUDA_CHECK(cudaMalloc(&s.grid_out, 2 * sizeof(uint32_t)));
-	}
+	if (ts_bytes + 16 > s.ts.size()) s.ts.reserve(ts_bytes + ts_bytes / 4 + 16);
+	s.bound.reserve(8192);
+	s.misaligned.reserve(1);
+	s.pes_count.reserve(1);
+	s.ev_count.reserve(1);
+	s.grid_out.reserve(2);
 	if (n > s.n_cap) {
-		void *old[] = {s.grid, s.info, s.use, s.lens, s.offsets, s.is_pes, s.pts, s.ev_key, s.ev_key2, s.ev_val, s.ev_val2,
-		               s.pes_offset, s.pes_pts, s.scan_temp, s.sort_temp};
-		for (void *p : old) if (p) CUDA_CHECK(cudaFree(p));
-		s.grid = nullptr; s.info = nullptr; s.use = nullptr; s.lens = s.offsets = nullptr; s.is_pes = nullptr; s.pts = nullptr;
-		s.ev_key = s.ev_key2 = nullptr; s.ev_val = s.ev_val2 = nullptr; s.pes_offset = nullptr; s.pes_pts = nullptr;
-		s.scan_temp = s.sort_temp = nullptr;
-		s.n_cap = 0;
 		const size_t cap = n + n / 4 + 8;
 		const size_t ev_cap = cap + 8192;  // one event per packet at most, plus the carried bindings
-		CUDA_CHECK(cudaMalloc(&s.grid, cap * sizeof(uint32_t)));
-		CUDA_CHECK(cudaMalloc(&s.info, cap * sizeof(PacketInfo)));
-		CUDA_CHECK(cudaMalloc(&s.use, cap * sizeof(PacketUse)));
-		CUDA_CHECK(cudaMalloc(&s.lens, (cap + 1) * sizeof(uint32_t)));
-		CUDA_CHECK(cudaMalloc(&s.offsets, (cap + 1) * sizeof(uint32_t)));
-		CUDA_CHECK(cudaMalloc(&s.is_pes, cap));
-		CUDA_CHECK(cudaMalloc(&s.pts, cap * sizeof(uint64_t)));
-		CUDA_CHECK(cudaMalloc(&s.ev_key, ev_cap * sizeof(uint64_t)));
-		CUDA_CHECK(cudaMalloc(&s.ev_key2, ev_cap * sizeof(uint64_t)));
-		CUDA_CHECK(cudaMalloc(&s.ev_val, ev_cap * sizeof(uint32_t)));
-		CUDA_CHECK(cudaMalloc(&s.ev_val2, ev_cap * sizeof(uint32_t)));
-		CUDA_CHECK(cudaMalloc(&s.pes_offset, cap * sizeof(uint32_t)));
-		CUDA_CHECK(cudaMalloc(&s.pes_pts, cap * sizeof(uint64_t)));
-		s.scan_bytes = 0;
-		cub::DeviceScan::ExclusiveSum(nullptr, s.scan_bytes, s.lens, s.offsets, (int)(cap + 1));
-		CUDA_CHECK(cudaMalloc(&s.scan_temp, s.scan_bytes));
-		s.sort_bytes = 0;
-		cub::DeviceRadixSort::SortPairs(nullptr, s.sort_bytes, s.ev_key, s.ev_key2, s.ev_val, s.ev_val2, (int)ev_cap, 0, 45);
-		CUDA_CHECK(cudaMalloc(&s.sort_temp, s.sort_bytes));
+		s.grid.reserve(cap);
+		s.info.reserve(cap);
+		s.use.reserve(cap);
+		s.lens.reserve(cap + 1);
+		s.offsets.reserve(cap + 1);
+		s.is_pes.reserve(cap);
+		s.pts.reserve(cap);
+		s.ev_key.reserve(ev_cap);
+		s.ev_key2.reserve(ev_cap);
+		s.ev_val.reserve(ev_cap);
+		s.ev_val2.reserve(ev_cap);
+		s.pes_offset.reserve(cap);
+		s.pes_pts.reserve(cap);
+		size_t bytes = 0;
+		cub::DeviceScan::ExclusiveSum(nullptr, bytes, s.lens.data(), s.offsets.data(), (int)(cap + 1));
+		s.scan_temp.reserve(bytes);
+		bytes = 0;
+		cub::DeviceRadixSort::SortPairs(nullptr, bytes, s.ev_key.data(), s.ev_key2.data(), s.ev_val.data(), s.ev_val2.data(), (int)ev_cap,
+		                                0, 45);
+		s.sort_temp.reserve(bytes);
 		s.n_cap = cap;
 	}
 }
 
 TsScratch *ts_scratch_create() { return new TsScratch(); }
-void ts_scratch_destroy(TsScratch *s) {
-	if (!s) return;
-	void *all[] = {s->ts, s->grid, s->grid_out, s->info, s->use, s->lens, s->offsets, s->is_pes, s->pts, s->ev_key, s->ev_key2, s->ev_val,
-	               s->ev_val2, s->ev_count, s->bound, s->pes_count, s->pes_offset, s->pes_pts, s->misaligned, s->scan_temp, s->sort_temp};
-	for (void *p : all) if (p) cudaFree(p);
-	delete s;
-}
+void ts_scratch_destroy(TsScratch *s) { delete s; }
 
 // Phase 1: upload + grid + classify + bind + scan.  `bound` [8192]: the stream id every PID is bound to
 // (0 = none), in/out (pidsToStreamIds lives across write() calls, ts.js:9).  Returns the ES byte count;
@@ -283,21 +263,21 @@ long ts_demux_measure(TsScratch *s, const uint8_t *ts_host, size_t ts_bytes, int
 	const size_t n_max = ts_bytes / 188;
 	ts_reserve(*s, ts_bytes, n_max);
 	const uint32_t n = (uint32_t)ts_bytes;
-	CUDA_CHECK(cudaMemcpyAsync(s->ts, ts_host, ts_bytes, cudaMemcpyHostToDevice, st));
-	CUDA_CHECK(cudaMemsetAsync(s->misaligned, 0, sizeof(int), st));
-	CUDA_CHECK(cudaMemsetAsync(s->pes_count, 0, sizeof(uint32_t), st));
+	CUDA_CHECK(cudaMemcpyAsync(s->ts.data(), ts_host, ts_bytes, cudaMemcpyHostToDevice, st));
+	CUDA_CHECK(cudaMemsetAsync(s->misaligned.data(), 0, sizeof(int), st));
+	CUDA_CHECK(cudaMemsetAsync(s->pes_count.data(), 0, sizeof(uint32_t), st));
 	const int block = 256;
 	int grid_n = (int)((n_max + block - 1) / block);
-	ts_check_grid_kernel<<<grid_n, block, 0, st>>>(s->ts, (uint32_t)n_max, s->misaligned);
+	ts_check_grid_kernel<<<grid_n, block, 0, st>>>(s->ts.data(), (uint32_t)n_max, s->misaligned.data());
 	int misaligned = 0;
-	CUDA_CHECK(cudaMemcpyAsync(&misaligned, s->misaligned, sizeof(int), cudaMemcpyDeviceToHost, st));
+	CUDA_CHECK(cudaMemcpyAsync(&misaligned, s->misaligned.data(), sizeof(int), cudaMemcpyDeviceToHost, st));
 	CUDA_CHECK(cudaStreamSynchronize(st));
 	uint32_t n_packets = (uint32_t)n_max, stop = (uint32_t)(n_max * 188);
 	s->grid_in_use = misaligned != 0;
 	if (misaligned) {  // sync was lost somewhere: one warp walks the buffer the way the reference does
-		ts_walk_grid_kernel<<<1, 32, 0, st>>>(s->ts, n, s->grid, s->grid_out);
+		ts_walk_grid_kernel<<<1, 32, 0, st>>>(s->ts.data(), n, s->grid.data(), s->grid_out.data());
 		uint32_t out[2] = {0, 0};
-		CUDA_CHECK(cudaMemcpyAsync(out, s->grid_out, sizeof(out), cudaMemcpyDeviceToHost, st));
+		CUDA_CHECK(cudaMemcpyAsync(out, s->grid_out.data(), sizeof(out), cudaMemcpyDeviceToHost, st));
 		CUDA_CHECK(cudaStreamSynchronize(st));
 		n_packets = out[0];
 		stop = out[1];
@@ -305,7 +285,7 @@ long ts_demux_measure(TsScratch *s, const uint8_t *ts_host, size_t ts_bytes, int
 	*consumed = stop;
 	s->n_packets = n_packets;
 	if (n_packets == 0) return 0;
-	const uint32_t *grid = s->grid_in_use ? s->grid : nullptr;
+	const uint32_t *grid = s->grid_in_use ? s->grid.data() : nullptr;
 	// events: the carried bindings first (index 0 of their PID), then the PES headers of this buffer
 	static thread_local uint64_t carry_key[8192];
 	static thread_local uint32_t carry_val[8192];
@@ -313,38 +293,41 @@ long ts_demux_measure(TsScratch *s, const uint8_t *ts_host, size_t ts_bytes, int
 	for (uint32_t pid = 0; pid < 8192; pid++)
 		if (bound[pid]) { carry_key[n_carry] = (uint64_t)pid << 32; carry_val[n_carry] = (uint32_t)(uint16_t)bound[pid]; n_carry++; }
 	if (n_carry) {
-		CUDA_CHECK(cudaMemcpyAsync(s->ev_key, carry_key, n_carry * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-		CUDA_CHECK(cudaMemcpyAsync(s->ev_val, carry_val, n_carry * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+		CUDA_CHECK(cudaMemcpyAsync(s->ev_key.data(), carry_key, n_carry * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+		CUDA_CHECK(cudaMemcpyAsync(s->ev_val.data(), carry_val, n_carry * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
 	}
-	CUDA_CHECK(cudaMemcpyAsync(s->ev_count, &n_carry, sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+	CUDA_CHECK(cudaMemcpyAsync(s->ev_count.data(), &n_carry, sizeof(uint32_t), cudaMemcpyHostToDevice, st));
 	grid_n = (int)((n_packets + block - 1) / block);
-	ts_classify_kernel<<<grid_n, block, 0, st>>>(s->ts, n, grid, n_packets, s->info, s->pts, s->ev_key, s->ev_val, s->ev_count);
+	ts_classify_kernel<<<grid_n, block, 0, st>>>(s->ts.data(), n, grid, n_packets, s->info.data(), s->pts.data(), s->ev_key.data(),
+	                                             s->ev_val.data(), s->ev_count.data());
 	uint32_t n_events = 0;
-	CUDA_CHECK(cudaMemcpyAsync(&n_events, s->ev_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+	CUDA_CHECK(cudaMemcpyAsync(&n_events, s->ev_count.data(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 	CUDA_CHECK(cudaStreamSynchronize(st));  // (also: carry_key / carry_val / n_carry have been read)
-	const uint64_t *keys = s->ev_key;
-	const uint32_t *vals = s->ev_val;
+	const uint64_t *keys = s->ev_key.data();
+	const uint32_t *vals = s->ev_val.data();
 	if (n_events > 1) {
-		size_t bytes = s->sort_bytes;
-		cub::DeviceRadixSort::SortPairs(s->sort_temp, bytes, s->ev_key, s->ev_key2, s->ev_val, s->ev_val2, (int)n_events, 0, 45, st);
-		keys = s->ev_key2;
-		vals = s->ev_val2;
+		size_t bytes = s->sort_temp.size();
+		cub::DeviceRadixSort::SortPairs(s->sort_temp.data(), bytes, s->ev_key.data(), s->ev_key2.data(), s->ev_val.data(), s->ev_val2.data(),
+		                                (int)n_events, 0, 45, st);
+		keys = s->ev_key2.data();
+		vals = s->ev_val2.data();
 	}
-	ts_bind_kernel<<<grid_n, block, 0, st>>>(n_packets, s->info, keys, vals, n_events, stream_id, s->use, s->lens, s->is_pes);
+	ts_bind_kernel<<<grid_n, block, 0, st>>>(n_packets, s->info.data(), keys, vals, n_events, stream_id, s->use.data(), s->lens.data(),
+	                                         s->is_pes.data());
 	if (n_events) {
 		static thread_local int16_t host_bound[8192];
 		memcpy(host_bound, bound, sizeof(host_bound));
-		CUDA_CHECK(cudaMemcpyAsync(s->bound, host_bound, sizeof(host_bound), cudaMemcpyHostToDevice, st));
-		ts_carry_kernel<<<(int)((n_events + block - 1) / block), block, 0, st>>>(keys, vals, n_events, s->bound);
-		CUDA_CHECK(cudaMemcpyAsync(host_bound, s->bound, sizeof(host_bound), cudaMemcpyDeviceToHost, st));
+		CUDA_CHECK(cudaMemcpyAsync(s->bound.data(), host_bound, sizeof(host_bound), cudaMemcpyHostToDevice, st));
+		ts_carry_kernel<<<(int)((n_events + block - 1) / block), block, 0, st>>>(keys, vals, n_events, s->bound.data());
+		CUDA_CHECK(cudaMemcpyAsync(host_bound, s->bound.data(), sizeof(host_bound), cudaMemcpyDeviceToHost, st));
 		CUDA_CHECK(cudaStreamSynchronize(st));
 		memcpy(bound, host_bound, sizeof(host_bound));
 	}
-	CUDA_CHECK(cudaMemsetAsync(s->lens + n_packets, 0, sizeof(uint32_t), st));
-	size_t bytes = s->scan_bytes;
-	cub::DeviceScan::ExclusiveSum(s->scan_temp, bytes, s->lens, s->offsets, (int)(n_packets + 1), st);
+	CUDA_CHECK(cudaMemsetAsync(s->lens.data() + n_packets, 0, sizeof(uint32_t), st));
+	size_t bytes = s->scan_temp.size();
+	cub::DeviceScan::ExclusiveSum(s->scan_temp.data(), bytes, s->lens.data(), s->offsets.data(), (int)(n_packets + 1), st);
 	uint32_t total = 0;
-	CUDA_CHECK(cudaMemcpyAsync(&total, s->offsets + n_packets, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+	CUDA_CHECK(cudaMemcpyAsync(&total, s->offsets.data() + n_packets, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 	CUDA_CHECK(cudaStreamSynchronize(st));
 	return (long)total;
 }
@@ -355,15 +338,16 @@ int ts_demux_gather(TsScratch *s, uint8_t *es, uint32_t es_base, uint64_t *pts_o
 	if (n == 0) return 0;
 	const int block = 256;
 	const int grid = (int)((n * 32 + block - 1) / block);
-	ts_gather_kernel<<<grid, block, 0, st>>>(s->ts, s->grid_in_use ? s->grid : nullptr, (uint32_t)n, s->use, s->offsets, s->is_pes, s->pts,
-	                                         es, es_base, s->pes_count, (uint32_t)s->n_cap, s->pes_offset, s->pes_pts);
+	ts_gather_kernel<<<grid, block, 0, st>>>(s->ts.data(), s->grid_in_use ? s->grid.data() : nullptr, (uint32_t)n, s->use.data(),
+	                                         s->offsets.data(), s->is_pes.data(), s->pts.data(), es, es_base, s->pes_count.data(),
+	                                         (uint32_t)s->n_cap, s->pes_offset.data(), s->pes_pts.data());
 	uint32_t count = 0;
-	CUDA_CHECK(cudaMemcpyAsync(&count, s->pes_count, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+	CUDA_CHECK(cudaMemcpyAsync(&count, s->pes_count.data(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 	CUDA_CHECK(cudaStreamSynchronize(st));
 	if (pts_out && offset_out && n_max > 0) {
 		const uint32_t m = count < (uint32_t)n_max ? count : (uint32_t)n_max;
-		CUDA_CHECK(cudaMemcpyAsync(pts_out, s->pes_pts, m * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-		CUDA_CHECK(cudaMemcpyAsync(offset_out, s->pes_offset, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+		CUDA_CHECK(cudaMemcpyAsync(pts_out, s->pes_pts.data(), m * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+		CUDA_CHECK(cudaMemcpyAsync(offset_out, s->pes_offset.data(), m * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 		CUDA_CHECK(cudaStreamSynchronize(st));
 	}
 	return (int)count;
