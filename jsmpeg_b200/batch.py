@@ -258,18 +258,21 @@ class BatchDecoder:
         """The I pictures of `stream` that decode_intra can decode now (include/jsmpeg_b200.h): one dict per picture,
         {"picture": k, "byte_pos", "temporal_reference", "pts"}.  `pts` (seconds) is that of the last PES packet
         write_ts / write_ps reported at or before the picture's start code (src/decoder.js:36-47), or None."""
-        n = self.lib.jsmpeg_b200_batch_intra_index(self.handle, stream, None, None, None, 0)
+        return self._index(self.lib.jsmpeg_b200_batch_intra_index, stream,
+                           [("picture", np.uint32), ("byte_pos", np.uint32), ("temporal_reference", np.int32)])
+
+    def _index(self, fn, stream, fields):
+        """The index `fn` (jsmpeg_b200_batch_*_index) of `stream`: one dict per picture with the (key, dtype) `fields`
+        in the order of fn's output arrays ("picture" and "byte_pos" first), then "pts"."""
+        n = fn(self.handle, stream, *[None] * len(fields), 0)
         if n == -2:
             raise ValueError(f"stream {stream} out of range")
         if n < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_intra_index failed")
-        pic, pos, tr = np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.int32)
-        n = self.lib.jsmpeg_b200_batch_intra_index(self.handle, stream, pic.ctypes.data, pos.ctypes.data, tr.ctypes.data, n)
-        out = []
-        for i in range(min(n, len(pic))):
-            out.append({"picture": int(pic[i]), "byte_pos": int(pos[i]), "temporal_reference": int(tr[i]),
-                        "pts": self._pts(stream, int(pos[i]))})
-        return out
+            raise RuntimeError(self.last_error() or f"{fn.__name__} failed")
+        arrays = [np.zeros(n, dtype) for _, dtype in fields]
+        n = fn(self.handle, stream, *[a.ctypes.data for a in arrays], n)
+        return [{**{key: int(a[i]) for (key, _), a in zip(fields, arrays)}, "pts": self._pts(stream, int(arrays[1][i]))}
+                for i in range(min(n, len(arrays[0])))]
 
     def _pts(self, stream, byte_pos):
         """PTS (seconds) of the last PES packet write_ts / write_ps reported at or before `byte_pos`, or None."""
@@ -281,17 +284,9 @@ class BatchDecoder:
         """The pictures of `stream` that decode_pictures can decode now (include/jsmpeg_b200.h): one dict per picture,
         {"picture": k, "byte_pos", "type" (picture_coding_type), "temporal_reference", "chain_start", "pts"}; `pts`
         as in intra_index.  Follows the decode_b option's current value."""
-        n = self.lib.jsmpeg_b200_batch_picture_index(self.handle, stream, None, None, None, None, None, 0)
-        if n == -2:
-            raise ValueError(f"stream {stream} out of range")
-        if n < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_picture_index failed")
-        pic, pos, start = np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.uint32)
-        kind, tr = np.zeros(n, np.int32), np.zeros(n, np.int32)
-        n = self.lib.jsmpeg_b200_batch_picture_index(self.handle, stream, pic.ctypes.data, pos.ctypes.data,
-                                                     kind.ctypes.data, tr.ctypes.data, start.ctypes.data, n)
-        return [{"picture": int(pic[i]), "byte_pos": int(pos[i]), "type": int(kind[i]), "temporal_reference": int(tr[i]),
-                 "chain_start": int(start[i]), "pts": self._pts(stream, int(pos[i]))} for i in range(min(n, len(pic)))]
+        return self._index(self.lib.jsmpeg_b200_batch_picture_index, stream,
+                           [("picture", np.uint32), ("byte_pos", np.uint32), ("type", np.int32),
+                            ("temporal_reference", np.int32), ("chain_start", np.uint32)])
 
     def decode_pictures(self, requests, rgba=False):
         """Decode pictures listed by picture_index, of any streams, in one call: `requests` is an iterable of (stream,
@@ -318,16 +313,9 @@ class BatchDecoder:
         """The pictures of `stream` that decode_macroblocks can describe now (include/jsmpeg_b200.h): one dict per
         picture, {"picture": k, "byte_pos", "type" (picture_coding_type), "temporal_reference", "pts"}; `pts` as in
         intra_index.  B pictures are listed whatever the decode_b option says."""
-        n = self.lib.jsmpeg_b200_batch_macroblock_index(self.handle, stream, None, None, None, None, 0)
-        if n == -2:
-            raise ValueError(f"stream {stream} out of range")
-        if n < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_macroblock_index failed")
-        pic, pos, kind, tr = np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros(n, np.int32), np.zeros(n, np.int32)
-        n = self.lib.jsmpeg_b200_batch_macroblock_index(self.handle, stream, pic.ctypes.data, pos.ctypes.data,
-                                                        kind.ctypes.data, tr.ctypes.data, n)
-        return [{"picture": int(pic[i]), "byte_pos": int(pos[i]), "type": int(kind[i]), "temporal_reference": int(tr[i]),
-                 "pts": self._pts(stream, int(pos[i]))} for i in range(min(n, len(pic)))]
+        return self._index(self.lib.jsmpeg_b200_batch_macroblock_index, stream,
+                           [("picture", np.uint32), ("byte_pos", np.uint32), ("type", np.int32),
+                            ("temporal_reference", np.int32)])
 
     def decode_macroblocks(self, requests):
         """Macroblock types and motion vectors of pictures listed by macroblock_index, of any streams, in one call:
@@ -340,14 +328,9 @@ class BatchDecoder:
         n = len(reqs)
         shapes = {}  # per stream: (mb_height, mb_width)
         for s, _ in reqs:
-            if s in shapes:
-                continue
-            if not 0 <= s < self.n_streams:
-                raise ValueError(f"stream {s} out of range")
-            info = self.stream_info(s)
-            if not info["has_sequence_header"]:
-                raise ValueError(f"stream {s} has no sequence header yet")
-            shapes[s] = ((info["height"] + 15) // 16, (info["width"] + 15) // 16)
+            if s not in shapes:
+                info = self._request_stream_info(s)
+                shapes[s] = ((info["height"] + 15) // 16, (info["width"] + 15) // 16)
         dev = torch.device("cuda", self.device)
         by_shape = {}  # per picture size: the requests of that size
         for i, (s, _) in enumerate(reqs):
@@ -371,6 +354,15 @@ class BatchDecoder:
         self.last_macroblocks_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
         return out
 
+    def _request_stream_info(self, s):
+        """stream_info of the stream a request names; ValueError unless it is in range and has a sequence header."""
+        if not 0 <= s < self.n_streams:
+            raise ValueError(f"stream {s} out of range")
+        info = self.stream_info(s)
+        if not info["has_sequence_header"]:
+            raise ValueError(f"stream {s} has no sequence header yet")
+        return info
+
     def _decode_requests(self, fn, reqs, rgba, extra_out, refused):
         """Allocate the destinations of (stream, picture) requests and call `fn` (decode_intra / decode_pictures) with
         `extra_out` before n_present and error.  Returns (outputs, n_present, errors)."""
@@ -379,11 +371,7 @@ class BatchDecoder:
         dev = torch.device("cuda", self.device)
         planes, images = [], []
         for s, _ in reqs:
-            if not 0 <= s < self.n_streams:
-                raise ValueError(f"stream {s} out of range")
-            info = self.stream_info(s)
-            if not info["has_sequence_header"]:
-                raise ValueError(f"stream {s} has no sequence header yet")
+            info = self._request_stream_info(s)
             planes.append(torch.empty(info["coded_size"] * 3 // 2, dtype=torch.uint8, device=dev))
             if rgba:
                 images.append(torch.empty((info["height"], info["width"], 4), dtype=torch.uint8, device=dev))

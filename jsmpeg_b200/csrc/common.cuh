@@ -124,26 +124,24 @@ struct ParseFork {
 	cudaStream_t side[PARSE_GROUPS];
 	cudaEvent_t fork, join[PARSE_GROUPS];
 };
-// Stage 1 of I/P pictures: a walk + an expand launch per size group (one group without `fork`); walk_done, unless
-// nullptr, is recorded behind the first group's walk.  expand = false: the walk alone (macroblock records without
-// coefficients), in one group.  Returns the number of kernels launched.
-int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream,
-                          cudaEvent_t walk_done = nullptr, const ParseFork *fork = nullptr);
-// Stage 2.  `tasks_host` is read on the host at launch time: the table travels in the kernel parameters.  Each
-// launcher returns the number of kernels it launched.
-int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
-// the same with the planar -> RGBA conversion fused in (tasks' rgba / width / height)
-int launch_reconstruct_rgba(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
-// B pictures (every task has `bwd`): prediction from two references; `rgba` = with the fused conversion
-int launch_reconstruct_b(const ReconTask *tasks_host, int n_tasks, bool rgba, cudaStream_t stream);
-// stage 1 for B pictures: the serial walk with the B-picture macroblock layer (walk_b.cuh) + the same expand unless
-// `expand` is false; returns the number of kernels launched
-int launch_parse_pictures_b(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream);
-// stage 1 for I/P pictures of many slices (opt-in, walk_slices.cuh): a lane per slice + the same expand unless
-// `expand` is false; returns the number of kernels launched
-int launch_parse_pictures_slices(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream);
-// the host routes an I/P picture to it when it has at least this many slices
+// The walk kernels of stage 1a, in the order a wave launches them:
+//   WALK_LANES   I/P pictures: the lane-parallel walk (walk.cuh), or with JSMPEG_B200_WALK=serial the serial walk
+//   WALK_SLICES  I/P pictures of many slices (opt-in "slice_walk", walk_slices.cuh): a lane per slice
+//   WALK_B       B pictures (opt-in "decode_b", walk_b.cuh): the serial walk with the B-picture macroblock layer
+enum WalkKind { WALK_LANES, WALK_SLICES, WALK_B, N_WALK_KINDS };
+// the host routes an I/P picture to the slice walk when it has at least this many slices
 constexpr int SLICE_WALK_MIN_SLICES = 4;
+// Stage 1 of n_tasks pictures of walk kernel `kind`: the walk + the expand, or with expand = false the walk alone
+// (macroblock records without coefficients).  A WALK_LANES wave with expand and `fork` is cut into size groups, a walk
+// + an expand launch per group; every other call is one group.  walk_done, unless nullptr, is recorded behind the first
+// group's walk.  Returns the number of kernels launched.
+int launch_parse_pictures(WalkKind kind, const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand,
+                          cudaStream_t stream, cudaEvent_t walk_done = nullptr, const ParseFork *fork = nullptr);
+// Stage 2 of n_tasks pictures, by kernel: I/P pictures, then I/P pictures with the planar -> RGBA conversion fused in
+// (tasks with `rgba`), then B pictures (tasks with `bwd`: prediction from two references), then B pictures with the
+// conversion; each kernel's tasks in their order.  `tasks_host` is read on the host at launch time: the table travels
+// in the kernel parameters.  Returns the number of kernels launched.
+int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
 
 // Macroblock export (macroblocks.cu): request i converts the records of one picture (`mb_size` of them at `src`, a
 // picture of picture_coding_type `picture_type`) into the public jsmpeg_b200_macroblock_t layout at `dst`; `first` is

@@ -23,7 +23,7 @@
 // Pipeline.  decode() and decode_pictures / decode_intra share it.  A round plans its pictures, parses
 // them in one stage-1 wave (parse_wave: walk + expand per walk kernel, the kernels beside each other on
 // side streams) and waits for the picture infos; the host then consumes them in decode() order and
-// queues one reconstruct step per picture depth (ReconStep, launch_step) on the reconstruct stream.
+// queues one reconstruct step per picture depth (ReconStep, launch_reconstruct) on the reconstruct stream.
 // Cutting the wave into chunks to overlap stage 1 with stage 2 was measured not to pay (DESIGN 8).
 // decode_macroblocks runs the same waves walk-only (no expand, no reconstruct) and exports the records (DESIGN 3.8).
 #include <sched.h>
@@ -221,15 +221,21 @@ void *stream_get_write_ptr(Batch *b, Stream &s, uint32_t n) {
 	return p;
 }
 
-// MSB-first reader for the (tiny, once-per-stream) sequence header on the host
+// MSB-first reader for the headers the host reads itself (sequence header, picture headers); bytes beyond `len` read
+// as 0, as they do to the walks
 struct HostBits {
 	const uint8_t *p;
-	uint32_t len, idx;
-	uint32_t read(int n) {
+	uint32_t len;
+	uint64_t idx;
+	uint32_t read(int n) {  // n <= 32
 		uint32_t v = 0;
-		for (int i = 0; i < n; i++, idx++) {
-			uint32_t byte = idx >> 3;
-			v = (v << 1) | (byte < len ? (p[byte] >> (7 - (idx & 7))) & 1u : 0u);
+		while (n > 0) {  // the bits of one byte at a time
+			const uint64_t byte = idx >> 3;
+			const int left = 8 - (int)(idx & 7), take = n < left ? n : left;
+			const uint32_t bits = byte < len ? p[byte] : 0u;
+			v = v << take | ((bits >> (left - take)) & ((1u << take) - 1u));
+			idx += take;
+			n -= take;
 		}
 		return v;
 	}
@@ -257,9 +263,9 @@ void parse_sequence_header(Batch *b, Stream &s, uint32_t bit_index) {
 	if (hb.read(1)) { for (int i = 0; i < 64; i++) s.seq.non_intra_q[kZigZag[i]] = (uint8_t)hb.read(8); }
 	else memset(s.seq.non_intra_q, 16, 64);
 	seq_fill_xq(s.seq);
-	s.bb.index = hb.idx;
-	s.seq_end_index = hb.idx;
-	s.seq_floor = (hb.idx + 7) >> 3;  // where decode() starts looking for the first picture
+	s.bb.index = (uint32_t)hb.idx;
+	s.seq_end_index = (uint32_t)hb.idx;
+	s.seq_floor = (uint32_t)((hb.idx + 7) >> 3);  // where decode() starts looking for the first picture
 	s.seq.mb_width = (s.width + 15) >> 4;
 	s.seq.mb_height = (s.height + 15) >> 4;
 	s.seq.mb_size = s.seq.mb_width * s.seq.mb_height;
@@ -545,28 +551,18 @@ void copy_batch(Batch *b, std::vector<void *> &dst, std::vector<void *> &src, st
 		for (size_t i = 0; i < n_copy; i++) CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], size[i], cudaMemcpyDefault, st));
 }
 
-// The reconstruct launches of one step of decode() (or one depth of decode_chains), by kernel: I/P and B pictures,
-// each without and with the fused RGBA conversion; and the copies of its pictures that follow them
+// The reconstruct tasks of one step of decode() (or one depth of decode_chains), queued by launch_reconstruct; and
+// the copies of its pictures that follow them
 struct ReconStep {
-	std::vector<ReconTask> ip, ip_rgba, bi, bi_rgba;
+	std::vector<ReconTask> tasks;
 	std::vector<void *> dst, src;
 	std::vector<size_t> size;
-	void add(const ReconTask &t) { (t.bwd.y ? (t.rgba ? bi_rgba : bi) : (t.rgba ? ip_rgba : ip)).push_back(t); }
 	void copy(void *to, void *from, size_t n) {
 		dst.push_back(to);
 		src.push_back(from);
 		size.push_back(n);
 	}
 };
-
-// Queues a step's reconstruct launches on `st`; returns the number of kernels launched
-int launch_step(const ReconStep &r, cudaStream_t st) {
-	int n = launch_reconstruct(r.ip.data(), (int)r.ip.size(), st);
-	n += launch_reconstruct_rgba(r.ip_rgba.data(), (int)r.ip_rgba.size(), st);
-	n += launch_reconstruct_b(r.bi.data(), (int)r.bi.size(), false, st);
-	n += launch_reconstruct_b(r.bi_rgba.data(), (int)r.bi_rgba.size(), true, st);
-	return n;
-}
 
 // The copy-out of one step's pictures (OUT_HOST) on the copy stream, behind the step's launches
 void copy_out_step(Batch *b, ReconStep &r) {
@@ -577,19 +573,27 @@ void copy_out_step(Batch *b, ReconStep &r) {
 	b->copy_steps++;
 }
 
-// picture_coding_type of picture `pic` of a stream (ISO 11172-2 2.4.2.5: 10 bits temporal_reference, 3 bits
-// picture_coding_type); 0 while its header byte is not in the buffer yet
-int picture_type_of(const Stream &s, uint32_t pic) {
-	const uint32_t pos = s.pics[pic];
-	return (uint64_t)pos + 5 < s.bb.length ? (s.bb.bytes[pos + 5] >> 3) & 7 : 0;
+// The header of the picture whose start code is at byte `pos` (ISO 11172-2 2.4.2.5); fields whose bytes are not in the
+// buffer yet read as 0
+struct PictureHeader {
+	int temporal_reference, type;  // type: picture_coding_type
+	int full_pel_forward, forward_f_code, full_pel_backward, backward_f_code;
+};
+PictureHeader picture_header(const Stream &s, uint32_t pos) {
+	// the 40 bits after the start code: temporal_reference 10, picture_coding_type 3, vbv_delay 16,
+	// full_pel_forward_vector 1, forward_f_code 3, full_pel_backward_vector 1, backward_f_code 3 (and one more).
+	// (Read as two words: decode() reads a header per picture.)
+	HostBits hb{s.bb.bytes, s.bb.length, ((uint64_t)pos + 4) * 8};
+	const uint64_t w = (uint64_t)hb.read(32) << 8 | hb.read(8);
+	auto field = [w](int first, int n) { return (int)(w >> (40 - first - n)) & ((1 << n) - 1); };
+	return {field(0, 10), field(10, 3), field(29, 1), field(30, 3), field(33, 1), field(34, 3)};
 }
 
-// Which walk kernel takes picture `pic` of a stream: 0 the lane-parallel walk, 1 the slice walk, 2 the B-picture walk.
-// b_walk: a type 3 picture goes to the B-picture walk (decode() and decode_pictures: the decode_b option); everything
-// else, and everything without it, to the I/P walk
-int walk_kind(const Batch *b, const Stream &s, uint32_t pic, bool b_walk) {
-	const int type = picture_type_of(s, pic);
-	int kind = (b_walk && type == 3) ? 2 : 0;
+// Which walk kernel takes picture `pic` of a stream.  b_walk: a type 3 picture goes to the B-picture walk (decode() and
+// decode_pictures: the decode_b option); everything else, and everything without it, to an I/P walk
+WalkKind walk_kind(const Batch *b, const Stream &s, uint32_t pic, bool b_walk) {
+	const int type = picture_header(s, s.pics[pic]).type;
+	WalkKind kind = (b_walk && type == 3) ? WALK_B : WALK_LANES;
 	if (b->slice_walk && (type == 1 || type == 2)) {  // enough slice start codes between this picture's and the next one's?
 		const uint32_t hi = pic + 1 < s.pic_code.size() ? s.pic_code[pic + 1] : (uint32_t)s.codes.size();
 		int n_slices = 0;
@@ -597,7 +601,7 @@ int walk_kind(const Batch *b, const Stream &s, uint32_t pic, bool b_walk) {
 			const uint32_t q = s.codes[k];
 			if (q + 3u < s.bb.length && s.bb.bytes[q + 3u] >= 0x01 && s.bb.bytes[q + 3u] <= 0xAF) n_slices++;
 		}
-		if (n_slices >= SLICE_WALK_MIN_SLICES) kind = 1;
+		if (n_slices >= SLICE_WALK_MIN_SLICES) kind = WALK_SLICES;
 	}
 	return kind;
 }
@@ -630,9 +634,26 @@ struct WaveItem {
 	int stream;
 	uint32_t pic;
 	int slot;
-	int kind;
+	WalkKind kind;
 	uint32_t bytes;
 };
+
+// Picture `pic` of stream `si` as an item of a stage-1 wave, in a record slot it takes from the free ones; b_walk as in
+// walk_kind
+WaveItem take_slot(Batch *b, int si, uint32_t pic, bool b_walk) {
+	const Stream &s = b->streams[si];
+	const int slot = b->free_slots.back();
+	b->free_slots.pop_back();
+	const uint32_t end = pic + 1 < s.pics.size() ? s.pics[pic + 1] : s.bb.length;
+	return {si, pic, slot, walk_kind(b, s, pic, b_walk), end - s.pics[pic]};
+}
+
+// Frees the look-ahead's record slots too when the free ones do not cover `need` pictures (decode() parses the
+// look-ahead again)
+void free_slots_for(Batch *b, size_t need) {
+	if (b->free_slots.size() < need)
+		for (auto &s : b->streams) flush_cache(b, s);
+}
 
 // Stage 1 of `wave` as one wave, for decode(), decode_chains and decode_macroblocks alike; expand = false runs the walks
 // alone (records without coefficients: decode_macroblocks).  The tasks are grouped by walk kernel and,
@@ -650,7 +671,7 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 		return wave[x].kind != wave[y].kind ? wave[x].kind < wave[y].kind : wave[x].bytes > wave[y].bytes;
 	});
 	ensure_task_caps(b, n);
-	int cnt[3] = {0, 0, 0};
+	int cnt[N_WALK_KINDS] = {};
 	for (int j = 0; j < n; j++) {
 		const WaveItem &w = wave[order[j]];
 		b->h_ptasks[j] = parse_task(b, w.stream, w.pic, w.slot, order[j]);
@@ -665,19 +686,17 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 	int primary = 0;
 	while (cnt[primary] == 0) primary++;
 	if (cnt[primary] < n) CUDA_CHECK(cudaEventRecord(b->ev_sfork, b->st_main));
-	// the wave's pictures by walk kernel: [0, cnt[0]) lane-parallel walk, then the slice walk's, then the B pictures
-	const int off[3] = {0, cnt[0], cnt[0] + cnt[1]};
+	// the wave's pictures by walk kernel, in WalkKind order
 	int launches = 0, n_side = 0;
-	for (int kind = 0; kind < 3; kind++) {
+	for (int kind = 0, off = 0; kind < N_WALK_KINDS; off += cnt[kind++]) {
 		if (cnt[kind] == 0) continue;
 		cudaStream_t st = b->st_main;
 		if (kind != primary) {
 			st = b->st_side[n_side];
 			CUDA_CHECK(cudaStreamWaitEvent(st, b->ev_sfork, 0));
 		}
-		if (kind == 0) launches += launch_parse_pictures(b->d_ptasks.data(), cnt[0], b->slot_mb, expand, st, b->ev_mid, &b->fork);
-		else if (kind == 1) launches += launch_parse_pictures_slices(b->d_ptasks.data() + off[1], cnt[1], b->slot_mb, expand, st);
-		else launches += launch_parse_pictures_b(b->d_ptasks.data() + off[2], cnt[2], b->slot_mb, expand, st);
+		launches += launch_parse_pictures((WalkKind)kind, b->d_ptasks.data() + off, cnt[kind], b->slot_mb, expand, st,
+		                                  kind == WALK_LANES ? b->ev_mid : nullptr, &b->fork);
 		if (kind != primary) {
 			CUDA_CHECK(cudaEventRecord(b->ev_sjoin[n_side], st));
 			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_sjoin[n_side], 0));
@@ -685,7 +704,7 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 		}
 	}
 	CUDA_CHECK(cudaMemcpyAsync(b->h_info.data(), b->d_info.data(), n * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
-	if (cnt[0] == 0) CUDA_CHECK(cudaEventRecord(b->ev_mid, b->st_main));  // (a wave without the lane-parallel walk)
+	if (cnt[WALK_LANES] == 0) CUDA_CHECK(cudaEventRecord(b->ev_mid, b->st_main));  // (a wave without the lane-parallel walk)
 	CUDA_CHECK(cudaEventRecord(b->ev_b, b->st_main));
 	CUDA_CHECK(cudaEventSynchronize(b->ev_b));
 	return launches;
@@ -739,15 +758,12 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 		auto next = it + (ptrdiff_t)s.cache.size();
 		// `it` may be end(); cache is then empty
 		while ((int)s.cache.size() < target && next < s.pics.end() && !b->free_slots.empty()) {
+			wave.push_back(take_slot(b, si, (uint32_t)(next - s.pics.begin()), b->decode_b));
 			Parsed p{};
-			p.pos = *next;
+			p.pos = *next++;
 			p.len_at_parse = s.bb.length;
-			p.slot = b->free_slots.back();
-			b->free_slots.pop_back();
+			p.slot = wave.back().slot;
 			s.cache.push_back(p);
-			++next;
-			const uint32_t pic = (uint32_t)(next - 1 - s.pics.begin());
-			wave.push_back({si, pic, p.slot, walk_kind(b, s, pic, b->decode_b), (next < s.pics.end() ? *next : s.bb.length) - p.pos});
 		}
 	}
 	// ---- 2. stage 1: the wave, every picture's info on the host before consumption starts
@@ -795,7 +811,8 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			b->stats.pictures++;
 			b->stats.es_bytes += (e.info.end_bit >> 3) - e.pos;
 			s.last_type = e.info.picture_type;
-			s.last_temporal = (uint64_t)e.pos + 5 < s.bb.length ? (s.bb.bytes[e.pos + 4] << 2 | s.bb.bytes[e.pos + 5] >> 6) : 0;
+			// (0 unless both of its bytes are in the buffer)
+			s.last_temporal = (uint64_t)e.pos + 5 < s.bb.length ? picture_header(s, e.pos).temporal_reference : 0;
 			if (e.info.status == PIC_DECODED) {
 				const bool is_b = e.info.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
 				uint8_t *rgba = nullptr;
@@ -826,7 +843,7 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 				s.d_last = t.cur.y;
 				const uint64_t planes = (uint64_t)s.coded_size * 3 / 2;
 				if (steps.size() <= step) steps.emplace_back();
-				steps[step].add(t);
+				steps[step].tasks.push_back(t);
 				if (flags & JSMPEG_B200_OUT_HOST) {  // into the next slot of the stream's host ring
 					s.h_head = (s.h_head + 1) % HOST_RING;
 					steps[step].copy(s.h_planes[s.h_head].data(), t.cur.y, planes);
@@ -851,7 +868,7 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			// (the copy stream is in order, so that covers every earlier one).
 			if ((flags & JSMPEG_B200_OUT_HOST) && b->copy_steps >= 2)
 				CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_copied[b->copy_steps & 1], 0));
-			b->stats.kernel_launches += launch_step(r, b->st_recon);
+			b->stats.kernel_launches += launch_reconstruct(r.tasks.data(), (int)r.tasks.size(), b->st_recon);
 			b->stats.recon_launches++;
 			if (flags & JSMPEG_B200_OUT_HOST) copy_out_step(b, r);  // while the next step reconstructs
 		}
@@ -915,46 +932,31 @@ bool picture_closed(const Stream &s, uint32_t k) {
 	return false;
 }
 
+// Whether the walks decode a picture (PIC_DECODED), by their rule (walk.cuh, walk_b.cuh): an I picture, a P picture with
+// forward_f_code != 0, and when B pictures go to the B walk (b_walk) a B picture with both f_codes != 0
+bool picture_decoded(const PictureHeader &h, bool b_walk) {
+	if (h.type == 1) return true;
+	if (h.type == 2) return h.forward_f_code != 0;
+	return h.type == 3 && b_walk && h.forward_f_code != 0 && h.backward_f_code != 0;
+}
+
 // An entry of an index: picture `pic` (an index into s.pics) and its chain start
 struct IndexEntry {
 	uint32_t pic, chain_start;
 };
 
-// The pictures decode_intra can decode now: after the first sequence header, picture_coding_type 1, and closed.  Each
-// is its own chain start.
-std::vector<IndexEntry> intra_index(const Stream &s) {
-	std::vector<IndexEntry> out;
-	if (!s.has_seq) return out;
-	for (uint32_t k = 0; k < s.pics.size(); k++)
-		if (s.pics[k] >= s.seq_floor && picture_type_of(s, k) == 1 && picture_closed(s, k)) out.push_back({k, k});
-	return out;
-}
+// The random-access calls, by the index each serves
+enum class Listing {
+	Intra,        // decode_intra: the I pictures, each its own chain start
+	Pictures,     // decode_pictures: the pictures decode() reconstructs under the current decode_b, with a chain start
+	Macroblocks,  // decode_macroblocks: B pictures whatever decode_b says, no chain start needed (a picture's
+	              // macroblock layer depends on its own bits only)
+};
 
-// `n` bits of picture `pic`'s header, from bit `bit` after its start code (ISO 11172-2 2.4.2.5: temporal_reference 10,
-// picture_coding_type 3, vbv_delay 16, full_pel_forward_vector 1, forward_f_code 3, full_pel_backward_vector 1,
-// backward_f_code 3).  Bytes beyond the buffer read as 0, as they do to the walks.
-uint32_t picture_header_bits(const Stream &s, uint32_t pic, int bit, int n) {
-	uint32_t v = 0;
-	for (int i = 0; i < n; i++, bit++) {
-		const uint64_t byte = (uint64_t)s.pics[pic] + 4 + (bit >> 3);
-		v = v << 1 | (byte < s.bb.length ? (s.bb.bytes[byte] >> (7 - (bit & 7))) & 1u : 0u);
-	}
-	return v;
-}
-
-// Whether the walks decode picture k (PIC_DECODED), by their rule (walk.cuh, walk_b.cuh): an I picture, a P picture with
-// forward_f_code != 0, and when B pictures go to the B walk (decode_b) a B picture with both f_codes != 0
-bool picture_decoded(const Stream &s, uint32_t k, bool decode_b) {
-	const int type = picture_type_of(s, k);
-	if (type == 1) return true;
-	if (type == 2) return picture_header_bits(s, k, 30, 3) != 0;
-	return type == 3 && decode_b && picture_header_bits(s, k, 30, 3) != 0 && picture_header_bits(s, k, 34, 3) != 0;
-}
-
-// The pictures decode_pictures can decode now: after the first sequence header, closed, reconstructed by decode(),
-// and with a chain start -- the greatest picture j <= k of the intra index such that at least r(k) pictures of
+// The pictures a random-access call can serve now: after the first sequence header, closed, decoded by the walks, and
+// with a chain start where the call needs one -- the greatest I picture j <= k such that at least r(k) pictures of
 // [j, k) are references (I, or P with forward_f_code != 0); r = 0 for I, 1 for P, 2 for B.
-std::vector<IndexEntry> picture_index(const Batch *b, const Stream &s) {
+std::vector<IndexEntry> list_pictures(const Batch *b, const Stream &s, Listing what) {
 	std::vector<IndexEntry> out;
 	if (!s.has_seq) return out;
 	std::vector<uint32_t> keys;      // the I pictures after the sequence header so far
@@ -962,12 +964,17 @@ std::vector<IndexEntry> picture_index(const Batch *b, const Stream &s) {
 	uint32_t refs = 0;
 	for (uint32_t k = 0; k < s.pics.size(); k++) {
 		refs_upto.push_back(refs);
-		const int type = picture_type_of(s, k);
+		const PictureHeader h = picture_header(s, s.pics[k]);
 		const bool after = s.pics[k] >= s.seq_floor;
-		if (after && type == 1) keys.push_back(k);
-		refs += type == 1 || (type == 2 && picture_header_bits(s, k, 30, 3) != 0);
-		if (!after || !picture_decoded(s, k, b->decode_b) || !picture_closed(s, k)) continue;
-		const uint32_t need = type == 1 ? 0 : type - 1;
+		if (after && h.type == 1) keys.push_back(k);
+		refs += h.type == 1 || (h.type == 2 && h.forward_f_code != 0);
+		const bool listed = what == Listing::Intra ? h.type == 1 : picture_decoded(h, what == Listing::Macroblocks || b->decode_b);
+		if (!after || !listed || !picture_closed(s, k)) continue;
+		if (what == Listing::Macroblocks) {
+			out.push_back({k, k});
+			continue;
+		}
+		const uint32_t need = h.type == 1 ? 0 : h.type - 1;
 		// (every key is a reference: this looks at most three keys back)
 		for (auto j = keys.rbegin(); j != keys.rend(); ++j)
 			if (refs_upto[k] - refs_upto[*j] >= need) {
@@ -977,6 +984,23 @@ std::vector<IndexEntry> picture_index(const Batch *b, const Stream &s) {
 	}
 	return out;
 }
+
+// What a random-access call reports per request (picture_info_t's status, n_present and error)
+struct RequestInfo {
+	std::vector<int32_t> status, n_present, error;
+	explicit RequestInfo(int n) : status(n, 0), n_present(n, 0), error(n, 0) {}
+	void set(int i, const picture_info_t &e) {
+		status[i] = e.status;
+		n_present[i] = e.n_present;
+		error[i] = e.error;
+	}
+	// into the caller's arrays, those that are not nullptr
+	void copy_out(int32_t *status_out, int32_t *n_present_out, int32_t *error_out) const {
+		if (status_out) std::copy(status.begin(), status.end(), status_out);
+		if (n_present_out) std::copy(n_present.begin(), n_present.end(), n_present_out);
+		if (error_out) std::copy(error.begin(), error.end(), error_out);
+	}
+};
 
 // One request: picture `pic` of stream `stream`, decoded by a fresh decoder from picture `from` (its chain start) on
 struct PictureRequest {
@@ -1025,7 +1049,7 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 		c.first = c.next = r.from;
 		c.last = req[order[hi - 1]].pic;
 		for (int i = lo; i < hi; i++)
-			if (picture_type_of(s, req[order[i]].pic) == 3) c.b_end = req[order[i]].pic + 1;
+			if (picture_header(s, s.pics[req[order[i]].pic]).type == 3) c.b_end = req[order[i]].pic + 1;
 		c.req_lo = c.req_next = lo;
 		c.req_hi = hi;
 		c.n_sets = c.last == c.first ? 0 : (c.b_end ? 4 : 2);
@@ -1052,10 +1076,8 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 			if (c.n_sets == 0) CUDA_CHECK(cudaMemsetAsync(planes_dst[i], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
 			if (rgba) CUDA_CHECK(cudaMemsetAsync(rgba_dst[i], 0xff, (size_t)s.width * s.height * 4, b->st_recon));
 		}
-	std::vector<int32_t> status(n, 0), n_present(n, 0), error(n, 0);
-	// record slots: the free ones; when they do not cover the call, the look-ahead's too (decode() parses those again)
-	if (b->free_slots.size() < n_tasks)
-		for (auto &s : b->streams) flush_cache(b, s);
+	RequestInfo out(n);
+	free_slots_for(b, n_tasks);
 	const int wave_max = (int)b->free_slots.size();
 	// chain groups: at most wave_max chains (a wave parses at least one picture of each), and plane sets within half
 	// of the free device memory -- a request beyond the device is cut into groups, not refused
@@ -1089,13 +1111,9 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 			for (size_t c = glo; c < ghi; c++) {
 				Chain &ch = chains[c];
 				if (ch.next > ch.last) continue;
-				const Stream &s = b->streams[ch.stream];
 				for (uint32_t p = ch.first + lo; p <= ch.last && p - ch.first < lo + width; p++) {
-					const uint32_t end = p + 1 < s.pics.size() ? s.pics[p + 1] : s.bb.length;
-					const int slot = b->free_slots.back();
-					b->free_slots.pop_back();
-					ch.slot[p - ch.first] = slot;
-					wave.push_back({ch.stream, p, slot, walk_kind(b, s, p, b->decode_b), end - s.pics[p]});
+					wave.push_back(take_slot(b, ch.stream, p, b->decode_b));
+					ch.slot[p - ch.first] = wave.back().slot;
 					wave_chain.push_back((int)c);
 				}
 			}
@@ -1119,11 +1137,7 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 					const int q_lo = ch.req_next;
 					while (ch.req_next < ch.req_hi && req[order[ch.req_next]].pic == k) ch.req_next++;
 					const int q_hi = ch.req_next;
-					for (int q = q_lo; q < q_hi; q++) {
-						status[order[q]] = e.status;
-						n_present[order[q]] = e.n_present;
-						error[order[q]] = e.error;
-					}
+					for (int q = q_lo; q < q_hi; q++) out.set(order[q], e);
 					const bool is_b = e.picture_type == 3;  // (only the B walk answers PIC_DECODED for one)
 					if (e.status == PIC_DECODED && (!is_b || k < ch.b_end)) {
 						const int slot = ch.slot[k - ch.first];
@@ -1138,7 +1152,7 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 							t = recon_task(b, s, slot, ch.set[ch.cur], ch.set[1 - ch.cur], nullptr, out_rgba);
 						if (depths.size() <= d) depths.emplace_back();
 						ReconStep &dp = depths[d++];
-						dp.add(t);
+						dp.tasks.push_back(t);
 						for (int q = q_lo; q < q_hi; q++) {  // the first request gets the picture, duplicates a copy of it
 							if (!leaf || q > q_lo) dp.copy(planes_dst[order[q]], t.cur.y, (size_t)s.coded_size * 3 / 2);
 							if (rgba && q > q_lo) dp.copy(rgba_dst[order[q]], t.rgba, (size_t)s.width * s.height * 4);
@@ -1153,7 +1167,7 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 			// ---- stage 2: one depth after the other on the reconstruct stream, each followed by its copies (a set is
 			// overwritten two references later, by a later launch on the same stream)
 			for (ReconStep &dp : depths) {
-				launch_step(dp, b->st_recon);
+				launch_reconstruct(dp.tasks.data(), (int)dp.tasks.size(), b->st_recon);
 				if (!dp.dst.empty()) copy_batch(b, dp.dst, dp.src, dp.size, b->st_recon);
 			}
 			CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
@@ -1163,50 +1177,52 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 		for (size_t c = glo; c < ghi; c++)  // never consumed: planes 0 (a copied destination was not zeroed)
 			if (chains[c].n_sets)
 				for (int q = chains[c].req_lo; q < chains[c].req_hi; q++)
-					if (status[order[q]] == 0) {
+					if (out.status[order[q]] == 0) {
 						const Stream &s = b->streams[chains[c].stream];
 						CUDA_CHECK(cudaMemsetAsync(planes_dst[order[q]], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
 					}
 	}
 	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
 	b->recon_pending = false;
-	for (int i = 0; i < n; i++) {
-		if (status_out) status_out[i] = status[i];
-		if (n_present_out) n_present_out[i] = n_present[i];
-		if (error_out) error_out[i] = error[i];
-	}
+	out.copy_out(status_out, n_present_out, error_out);
 }
 
-// The checks both front ends make of a request before anything changes: stream, sequence header, destinations
-bool request_valid(const Batch *b, int si, void *planes, void *image, bool rgba) {
-	auto aligned = [](const void *p) { return ((uintptr_t)p & 15u) == 0; };  // stage 2 stores 8 and 16 bytes at a time
-	if (si < 0 || si >= (int)b->streams.size() || !b->streams[si].has_seq || !planes || !aligned(planes)) return false;
-	return !rgba || (image && aligned(image));
+// The checks of a random-access call's requests, all before anything changes: the arrays are there; every request
+// names a stream with a sequence header and a picture of its `what` listing; its destination, and with `rgba` its image,
+// is 16-byte aligned (stage 2 stores 8 and 16 bytes at a time).  Fills `req` (with the chain starts) and returns true,
+// or returns false.
+bool check_requests(Batch *b, Listing what, int n, const int *streams, const uint32_t *pictures, void *const *dst,
+                    void *const *rgba_dst, bool rgba, std::vector<PictureRequest> &req) {
+	use_device(b);
+	if (n < 0 || (n > 0 && (!streams || !pictures || !dst || (rgba && !rgba_dst)))) return false;
+	upload_all(b);
+	auto aligned = [](const void *p) { return p && ((uintptr_t)p & 15u) == 0; };
+	std::vector<std::vector<IndexEntry>> listed(b->streams.size());
+	std::vector<char> indexed(b->streams.size(), 0);
+	req.resize(n);
+	for (int i = 0; i < n; i++) {
+		const int si = streams[i];
+		if (si < 0 || si >= (int)b->streams.size() || !b->streams[si].has_seq || !aligned(dst[i])) return false;
+		if (rgba && !aligned(rgba_dst[i])) return false;
+		if (!indexed[si]) {
+			listed[si] = list_pictures(b, b->streams[si], what);
+			indexed[si] = 1;
+		}
+		auto e = std::lower_bound(listed[si].begin(), listed[si].end(), pictures[i],
+		                          [](const IndexEntry &x, uint32_t k) { return x.pic < k; });
+		if (e == listed[si].end() || e->pic != pictures[i]) return false;
+		req[i] = {si, pictures[i], e->chain_start};
+	}
+	return true;
 }
 
 // decode_intra (`intra`: requests are looked up in the intra index) and decode_pictures (in the picture index)
 long batch_decode_chosen(Batch *b, bool intra, int n, const int *streams, const uint32_t *pictures, void *const *planes_dst,
                          void *const *rgba_dst, int flags, int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
-	use_device(b);
 	const bool rgba = (flags & JSMPEG_B200_OUT_RGBA) != 0;
-	if (n < 0 || (n > 0 && (!streams || !pictures || !planes_dst || (rgba && !rgba_dst)))) return -2;
-	upload_all(b);
-	// ---- every request is checked before anything changes
-	std::vector<std::vector<IndexEntry>> listed(b->streams.size());
-	std::vector<char> indexed(b->streams.size(), 0);
-	std::vector<PictureRequest> req(n);
-	for (int i = 0; i < n; i++) {
-		const int si = streams[i];
-		if (!request_valid(b, si, planes_dst[i], rgba ? rgba_dst[i] : nullptr, rgba)) return -2;
-		if (!indexed[si]) {
-			listed[si] = intra ? intra_index(b->streams[si]) : picture_index(b, b->streams[si]);
-			indexed[si] = 1;
-		}
-		auto e = std::lower_bound(listed[si].begin(), listed[si].end(), pictures[i],
-		                          [](const IndexEntry &x, uint32_t k) { return x.pic < k; });
-		if (e == listed[si].end() || e->pic != pictures[i]) return -2;
-		req[i] = {si, pictures[i], e->chain_start};
-	}
+	std::vector<PictureRequest> req;
+	if (!check_requests(b, intra ? Listing::Intra : Listing::Pictures, n, streams, pictures, planes_dst, rgba_dst, rgba, req))
+		return -2;
 	if (n == 0) return 0;
 	decode_chains(b, req, planes_dst, rgba_dst, rgba, status_out, n_present_out, error_out);
 	return n;
@@ -1214,51 +1230,33 @@ long batch_decode_chosen(Batch *b, bool intra, int n, const int *streams, const 
 
 // ---- decode_macroblocks: the walks' records of chosen pictures of any streams, in the public layout (DESIGN 3.8) ----
 
-// The pictures decode_macroblocks can describe now: after the first sequence header, closed, and decoded by the walks
-// with B pictures going to the B walk whatever decode_b says.  No chain start: a picture's macroblock layer depends on
-// its own bits only.
-std::vector<uint32_t> macroblock_index(const Stream &s) {
-	std::vector<uint32_t> out;
-	if (!s.has_seq) return out;
-	for (uint32_t k = 0; k < s.pics.size(); k++)
-		if (s.pics[k] >= s.seq_floor && picture_decoded(s, k, true) && picture_closed(s, k)) out.push_back(k);
-	return out;
-}
-
 // Each unique (stream, picture) of the requests takes a record slot; waves of as many as there are free slots (after
 // flushing the look-ahead when they do not cover the call) run the walks alone, and one export launch per wave, on the
 // main stream behind the walks and before the slots are released, writes every request of the wave to its
 // destination.  The next wave's walks are queued behind it.  The requests are valid (the caller checked them).
-void decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *dst,
-                        int32_t *n_present_out, int32_t *error_out) {
+void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *const *dst, int32_t *n_present_out,
+                        int32_t *error_out) {
+	const int n = (int)req.size();
 	ensure_pool(b);
 	std::vector<std::pair<int, uint32_t>> uniq(n);
-	for (int i = 0; i < n; i++) uniq[i] = {streams[i], pictures[i]};
+	for (int i = 0; i < n; i++) uniq[i] = {req[i].stream, req[i].pic};
 	std::sort(uniq.begin(), uniq.end());
 	uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
 	std::vector<size_t> uniq_of(n);  // request i describes picture uniq[uniq_of[i]]
 	for (int i = 0; i < n; i++)
-		uniq_of[i] = std::lower_bound(uniq.begin(), uniq.end(), std::make_pair(streams[i], pictures[i])) - uniq.begin();
-	if (b->free_slots.size() < uniq.size())  // decode() parses the look-ahead again
-		for (auto &s : b->streams) flush_cache(b, s);
+		uniq_of[i] = std::lower_bound(uniq.begin(), uniq.end(), std::make_pair(req[i].stream, req[i].pic)) - uniq.begin();
+	free_slots_for(b, uniq.size());
 	if ((size_t)n > b->d_xtasks.size()) {
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 		b->h_xtasks.reserve(n);
 		b->d_xtasks.reserve(n);
 	}
 	const size_t wave_max = b->free_slots.size();
-	std::vector<int32_t> n_present(n, 0), error(n, 0);
+	RequestInfo out(n);
 	for (size_t lo = 0; lo < uniq.size(); lo += wave_max) {
 		const size_t hi = std::min(uniq.size(), lo + wave_max);
 		std::vector<WaveItem> wave;
-		for (size_t u = lo; u < hi; u++) {
-			const Stream &s = b->streams[uniq[u].first];
-			const uint32_t p = uniq[u].second;
-			const uint32_t end = p + 1 < s.pics.size() ? s.pics[p + 1] : s.bb.length;
-			const int slot = b->free_slots.back();
-			b->free_slots.pop_back();
-			wave.push_back({uniq[u].first, p, slot, walk_kind(b, s, p, true), end - s.pics[p]});
-		}
+		for (size_t u = lo; u < hi; u++) wave.push_back(take_slot(b, uniq[u].first, uniq[u].second, true));
 		// (parse_wave waits for the infos, which also means the previous wave's task upload has read h_xtasks)
 		parse_wave(b, wave, false);
 		int m = 0;
@@ -1267,8 +1265,7 @@ void decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pic
 			if (uniq_of[i] < lo || uniq_of[i] >= hi) continue;
 			const WaveItem &w = wave[uniq_of[i] - lo];
 			const picture_info_t &info = b->h_info[uniq_of[i] - lo];
-			n_present[i] = info.n_present;
-			error[i] = info.error;
+			out.set(i, info);
 			const int mb_size = b->streams[w.stream].seq.mb_size;
 			b->h_xtasks[m++] = MbExportTask{b->d_hdr.data() + (size_t)w.slot * b->slot_mb, dst[i], total, mb_size, info.picture_type, 0};
 			total += (uint32_t)mb_size;
@@ -1278,33 +1275,44 @@ void decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pic
 		for (const WaveItem &w : wave) release_slot(b, w.slot);  // the next wave's walks queue behind the export
 	}
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-	for (int i = 0; i < n; i++) {
-		if (n_present_out) n_present_out[i] = n_present[i];
-		if (error_out) error_out[i] = error[i];
-	}
+	out.copy_out(nullptr, n_present_out, error_out);
 }
 
 long batch_decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *mb_dst,
                               int32_t *n_present_out, int32_t *error_out) {
-	use_device(b);
-	if (n < 0 || (n > 0 && (!streams || !pictures || !mb_dst))) return -2;
-	upload_all(b);
-	// ---- every request is checked before anything changes
-	std::vector<std::vector<uint32_t>> listed(b->streams.size());
-	std::vector<char> indexed(b->streams.size(), 0);
-	for (int i = 0; i < n; i++) {
-		const int si = streams[i];
-		if (!request_valid(b, si, mb_dst[i], nullptr, false)) return -2;
-		if (!indexed[si]) {
-			listed[si] = macroblock_index(b->streams[si]);
-			indexed[si] = 1;
-		}
-		if (!std::binary_search(listed[si].begin(), listed[si].end(), pictures[i])) return -2;
-	}
+	std::vector<PictureRequest> req;
+	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, mb_dst, nullptr, false, req)) return -2;
 	if (n == 0) return 0;
-	decode_macroblocks(b, n, streams, pictures, mb_dst, n_present_out, error_out);
+	decode_macroblocks(b, req, mb_dst, n_present_out, error_out);
 	return n;
 }
+
+// The three *_index calls: the `what` listing of `stream`, its first n_max entries into the outputs that are not nullptr.
+// Returns the listing's length, -2 for a stream out of range.
+long write_index(Batch *b, int stream, Listing what, uint32_t *picture_out, uint32_t *byte_pos_out, int32_t *type_out,
+                 int32_t *temporal_reference_out, uint32_t *chain_start_out, long n_max) {
+	return guarded<long>(b, -1, [&]() -> long {
+		if (stream < 0 || stream >= (int)b->streams.size()) return -2;
+		use_device(b);
+		upload_all(b);
+		const Stream &s = b->streams[stream];
+		const std::vector<IndexEntry> listed = list_pictures(b, s, what);
+		for (long i = 0; i < std::min<long>((long)listed.size(), n_max); i++) {
+			const uint32_t k = listed[i].pic;
+			const PictureHeader h = picture_header(s, s.pics[k]);
+			if (picture_out) picture_out[i] = k;
+			if (byte_pos_out) byte_pos_out[i] = s.pics[k];
+			if (type_out) type_out[i] = h.type;
+			if (temporal_reference_out) temporal_reference_out[i] = h.temporal_reference;
+			if (chain_start_out) chain_start_out[i] = listed[i].chain_start;
+		}
+		return (long)listed.size();
+	});
+}
+
+// The planes of the stream's most recent picture: `forward` (mpeg1.c:841-851); with the B-picture extension it may be a
+// B picture's own set
+PlaneSet latest_planes(const Stream &s) { return plane_set(s, s.d_last ? s.d_last : s.d_planes[1 - s.cur].data()); }
 
 int env_int(const char *name, int fallback) {
 	const char *e = getenv(name);
@@ -1494,20 +1502,7 @@ long jsmpeg_b200_batch_decode(jsmpeg_b200_batch_t *b, int n_pictures, int flags)
 
 long jsmpeg_b200_batch_intra_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out, uint32_t *byte_pos_out,
                                    int32_t *temporal_reference_out, long n_max) {
-	return guarded<long>(b, -1, [&]() -> long {
-		if (stream < 0 || stream >= (int)b->streams.size()) return -2;
-		use_device(b);
-		upload_all(b);
-		const Stream &s = b->streams[stream];
-		const std::vector<IndexEntry> listed = intra_index(s);
-		for (long i = 0; i < std::min<long>((long)listed.size(), n_max); i++) {
-			const uint32_t pos = s.pics[listed[i].pic];
-			if (picture_out) picture_out[i] = listed[i].pic;
-			if (byte_pos_out) byte_pos_out[i] = pos;
-			if (temporal_reference_out) temporal_reference_out[i] = s.bb.bytes[pos + 4] << 2 | s.bb.bytes[pos + 5] >> 6;
-		}
-		return (long)listed.size();
-	});
+	return write_index(b, stream, Listing::Intra, picture_out, byte_pos_out, nullptr, temporal_reference_out, nullptr, n_max);
 }
 
 long jsmpeg_b200_batch_decode_intra(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
@@ -1521,22 +1516,8 @@ long jsmpeg_b200_batch_decode_intra(jsmpeg_b200_batch_t *b, int n, const int *st
 long jsmpeg_b200_batch_picture_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out, uint32_t *byte_pos_out,
                                      int32_t *type_out, int32_t *temporal_reference_out, uint32_t *chain_start_out,
                                      long n_max) {
-	return guarded<long>(b, -1, [&]() -> long {
-		if (stream < 0 || stream >= (int)b->streams.size()) return -2;
-		use_device(b);
-		upload_all(b);
-		const Stream &s = b->streams[stream];
-		const std::vector<IndexEntry> listed = picture_index(b, s);
-		for (long i = 0; i < std::min<long>((long)listed.size(), n_max); i++) {
-			const uint32_t k = listed[i].pic;
-			if (picture_out) picture_out[i] = k;
-			if (byte_pos_out) byte_pos_out[i] = s.pics[k];
-			if (type_out) type_out[i] = picture_type_of(s, k);
-			if (temporal_reference_out) temporal_reference_out[i] = (int32_t)picture_header_bits(s, k, 0, 10);
-			if (chain_start_out) chain_start_out[i] = listed[i].chain_start;
-		}
-		return (long)listed.size();
-	});
+	return write_index(b, stream, Listing::Pictures, picture_out, byte_pos_out, type_out, temporal_reference_out,
+	                   chain_start_out, n_max);
 }
 
 long jsmpeg_b200_batch_decode_pictures(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
@@ -1549,21 +1530,8 @@ long jsmpeg_b200_batch_decode_pictures(jsmpeg_b200_batch_t *b, int n, const int 
 
 long jsmpeg_b200_batch_macroblock_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out, uint32_t *byte_pos_out,
                                         int32_t *type_out, int32_t *temporal_reference_out, long n_max) {
-	return guarded<long>(b, -1, [&]() -> long {
-		if (stream < 0 || stream >= (int)b->streams.size()) return -2;
-		use_device(b);
-		upload_all(b);
-		const Stream &s = b->streams[stream];
-		const std::vector<uint32_t> listed = macroblock_index(s);
-		for (long i = 0; i < std::min<long>((long)listed.size(), n_max); i++) {
-			const uint32_t k = listed[i];
-			if (picture_out) picture_out[i] = k;
-			if (byte_pos_out) byte_pos_out[i] = s.pics[k];
-			if (type_out) type_out[i] = picture_type_of(s, k);
-			if (temporal_reference_out) temporal_reference_out[i] = (int32_t)picture_header_bits(s, k, 0, 10);
-		}
-		return (long)listed.size();
-	});
+	return write_index(b, stream, Listing::Macroblocks, picture_out, byte_pos_out, type_out, temporal_reference_out, nullptr,
+	                   n_max);
 }
 
 long jsmpeg_b200_batch_decode_macroblocks(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
@@ -1574,8 +1542,7 @@ long jsmpeg_b200_batch_decode_macroblocks(jsmpeg_b200_batch_t *b, int n, const i
 int jsmpeg_b200_batch_get_planes(jsmpeg_b200_batch_t *b, int stream, void **y, void **cr, void **cb) {
 	const Stream &s = b->streams[stream];
 	if (!s.has_seq) return -1;
-	// most recent picture = forward (mpeg1.c:841-851); with the B-picture extension it may be a B picture's own set
-	PlaneSet p = plane_set(s, s.d_last ? s.d_last : s.d_planes[1 - s.cur].data());
+	PlaneSet p = latest_planes(s);
 	if (y) *y = p.y;
 	if (cr) *cr = p.cr;
 	if (cb) *cb = p.cb;
@@ -1604,7 +1571,7 @@ int jsmpeg_b200_batch_read_planes(jsmpeg_b200_batch_t *b, int stream, void *y, v
 		use_device(b);
 		const Stream &s = b->streams[stream];
 		if (!s.has_seq) return -1;
-		PlaneSet p = plane_set(s, s.d_last ? s.d_last : s.d_planes[1 - s.cur].data());
+		PlaneSet p = latest_planes(s);
 		if (y) CUDA_CHECK(cudaMemcpy(y, p.y, s.coded_size, cudaMemcpyDeviceToHost));
 		if (cr) CUDA_CHECK(cudaMemcpy(cr, p.cr, s.coded_size >> 2, cudaMemcpyDeviceToHost));
 		if (cb) CUDA_CHECK(cudaMemcpy(cb, p.cb, s.coded_size >> 2, cudaMemcpyDeviceToHost));
@@ -1839,7 +1806,7 @@ int jsmpeg_b200_debug_parse_picture(const uint8_t *es, uint32_t es_len, uint32_t
 		t.stage = d_stage.data(); t.stage_entries = stage_entries_for(sp.mb_size);
 		t.codes = nullptr; t.n_codes = 0; t.code_hint = 0;  // this hook lets the walk search the slice end itself
 		CUDA_CHECK(cudaMemcpy(d_task.data(), &t, sizeof(t), cudaMemcpyHostToDevice));
-		launch_parse_pictures(d_task.data(), 1, sp.mb_size, true, 0);
+		launch_parse_pictures(WALK_LANES, d_task.data(), 1, sp.mb_size, true, 0);
 		CUDA_CHECK(cudaGetLastError());
 		CUDA_CHECK(cudaDeviceSynchronize());
 		CUDA_CHECK(cudaMemcpy(info_out, d_info.data(), sizeof(picture_info_t), cudaMemcpyDeviceToHost));

@@ -166,6 +166,25 @@ void launch_expand(const ParseTask *tasks, int n_tasks, int max_mb_size, cudaStr
 	expand_blocks_kernel<<<grid, CTA_THREADS, EXPAND_SMEM, stream>>>(tasks);
 }
 
+// The walk kernel of each WalkKind and its dynamic shared memory.  The lane-parallel walk is the default for WALK_LANES;
+// JSMPEG_B200_WALK=serial selects the one-chain-per-warp walk instead.
+struct WalkKernel {
+	void (*fn)(const ParseTask *, int, const uint4 *);
+	size_t smem;
+};
+const WalkKernel *walk_kernels() {
+	static const bool serial = [] {
+		const char *e = getenv("JSMPEG_B200_WALK");
+		return e && !strcmp(e, "serial");
+	}();
+	static const WalkKernel table[N_WALK_KINDS] = {
+	    serial ? WalkKernel{walk_pictures_kernel, WALK_SMEM_SERIAL} : WalkKernel{walk_pictures_lanes_kernel, WALK_SMEM_LANES},
+	    {walk_pictures_slices_kernel, WALK_SMEM_LANES},
+	    {walk_pictures_b_kernel, WALK_SMEM_SERIAL},
+	};
+	return table;
+}
+
 }  // namespace
 
 // The multi-symbol walk table (walk.cuh: build_ms_table), built once per device from the generated DCT table.
@@ -176,14 +195,8 @@ static const uint16_t *ms_table_for_current_device() {
 	int dev = 0;
 	CUDA_CHECK(cudaGetDevice(&dev));
 	if (tables[dev]) return tables[dev];
-	CUDA_CHECK(cudaFuncSetAttribute(walk_pictures_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-	                                (int)WALK_SMEM_SERIAL));  // per device, once
-	CUDA_CHECK(cudaFuncSetAttribute(walk_pictures_lanes_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-	                                (int)WALK_SMEM_LANES));
-	CUDA_CHECK(cudaFuncSetAttribute(walk_pictures_b_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-	                                (int)WALK_SMEM_SERIAL));
-	CUDA_CHECK(cudaFuncSetAttribute(walk_pictures_slices_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-	                                (int)WALK_SMEM_LANES));
+	for (int k = 0; k < N_WALK_KINDS; k++)  // per device, once
+		CUDA_CHECK(cudaFuncSetAttribute(walk_kernels()[k].fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)walk_kernels()[k].smem));
 	std::vector<uint16_t> dct((VLC_DCT_MAX_Z + 1) * 32);
 	CUDA_CHECK(cudaMemcpyFromSymbol(dct.data(), VLC_DCT_COEFF, dct.size() * sizeof(uint16_t)));
 	std::vector<uint16_t> ms(MS_TABLE_ENTRIES);
@@ -195,35 +208,26 @@ static const uint16_t *ms_table_for_current_device() {
 	return d;
 }
 
-int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream,
-                          cudaEvent_t walk_done, const ParseFork *fork) {
+int launch_parse_pictures(WalkKind kind, const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand,
+                          cudaStream_t stream, cudaEvent_t walk_done, const ParseFork *fork) {
 	if (n_tasks <= 0) return 0;
-	const uint16_t *ms = ms_table_for_current_device();
+	const uint4 *ms = reinterpret_cast<const uint4 *>(ms_table_for_current_device());
+	const WalkKernel walk = walk_kernels()[kind];
 	const int per_cta = WALK_THREADS / 32;
-	// the lane-parallel walk (walk.cuh) is the default; JSMPEG_B200_WALK=serial selects the one-chain-per-warp walk
-	static const bool lane_walk = [] {
-		const char *e = getenv("JSMPEG_B200_WALK");
-		return !(e && !strcmp(e, "serial"));
-	}();
-	const size_t walk_smem = lane_walk ? WALK_SMEM_LANES : WALK_SMEM_SERIAL;
-	// The wave arrives sorted by picture size, largest first.  A wave of at least 64 pictures per group is cut into
-	// PARSE_GROUPS equal groups: group 0 (largest pictures) stays on `stream`, the others go to side streams, each walk
-	// followed by its own expand, so that the expand of the smaller pictures runs while the walk of the bigger ones is
-	// still going.  On an H100 this takes 3 ms off stage 1 of a 3840-picture 1080p wave (DESIGN 8).  A walk-only wave
-	// has no expand to overlap: one group.
-	const int groups = (expand && fork && n_tasks >= 64 * PARSE_GROUPS) ? PARSE_GROUPS : 1;
+	// The wave arrives sorted by picture size, largest first.  A lane-parallel wave of at least 64 pictures per group
+	// is cut into PARSE_GROUPS equal groups: group 0 (largest pictures) stays on `stream`, the others go to side
+	// streams, each walk followed by its own expand, so that the expand of the smaller pictures runs while the walk of
+	// the bigger ones is still going.  On an H100 this takes 3 ms off stage 1 of a 3840-picture 1080p wave (DESIGN 8).
+	// A walk-only wave has no expand to overlap: one group.  The slice and B walks take one group: B pictures are the
+	// small ones of a stream.
+	const int groups = (kind == WALK_LANES && expand && fork && n_tasks >= 64 * PARSE_GROUPS) ? PARSE_GROUPS : 1;
 	if (groups > 1) CUDA_CHECK(cudaEventRecord(fork->fork, stream));
 	for (int g = 0; g < groups; g++) {
 		const int lo = (int)((long)n_tasks * g / groups), hi = (int)((long)n_tasks * (g + 1) / groups);
 		const int n = hi - lo;
 		cudaStream_t st = g == 0 ? stream : fork->side[g];
 		if (g > 0) CUDA_CHECK(cudaStreamWaitEvent(st, fork->fork, 0));
-		if (lane_walk)
-			walk_pictures_lanes_kernel<<<(n + per_cta - 1) / per_cta, WALK_THREADS, walk_smem, st>>>(
-			    tasks + lo, n, reinterpret_cast<const uint4 *>(ms));
-		else
-			walk_pictures_kernel<<<(n + per_cta - 1) / per_cta, WALK_THREADS, walk_smem, st>>>(
-			    tasks + lo, n, reinterpret_cast<const uint4 *>(ms));
+		walk.fn<<<(n + per_cta - 1) / per_cta, WALK_THREADS, walk.smem, st>>>(tasks + lo, n, ms);
 		if (g == 0 && walk_done) CUDA_CHECK(cudaEventRecord(walk_done, st));
 		if (expand) launch_expand(tasks + lo, n, max_mb_size, st);
 		if (g > 0) {
@@ -232,26 +236,4 @@ int launch_parse_pictures(const ParseTask *tasks, int n_tasks, int max_mb_size, 
 		}
 	}
 	return (expand ? 2 : 1) * groups;
-}
-
-// B pictures: one walk (+ one expand) launch on `stream` (no size groups: B pictures are the small ones of a stream)
-int launch_parse_pictures_b(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream) {
-	if (n_tasks <= 0) return 0;
-	const uint16_t *ms = ms_table_for_current_device();
-	const int per_cta = WALK_THREADS / 32;
-	walk_pictures_b_kernel<<<(n_tasks + per_cta - 1) / per_cta, WALK_THREADS, WALK_SMEM_SERIAL, stream>>>(
-	    tasks, n_tasks, reinterpret_cast<const uint4 *>(ms));
-	if (expand) launch_expand(tasks, n_tasks, max_mb_size, stream);
-	return expand ? 2 : 1;
-}
-
-// Pictures of many slices (opt-in): one walk (a lane per slice) (+ one expand) launch on `stream`
-int launch_parse_pictures_slices(const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand, cudaStream_t stream) {
-	if (n_tasks <= 0) return 0;
-	const uint16_t *ms = ms_table_for_current_device();
-	const int per_cta = WALK_THREADS / 32;
-	walk_pictures_slices_kernel<<<(n_tasks + per_cta - 1) / per_cta, WALK_THREADS, WALK_SMEM_LANES, stream>>>(
-	    tasks, n_tasks, reinterpret_cast<const uint4 *>(ms));
-	if (expand) launch_expand(tasks, n_tasks, max_mb_size, stream);
-	return expand ? 2 : 1;
 }

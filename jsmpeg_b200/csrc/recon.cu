@@ -37,6 +37,9 @@
 // HBM roofline accounting (DESIGN.md): per macroblock 16 B header + 32 B per coded block (its
 // compact record; the about 0.5 % of blocks with a dense record are not counted) + 384 B written +
 // 384 B of forward-plane samples (P pictures), each counted once.
+#include <algorithm>
+#include <vector>
+
 #include "recon.cuh"
 
 namespace {
@@ -99,82 +102,45 @@ void fill_task(CompactTask &c, const ReconTask &t) {
 	c.flags = 0;
 }
 
+// One kernel's tasks, cut into launches of at most `per`: B = the kernel takes `bwd`, RGBA = it takes the fused
+// conversion's target.  The plain kernels' grid covers the largest picture's block slots, the RGBA kernels' its
+// macroblock rows and columns.
+template <bool B, bool RGBA, class Params>
+int launch_kernel(void (*kernel)(Params), int per, const std::vector<const ReconTask *> &tasks, cudaStream_t stream) {
+	int launches = 0;
+	for (size_t first = 0; first < tasks.size(); first += per, launches++) {
+		const int n = (int)std::min<size_t>(per, tasks.size() - first);
+		Params p;
+		auto &table = [&]() -> auto & { if constexpr (RGBA) return p.p; else return p; }();
+		int max_slots = 0, max_w = 0, max_h = 0;
+		for (int i = 0; i < n; i++) {
+			const ReconTask &t = *tasks[first + i];
+			fill_task(table.t[i], t);
+			if constexpr (B) table.t[i].bwd = t.bwd.y;
+			if constexpr (RGBA) p.out[i] = RgbaTarget{t.rgba, t.width, t.height};
+			max_slots = std::max(max_slots, t.mb_size * 6);
+			max_w = std::max(max_w, t.mb_width);
+			max_h = std::max(max_h, t.mb_size / t.mb_width);
+		}
+		table.n_tasks = n;
+		if constexpr (RGBA) kernel<<<dim3((max_w + RGBA_MBS - 1) / RGBA_MBS, max_h, n), RGBA_THREADS, 0, stream>>>(p);
+		else kernel<<<dim3((max_slots + THREADS - 1) / THREADS, n), THREADS, 0, stream>>>(p);
+	}
+	return launches;
+}
+
 }  // namespace
 
 int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream) {
-	int launches = 0;
-	for (int first = 0; first < n_tasks; first += MAX_TASKS, launches++) {
-		const int n = n_tasks - first < MAX_TASKS ? n_tasks - first : MAX_TASKS;
-		ReconParams p;
-		int max_slots = 0;
-		for (int i = 0; i < n; i++) {
-			const ReconTask &t = tasks_host[first + i];
-			fill_task(p.t[i], t);
-			max_slots = max_slots > t.mb_size * 6 ? max_slots : t.mb_size * 6;
-		}
-		p.n_tasks = n;
-		dim3 grid((max_slots + THREADS - 1) / THREADS, n);
-		reconstruct_kernel<<<grid, THREADS, 0, stream>>>(p);
+	std::vector<const ReconTask *> by_kernel[4];  // I/P, I/P + RGBA, B, B + RGBA
+	for (int i = 0; i < n_tasks; i++) {
+		const ReconTask &t = tasks_host[i];
+		by_kernel[(t.bwd.y ? 2 : 0) + (t.rgba ? 1 : 0)].push_back(&t);
 	}
-	return launches;
-}
-
-int launch_reconstruct_rgba(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream) {
-	int launches = 0;
-	for (int first = 0; first < n_tasks; first += MAX_TASKS_RGBA, launches++) {
-		const int n = n_tasks - first < MAX_TASKS_RGBA ? n_tasks - first : MAX_TASKS_RGBA;
-		ReconRgbaParams p;
-		int max_w = 0, max_h = 0;
-		for (int i = 0; i < n; i++) {
-			const ReconTask &t = tasks_host[first + i];
-			fill_task(p.p.t[i], t);
-			p.out[i] = RgbaTarget{t.rgba, t.width, t.height};
-			max_w = max_w > t.mb_width ? max_w : t.mb_width;
-			const int h = t.mb_size / t.mb_width;
-			max_h = max_h > h ? max_h : h;
-		}
-		p.p.n_tasks = n;
-		dim3 grid((max_w + RGBA_MBS - 1) / RGBA_MBS, max_h, n);
-		reconstruct_rgba_kernel<<<grid, RGBA_THREADS, 0, stream>>>(p);
-	}
-	return launches;
-}
-
-int launch_reconstruct_b(const ReconTask *tasks_host, int n_tasks, bool rgba, cudaStream_t stream) {
-	int launches = 0;
-	const int per = rgba ? MAX_TASKS_RGBA_B : MAX_TASKS_B;
-	for (int first = 0; first < n_tasks; first += per, launches++) {
-		const int n = n_tasks - first < per ? n_tasks - first : per;
-		int max_slots = 0, max_w = 0, max_h = 0;
-		for (int i = 0; i < n; i++) {
-			const ReconTask &t = tasks_host[first + i];
-			max_slots = max_slots > t.mb_size * 6 ? max_slots : t.mb_size * 6;
-			max_w = max_w > t.mb_width ? max_w : t.mb_width;
-			const int h = t.mb_size / t.mb_width;
-			max_h = max_h > h ? max_h : h;
-		}
-		if (rgba) {
-			ReconRgbaParamsB p;
-			for (int i = 0; i < n; i++) {
-				const ReconTask &t = tasks_host[first + i];
-				fill_task(p.p.t[i], t);
-				p.p.t[i].bwd = t.bwd.y;
-				p.out[i] = RgbaTarget{t.rgba, t.width, t.height};
-			}
-			p.p.n_tasks = n;
-			dim3 grid((max_w + RGBA_MBS - 1) / RGBA_MBS, max_h, n);
-			reconstruct_rgba_b_kernel<<<grid, RGBA_THREADS, 0, stream>>>(p);
-		} else {
-			ReconParamsB p;
-			for (int i = 0; i < n; i++) {
-				const ReconTask &t = tasks_host[first + i];
-				fill_task(p.t[i], t);
-				p.t[i].bwd = t.bwd.y;
-			}
-			p.n_tasks = n;
-			dim3 grid((max_slots + THREADS - 1) / THREADS, n);
-			reconstruct_b_kernel<<<grid, THREADS, 0, stream>>>(p);
-		}
-	}
+	// (one statement per kernel: the launch order is the order above)
+	int launches = launch_kernel<false, false>(reconstruct_kernel, MAX_TASKS, by_kernel[0], stream);
+	launches += launch_kernel<false, true>(reconstruct_rgba_kernel, MAX_TASKS_RGBA, by_kernel[1], stream);
+	launches += launch_kernel<true, false>(reconstruct_b_kernel, MAX_TASKS_B, by_kernel[2], stream);
+	launches += launch_kernel<true, true>(reconstruct_rgba_b_kernel, MAX_TASKS_RGBA_B, by_kernel[3], stream);
 	return launches;
 }
