@@ -280,6 +280,39 @@ long jsmpeg_b200_batch_macroblock_index(jsmpeg_b200_batch_t *b, int stream, uint
 long jsmpeg_b200_batch_decode_macroblocks(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
                                           void *const *mb_dst, int32_t *n_present_out, int32_t *error_out);
 
+/* COEFFICIENTS (DC images for shot-boundary detection and thumbnails, residual-energy and texture features,
+ * DCT-domain learning): each block's 64 dequantised DCT coefficients of chosen pictures of any streams, as the
+ * inverse transform consumes them -- no pixels and no reference pictures, so every request of a call is one wave of
+ * the walks and the coefficient expansion.  The pictures are those of the macroblock index above, for the same reason
+ * (a picture's coefficients depend on its own bits only: the intra DC predictors reset at every slice).
+ *
+ * Request i = picture pictures[i] of stream streams[i] into coef_dst[i]: DEVICE memory, 16-byte aligned, of
+ * mb_height * mb_width * 6 * 64 int16 (768 bytes per macroblock): macroblocks in raster order; per macroblock the
+ * blocks 0-3 luma (top-left, top-right, bottom-left, bottom-right), 4 Cb, 5 Cr (the cbp bits' order); per block the
+ * 64 values in RASTER (de-zig-zagged) order, row-major 8 x 8.  Each value is dequantised, made odd toward zero and
+ * clipped to [-2048, 2047], the intra DC as 8 * dc: ISO 11172-2's dct_recon, with ONE deviation, kept because these
+ * are the values the pictures' samples are made from: the product level * quantiser_scale * Q is shifted right
+ * arithmetically by 4, so a negative product is rounded toward minus infinity where ISO truncates toward zero.
+ * Every value of a block whose cbp bit is clear, and of a macroblock without PRESENT, is 0: every byte of
+ * coef_dst[i] is written.  mb_dst may be NULL; otherwise mb_dst[i] (16-byte aligned) gets exactly what
+ * decode_macroblocks writes for the request, from the same walk.
+ *
+ * Each picture is what the walk and the expansion give when they start at the picture's own start code: for a clean
+ * stream, what a fresh decoder (B pictures on) gives for the first sequence header + the picture + its closing code,
+ * and the coefficients decode() uses for picture k.  A damaged picture: the walk reads the resident stream past the
+ * closing code (as decode_intra).  Where it stops inside a macroblock header the macroblock is absent (all 0); where
+ * it stops inside a block the macroblock is PRESENT with the cbp bits of the blocks it finished -- the block whose
+ * codes it could not read, and those after it, have their bit clear and are 0 (not the values read before the bad
+ * code) -- and every finished block holds the values of its codes.
+ *
+ * Synchronous; duplicates each get the data.  n_present_out / error_out (may be NULL) as decode_macroblocks.  Returns
+ * n; -1 dead; -2 a request is invalid (stream out of range or without sequence header, picture not in the macroblock
+ * index, NULL or misaligned coef_dst[i], misaligned or NULL mb_dst[i] when mb_dst is given) -- checked before any
+ * work, and then nothing changed.  Changes nothing decode() observes, as decode_intra. */
+long jsmpeg_b200_batch_decode_coefficients(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                           void *const *coef_dst, void *const *mb_dst,
+                                           int32_t *n_present_out, int32_t *error_out);
+
 void jsmpeg_b200_batch_get_stats(jsmpeg_b200_batch_t *b, jsmpeg_b200_stats_t *out);
 void jsmpeg_b200_batch_reset_stats(jsmpeg_b200_batch_t *b);
 

@@ -59,6 +59,7 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_decode_pictures": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_macroblock_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_macroblocks": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP]),
+    "jsmpeg_b200_batch_decode_coefficients": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_get_stats": (None, [_VP, ctypes.POINTER(Stats)]),
     "jsmpeg_b200_batch_reset_stats": (None, [_VP]),
     "jsmpeg_b200_debug_parse_picture": (ctypes.c_int, [_VP, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int, ctypes.c_int,
@@ -117,6 +118,7 @@ class BatchDecoder:
         self.last_intra_info = []  # per request of the last decode_intra: {"n_present", "error"} (picture_info_t)
         self.last_pictures_info = []  # per request of the last decode_pictures: {"status", "n_present", "error"}
         self.last_macroblocks_info = []  # per request of the last decode_macroblocks: {"n_present", "error"}
+        self.last_coefficients_info = []  # per request of the last decode_coefficients: {"n_present", "error"}
         self.handle = self.lib.jsmpeg_b200_batch_create(n_streams, device, max_slots)
         err = self.lib.jsmpeg_b200_batch_last_error(self.handle)
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
@@ -326,26 +328,10 @@ class BatchDecoder:
         import torch
         reqs = [(int(s), int(p)) for s, p in requests]
         n = len(reqs)
-        shapes = {}  # per stream: (mb_height, mb_width)
-        for s, _ in reqs:
-            if s not in shapes:
-                info = self._request_stream_info(s)
-                shapes[s] = ((info["height"] + 15) // 16, (info["width"] + 15) // 16)
-        dev = torch.device("cuda", self.device)
-        by_shape = {}  # per picture size: the requests of that size
-        for i, (s, _) in enumerate(reqs):
-            by_shape.setdefault(shapes[s], []).append(i)
-        out = [None] * n
-        for shape, idx in by_shape.items():  # (entries are 16 bytes: every view is 16-byte aligned)
-            views = torch.empty((len(idx), *shape, MACROBLOCK_BYTES), dtype=torch.uint8, device=dev).unbind(0)
-            for i, t in zip(idx, views):
-                out[i] = t
-        streams = (ctypes.c_int * max(n, 1))(*[s for s, _ in reqs])
-        pictures = (ctypes.c_uint32 * max(n, 1))(*[p for _, p in reqs])
+        out = self._per_macroblock_views(reqs, (MACROBLOCK_BYTES,), torch.uint8)
+        streams, pictures, n_present, errors = self._request_arrays(reqs)
         dst = (_VP * max(n, 1))(*[t.data_ptr() for t in out])
-        n_present = (ctypes.c_int32 * max(n, 1))()
-        errors = (ctypes.c_int32 * max(n, 1))()
-        torch.cuda.current_stream(dev).synchronize()  # the allocations are the caller's stream's; the call uses its own
+        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # the allocations are the caller's stream's; the call uses its own
         got = self.lib.jsmpeg_b200_batch_decode_macroblocks(self.handle, n, streams, pictures, dst, n_present, errors)
         if got == -2:
             raise ValueError("a request names a picture that is not in the stream's macroblock index")
@@ -353,6 +339,59 @@ class BatchDecoder:
             raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_macroblocks failed")
         self.last_macroblocks_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
         return out
+
+    def decode_coefficients(self, requests, macroblocks=False):
+        """Dequantised DCT coefficients of pictures listed by macroblock_index, of any streams, in one call: `requests`
+        is an iterable of (stream, picture).  Returns per request a torch.int16 CUDA tensor [mb_height, mb_width, 6, 8,
+        8]: per macroblock the blocks 0-3 luma, 4 Cb, 5 Cr, each in raster order, as the inverse transform consumes
+        them (include/jsmpeg_b200.h); 0 for uncoded blocks and absent macroblocks.  A DC image is c[..., 0, 0] (8 x the
+        DC of intra blocks).  With macroblocks=True each item is a pair (coefficients, entries), entries as
+        decode_macroblocks returns them, from the same walk.  last_coefficients_info gets {"n_present", "error"} per
+        request.  The tensors are views of one allocation per picture size."""
+        import torch
+        reqs = [(int(s), int(p)) for s, p in requests]
+        n = len(reqs)
+        coefs = self._per_macroblock_views(reqs, (6, 8, 8), torch.int16)
+        entries = self._per_macroblock_views(reqs, (MACROBLOCK_BYTES,), torch.uint8) if macroblocks else None
+        streams, pictures, n_present, errors = self._request_arrays(reqs)
+        coef_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in coefs])
+        mb_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in entries]) if macroblocks else None
+        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # as in decode_macroblocks
+        got = self.lib.jsmpeg_b200_batch_decode_coefficients(self.handle, n, streams, pictures, coef_dst, mb_dst,
+                                                             n_present, errors)
+        if got == -2:
+            raise ValueError("a request names a picture that is not in the stream's macroblock index")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_coefficients failed")
+        self.last_coefficients_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
+        return list(zip(coefs, entries)) if macroblocks else coefs
+
+    def _per_macroblock_views(self, reqs, per_mb, dtype):
+        """Per (stream, picture) request a CUDA tensor [mb_height, mb_width, *per_mb] of `dtype`, the views of one
+        allocation per picture size (thousands of requests cost a few allocations, not thousands).  A view starts a
+        whole number of macroblocks into its allocation: with 16 * k bytes per macroblock it is 16-byte aligned."""
+        import torch
+        shapes = {}  # per stream: (mb_height, mb_width)
+        for s, _ in reqs:
+            if s not in shapes:
+                info = self._request_stream_info(s)
+                shapes[s] = ((info["height"] + 15) // 16, (info["width"] + 15) // 16)
+        by_shape = {}  # per picture size: the requests of that size
+        for i, (s, _) in enumerate(reqs):
+            by_shape.setdefault(shapes[s], []).append(i)
+        out = [None] * len(reqs)
+        for shape, idx in by_shape.items():
+            views = torch.empty((len(idx), *shape, *per_mb), dtype=dtype, device=torch.device("cuda", self.device)).unbind(0)
+            for i, t in zip(idx, views):
+                out[i] = t
+        return out
+
+    @staticmethod
+    def _request_arrays(reqs):
+        """ctypes arrays of (stream, picture) requests: streams, pictures, and n_present / error outputs."""
+        n = max(len(reqs), 1)
+        return ((ctypes.c_int * n)(*[s for s, _ in reqs]), (ctypes.c_uint32 * n)(*[p for _, p in reqs]),
+                (ctypes.c_int32 * n)(), (ctypes.c_int32 * n)())
 
     def _request_stream_info(self, s):
         """stream_info of the stream a request names; ValueError unless it is in range and has a sequence header."""

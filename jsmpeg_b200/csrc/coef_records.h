@@ -11,8 +11,8 @@
  * A block with more than COEF_RECORD_LEVELS positions has mask == COEF_RECORD_DENSE: its dense 128-byte record
  * holds it, at its usual place in the coefficient plane.  Uncoded blocks write and read nothing.
  *
- * This header is the only place that knows the layout; the expand and reconstruct kernels, the host engine's
- * debug hooks and the tests all go through it.  It compiles as CUDA (host and device) and as plain C++.
+ * This header is the only place that knows the layout; the expand, reconstruct and coefficient export kernels, the
+ * host engine's debug hooks and the tests all go through it.  It compiles as CUDA (host and device) and as plain C++.
  */
 #ifndef JSMPEG_B200_COEF_RECORDS_H
 #define JSMPEG_B200_COEF_RECORDS_H
@@ -62,6 +62,33 @@ COEF_FN int coef_zigzag_raster(int k) {
 	const int row = (d & 1) ? o : d - o;
 	const int r = row * 8 + (d - row);
 	return first ? r : 63 - r;
+}
+
+// zig-zag position of raster index r (0..63), the inverse of coef_zigzag_raster: on anti-diagonal d = row + col < 8
+// the position is d (d + 1) / 2 plus the step along it (row on odd d, col on even d); the rest mirrors about the centre.
+COEF_FN int coef_raster_zigzag(int r) {
+	const bool first = (r >> 3) + (r & 7) < 8;
+	const int j = first ? r : 63 - r;
+	const int row = j >> 3, col = j & 7, d = row + col;
+	const int k = d * (d + 1) / 2 + ((d & 1) ? row : col);
+	return first ? k : 63 - k;
+}
+
+// raster row `row` (0..7) of a compact record (mask != COEF_RECORD_DENSE): out[c] = value at raster row * 8 + c.
+// Per value: its zig-zag position k, bit k of the mask, and the level index popc(mask & ((1 << k) - 1)); the levels
+// are read as three 64-bit words selected by that index, so nothing is indexed at run time (no local memory on the
+// device) and no value takes a branch.  An index of 12 (bit clear, 12 positions below) selects a word too; the clear
+// bit discards it.
+COEF_FN void coef_record_row(const coef_record_t &r, int row, int16_t out[8]) {
+	uint64_t w[3] = {0, 0, 0};
+	for (int i = 0; i < COEF_RECORD_LEVELS; i++) w[i >> 2] |= (uint64_t)(uint16_t)r.level[i] << (16 * (i & 3));
+	for (int c = 0; c < 8; c++) {
+		const int k = coef_raster_zigzag(row * 8 + c);
+		const int idx = coef_popc64(r.mask & ((((uint64_t)1) << k) - 1));
+		const uint64_t word = idx < 4 ? w[0] : (idx < 8 ? w[1] : w[2]);
+		const int16_t v = (int16_t)(uint16_t)(word >> (16 * (idx & 3)));
+		out[c] = ((r.mask >> k) & 1) ? v : (int16_t)0;
+	}
 }
 
 // whether a block with the zig-zag positions `written` fits a compact record

@@ -156,6 +156,21 @@ struct MbExportTask {
 };
 void launch_export_macroblocks(const MbExportTask *tasks, int n_tasks, uint32_t total_mb, cudaStream_t stream);
 
+// Coefficient export (coefficients.cu): request i writes the dequantised coefficients of one picture (`mb_size`
+// macroblocks; records at `hdr`, stage 1b's compact plane at `compact` and dense records at `coef`, as stage 2 reads
+// them) to `dst` in the public layout of jsmpeg_b200_batch_decode_coefficients: per macroblock 6 blocks of 64 int16 in
+// raster order, 0 for uncoded blocks and absent macroblocks.  `first` is the number of macroblocks of requests
+// 0 .. i-1.  One thread per 16-byte output row (48 per macroblock) of all requests, one launch.
+struct CoefExportTask {
+	const mb_record_t *hdr;
+	const int16_t *coef;
+	const coef_record_t *compact;
+	void *dst;
+	uint32_t first;
+	int32_t mb_size;
+};
+void launch_export_coefficients(const CoefExportTask *tasks, int n_tasks, uint32_t total_mb, cudaStream_t stream);
+
 // device MPEG-TS demux (tsdemux.cu)
 struct TsScratch;
 TsScratch *ts_scratch_create();

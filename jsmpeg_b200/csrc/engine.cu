@@ -25,7 +25,8 @@
 // side streams) and waits for the picture infos; the host then consumes them in decode() order and
 // queues one reconstruct step per picture depth (ReconStep, launch_reconstruct) on the reconstruct stream.
 // Cutting the wave into chunks to overlap stage 1 with stage 2 was measured not to pay (DESIGN 8).
-// decode_macroblocks runs the same waves walk-only (no expand, no reconstruct) and exports the records (DESIGN 3.8).
+// decode_macroblocks runs the same waves walk-only (no expand, no reconstruct) and exports the records (DESIGN 3.8);
+// decode_coefficients runs them with expand and exports the coefficients too (DESIGN 3.9).
 #include <sched.h>
 
 #include <algorithm>
@@ -155,6 +156,9 @@ struct jsmpeg_b200_batch_t {
 	// decode_macroblocks: the export tasks of a wave (DESIGN 3.8)
 	PinnedBuffer<MbExportTask> h_xtasks;
 	DeviceBuffer<MbExportTask> d_xtasks;
+	// decode_coefficients: the coefficient export tasks of a wave (DESIGN 3.9)
+	PinnedBuffer<CoefExportTask> h_ctasks;
+	DeviceBuffer<CoefExportTask> d_ctasks;
 	jsmpeg_b200_stats_t stats{};
 };
 
@@ -710,13 +714,26 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 	return launches;
 }
 
+// What stage 1 left in record `slot`, as its readers (stage 2, the coefficient export) take it: the macroblock records,
+// the dense coefficient records and the compact coefficient plane
+struct SlotRecords {
+	const mb_record_t *hdr;
+	const int16_t *coef;
+	const coef_record_t *compact;
+};
+SlotRecords slot_records(const Batch *b, int slot) {
+	return {b->d_hdr.data() + (size_t)slot * b->slot_mb, b->d_coef.data() + (size_t)slot * b->slot_mb * MB_COEF_INT16,
+	        compact_plane(b->d_stage.data() + (size_t)slot * stage_entries_for(b->slot_mb) * 4)};  // (stage 1b wrote it: parse_task)
+}
+
 // The reconstruct task of a picture of `s` whose records are in `slot`: written into the plane set at `cur`, predicted
 // from `fwd` (and, for a B picture, `bwd`), with the fused RGBA conversion into `rgba` unless that is nullptr
 ReconTask recon_task(const Batch *b, const Stream &s, int slot, uint8_t *cur, uint8_t *fwd, uint8_t *bwd, uint8_t *rgba) {
 	ReconTask t{};
-	t.hdr = b->d_hdr.data() + (size_t)slot * b->slot_mb;
-	t.coef = b->d_coef.data() + (size_t)slot * b->slot_mb * MB_COEF_INT16;
-	t.compact = compact_plane(b->d_stage.data() + (size_t)slot * stage_entries_for(b->slot_mb) * 4);  // (stage 1b wrote it: parse_task)
+	const SlotRecords sr = slot_records(b, slot);
+	t.hdr = sr.hdr;
+	t.coef = sr.coef;
+	t.compact = sr.compact;
 	t.cur = plane_set(s, cur);
 	t.fwd = plane_set(s, fwd);
 	if (bwd) t.bwd = plane_set(s, bwd);
@@ -1231,11 +1248,13 @@ long batch_decode_chosen(Batch *b, bool intra, int n, const int *streams, const 
 // ---- decode_macroblocks: the walks' records of chosen pictures of any streams, in the public layout (DESIGN 3.8) ----
 
 // Each unique (stream, picture) of the requests takes a record slot; waves of as many as there are free slots (after
-// flushing the look-ahead when they do not cover the call) run the walks alone, and one export launch per wave, on the
-// main stream behind the walks and before the slots are released, writes every request of the wave to its
-// destination.  The next wave's walks are queued behind it.  The requests are valid (the caller checked them).
-void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *const *dst, int32_t *n_present_out,
-                        int32_t *error_out) {
+// flushing the look-ahead when they do not cover the call) run the walks alone -- or, with `coef_dst` (decode_coefficients,
+// DESIGN 3.9), the walks and the expand -- and one export launch per wave and destination kind, on the main stream
+// behind stage 1 and before the slots are released, writes every request of the wave to its destination: `dst` (may be
+// nullptr) gets the macroblock entries, `coef_dst` (nullptr: none) the coefficients.  The requests are valid (the
+// caller checked them).
+void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *const *dst, void *const *coef_dst,
+                        int32_t *n_present_out, int32_t *error_out) {
 	const int n = (int)req.size();
 	ensure_pool(b);
 	std::vector<std::pair<int, uint32_t>> uniq(n);
@@ -1246,10 +1265,15 @@ void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *
 	for (int i = 0; i < n; i++)
 		uniq_of[i] = std::lower_bound(uniq.begin(), uniq.end(), std::make_pair(req[i].stream, req[i].pic)) - uniq.begin();
 	free_slots_for(b, uniq.size());
-	if ((size_t)n > b->d_xtasks.size()) {
+	if (dst && (size_t)n > b->d_xtasks.size()) {
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 		b->h_xtasks.reserve(n);
 		b->d_xtasks.reserve(n);
+	}
+	if (coef_dst && (size_t)n > b->d_ctasks.size()) {
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		b->h_ctasks.reserve(n);
+		b->d_ctasks.reserve(n);
 	}
 	const size_t wave_max = b->free_slots.size();
 	RequestInfo out(n);
@@ -1257,8 +1281,8 @@ void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *
 		const size_t hi = std::min(uniq.size(), lo + wave_max);
 		std::vector<WaveItem> wave;
 		for (size_t u = lo; u < hi; u++) wave.push_back(take_slot(b, uniq[u].first, uniq[u].second, true));
-		// (parse_wave waits for the infos, which also means the previous wave's task upload has read h_xtasks)
-		parse_wave(b, wave, false);
+		// (parse_wave waits for the infos, which also means the previous wave's task uploads have read h_xtasks / h_ctasks)
+		parse_wave(b, wave, coef_dst != nullptr);
 		int m = 0;
 		uint32_t total = 0;
 		for (int i = 0; i < n; i++) {
@@ -1267,12 +1291,25 @@ void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *
 			const picture_info_t &info = b->h_info[uniq_of[i] - lo];
 			out.set(i, info);
 			const int mb_size = b->streams[w.stream].seq.mb_size;
-			b->h_xtasks[m++] = MbExportTask{b->d_hdr.data() + (size_t)w.slot * b->slot_mb, dst[i], total, mb_size, info.picture_type, 0};
+			const SlotRecords sr = slot_records(b, w.slot);
+			if (dst) b->h_xtasks[m] = MbExportTask{sr.hdr, dst[i], total, mb_size, info.picture_type, 0};
+			if (coef_dst) b->h_ctasks[m] = CoefExportTask{sr.hdr, sr.coef, sr.compact, coef_dst[i], total, mb_size};
+			m++;
 			total += (uint32_t)mb_size;
 		}
-		CUDA_CHECK(cudaMemcpyAsync(b->d_xtasks.data(), b->h_xtasks.data(), m * sizeof(MbExportTask), cudaMemcpyHostToDevice, b->st_main));
-		launch_export_macroblocks(b->d_xtasks.data(), m, total, b->st_main);
-		for (const WaveItem &w : wave) release_slot(b, w.slot);  // the next wave's walks queue behind the export
+		if (dst) {
+			CUDA_CHECK(cudaMemcpyAsync(b->d_xtasks.data(), b->h_xtasks.data(), m * sizeof(MbExportTask), cudaMemcpyHostToDevice, b->st_main));
+			launch_export_macroblocks(b->d_xtasks.data(), m, total, b->st_main);
+		}
+		if (coef_dst) {
+			CUDA_CHECK(cudaMemcpyAsync(b->d_ctasks.data(), b->h_ctasks.data(), m * sizeof(CoefExportTask), cudaMemcpyHostToDevice, b->st_main));
+			launch_export_coefficients(b->d_ctasks.data(), m, total, b->st_main);
+		}
+		// Released right behind the exports, which read the slots on st_main: the next wave's stage 1 rewrites them
+		// (records, dense records and -- through its walks and expands -- the compact planes) only after them.  Its
+		// kernels on st_main queue behind the exports; those on the side streams (parse_wave's st_side, and the size
+		// groups of launch_parse_pictures) start from an event recorded on st_main after them (ev_sfork, fork.fork).
+		for (const WaveItem &w : wave) release_slot(b, w.slot);
 	}
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 	out.copy_out(nullptr, n_present_out, error_out);
@@ -1283,7 +1320,18 @@ long batch_decode_macroblocks(Batch *b, int n, const int *streams, const uint32_
 	std::vector<PictureRequest> req;
 	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, mb_dst, nullptr, false, req)) return -2;
 	if (n == 0) return 0;
-	decode_macroblocks(b, req, mb_dst, n_present_out, error_out);
+	decode_macroblocks(b, req, mb_dst, nullptr, n_present_out, error_out);
+	return n;
+}
+
+// decode_coefficients: decode_macroblocks' requests and schedule with stage 1b on and the coefficient export
+// (DESIGN 3.9); mb_dst, when given, is checked as decode_macroblocks' destinations are
+long batch_decode_coefficients(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *coef_dst,
+                               void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
+	std::vector<PictureRequest> req;
+	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, coef_dst, mb_dst, mb_dst != nullptr, req)) return -2;
+	if (n == 0) return 0;
+	decode_macroblocks(b, req, mb_dst, coef_dst, n_present_out, error_out);
 	return n;
 }
 
@@ -1537,6 +1585,14 @@ long jsmpeg_b200_batch_macroblock_index(jsmpeg_b200_batch_t *b, int stream, uint
 long jsmpeg_b200_batch_decode_macroblocks(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
                                           void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
 	return guarded<long>(b, -1, [&] { return batch_decode_macroblocks(b, n, streams, pictures, mb_dst, n_present_out, error_out); });
+}
+
+long jsmpeg_b200_batch_decode_coefficients(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                           void *const *coef_dst, void *const *mb_dst, int32_t *n_present_out,
+                                           int32_t *error_out) {
+	return guarded<long>(b, -1, [&] {
+		return batch_decode_coefficients(b, n, streams, pictures, coef_dst, mb_dst, n_present_out, error_out);
+	});
 }
 
 int jsmpeg_b200_batch_get_planes(jsmpeg_b200_batch_t *b, int stream, void **y, void **cr, void **cb) {

@@ -6,7 +6,8 @@ Picture k of a stream is the k-th picture start code (00 00 01 00) in its buffer
   3. the walks decode it with B pictures on: picture_coding_type 1; 2 with forward_f_code != 0; 3 with both f_codes
      != 0 (tools/chain_model.py: is_decoded) -- whatever the decode_b option says, and with no chain start.
 A listed picture's entries are export() of the records a fresh decoder with B pictures on gives for fresh_bytes(): the
-first sequence header, the picture's bytes up to its closing code, and the closing code itself.
+first sequence header, the picture's bytes up to its closing code, and the closing code itself.  decode_coefficients
+lists the same pictures; its coefficients are coefficients() of the same decoder's records and coefficient plane.
 """
 from __future__ import annotations
 
@@ -75,3 +76,14 @@ def export(records, picture_type):
     e["cbp"] = np.where(present, r["cbp"], 0)
     e["qscale"] = np.where(present, r["qscale"], 0)
     return e.view(np.uint8).reshape(len(r), 16)
+
+
+def coefficients(records, coef):
+    """What decode_coefficients gives (int16 [n, 6, 64], each block in raster order) for n mb_record_t (any 16-byte-
+    per-record buffer) and the int16 coefficient plane of the same picture ([n * 6 * 64] values in the oracle's layout,
+    which is the public one): the plane, with every value 0 where the macroblock is not PRESENT or the block's cbp bit
+    (bit 5 - block) is clear."""
+    r = np.frombuffer(np.ascontiguousarray(records).tobytes(), RECORD)
+    c = np.frombuffer(np.ascontiguousarray(coef).tobytes(), np.int16).reshape(len(r), 6, 64)
+    coded = ((r["flags"] & MBF_PRESENT) != 0)[:, None] & ((r["cbp"][:, None] >> (5 - np.arange(6))) & 1).astype(bool)
+    return np.where(coded[:, :, None], c, np.int16(0)).astype(np.int16)
