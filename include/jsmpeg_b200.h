@@ -313,6 +313,35 @@ long jsmpeg_b200_batch_decode_coefficients(jsmpeg_b200_batch_t *b, int n, const 
                                            void *const *coef_dst, void *const *mb_dst,
                                            int32_t *n_present_out, int32_t *error_out);
 
+/* RESIDUALS (compressed-domain video models -- I frames, motion vectors and residuals -- residual-energy motion and
+ * saliency cues): the pixel-domain residual of chosen pictures of any streams, the inverse transform of every coded
+ * block -- what stage 2 adds to the motion-compensated prediction (or, for an intra macroblock, clamps) -- with no
+ * reference pictures, so every request of a call is one wave of the walks, the coefficient expansion and one
+ * transform-and-store kernel.  The pictures are those of the macroblock index, as for decode_coefficients.
+ *
+ * Request i = picture pictures[i] of stream streams[i] into res_dst[i]: DEVICE memory, 16-byte aligned, of
+ * coded_size * 3 / 2 int16 (coded_size * 3 bytes) in the planes' layout, in samples: Y at 0 (coded_height x
+ * coded_width), Cr at coded_size, Cb at coded_size * 5 / 4 (each coded_height / 2 x coded_width / 2) -- the order and
+ * offsets of get_planes and of decode_pictures' planes_dst, so residual and picture line up sample for sample.
+ * Every 8 x 8 block is the reference's integer IDCT (src/mpeg1.js:916-983, with PREMULTIPLIER_MATRIX) of the block
+ * decode_coefficients writes for the same request, before any add or clamp: 0 where the cbp bit is clear or the
+ * macroblock is not PRESENT (every byte of res_dst[i] is written), (c0 * 32 + 128) >> 8 everywhere for a DC-only
+ * block (the reference's shortcut, which the transform equals), and a damaged picture follows decode_coefficients'
+ * rule (the block with the bad code, and those after it, are 0).  For a clean stream, the residual of an intra
+ * macroblock is its samples before the clamp (its prediction is 0), that of any other PRESENT macroblock what stage 2
+ * adds to its prediction when decode() reconstructs the picture.  Coefficients are clipped to [-2048, 2047], which
+ * bounds every value well inside int16 (|r| <= 14,314; tests/test_residual_export.py).  mb_dst may be NULL; otherwise
+ * mb_dst[i] (16-byte aligned) gets exactly what decode_macroblocks writes for the request, from the same walk: its
+ * INTRA / FORWARD / BACKWARD flags say how to read the residual.
+ *
+ * Synchronous; duplicates each get the data.  n_present_out / error_out (may be NULL) as decode_macroblocks.  Returns
+ * n; -1 dead; -2 a request is invalid (stream out of range or without sequence header, picture not in the macroblock
+ * index, NULL or misaligned res_dst[i], misaligned or NULL mb_dst[i] when mb_dst is given) -- checked before any
+ * work, and then nothing changed.  Changes nothing decode() observes, as decode_intra. */
+long jsmpeg_b200_batch_decode_residuals(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                        void *const *res_dst, void *const *mb_dst,
+                                        int32_t *n_present_out, int32_t *error_out);
+
 void jsmpeg_b200_batch_get_stats(jsmpeg_b200_batch_t *b, jsmpeg_b200_stats_t *out);
 void jsmpeg_b200_batch_reset_stats(jsmpeg_b200_batch_t *b);
 

@@ -60,6 +60,7 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_macroblock_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_macroblocks": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_decode_coefficients": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "jsmpeg_b200_batch_decode_residuals": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_get_stats": (None, [_VP, ctypes.POINTER(Stats)]),
     "jsmpeg_b200_batch_reset_stats": (None, [_VP]),
     "jsmpeg_b200_debug_parse_picture": (ctypes.c_int, [_VP, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int, ctypes.c_int,
@@ -78,8 +79,8 @@ _BATCH_ABI = {
 
 
 def planes_view(t, info):
-    """Y [coded_h, coded_w], Cr and Cb [coded_h / 2, coded_w / 2] as views of a decode_intra planes tensor; `info` is
-    the stream's BatchDecoder.stream_info."""
+    """Y [coded_h, coded_w], Cr and Cb [coded_h / 2, coded_w / 2] as views of a decode_intra planes tensor (or of a
+    decode_residuals tensor, which has the same layout); `info` is the stream's BatchDecoder.stream_info."""
     cw, ch = (info["width"] + 15) // 16 * 16, (info["height"] + 15) // 16 * 16
     n = cw * ch
     return t[:n].view(ch, cw), t[n:n + n // 4].view(ch // 2, cw // 2), t[n + n // 4:n + n // 2].view(ch // 2, cw // 2)
@@ -119,6 +120,7 @@ class BatchDecoder:
         self.last_pictures_info = []  # per request of the last decode_pictures: {"status", "n_present", "error"}
         self.last_macroblocks_info = []  # per request of the last decode_macroblocks: {"n_present", "error"}
         self.last_coefficients_info = []  # per request of the last decode_coefficients: {"n_present", "error"}
+        self.last_residuals_info = []  # per request of the last decode_residuals: {"n_present", "error"}
         self.handle = self.lib.jsmpeg_b200_batch_create(n_streams, device, max_slots)
         err = self.lib.jsmpeg_b200_batch_last_error(self.handle)
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
@@ -328,7 +330,7 @@ class BatchDecoder:
         import torch
         reqs = [(int(s), int(p)) for s, p in requests]
         n = len(reqs)
-        out = self._per_macroblock_views(reqs, (MACROBLOCK_BYTES,), torch.uint8)
+        out = self._per_picture_views(reqs, lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8)
         streams, pictures, n_present, errors = self._request_arrays(reqs)
         dst = (_VP * max(n, 1))(*[t.data_ptr() for t in out])
         torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # the allocations are the caller's stream's; the call uses its own
@@ -351,8 +353,8 @@ class BatchDecoder:
         import torch
         reqs = [(int(s), int(p)) for s, p in requests]
         n = len(reqs)
-        coefs = self._per_macroblock_views(reqs, (6, 8, 8), torch.int16)
-        entries = self._per_macroblock_views(reqs, (MACROBLOCK_BYTES,), torch.uint8) if macroblocks else None
+        coefs = self._per_picture_views(reqs, lambda h, w: (h, w, 6, 8, 8), torch.int16)
+        entries = self._per_picture_views(reqs, lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8) if macroblocks else None
         streams, pictures, n_present, errors = self._request_arrays(reqs)
         coef_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in coefs])
         mb_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in entries]) if macroblocks else None
@@ -366,10 +368,37 @@ class BatchDecoder:
         self.last_coefficients_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
         return list(zip(coefs, entries)) if macroblocks else coefs
 
-    def _per_macroblock_views(self, reqs, per_mb, dtype):
-        """Per (stream, picture) request a CUDA tensor [mb_height, mb_width, *per_mb] of `dtype`, the views of one
+    def decode_residuals(self, requests, macroblocks=False):
+        """Pixel-domain residuals of pictures listed by macroblock_index, of any streams, in one call: `requests` is an
+        iterable of (stream, picture).  Returns per request a flat torch.int16 CUDA tensor of coded_size * 3 // 2 values
+        in the planes' layout (Y | Cr | Cb, see planes_view): every 8 x 8 block the reference's integer inverse
+        transform of what decode_coefficients gives for it (include/jsmpeg_b200.h), 0 for uncoded blocks and absent
+        macroblocks -- what stage 2 adds to the prediction, or for an intra macroblock clamps.  With macroblocks=True
+        each item is a pair (residual, entries), entries as decode_macroblocks returns them, from the same walk.
+        last_residuals_info gets {"n_present", "error"} per request.  The tensors are views of one allocation per
+        picture size."""
+        import torch
+        reqs = [(int(s), int(p)) for s, p in requests]
+        n = len(reqs)
+        res = self._per_picture_views(reqs, lambda h, w: (h * w * 384,), torch.int16)
+        entries = self._per_picture_views(reqs, lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8) if macroblocks else None
+        streams, pictures, n_present, errors = self._request_arrays(reqs)
+        res_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in res])
+        mb_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in entries]) if macroblocks else None
+        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # as in decode_macroblocks
+        got = self.lib.jsmpeg_b200_batch_decode_residuals(self.handle, n, streams, pictures, res_dst, mb_dst,
+                                                          n_present, errors)
+        if got == -2:
+            raise ValueError("a request names a picture that is not in the stream's macroblock index")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_residuals failed")
+        self.last_residuals_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
+        return list(zip(res, entries)) if macroblocks else res
+
+    def _per_picture_views(self, reqs, shape, dtype):
+        """Per (stream, picture) request a CUDA tensor of shape shape(mb_height, mb_width) and `dtype`, the views of one
         allocation per picture size (thousands of requests cost a few allocations, not thousands).  A view starts a
-        whole number of macroblocks into its allocation: with 16 * k bytes per macroblock it is 16-byte aligned."""
+        whole number of pictures into its allocation: with 16 * k bytes per macroblock it is 16-byte aligned."""
         import torch
         shapes = {}  # per stream: (mb_height, mb_width)
         for s, _ in reqs:
@@ -380,8 +409,8 @@ class BatchDecoder:
         for i, (s, _) in enumerate(reqs):
             by_shape.setdefault(shapes[s], []).append(i)
         out = [None] * len(reqs)
-        for shape, idx in by_shape.items():
-            views = torch.empty((len(idx), *shape, *per_mb), dtype=dtype, device=torch.device("cuda", self.device)).unbind(0)
+        for mb_shape, idx in by_shape.items():
+            views = torch.empty((len(idx), *shape(*mb_shape)), dtype=dtype, device=torch.device("cuda", self.device)).unbind(0)
             for i, t in zip(idx, views):
                 out[i] = t
         return out

@@ -11,8 +11,8 @@
  * A block with more than COEF_RECORD_LEVELS positions has mask == COEF_RECORD_DENSE: its dense 128-byte record
  * holds it, at its usual place in the coefficient plane.  Uncoded blocks write and read nothing.
  *
- * This header is the only place that knows the layout; the expand, reconstruct and coefficient export kernels, the
- * host engine's debug hooks and the tests all go through it.  It compiles as CUDA (host and device) and as plain C++.
+ * This header is the only place that knows the layout; the expand, reconstruct, coefficient and residual export
+ * kernels, the host engine's debug hooks and the tests all go through it.  It compiles as CUDA (host and device) and as plain C++.
  */
 #ifndef JSMPEG_B200_COEF_RECORDS_H
 #define JSMPEG_B200_COEF_RECORDS_H
@@ -90,6 +90,21 @@ COEF_FN void coef_record_row(const coef_record_t &r, int row, int16_t out[8]) {
 		out[c] = ((r.mask >> k) & 1) ? v : (int16_t)0;
 	}
 }
+
+// the values of a compact record (mask != COEF_RECORD_DENSE) into their raster places of a block whose other values
+// the caller has set: at most COEF_RECORD_LEVELS stores, and no index into the record at run time
+COEF_FN void coef_record_scatter(const coef_record_t &r, int16_t *raster) {
+	uint64_t m = r.mask;
+	for (int k = 0; k < COEF_RECORD_LEVELS; k++) {
+		if (m) {
+			raster[coef_zigzag_raster(coef_lowest64(m))] = r.level[k];
+			m &= m - 1;
+		}
+	}
+}
+
+// coefficient 0 of a compact record (mask != COEF_RECORD_DENSE): the first level when zig-zag position 0 is written
+COEF_FN int coef_record_dc(const coef_record_t &r) { return (r.mask & 1) ? r.level[0] : 0; }
 
 // whether a block with the zig-zag positions `written` fits a compact record
 COEF_FN bool coef_record_fits(uint64_t written) { return coef_popc64(written) <= COEF_RECORD_LEVELS; }

@@ -171,6 +171,25 @@ struct CoefExportTask {
 };
 void launch_export_coefficients(const CoefExportTask *tasks, int n_tasks, uint32_t total_mb, cudaStream_t stream);
 
+// Residual export (residuals.cu): request i writes the inverse transform of every block of one picture (`mb_width` x
+// `mb_height` macroblocks; records as CoefExportTask's) to `dst` in the public layout of
+// jsmpeg_b200_batch_decode_residuals: int16 planes Y | Cr | Cb of the coded size, 0 for uncoded blocks and absent
+// macroblocks.  One thread per block, a warp per 32 blocks of one request (6 * mb_size block slots rounded up to
+// whole warps); `first` is the number of warps of requests 0 .. i-1.  One launch for all requests.
+// (A type of its own: CoefExportTask, and so export_coefficients_kernel, stay as they are.)
+struct ResExportTask {
+	const mb_record_t *hdr;
+	const int16_t *coef;
+	const coef_record_t *compact;
+	int16_t *dst;
+	uint32_t first;
+	int32_t mb_width, mb_height;
+	int32_t pad;
+};
+// the warps of a request of mb_size macroblocks
+constexpr uint32_t res_export_warps(int mb_size) { return ((uint32_t)mb_size * 6 + 31) / 32; }
+void launch_export_residuals(const ResExportTask *tasks, int n_tasks, uint32_t total_warps, cudaStream_t stream);
+
 // device MPEG-TS demux (tsdemux.cu)
 struct TsScratch;
 TsScratch *ts_scratch_create();

@@ -26,7 +26,8 @@
 // queues one reconstruct step per picture depth (ReconStep, launch_reconstruct) on the reconstruct stream.
 // Cutting the wave into chunks to overlap stage 1 with stage 2 was measured not to pay (DESIGN 8).
 // decode_macroblocks runs the same waves walk-only (no expand, no reconstruct) and exports the records (DESIGN 3.8);
-// decode_coefficients runs them with expand and exports the coefficients too (DESIGN 3.9).
+// decode_coefficients runs them with expand and exports the coefficients too (DESIGN 3.9), decode_residuals their
+// inverse transform (DESIGN 3.10).
 #include <sched.h>
 
 #include <algorithm>
@@ -159,6 +160,9 @@ struct jsmpeg_b200_batch_t {
 	// decode_coefficients: the coefficient export tasks of a wave (DESIGN 3.9)
 	PinnedBuffer<CoefExportTask> h_ctasks;
 	DeviceBuffer<CoefExportTask> d_ctasks;
+	// decode_residuals: the residual export tasks of a wave (DESIGN 3.10)
+	PinnedBuffer<ResExportTask> h_rtasks;
+	DeviceBuffer<ResExportTask> d_rtasks;
 	jsmpeg_b200_stats_t stats{};
 };
 
@@ -1249,12 +1253,12 @@ long batch_decode_chosen(Batch *b, bool intra, int n, const int *streams, const 
 
 // Each unique (stream, picture) of the requests takes a record slot; waves of as many as there are free slots (after
 // flushing the look-ahead when they do not cover the call) run the walks alone -- or, with `coef_dst` (decode_coefficients,
-// DESIGN 3.9), the walks and the expand -- and one export launch per wave and destination kind, on the main stream
-// behind stage 1 and before the slots are released, writes every request of the wave to its destination: `dst` (may be
-// nullptr) gets the macroblock entries, `coef_dst` (nullptr: none) the coefficients.  The requests are valid (the
-// caller checked them).
+// DESIGN 3.9) or `res_dst` (decode_residuals, DESIGN 3.10), the walks and the expand -- and one export launch per wave
+// and destination kind, on the main stream behind stage 1 and before the slots are released, writes every request of
+// the wave to its destination: `dst` (may be nullptr) gets the macroblock entries, `coef_dst` (nullptr: none) the
+// coefficients, `res_dst` (nullptr: none) the residuals.  The requests are valid (the caller checked them).
 void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *const *dst, void *const *coef_dst,
-                        int32_t *n_present_out, int32_t *error_out) {
+                        void *const *res_dst, int32_t *n_present_out, int32_t *error_out) {
 	const int n = (int)req.size();
 	ensure_pool(b);
 	std::vector<std::pair<int, uint32_t>> uniq(n);
@@ -1275,25 +1279,36 @@ void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *
 		b->h_ctasks.reserve(n);
 		b->d_ctasks.reserve(n);
 	}
+	if (res_dst && (size_t)n > b->d_rtasks.size()) {
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		b->h_rtasks.reserve(n);
+		b->d_rtasks.reserve(n);
+	}
 	const size_t wave_max = b->free_slots.size();
 	RequestInfo out(n);
 	for (size_t lo = 0; lo < uniq.size(); lo += wave_max) {
 		const size_t hi = std::min(uniq.size(), lo + wave_max);
 		std::vector<WaveItem> wave;
 		for (size_t u = lo; u < hi; u++) wave.push_back(take_slot(b, uniq[u].first, uniq[u].second, true));
-		// (parse_wave waits for the infos, which also means the previous wave's task uploads have read h_xtasks / h_ctasks)
-		parse_wave(b, wave, coef_dst != nullptr);
+		// (parse_wave waits for the infos, which also means the previous wave's task uploads have read the task tables)
+		parse_wave(b, wave, coef_dst != nullptr || res_dst != nullptr);
 		int m = 0;
-		uint32_t total = 0;
+		uint32_t total = 0, res_warps = 0;
 		for (int i = 0; i < n; i++) {
 			if (uniq_of[i] < lo || uniq_of[i] >= hi) continue;
 			const WaveItem &w = wave[uniq_of[i] - lo];
 			const picture_info_t &info = b->h_info[uniq_of[i] - lo];
 			out.set(i, info);
-			const int mb_size = b->streams[w.stream].seq.mb_size;
+			const SeqParams &seq = b->streams[w.stream].seq;
+			const int mb_size = seq.mb_size;
 			const SlotRecords sr = slot_records(b, w.slot);
 			if (dst) b->h_xtasks[m] = MbExportTask{sr.hdr, dst[i], total, mb_size, info.picture_type, 0};
 			if (coef_dst) b->h_ctasks[m] = CoefExportTask{sr.hdr, sr.coef, sr.compact, coef_dst[i], total, mb_size};
+			if (res_dst) {
+				b->h_rtasks[m] = ResExportTask{sr.hdr, sr.coef, sr.compact, static_cast<int16_t *>(res_dst[i]), res_warps,
+				                               seq.mb_width, seq.mb_height, 0};
+				res_warps += res_export_warps(mb_size);
+			}
 			m++;
 			total += (uint32_t)mb_size;
 		}
@@ -1304,6 +1319,10 @@ void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *
 		if (coef_dst) {
 			CUDA_CHECK(cudaMemcpyAsync(b->d_ctasks.data(), b->h_ctasks.data(), m * sizeof(CoefExportTask), cudaMemcpyHostToDevice, b->st_main));
 			launch_export_coefficients(b->d_ctasks.data(), m, total, b->st_main);
+		}
+		if (res_dst) {
+			CUDA_CHECK(cudaMemcpyAsync(b->d_rtasks.data(), b->h_rtasks.data(), m * sizeof(ResExportTask), cudaMemcpyHostToDevice, b->st_main));
+			launch_export_residuals(b->d_rtasks.data(), m, res_warps, b->st_main);
 		}
 		// Released right behind the exports, which read the slots on st_main: the next wave's stage 1 rewrites them
 		// (records, dense records and -- through its walks and expands -- the compact planes) only after them.  Its
@@ -1320,7 +1339,7 @@ long batch_decode_macroblocks(Batch *b, int n, const int *streams, const uint32_
 	std::vector<PictureRequest> req;
 	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, mb_dst, nullptr, false, req)) return -2;
 	if (n == 0) return 0;
-	decode_macroblocks(b, req, mb_dst, nullptr, n_present_out, error_out);
+	decode_macroblocks(b, req, mb_dst, nullptr, nullptr, n_present_out, error_out);
 	return n;
 }
 
@@ -1331,7 +1350,18 @@ long batch_decode_coefficients(Batch *b, int n, const int *streams, const uint32
 	std::vector<PictureRequest> req;
 	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, coef_dst, mb_dst, mb_dst != nullptr, req)) return -2;
 	if (n == 0) return 0;
-	decode_macroblocks(b, req, mb_dst, coef_dst, n_present_out, error_out);
+	decode_macroblocks(b, req, mb_dst, coef_dst, nullptr, n_present_out, error_out);
+	return n;
+}
+
+// decode_residuals: decode_coefficients' requests and schedule with the residual export in place of the coefficient
+// export (DESIGN 3.10)
+long batch_decode_residuals(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *res_dst,
+                            void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
+	std::vector<PictureRequest> req;
+	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, res_dst, mb_dst, mb_dst != nullptr, req)) return -2;
+	if (n == 0) return 0;
+	decode_macroblocks(b, req, mb_dst, nullptr, res_dst, n_present_out, error_out);
 	return n;
 }
 
@@ -1592,6 +1622,14 @@ long jsmpeg_b200_batch_decode_coefficients(jsmpeg_b200_batch_t *b, int n, const 
                                            int32_t *error_out) {
 	return guarded<long>(b, -1, [&] {
 		return batch_decode_coefficients(b, n, streams, pictures, coef_dst, mb_dst, n_present_out, error_out);
+	});
+}
+
+long jsmpeg_b200_batch_decode_residuals(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                        void *const *res_dst, void *const *mb_dst, int32_t *n_present_out,
+                                        int32_t *error_out) {
+	return guarded<long>(b, -1, [&] {
+		return batch_decode_residuals(b, n, streams, pictures, res_dst, mb_dst, n_present_out, error_out);
 	});
 }
 
