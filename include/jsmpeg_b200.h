@@ -342,6 +342,52 @@ long jsmpeg_b200_batch_decode_residuals(jsmpeg_b200_batch_t *b, int n, const int
                                         void *const *res_dst, void *const *mb_dst,
                                         int32_t *n_present_out, int32_t *error_out);
 
+/* ACCUMULATED MOTION AND RESIDUALS (compressed-domain video models in the CoViAR style): chosen I and P pictures of any
+ * streams traced back through their reference chain to the key picture.  Every sample of a P picture follows its
+ * block's forward vector into the previous reference picture, and that sample's trace on, to the I picture or to
+ * where the trace ends; its motion is the sum of the vectors along the way and its residual the sum of the
+ * residuals.  So P picture k ~ the picture `back` references earlier, warped by the accumulated motion, plus the
+ * accumulated residual, and a model can take any picture of a GOP without its neighbours.
+ *
+ * The pictures are the I and P entries of the picture index (type 1 or 2), with the same chain start.  The chain is
+ * consumed by decode()'s rule with decode_b OFF: B pictures between references are skipped after their header, so
+ * neither the listing nor the result depends on decode_b.  B pictures are not accepted.
+ *
+ * Request i = picture pictures[i] of stream streams[i] into acc_dst[i]: DEVICE memory, 16-byte aligned, of
+ * coded_size * 3 / 2 records of jsmpeg_b200_accumulated_t (coded_size * 12 bytes), in the planes' layout counted in
+ * samples: Y at 0, Cr at coded_size, Cb at coded_size * 5 / 4 -- the map lines up sample for sample with
+ * decode_pictures' planes and decode_residuals' residual.  Every byte is written.
+ *
+ * The rule.  Let p0 (the I picture), p1, ..., pn = k be the chain's reference pictures as the fresh decoder of
+ * decode_pictures reconstructs them.  The map M_m of p_m, per sample i (its flat index in its plane), with the
+ * sample's macroblock in p_m's records and its 8 x 8 block:
+ *   1. macroblock not PRESENT: untraced, back = -1, dx = dy = residual = 0;
+ *   2. macroblock INTRA, or the block's prediction not inside the plane (stage 2's flat-index rule, half-sample taps
+ *      included; stage 2 predicts 0 for such a block): back = 0, dx = dy = residual = 0 (every macroblock of p0 is
+ *      under rule 1 or 2);
+ *   3. otherwise (forward-predicted, skipped and zero-vector macroblocks included), v = the forward vector, luma as
+ *      decode_macroblocks exports it, chroma each component halved with truncation toward zero (as stage 2), and
+ *      i' = i + (v_y >> 1) * stride + (v_x >> 1), the sample's first prediction tap in p_{m-1}: if M_{m-1}(i') is
+ *      untraced, so is the sample; else back = M_{m-1}(i').back + 1, (dx, dy) = sat16(M_{m-1}(i').d + v) and
+ *      residual = sat16(M_{m-1}(i').residual + r_m(i)), r_m being decode_residuals' residual of p_m.  sat16 saturates
+ *      to [-32768, 32767] at every depth.
+ * For a clean stream, k(x) ~ clamp(p_{n-back}(x + d / 2) + residual), exact with full-sample vectors and no clamping
+ * along the trace.
+ *
+ * status_out[i] (may be NULL) is PIC_DECODED, or 0 when the fresh decoder never consumes picture k: every record is
+ * then untraced.  n_present_out / error_out (may be NULL) are those of picture k.  Synchronous; duplicates each get
+ * the map.  Returns n; -1 dead; -2 a request is invalid (stream out of range or without sequence header, picture not
+ * an I or P entry of the picture index, NULL or misaligned acc_dst[i], a chain of more than 32,767 reference pictures)
+ * -- checked before any work, and then nothing changed.  Changes nothing decode() observes, as decode_intra. */
+typedef struct jsmpeg_b200_accumulated_t {
+	int16_t dx, dy;   /* accumulated motion, half-sample units of the sample's own plane */
+	int16_t residual; /* accumulated residual */
+	int16_t back;     /* reference pictures back to where the trace ends; -1: untraced */
+} jsmpeg_b200_accumulated_t; /* 8 bytes */
+long jsmpeg_b200_batch_decode_accumulated(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                          void *const *acc_dst, int32_t *status_out, int32_t *n_present_out,
+                                          int32_t *error_out);
+
 void jsmpeg_b200_batch_get_stats(jsmpeg_b200_batch_t *b, jsmpeg_b200_stats_t *out);
 void jsmpeg_b200_batch_reset_stats(jsmpeg_b200_batch_t *b);
 

@@ -61,6 +61,7 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_decode_macroblocks": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_decode_coefficients": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_decode_residuals": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "jsmpeg_b200_batch_decode_accumulated": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_get_stats": (None, [_VP, ctypes.POINTER(Stats)]),
     "jsmpeg_b200_batch_reset_stats": (None, [_VP]),
     "jsmpeg_b200_debug_parse_picture": (ctypes.c_int, [_VP, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int, ctypes.c_int,
@@ -99,6 +100,18 @@ def macroblocks_view(t):
             "qscale": t[..., 10]}
 
 
+ACCUMULATED_BYTES = 8  # sizeof(jsmpeg_b200_accumulated_t)
+
+
+def accumulated_view(t, info):
+    """Per plane (Y, Cr, Cb) of a decode_accumulated map [coded_size * 3 // 2, 4]: {"motion": int16 [h, w, 2] (dx, dy in
+    half-sample units of the plane), "residual": [h, w], "back": [h, w] (-1: untraced)}; `info` as in planes_view."""
+    cw, ch = (info["width"] + 15) // 16 * 16, (info["height"] + 15) // 16 * 16
+    n = cw * ch
+    planes = (t[:n].view(ch, cw, 4), t[n:n + n // 4].view(ch // 2, cw // 2, 4), t[n + n // 4:n + n // 2].view(ch // 2, cw // 2, 4))
+    return tuple({"motion": p[..., 0:2], "residual": p[..., 2], "back": p[..., 3]} for p in planes)
+
+
 def bind_batch_abi(lib):
     for name, (res, args) in _BATCH_ABI.items():
         fn = getattr(lib, name)
@@ -121,6 +134,7 @@ class BatchDecoder:
         self.last_macroblocks_info = []  # per request of the last decode_macroblocks: {"n_present", "error"}
         self.last_coefficients_info = []  # per request of the last decode_coefficients: {"n_present", "error"}
         self.last_residuals_info = []  # per request of the last decode_residuals: {"n_present", "error"}
+        self.last_accumulated_info = []  # per request of the last decode_accumulated: {"status", "n_present", "error"}
         self.handle = self.lib.jsmpeg_b200_batch_create(n_streams, device, max_slots)
         err = self.lib.jsmpeg_b200_batch_last_error(self.handle)
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
@@ -394,6 +408,32 @@ class BatchDecoder:
             raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_residuals failed")
         self.last_residuals_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
         return list(zip(res, entries)) if macroblocks else res
+
+    def decode_accumulated(self, requests):
+        """Accumulated motion and residuals of I and P pictures listed by picture_index (type 1 or 2), of any streams,
+        in one call: `requests` is an iterable of (stream, picture).  Returns per request a torch.int16 CUDA tensor
+        [coded_size * 3 // 2, 4] in the planes' layout (see accumulated_view): per sample (dx, dy, residual, back), the
+        sample traced through the reference chain to its key picture (include/jsmpeg_b200.h).  B pictures between
+        references are skipped, whatever the decode_b option says.  last_accumulated_info gets {"status",
+        "n_present", "error"} per request (status 0: the fresh decoder never reached the picture, whose samples are
+        then all untraced).  The tensors are views of one allocation per picture size."""
+        import torch
+        reqs = [(int(s), int(p)) for s, p in requests]
+        n = len(reqs)
+        maps = self._per_picture_views(reqs, lambda h, w: (h * w * 384, 4), torch.int16)
+        streams, pictures, n_present, errors = self._request_arrays(reqs)
+        status = (ctypes.c_int32 * max(n, 1))()
+        acc_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in maps])
+        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # as in decode_macroblocks
+        got = self.lib.jsmpeg_b200_batch_decode_accumulated(self.handle, n, streams, pictures, acc_dst, status,
+                                                            n_present, errors)
+        if got == -2:
+            raise ValueError("a request names a picture that is not an I or P picture of the stream's picture index")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_accumulated failed")
+        self.last_accumulated_info = [{"status": status[i], "n_present": n_present[i], "error": errors[i]}
+                                      for i in range(n)]
+        return maps
 
     def _per_picture_views(self, reqs, shape, dtype):
         """Per (stream, picture) request a CUDA tensor of shape shape(mb_height, mb_width) and `dtype`, the views of one

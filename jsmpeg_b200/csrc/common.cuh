@@ -93,6 +93,14 @@ struct PlaneSet {
 	uint8_t *y, *cr, *cb;
 };
 
+// PREDICTION_INSIDE: whether every tap an 8x8 block's prediction USES lies inside its plane of plane_size samples: the block's first tap
+// at flat index src (origin + (mv >> 1) * stride + (mh >> 1), mpeg1.js:479, 567), oh / ov its horizontal / vertical
+// half-sample flags.  A flat-index rule: a vector past a row's end wraps into the next row.  Stage 2 predicts 0 for a
+// block outside (recon.cuh), and the accumulated map ends its trace there (accumulate.cuh).  A macro: stage 2's machine
+// code is the same as with the expression written out (an inline function reorders it).
+#define PREDICTION_INSIDE(src, stride, plane_size, oh, ov) \
+	((src) >= 0 && (src) + 7 * (stride) + 7 + ((ov) ? (stride) : 0) + ((oh) ? 1 : 0) < (plane_size))
+
 // Stage 2: one task per (stream, picture); blockIdx.y selects the task.
 struct ReconTask {
 	const mb_record_t *hdr;
@@ -189,6 +197,22 @@ struct ResExportTask {
 // the warps of a request of mb_size macroblocks
 constexpr uint32_t res_export_warps(int mb_size) { return ((uint32_t)mb_size * 6 + 31) / 32; }
 void launch_export_residuals(const ResExportTask *tasks, int n_tasks, uint32_t total_warps, cudaStream_t stream);
+
+// Accumulated map (accumulate.cu, DESIGN 3.11): task i writes the map of one reference picture of a chain (records as
+// ResExportTask's) to `dst` from `prev`, the map of the chain's previous reference picture (nullptr: the chain's first
+// picture, which traces nothing back).  A map is one 8-byte record {dx, dy, residual, back} (int16 each, the public
+// jsmpeg_b200_accumulated_t) per sample of the planes Y | Cr | Cb.  The geometry of ResExportTask: a thread per block,
+// `first` warps before task i; one launch per chain depth.
+struct AccTask {
+	const mb_record_t *hdr;
+	const int16_t *coef;
+	const coef_record_t *compact;
+	const uint2 *prev;
+	uint2 *dst;
+	uint32_t first;
+	int32_t mb_width, mb_height;
+};
+void launch_accumulate(const AccTask *tasks, int n_tasks, uint32_t total_warps, cudaStream_t stream);
 
 // device MPEG-TS demux (tsdemux.cu)
 struct TsScratch;

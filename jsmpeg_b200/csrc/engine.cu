@@ -33,6 +33,7 @@
 #include <algorithm>
 #include <cstring>
 #include <deque>
+#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -163,6 +164,10 @@ struct jsmpeg_b200_batch_t {
 	// decode_residuals: the residual export tasks of a wave (DESIGN 3.10)
 	PinnedBuffer<ResExportTask> h_rtasks;
 	DeviceBuffer<ResExportTask> d_rtasks;
+	// decode_accumulated: the pool of the chains' two scratch map sets, and the tasks of a wave's depths (DESIGN 3.11)
+	DeviceBuffer<uint8_t> d_map_sets;
+	PinnedBuffer<AccTask> h_atasks;
+	DeviceBuffer<AccTask> d_atasks;
 	jsmpeg_b200_stats_t stats{};
 };
 
@@ -972,6 +977,7 @@ enum class Listing {
 	Pictures,     // decode_pictures: the pictures decode() reconstructs under the current decode_b, with a chain start
 	Macroblocks,  // decode_macroblocks: B pictures whatever decode_b says, no chain start needed (a picture's
 	              // macroblock layer depends on its own bits only)
+	Accumulated,  // decode_accumulated: the I and P pictures of Pictures, whatever decode_b says
 };
 
 // The pictures a random-access call can serve now: after the first sequence header, closed, decoded by the walks, and
@@ -989,7 +995,9 @@ std::vector<IndexEntry> list_pictures(const Batch *b, const Stream &s, Listing w
 		const bool after = s.pics[k] >= s.seq_floor;
 		if (after && h.type == 1) keys.push_back(k);
 		refs += h.type == 1 || (h.type == 2 && h.forward_f_code != 0);
-		const bool listed = what == Listing::Intra ? h.type == 1 : picture_decoded(h, what == Listing::Macroblocks || b->decode_b);
+		const bool listed = what == Listing::Intra         ? h.type == 1
+		                    : what == Listing::Accumulated ? picture_decoded(h, false)
+		                                                   : picture_decoded(h, what == Listing::Macroblocks || b->decode_b);
 		if (!after || !listed || !picture_closed(s, k)) continue;
 		if (what == Listing::Macroblocks) {
 			out.push_back({k, k});
@@ -1029,37 +1037,33 @@ struct PictureRequest {
 	uint32_t pic, from;
 };
 
-// The schedule behind decode_pictures and decode_intra (DESIGN 3.7).  Requests with the same stream and chain start
-// form a chain: pictures [first, last], parsed in waves over consecutive positions of every chain, consumed on the
-// host by decode()'s rule and reconstructed in launches by depth (launch d: the d-th reconstructed picture of every
-// chain of the wave).  A requested picture is copied to its destination right behind its launch -- or, in a chain
-// that reconstructs nothing else, reconstructed straight into it.  The requests are valid (the caller checked them).
-void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const *planes_dst, void *const *rgba_dst,
-                   bool rgba, int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
+// One chain of the random-access schedule: the requests with the same stream and chain start
+struct Chain {
+	int stream;
+	uint32_t first, last;  // chain start, last requested picture
+	uint32_t b_end;        // last requested B picture + 1; 0: none (B pictures after it are not reconstructed)
+	int req_lo, req_hi;    // its requests: order[req_lo .. req_hi)
+	int req_next;          // the first of them not consumed yet
+	int n_sets;            // sets from the caller's pool: 0 (a leaf: its one picture goes to its destination), 2, 4
+	uint8_t *set[4];
+	int cur, b_cur;        // as Stream::cur / b_cur
+	const uint2 *map;      // decode_accumulated: the map of the newest reference picture (nullptr: none yet)
+	uint32_t next;         // the picture decode() consumes next; beyond `last`: the chain is done
+	std::vector<picture_info_t> info;  // per picture of the chain, once parsed
+	std::vector<int> slot;
+};
+
+// The requests in chain order (by stream, chain start and picture) and their chains, with n_sets 0 for a chain of one
+// picture and 2 (4 with a B picture requested) otherwise
+std::vector<Chain> make_chains(const Batch *b, const std::vector<PictureRequest> &req, std::vector<int> &order) {
 	const int n = (int)req.size();
-	ensure_pool(b);
-	std::vector<int> order(n);  // the requests by stream, chain start and picture
+	order.resize(n);
 	for (int i = 0; i < n; i++) order[i] = i;
 	std::sort(order.begin(), order.end(), [&](int x, int y) {
 		const PictureRequest &p = req[x], &q = req[y];
 		return p.stream != q.stream ? p.stream < q.stream : p.from != q.from ? p.from < q.from : p.pic != q.pic ? p.pic < q.pic : x < y;
 	});
-	struct Chain {
-		int stream;
-		uint32_t first, last;  // chain start, last requested picture
-		uint32_t b_end;        // last requested B picture + 1; 0: none (B pictures after it are not reconstructed)
-		int req_lo, req_hi;    // its requests: order[req_lo .. req_hi)
-		int req_next;          // the first of them not consumed yet
-		int n_sets;            // plane sets: 0 (a leaf: it reconstructs the one picture requested), 2 (I/P), 4 (+ B)
-		uint8_t *set[4];
-		int cur, b_cur;        // as Stream::cur / b_cur
-		uint32_t next;         // the picture decode() consumes next; beyond `last`: the chain is done
-		std::vector<picture_info_t> info;  // per picture of the chain, once parsed
-		std::vector<int> slot;
-	};
 	std::vector<Chain> chains;
-	size_t set_bytes = 0, n_tasks = 0;
-	bool leaves = false;
 	for (int lo = 0; lo < n;) {
 		const PictureRequest &r = req[order[lo]];
 		int hi = lo + 1;
@@ -1076,12 +1080,165 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 		c.n_sets = c.last == c.first ? 0 : (c.b_end ? 4 : 2);
 		c.info.resize(c.last - c.first + 1);
 		c.slot.resize(c.last - c.first + 1);
+		chains.push_back(std::move(c));
+		lo = hi;
+	}
+	return chains;
+}
+
+// What a caller of run_chains does with the pictures its chains consume
+struct ChainWork {
+	// picture e of chain `ch` (stream s) is consumed and decoded, the d-th of its chain in this wave: records in `slot`,
+	// named by requests order[q_lo .. q_hi)
+	virtual void picture(Chain &ch, const Stream &s, int slot, const picture_info_t &e, size_t d, int q_lo, int q_hi) = 0;
+	// the wave's depths, one after the other on the reconstruct stream
+	virtual void depths() = 0;
+	virtual ~ChainWork() = default;
+};
+
+// The schedule behind decode_pictures, decode_intra and decode_accumulated (DESIGN 3.7).  The chains' pictures
+// [first, last] are parsed in waves over consecutive positions of every chain, consumed on the host by decode()'s rule
+// (b_walk: B pictures go to the B walk, as decode_b; else they are skipped after their header) and handed to `work`
+// by depth (depth d: the d-th decoded picture of every chain of the wave).  Chains run in groups of at most a wave's
+// slots, each chain's sets (set_bytes each, zeroed first with zero_sets) within half of the free device memory, from
+// `pool` -- a request beyond the device is cut into groups, not refused.  The requests are valid (the caller checked
+// them); on return the work is queued on the reconstruct stream, and the infos are the consumed pictures'.
+RequestInfo run_chains(Batch *b, const std::vector<PictureRequest> &req, const std::vector<int> &order,
+                       std::vector<Chain> &chains, bool b_walk, size_t set_bytes, DeviceBuffer<uint8_t> &pool,
+                       bool zero_sets, ChainWork &work) {
+	size_t n_tasks = 0;
+	for (const Chain &c : chains) n_tasks += c.info.size();
+	RequestInfo out((int)req.size());
+	free_slots_for(b, n_tasks);
+	const int wave_max = (int)b->free_slots.size();
+	size_t free_b = 0, total_b = 0;
+	CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+	const size_t max_sets = std::max<size_t>(4, ((size_t)(0.5 * (double)free_b) + pool.size()) / set_bytes);
+	std::vector<std::pair<size_t, size_t>> groups;
+	size_t most_sets = 0;
+	for (size_t lo = 0; lo < chains.size();) {
+		size_t hi = lo, sets = 0;
+		while (hi < chains.size() && hi - lo < (size_t)wave_max && sets + chains[hi].n_sets <= max_sets) sets += chains[hi++].n_sets;
+		groups.push_back({lo, hi});
+		most_sets = std::max(most_sets, sets);
+		lo = hi;
+	}
+	if (most_sets * set_bytes > pool.size()) {
+		if (pool.data()) CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+		pool.reserve(most_sets * set_bytes);
+	}
+	for (const auto &[glo, ghi] : groups) {
+		size_t sets = 0;
+		for (size_t c = glo; c < ghi; c++)
+			for (int k = 0; k < chains[c].n_sets; k++) chains[c].set[k] = pool.data() + set_bytes * sets++;
+		if (sets && zero_sets)  // (the previous group's copies are queued before)
+			CUDA_CHECK(cudaMemsetAsync(pool.data(), 0, set_bytes * sets, b->st_recon));
+		const uint32_t width = (uint32_t)std::max<size_t>(1, (size_t)wave_max / (ghi - glo));
+		for (uint32_t lo = 0;; lo += width) {
+			// ---- stage 1: positions [lo, lo + width) of every chain still consuming
+			std::vector<WaveItem> wave;
+			std::vector<int> wave_chain;  // the chain of each picture of the wave
+			for (size_t c = glo; c < ghi; c++) {
+				Chain &ch = chains[c];
+				if (ch.next > ch.last) continue;
+				for (uint32_t p = ch.first + lo; p <= ch.last && p - ch.first < lo + width; p++) {
+					wave.push_back(take_slot(b, ch.stream, p, b_walk));
+					ch.slot[p - ch.first] = wave.back().slot;
+					wave_chain.push_back((int)c);
+				}
+			}
+			if (wave.empty()) break;
+			parse_wave(b, wave, true);
+			for (size_t t = 0; t < wave.size(); t++) {
+				Chain &ch = chains[wave_chain[t]];
+				ch.info[wave[t].pic - ch.first] = b->h_info[t];
+			}
+			// ---- decode()'s consumption rule over the infos (decode_round): which pictures are decoded, at which depth
+			for (size_t c = glo; c < ghi; c++) {
+				Chain &ch = chains[c];
+				const Stream &s = b->streams[ch.stream];
+				const uint32_t parsed_end = std::min(ch.last + 1, ch.first + lo + width);
+				size_t d = 0;
+				while (ch.next < parsed_end) {
+					const uint32_t k = ch.next;
+					const picture_info_t &e = ch.info[k - ch.first];
+					while (ch.req_next < ch.req_hi && req[order[ch.req_next]].pic < k) ch.req_next++;  // passed over: status 0
+					const int q_lo = ch.req_next;
+					while (ch.req_next < ch.req_hi && req[order[ch.req_next]].pic == k) ch.req_next++;
+					const int q_hi = ch.req_next;
+					for (int q = q_lo; q < q_hi; q++) out.set(order[q], e);
+					const bool is_b = e.picture_type == 3;  // (only the B walk answers PIC_DECODED for one)
+					if (e.status == PIC_DECODED && (!is_b || k < ch.b_end))
+						work.picture(ch, s, ch.slot[k - ch.first], e, d++, q_lo, q_hi);
+					// the next picture: the first picture start code at or after where this one's parse ended
+					ch.next = (uint32_t)(std::lower_bound(s.pics.begin(), s.pics.end(), (e.end_bit + 7) >> 3) - s.pics.begin());
+				}
+			}
+			// ---- stage 2, then the slots go back: the next wave's parse waits for ev_round
+			work.depths();
+			CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
+			b->recon_pending = true;
+			for (const WaveItem &w : wave) release_slot(b, w.slot);
+		}
+	}
+	return out;
+}
+
+// decode_pictures and decode_intra: each depth is one launch_reconstruct, followed by the copies of its requested
+// pictures.  A requested picture is copied to its destination right behind its launch -- or, in a chain that
+// reconstructs nothing else, reconstructed straight into it.
+struct PlaneWork : ChainWork {
+	Batch *b;
+	const std::vector<int> &order;
+	void *const *planes_dst, *const *rgba_dst;
+	bool rgba;
+	std::vector<ReconStep> steps;
+	PlaneWork(Batch *b, const std::vector<int> &order, void *const *planes_dst, void *const *rgba_dst, bool rgba)
+	    : b(b), order(order), planes_dst(planes_dst), rgba_dst(rgba_dst), rgba(rgba) {}
+	void picture(Chain &ch, const Stream &s, int slot, const picture_info_t &e, size_t d, int q_lo, int q_hi) override {
+		const bool is_b = e.picture_type == 3;
+		const bool leaf = ch.n_sets == 0;
+		uint8_t *out_rgba = rgba && q_hi > q_lo ? static_cast<uint8_t *>(rgba_dst[order[q_lo]]) : nullptr;
+		ReconTask t;
+		if (is_b)  // the two I/P sets: `cur` the older (forward), `1 - cur` the newer (backward) reference
+			t = recon_task(b, s, slot, ch.set[2 + ch.b_cur], ch.set[ch.cur], ch.set[1 - ch.cur], out_rgba);
+		else if (leaf)  // into the destination, predicted (skipped macroblocks) from the zeroed scratch set
+			t = recon_task(b, s, slot, static_cast<uint8_t *>(planes_dst[order[q_lo]]), b->d_intra_fwd.data(), nullptr, out_rgba);
+		else
+			t = recon_task(b, s, slot, ch.set[ch.cur], ch.set[1 - ch.cur], nullptr, out_rgba);
+		if (steps.size() <= d) steps.emplace_back();
+		ReconStep &dp = steps[d];
+		dp.tasks.push_back(t);
+		for (int q = q_lo; q < q_hi; q++) {  // the first request gets the picture, duplicates a copy of it
+			if (!leaf || q > q_lo) dp.copy(planes_dst[order[q]], t.cur.y, (size_t)s.coded_size * 3 / 2);
+			if (rgba && q > q_lo) dp.copy(rgba_dst[order[q]], t.rgba, (size_t)s.width * s.height * 4);
+		}
+		if (is_b) ch.b_cur ^= 1;
+		else ch.cur ^= 1;
+	}
+	// (a set is overwritten two references later, by a later launch on the same stream)
+	void depths() override {
+		for (ReconStep &dp : steps) {
+			launch_reconstruct(dp.tasks.data(), (int)dp.tasks.size(), b->st_recon);
+			if (!dp.dst.empty()) copy_batch(b, dp.dst, dp.src, dp.size, b->st_recon);
+		}
+		steps.clear();
+	}
+};
+
+// decode_pictures and decode_intra (DESIGN 3.6, 3.7): run_chains with plane sets, B pictures as decode_b says
+void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const *planes_dst, void *const *rgba_dst,
+                   bool rgba, int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
+	ensure_pool(b);
+	std::vector<int> order;
+	std::vector<Chain> chains = make_chains(b, req, order);
+	size_t set_bytes = 0;
+	bool leaves = false;
+	for (const Chain &c : chains) {
+		const Stream &s = b->streams[c.stream];
 		leaves |= c.n_sets == 0;
 		// + coded_width + 64: parse_sequence_header's slack; a multiple of 256 keeps every set of the pool aligned
 		set_bytes = std::max(set_bytes, ((size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64 + 255) & ~(size_t)255);
-		n_tasks += c.info.size();
-		chains.push_back(std::move(c));
-		lo = hi;
 	}
 	if (leaves && set_bytes > b->d_intra_fwd.size()) {
 		if (b->d_intra_fwd.data()) CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
@@ -1097,112 +1254,16 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 			if (c.n_sets == 0) CUDA_CHECK(cudaMemsetAsync(planes_dst[i], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
 			if (rgba) CUDA_CHECK(cudaMemsetAsync(rgba_dst[i], 0xff, (size_t)s.width * s.height * 4, b->st_recon));
 		}
-	RequestInfo out(n);
-	free_slots_for(b, n_tasks);
-	const int wave_max = (int)b->free_slots.size();
-	// chain groups: at most wave_max chains (a wave parses at least one picture of each), and plane sets within half
-	// of the free device memory -- a request beyond the device is cut into groups, not refused
-	size_t free_b = 0, total_b = 0;
-	CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-	const size_t max_sets = std::max<size_t>(4, ((size_t)(0.5 * (double)free_b) + b->d_chain_sets.size()) / set_bytes);
-	std::vector<std::pair<size_t, size_t>> groups;
-	size_t most_sets = 0;
-	for (size_t lo = 0; lo < chains.size();) {
-		size_t hi = lo, sets = 0;
-		while (hi < chains.size() && hi - lo < (size_t)wave_max && sets + chains[hi].n_sets <= max_sets) sets += chains[hi++].n_sets;
-		groups.push_back({lo, hi});
-		most_sets = std::max(most_sets, sets);
-		lo = hi;
-	}
-	if (most_sets * set_bytes > b->d_chain_sets.size()) {
-		if (b->d_chain_sets.data()) CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-		b->d_chain_sets.reserve(most_sets * set_bytes);
-	}
-	for (const auto &[glo, ghi] : groups) {
-		size_t sets = 0;
-		for (size_t c = glo; c < ghi; c++)
-			for (int k = 0; k < chains[c].n_sets; k++) chains[c].set[k] = b->d_chain_sets.data() + set_bytes * sets++;
-		if (sets)  // a fresh decoder's planes start zeroed, the B sets too (the previous group's copies are queued before)
-			CUDA_CHECK(cudaMemsetAsync(b->d_chain_sets.data(), 0, set_bytes * sets, b->st_recon));
-		const uint32_t width = (uint32_t)std::max<size_t>(1, (size_t)wave_max / (ghi - glo));
-		for (uint32_t lo = 0;; lo += width) {
-			// ---- stage 1: positions [lo, lo + width) of every chain still consuming
-			std::vector<WaveItem> wave;
-			std::vector<int> wave_chain;  // the chain of each picture of the wave
-			for (size_t c = glo; c < ghi; c++) {
-				Chain &ch = chains[c];
-				if (ch.next > ch.last) continue;
-				for (uint32_t p = ch.first + lo; p <= ch.last && p - ch.first < lo + width; p++) {
-					wave.push_back(take_slot(b, ch.stream, p, b->decode_b));
-					ch.slot[p - ch.first] = wave.back().slot;
-					wave_chain.push_back((int)c);
+	PlaneWork work(b, order, planes_dst, rgba_dst, rgba);
+	// (a fresh decoder's planes start zeroed, the B sets too)
+	const RequestInfo out = run_chains(b, req, order, chains, b->decode_b, set_bytes, b->d_chain_sets, true, work);
+	for (const Chain &c : chains)  // never consumed: planes 0 (a copied destination was not zeroed)
+		if (c.n_sets)
+			for (int q = c.req_lo; q < c.req_hi; q++)
+				if (out.status[order[q]] == 0) {
+					const Stream &s = b->streams[c.stream];
+					CUDA_CHECK(cudaMemsetAsync(planes_dst[order[q]], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
 				}
-			}
-			if (wave.empty()) break;
-			parse_wave(b, wave, true);
-			for (size_t t = 0; t < wave.size(); t++) {
-				Chain &ch = chains[wave_chain[t]];
-				ch.info[wave[t].pic - ch.first] = b->h_info[t];
-			}
-			// ---- decode()'s consumption rule over the infos (decode_round): which pictures reconstruct, at which depth
-			std::vector<ReconStep> depths;
-			for (size_t c = glo; c < ghi; c++) {
-				Chain &ch = chains[c];
-				const Stream &s = b->streams[ch.stream];
-				const uint32_t parsed_end = std::min(ch.last + 1, ch.first + lo + width);
-				size_t d = 0;
-				while (ch.next < parsed_end) {
-					const uint32_t k = ch.next;
-					const picture_info_t &e = ch.info[k - ch.first];
-					while (ch.req_next < ch.req_hi && req[order[ch.req_next]].pic < k) ch.req_next++;  // passed over: status 0
-					const int q_lo = ch.req_next;
-					while (ch.req_next < ch.req_hi && req[order[ch.req_next]].pic == k) ch.req_next++;
-					const int q_hi = ch.req_next;
-					for (int q = q_lo; q < q_hi; q++) out.set(order[q], e);
-					const bool is_b = e.picture_type == 3;  // (only the B walk answers PIC_DECODED for one)
-					if (e.status == PIC_DECODED && (!is_b || k < ch.b_end)) {
-						const int slot = ch.slot[k - ch.first];
-						const bool leaf = ch.n_sets == 0;
-						uint8_t *out_rgba = rgba && q_hi > q_lo ? static_cast<uint8_t *>(rgba_dst[order[q_lo]]) : nullptr;
-						ReconTask t;
-						if (is_b)  // the two I/P sets: `cur` the older (forward), `1 - cur` the newer (backward) reference
-							t = recon_task(b, s, slot, ch.set[2 + ch.b_cur], ch.set[ch.cur], ch.set[1 - ch.cur], out_rgba);
-						else if (leaf)  // into the destination, predicted (skipped macroblocks) from the zeroed scratch set
-							t = recon_task(b, s, slot, static_cast<uint8_t *>(planes_dst[order[q_lo]]), b->d_intra_fwd.data(), nullptr, out_rgba);
-						else
-							t = recon_task(b, s, slot, ch.set[ch.cur], ch.set[1 - ch.cur], nullptr, out_rgba);
-						if (depths.size() <= d) depths.emplace_back();
-						ReconStep &dp = depths[d++];
-						dp.tasks.push_back(t);
-						for (int q = q_lo; q < q_hi; q++) {  // the first request gets the picture, duplicates a copy of it
-							if (!leaf || q > q_lo) dp.copy(planes_dst[order[q]], t.cur.y, (size_t)s.coded_size * 3 / 2);
-							if (rgba && q > q_lo) dp.copy(rgba_dst[order[q]], t.rgba, (size_t)s.width * s.height * 4);
-						}
-						if (is_b) ch.b_cur ^= 1;
-						else ch.cur ^= 1;
-					}
-					// the next picture: the first picture start code at or after where this one's parse ended
-					ch.next = (uint32_t)(std::lower_bound(s.pics.begin(), s.pics.end(), (e.end_bit + 7) >> 3) - s.pics.begin());
-				}
-			}
-			// ---- stage 2: one depth after the other on the reconstruct stream, each followed by its copies (a set is
-			// overwritten two references later, by a later launch on the same stream)
-			for (ReconStep &dp : depths) {
-				launch_reconstruct(dp.tasks.data(), (int)dp.tasks.size(), b->st_recon);
-				if (!dp.dst.empty()) copy_batch(b, dp.dst, dp.src, dp.size, b->st_recon);
-			}
-			CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
-			b->recon_pending = true;
-			for (const WaveItem &w : wave) release_slot(b, w.slot);  // reused by the next wave's parse, which waits for ev_round
-		}
-		for (size_t c = glo; c < ghi; c++)  // never consumed: planes 0 (a copied destination was not zeroed)
-			if (chains[c].n_sets)
-				for (int q = chains[c].req_lo; q < chains[c].req_hi; q++)
-					if (out.status[order[q]] == 0) {
-						const Stream &s = b->streams[chains[c].stream];
-						CUDA_CHECK(cudaMemsetAsync(planes_dst[order[q]], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
-					}
-	}
 	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
 	b->recon_pending = false;
 	out.copy_out(status_out, n_present_out, error_out);
@@ -1362,6 +1423,117 @@ long batch_decode_residuals(Batch *b, int n, const int *streams, const uint32_t 
 	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, res_dst, mb_dst, mb_dst != nullptr, req)) return -2;
 	if (n == 0) return 0;
 	decode_macroblocks(b, req, mb_dst, nullptr, res_dst, n_present_out, error_out);
+	return n;
+}
+
+// ---- decode_accumulated: chosen I and P pictures traced back to their key picture (DESIGN 3.11) ------------------
+
+// Each depth is one accumulate launch over the chains' pictures of that depth.  A requested picture's map is written
+// straight into its first destination, duplicates get a copy of it; an unrequested one's goes to the chain's scratch set
+// `cur` (the other set holds the map it reads, or an older one).  The next depth of the chain reads it where it is.
+struct MapWork : ChainWork {
+	Batch *b;
+	const std::vector<int> &order;
+	void *const *acc_dst;
+	std::vector<std::vector<AccTask>> tasks;  // per depth
+	std::vector<ReconStep> copies;           // per depth: its copy lists (no reconstruct task)
+	MapWork(Batch *b, const std::vector<int> &order, void *const *acc_dst) : b(b), order(order), acc_dst(acc_dst) {}
+	void picture(Chain &ch, const Stream &s, int slot, const picture_info_t &, size_t d, int q_lo, int q_hi) override {
+		uint2 *out;
+		if (q_hi > q_lo) {
+			out = static_cast<uint2 *>(acc_dst[order[q_lo]]);
+		} else {
+			out = reinterpret_cast<uint2 *>(ch.set[ch.cur]);
+			ch.cur ^= 1;
+		}
+		const SlotRecords sr = slot_records(b, slot);
+		if (tasks.size() <= d) {
+			tasks.emplace_back();
+			copies.emplace_back();
+		}
+		tasks[d].push_back(AccTask{sr.hdr, sr.coef, sr.compact, ch.map, out, 0, s.seq.mb_width, s.seq.mb_height});
+		ch.map = out;
+		for (int q = q_lo + 1; q < q_hi; q++) copies[d].copy(acc_dst[order[q]], out, (size_t)s.coded_size * 12);
+	}
+	// every depth's tasks in one upload (the previous wave's launches have read theirs: parse_wave waited for ev_round)
+	void depths() override {
+		size_t m = 0;
+		for (auto &dt : tasks) {
+			uint32_t warps = 0;
+			for (AccTask &t : dt) {
+				t.first = warps;
+				warps += res_export_warps(t.mb_width * t.mb_height);
+				b->h_atasks[m++] = t;
+			}
+		}
+		CUDA_CHECK(cudaMemcpyAsync(b->d_atasks.data(), b->h_atasks.data(), m * sizeof(AccTask), cudaMemcpyHostToDevice, b->st_recon));
+		size_t off = 0;
+		for (size_t d = 0; d < tasks.size(); d++) {
+			const AccTask &last = tasks[d].back();
+			launch_accumulate(b->d_atasks.data() + off, (int)tasks[d].size(), last.first + res_export_warps(last.mb_width * last.mb_height),
+			                  b->st_recon);
+			off += tasks[d].size();
+			if (!copies[d].dst.empty()) copy_batch(b, copies[d].dst, copies[d].src, copies[d].size, b->st_recon);
+		}
+		tasks.clear();
+		copies.clear();
+	}
+};
+
+// run_chains with two scratch map sets per chain (none for a chain of one picture) and B pictures skipped after their
+// header, whatever decode_b says.  The requests are valid (the caller checked them).
+void decode_accumulated(Batch *b, const std::vector<PictureRequest> &req, void *const *acc_dst, int32_t *status_out,
+                        int32_t *n_present_out, int32_t *error_out) {
+	ensure_pool(b);
+	std::vector<int> order;
+	std::vector<Chain> chains = make_chains(b, req, order);
+	size_t set_bytes = 0, n_tasks = 0;
+	for (Chain &c : chains) {
+		c.n_sets = c.n_sets ? 2 : 0;  // (no B picture is requested)
+		set_bytes = std::max(set_bytes, ((size_t)b->streams[c.stream].coded_size * 12 + 255) & ~(size_t)255);
+		n_tasks += c.info.size();
+	}
+	if (n_tasks > b->d_atasks.size()) {  // (a wave's tasks are at most the chains' pictures)
+		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+		b->h_atasks.reserve(n_tasks);
+		b->d_atasks.reserve(n_tasks);
+	}
+	MapWork work(b, order, acc_dst);
+	// (a scratch set is read only after the chain wrote it)
+	const RequestInfo out = run_chains(b, req, order, chains, false, set_bytes, b->d_map_sets, false, work);
+	for (int i = 0; i < (int)req.size(); i++)  // never consumed: every record untraced {0, 0, 0, -1}
+		if (out.status[i] != PIC_DECODED) {
+			const size_t n_rec = (size_t)b->streams[req[i].stream].coded_size * 3 / 2;
+			CUDA_CHECK(cudaMemsetAsync(acc_dst[i], 0, n_rec * 8, b->st_recon));
+			CUDA_CHECK(cudaMemset2DAsync(static_cast<uint8_t *>(acc_dst[i]) + 6, 8, 0xff, 2, n_rec, b->st_recon));
+		}
+	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+	b->recon_pending = false;
+	out.copy_out(status_out, n_present_out, error_out);
+}
+
+// decode_accumulated's requests: decode_pictures' checks over the I and P pictures, and no chain of more than 32,767
+// reference pictures (`back` is int16)
+long batch_decode_accumulated(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *acc_dst,
+                              int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
+	std::vector<PictureRequest> req;
+	if (!check_requests(b, Listing::Accumulated, n, streams, pictures, acc_dst, nullptr, false, req)) return -2;
+	std::map<std::pair<int, uint32_t>, uint32_t> chain_last;  // per (stream, chain start): the last picture requested
+	for (const PictureRequest &r : req) {
+		uint32_t &last = chain_last[{r.stream, r.from}];
+		last = std::max(last, r.pic);
+	}
+	for (const auto &[key, last] : chain_last) {
+		const Stream &s = b->streams[key.first];
+		uint32_t refs = 0;
+		for (uint32_t k = key.second; k <= last; k++) {
+			const PictureHeader h = picture_header(s, s.pics[k]);
+			refs += h.type == 1 || (h.type == 2 && h.forward_f_code != 0);
+		}
+		if (refs > 32767) return -2;
+	}
+	if (n == 0) return 0;
+	decode_accumulated(b, req, acc_dst, status_out, n_present_out, error_out);
 	return n;
 }
 
@@ -1630,6 +1802,14 @@ long jsmpeg_b200_batch_decode_residuals(jsmpeg_b200_batch_t *b, int n, const int
                                         int32_t *error_out) {
 	return guarded<long>(b, -1, [&] {
 		return batch_decode_residuals(b, n, streams, pictures, res_dst, mb_dst, n_present_out, error_out);
+	});
+}
+
+long jsmpeg_b200_batch_decode_accumulated(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                          void *const *acc_dst, int32_t *status_out, int32_t *n_present_out,
+                                          int32_t *error_out) {
+	return guarded<long>(b, -1, [&] {
+		return batch_decode_accumulated(b, n, streams, pictures, acc_dst, status_out, n_present_out, error_out);
 	});
 }
 

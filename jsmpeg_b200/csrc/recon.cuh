@@ -358,7 +358,7 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 	// every tap the prediction USES lies inside the plane.  (What the row loads touch beyond them -- the
 	// rest of the last word, row 8 of a lane without a vertical half -- is inside the allocation: planes
 	// are contiguous and followed by coded_width + 64 readable bytes.)
-	const bool inside = src >= 0 && src + 7 * stride + 7 + (ov ? stride : 0) + (oh ? 1 : 0) < plane_size;
+	const bool inside = PREDICTION_INSIDE(src, stride, plane_size, oh, ov);
 	// BIDIR: which references the block uses (a record with neither bit predicts forward, like the oracle), and the
 	// same geometry for the backward one
 	const bool use_b = BIDIR && (flags & MBF_MOTION_BWD);
@@ -371,7 +371,7 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		if (!use_b) bh = bv = 0;
 		ohb = bh & 1; ovb = bv & 1;
 		src_b = origin + (bv >> 1) * stride + (bh >> 1);
-		inside_b = src_b >= 0 && src_b + 7 * stride + 7 + (ovb ? stride : 0) + (ohb ? 1 : 0) < plane_size;
+		inside_b = PREDICTION_INSIDE(src_b, stride, plane_size, ohb, ovb);
 		if (present && !intra && use_b && inside_b) {
 #pragma unroll
 			for (int r = 0; r < 9; r++) prefetch_l2(t.bwd + plane_off + src_b + r * stride + 4);
