@@ -21,9 +21,9 @@
 //       chain) is its in-kernel fall-back and, with JSMPEG_B200_WALK=serial, a kernel of its own.
 //   1b  expand_blocks_kernel    one thread per coded BLOCK, all blocks of all pictures at once:
 //       re-reads the block's codes from its bit offset, does run/level -> zig-zag -> dequantise ->
-//       oddify -> clip (src/mpeg1.js:757-811) into a shared-memory tile; the block leaves as its 32-byte
-//       compact record (coef_records.h) or, with more than 12 values, as the 64 x int16 dense record,
-//       each as one TMA bulk store.
+//       oddify -> clip (src/mpeg1.js:757-811) straight into its 32-byte compact record (coef_records.h) in
+//       shared memory, which the warp stores with its neighbours' as whole 512-byte stretches; a block of more
+//       than 12 values is decoded again into a 64 x int16 tile and leaves as the dense record, one TMA bulk store.
 //
 // VLCs are decoded with clz-indexed look-up tables in shared memory (tools/gen_tables.py; pinned
 // to the reference's trees by tests/test_vlc_tables.py) instead of the reference's one-bit-per-step
@@ -42,8 +42,7 @@
 namespace {
 
 constexpr int CTA_THREADS = 128;       // expand kernel
-constexpr uint32_t TILE_PITCH = 144;   // bytes between the per-thread 64 x int16 tiles of the expand kernel (128 + 16: bank spread)
-constexpr uint32_t EXPAND_SMEM = EXP_OFF_TILES + CTA_THREADS * TILE_PITCH;
+constexpr uint32_t EXPAND_SMEM = EXP_OFF_TILES + CTA_THREADS * EXP_TILE_PITCH;
 
 // ==================================================================================================
 // 1a: one warp per picture (walk.cuh), serial or lane-parallel with serial fall-back
@@ -100,8 +99,8 @@ walk_pictures_slices_kernel(const ParseTask *__restrict__ tasks, int n_tasks, co
 // 1b: expand every coded block (one thread per block slot, grid.y = picture)
 //
 // A CTA stages the tables once and then takes EXPAND_GROUPS runs of CTA_THREADS consecutive slots, one after
-// the other: the warps go through their runs independently (tiles are per thread, the tables read-only, so
-// the one barrier is the one after staging), and a thread asks for the next run's inputs before it expands
+// the other: the warps go through their runs independently (staging areas are per warp, the tables read-only, so
+// the one CTA barrier is the one after staging), and a thread asks for the next run's inputs before it expands
 // the current block -- the staging, the barrier and the exposed load latency at the start of a CTA are paid
 // once per EXPAND_GROUPS runs.
 #ifndef JSMPEG_EXPAND_GROUPS
@@ -141,9 +140,9 @@ expand_blocks_kernel(const ParseTask *__restrict__ tasks) {
 	}
 	__syncthreads();
 	const uint32_t sbase = smem_base(smem);
-	// this thread's 64 x int16 tile, linear (it leaves as one bulk copy); tiles are 144 bytes apart so
-	// that lanes writing the same coefficient index spread over the banks
-	uint4 *tile = reinterpret_cast<uint4 *>(smem + EXP_OFF_TILES + threadIdx.x * TILE_PITCH);
+	// the warp's staging area (walk.cuh): its lanes' compact rows, or their 64 x int16 tiles
+	const int lane = threadIdx.x & 31;
+	const uint32_t wstage = sbase + EXP_OFF_TILES + (threadIdx.x - lane) * EXP_TILE_PITCH;
 #pragma unroll 1
 	for (int g = 0; g < EXPAND_GROUPS; g++) {
 		const uint32_t rec_now = rec;
@@ -152,11 +151,9 @@ expand_blocks_kernel(const ParseTask *__restrict__ tasks) {
 		slot_id += CTA_THREADS;
 		if (g + 1 < EXPAND_GROUPS) fetch(slot_id, rec, parked);  // the next run's, while this block is expanded
 		const int block = slot_now % 6;
-		if (slot_now >= n_slots || !(rec_now & MBF_PRESENT) || !((rec_now >> 8) & (0x20u >> block))) continue;
-#pragma unroll
-		for (int i = 0; i < 8; i++) tile[i] = make_uint4(0u, 0u, 0u, 0u);  // (the last bulk store has read the tile: expand_block waits)
-		expand_block(t, rec_now, parked_now, reinterpret_cast<uint4 *>(t.coef) + (size_t)slot_now * 8, sbase,
-		             sbase + EXP_OFF_TILES + threadIdx.x * TILE_PITCH, t.stage ? compact_plane(t.stage) + slot_now : nullptr);
+		const bool coded = slot_now < n_slots && (rec_now & MBF_PRESENT) && ((rec_now >> 8) & (0x20u >> block));
+		if (!__any_sync(0xffffffffu, coded)) continue;
+		expand_warp_run(t, coded, rec_now, parked_now, slot_now, lane, sbase, wstage);
 	}
 }
 

@@ -47,7 +47,7 @@ constexpr uint32_t OFF_TYPE_I = OFF_DC_CHROMA + 512;                   // uint16
 constexpr uint32_t OFF_TYPE_P = OFF_TYPE_I + 8;                        // uint16[64]
 static_assert(OFF_TYPE_P + 128 <= OFF_MS, "the per-symbol tables end before the multi-symbol table");
 // stage 1b (its own kernel, its own shared memory): the DCT table with values, the two quantiser tables
-// in zig-zag order (SeqParams::xq), one 64 x int16 tile per thread
+// in zig-zag order (SeqParams::xq), and per warp a staging area: the lanes' compact rows, or their 64 x int16 tiles
 constexpr uint32_t EXP_OFF_DCT = 0;                                     // uint32[384]: VLC_DCT_EXPAND (clz-indexed)
 constexpr uint32_t EXP_OFF_TOP8 = EXP_OFF_DCT + (VLC_DCT_MAX_Z + 1) * 128;  // uint32[256]: VLC_DCT_EXPAND_TOP8 (next 8 bits)
 constexpr uint32_t EXP_OFF_XQ = EXP_OFF_TOP8 + 1024;                    // uint16[2][64]
@@ -73,6 +73,9 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t addr) {
 __device__ __forceinline__ void sts_s16(uint32_t addr, int v) {
 	asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"((uint16_t)v) : "memory");
 }
+__device__ __forceinline__ void sts_u64(uint32_t addr, uint64_t v) {
+	asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(addr), "r"((uint32_t)v), "r"((uint32_t)(v >> 32)) : "memory");
+}
 #else
 // host emulation (tests only): `emu_smem` stands in for the CTA's shared memory, addresses are offsets into it
 constexpr uint32_t EMU_EXPAND_BASE = (WALK_SMEM_LANES + 127u) & ~127u;  // a second "CTA": stage 1b's own tables and tile
@@ -81,6 +84,7 @@ static inline uint32_t lds_u16(uint32_t addr) { uint16_t v; memcpy(&v, emu_smem 
 static inline uint32_t lds_u8(uint32_t addr) { return emu_smem[addr]; }
 static inline uint32_t lds_u32(uint32_t addr) { uint32_t v; memcpy(&v, emu_smem + addr, 4); return v; }
 static inline void sts_s16(uint32_t addr, int v) { const int16_t x = (int16_t)v; memcpy(emu_smem + addr, &x, 2); }
+static inline void sts_u64(uint32_t addr, uint64_t v) { memcpy(emu_smem + addr, &v, 8); }
 #endif
 // MSB-first bit window over a byte span (src/buffer.js:152-187); one copy per thread.
 //
@@ -1193,16 +1197,18 @@ __device__ void walk_picture(const ParseTask &t, uint32_t sbase, int lane, uint3
 }
 
 // ==================================================================================================
-// 1b: one coded block, from the offset the walk parked to the finished 64 x int16 record.
+// 1b: coded blocks, from the offset the walk parked to the finished record.
 // rec = the macroblock record's second word (flags | cbp << 8 | dc_only << 16 | quantiser scale << 24),
-// parked = {bit offset of the block's first coefficient code, intra dc * 8} from the walk's dense side
-// array, stile = the shared-memory address of this thread's (zeroed) 128-byte tile.  crec = the block's compact
-// record (coef_records.h), or nullptr: the block leaves as a dense record at `slot`.  With crec, a block of at most
-// COEF_RECORD_LEVELS positions leaves as its 32-byte compact record alone; a bigger one marks crec dense and leaves
-// as the dense record at `slot`.
+// parked = {bit offset of the block's first coefficient code, intra dc * 8} from the walk's dense side array.
 //
-// The kernel is bound by the integer ALU pipe, so the loop is built to need
-// few ALU instructions per code:
+// Run/level codes arrive in zig-zag order, and the compact record (coef_records.h) IS the position mask plus the
+// values in zig-zag order: the k-th value a block's codes give is level[k].  So a block is built as its compact
+// record directly, in a 32-byte row of its warp's staging area in shared memory (expand_compact_row), and the warp
+// stores the rows of its 32 consecutive slots itself, as whole 512-byte stretches (store_compact_rows).  Only a
+// block of more than COEF_RECORD_LEVELS positions is decoded a second time, into a zeroed 64 x int16 tile through
+// the raster offsets, and leaves as the dense record (expand_dense_record).
+//
+// The code loop (expand_codes) is built to need few instructions per code:
 //  * no bit window to maintain: the 32 bits at the current bit POSITION are two word loads (L1 hits: the
 //    blocks of a warp lie side by side in the stream) and one funnel shift -- the loads go to the LSU, the
 //    address to the FMA pipe; the window's shifts, counters and predicated refill were a quarter of the loop.
@@ -1225,8 +1231,11 @@ __device__ __forceinline__ int dequant_sm(int mag2_plus, int neg, int qs, uint32
 	const int r = min(max((t - 1) | 1, 1), 2047 + neg);
 	return (neg && t != 0) ? -r : r;
 }
-__device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, uint2 parked, uint4 *__restrict__ slot,
-                                             uint32_t sbase, uint32_t stile, coef_record_t *__restrict__ crec = nullptr) {
+// The codes of one block: put(q, value) for every value in zig-zag order, q = the position's quantiser entry (its
+// low byte: the raster offset in bytes; 0 for the intra DC).  Returns the zig-zag positions written (the compact
+// record's mask).
+template <class Put>
+__device__ __forceinline__ uint64_t expand_codes(const ParseTask &t, uint32_t rec, uint2 parked, uint32_t sbase, Put put) {
 	const bool intra = rec & MBF_INTRA;
 	const int ni = intra ? 0 : 1;
 	const int qs = (int)(rec >> 24);
@@ -1245,16 +1254,16 @@ __device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, u
 	uint32_t w = window(pos);
 
 	int n = 0;
-	uint64_t written = 0;  // zig-zag positions stored (the compact record's mask)
+	uint64_t written = 0;
 	if (intra) {
-		sts_s16(stile, (int)(int16_t)(parked.y & 0xffffu));  // coefficient 0
+		put(0u, (int)(int16_t)(parked.y & 0xffffu));  // coefficient 0
 		n = 1;
 		written = 1;
 	} else if (w >> 31) {
 		// dct_coeff_first of a non-intra block: a leading '1' is (run 0, level +-1) with its sign bit, never
 		// end_of_block (mpeg1.js:757-760, 781-787) -- handled here, once, instead of in every trip of the loop
 		const uint32_t q = lds_u16(xq);
-		sts_s16(stile + (q & 0xffu), dequant_sm(3, (int)((w >> 30) & 1u), qs, q));
+		put(q, dequant_sm(3, (int)((w >> 30) & 1u), qs, q));
 		pos += 2u;
 		w = window(pos);
 		n = 1;
@@ -1296,47 +1305,62 @@ __device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, u
 			continue;
 		}
 		const uint32_t q = lds_u16(xq + (uint32_t)(n - 1) * 2u);
-		sts_s16(stile + (q & 0xffu), dequant_sm(mag2 + ni, neg, qs, q));
+		put(q, dequant_sm(mag2 + ni, neg, qs, q));
 		written |= (uint64_t)1 << (n - 1);
 	}
-	if (crec && coef_record_fits(written)) {
-		// the compact record: the written values in zig-zag order, read back from the tile (its raster offsets come
-		// from the quantiser table's low byte), then written over the tile's first 32 bytes, which leave as one
-		// 32-byte bulk store -- whole sectors, like the dense record's
-		uint32_t lv[COEF_RECORD_LEVELS / 2] = {};
-		uint64_t m = written;
+	return written;
+}
+
+// A warp's staging area: the lanes' 32-byte compact rows EXP_ROW_PITCH bytes apart.  40 keeps a row 8-byte aligned
+// and starts the rows 10 banks apart: lanes storing their k-th value meet two to a bank (at 32 bytes: eight).
+// A lane's 64 x int16 tile for a dense block lies over the same memory, EXP_TILE_PITCH apart (128 + 16: bank spread).
+constexpr uint32_t EXP_ROW_PITCH = 40;
+constexpr uint32_t EXP_TILE_PITCH = 144;
+static_assert(32 * EXP_ROW_PITCH <= 32 * EXP_TILE_PITCH, "a warp's rows lie inside its tiles");
+
+// One block as its compact record in the row at srow: mask at +0, the values from +8 in the order the codes give
+// them, the unused levels 0.  Values past the record's twelve are dropped: the mask tells (coef_record_fits).
+__device__ __forceinline__ uint64_t expand_compact_row(const ParseTask &t, uint32_t rec, uint2 parked, uint32_t sbase, uint32_t srow) {
+	sts_u64(srow + 8u, 0);
+	sts_u64(srow + 16u, 0);
+	sts_u64(srow + 24u, 0);
+	uint32_t at = srow + 8u;
+	const uint64_t written = expand_codes(t, rec, parked, sbase, [&](uint32_t, int v) {
+		if (at < srow + (uint32_t)sizeof(coef_record_t)) sts_s16(at, v);
+		at += 2u;
+	});
+	sts_u64(srow, written);
+	return written;
+}
+
+// The rows of the lanes in `fits` to the warp's stretch of the compact plane (first = the record of lane 0's slot):
+// the kilobyte goes as 64 chunks of 16 bytes, lane l takes chunks l and l + 32, so one store instruction covers 512
+// contiguous bytes, whole sectors.  A chunk whose record is not in `fits` (uncoded, or dense) stays unwritten.
+__device__ __forceinline__ void store_compact_rows(coef_record_t *first, uint32_t wstage, int lane, uint32_t fits) {
 #pragma unroll
-		for (int k = 0; k < COEF_RECORD_LEVELS; k++) {
-			if (m) {
-				const uint32_t q = lds_u16(xq + (uint32_t)coef_lowest64(m) * 2u);
-				m &= m - 1;
-				uint32_t v;
+	for (int c = lane; c < 64; c += 32) {
+		if (!((fits >> (c >> 1)) & 1u)) continue;
+		const uint32_t src = wstage + (uint32_t)(c >> 1) * EXP_ROW_PITCH + (uint32_t)(c & 1) * 16u;
 #ifndef JSMPEG_WALK_EMU
-				asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(stile + (q & 0xffu)) : "memory");
+		uint4 v;
+		asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(src) : "memory");
+		asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.z), "=r"(v.w) : "r"(src + 8u) : "memory");
+		reinterpret_cast<uint4 *>(first)[c] = v;
 #else
-				v = lds_u16(stile + (q & 0xffu));
+		memcpy(reinterpret_cast<uint8_t *>(first) + c * 16, emu_smem + src, 16);
 #endif
-				lv[k >> 1] |= v << (16 * (k & 1));
-			}
-		}
-#ifndef JSMPEG_WALK_EMU
-		asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(stile), "r"((uint32_t)written), "r"((uint32_t)(written >> 32)),
-		             "r"(lv[0]), "r"(lv[1]) : "memory");
-		asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(stile + 16u), "r"(lv[2]), "r"(lv[3]), "r"(lv[4]), "r"(lv[5]) : "memory");
-		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-		asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], 32;" ::"l"(crec), "r"(stile) : "memory");
-		asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-		asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-#else
-		memcpy(crec, &written, 8);
-		memcpy(reinterpret_cast<uint8_t *>(crec) + 8, lv, sizeof lv);
-#endif
-		return;
 	}
-	if (crec) crec->mask = COEF_RECORD_DENSE;  // (rare: more positions than the compact record holds)
-	// The finished block leaves as ONE 128-byte TMA bulk store (shared -> global, SASS UBLKCP): whole
-	// lines reach L2, whereas eight 16-byte stores per thread half-fill 32-byte sectors and made L2
-	// read every sector back before merging (about as many bytes read as written).
+}
+
+// One block as the dense 64 x int16 record at `slot`, through the thread's tile at stile.
+// The finished block leaves as ONE 128-byte TMA bulk store (shared -> global, SASS UBLKCP): whole
+// lines reach L2, whereas eight 16-byte stores per thread half-fill 32-byte sectors and made L2
+// read every sector back before merging (about as many bytes read as written).
+__device__ __forceinline__ void expand_dense_record(const ParseTask &t, uint32_t rec, uint2 parked, uint4 *__restrict__ slot,
+                                                    uint32_t sbase, uint32_t stile) {
+#pragma unroll
+	for (uint32_t i = 0; i < 128u; i += 8u) sts_u64(stile + i, 0);
+	expand_codes(t, rec, parked, sbase, [&](uint32_t q, int v) { sts_s16(stile + (q & 0xffu), v); });
 #ifndef JSMPEG_WALK_EMU
 	asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the copy engine
 	asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], 128;" ::"l"(slot), "r"(stile) : "memory");
@@ -1346,6 +1370,49 @@ __device__ __forceinline__ void expand_block(const ParseTask &t, uint32_t rec, u
 	memcpy(slot, emu_smem + stile, 128);
 #endif
 }
+
+// One run of a warp: its 32 consecutive block slots, lane `lane` on slot_id (coded: the slot holds a coded block).
+// wstage = the warp's staging area in shared memory.  With a compact plane (t.stage) every coded block is built as
+// its compact record and the warp stores the rows; the few blocks that do not fit mark their record dense and leave
+// as dense records.  Without one (the host emulation's dense-only mode) every coded block leaves as a dense record.
+// All 32 lanes call it.
+__device__ __forceinline__ void expand_warp_run(const ParseTask &t, bool coded, uint32_t rec, uint2 parked, int slot_id, int lane,
+                                                uint32_t sbase, uint32_t wstage) {
+	bool dense = coded;
+	if (t.stage) {
+		uint64_t written = 0;
+		if (coded) written = expand_compact_row(t, rec, parked, sbase, wstage + (uint32_t)lane * EXP_ROW_PITCH);
+		const bool fits = coded && coef_record_fits(written);
+		dense = coded && !fits;
+		__syncwarp();  // the rows are written
+		coef_record_t *first = compact_plane(t.stage) + (slot_id - lane);
+		store_compact_rows(first, wstage, lane, __ballot_sync(0xffffffffu, fits));
+		if (dense) first[lane].mask = COEF_RECORD_DENSE;
+	}
+	if (__any_sync(0xffffffffu, dense)) {  // (rare: more positions than the compact record holds)
+		__syncwarp();  // the rows are read: the tiles lie over them
+		if (dense)
+			expand_dense_record(t, rec, parked, reinterpret_cast<uint4 *>(t.coef) + (size_t)slot_id * 8, sbase,
+			                    wstage + (uint32_t)lane * EXP_TILE_PITCH);
+	}
+	__syncwarp();  // the next run writes the rows again
+}
+
+#ifdef JSMPEG_WALK_EMU
+// One block on its own, for the host emulation's one-thread entry points: the row and the tile at stile, the record
+// to crec (nullptr: dense records only) or, dense, to `slot` -- expand_warp_run without the warp.
+static inline void expand_block(const ParseTask &t, uint32_t rec, uint2 parked, uint4 *slot, uint32_t sbase, uint32_t stile,
+                                coef_record_t *crec = nullptr) {
+	if (crec) {
+		if (coef_record_fits(expand_compact_row(t, rec, parked, sbase, stile))) {
+			memcpy(crec, emu_smem + stile, sizeof(coef_record_t));
+			return;
+		}
+		crec->mask = COEF_RECORD_DENSE;
+	}
+	expand_dense_record(t, rec, parked, slot, sbase, stile);
+}
+#endif
 
 // Multi-symbol walk table: for every MS_BITS-bit prefix, the complete dct_coeff_next codes (with their
 // sign bits) that fit, greedily.  Entry: bits 0..3 = bits to consume (0 = first code does not fit
