@@ -388,6 +388,42 @@ long jsmpeg_b200_batch_decode_accumulated(jsmpeg_b200_batch_t *b, int n, const i
                                           void *const *acc_dst, int32_t *status_out, int32_t *n_present_out,
                                           int32_t *error_out);
 
+/* SEEK (players, video walls, clip loaders): move decode() of chosen streams to a chosen picture each, and play on from
+ * there with decode() -- OUT_HOST, OUT_RGBA and the host ring as usual -- without stepping the other streams.  The
+ * reference chains of all requests run side by side, as for decode_pictures, but into the streams' own plane sets.
+ *
+ * Request i moves stream streams[i] to picture pictures[i], an entry of the stream's picture index under the batch's
+ * current decode_b (the listing and numbering of decode_pictures).  A stream may be named at most once per call.
+ *
+ * The seek chain start j is the index's chain start, except that under decode_b an I picture k needs ONE reference in
+ * [j, k), not zero: the greatest I picture before k (k itself where there is none), so that the B pictures after k
+ * of an open GOP are decoded from both their references.
+ *
+ * For each named stream, everything decode() observes afterwards is exactly what a FRESH decoder shows right after its
+ * decode() that consumes picture k, the fresh decoder having every plane set zeroed (the B sets too), the batch's
+ * decode_b, and being fed the first sequence header and then the stream's resident bytes from picture j to the end of
+ * the buffer.  Translated to the stream's buffer: the bit index is picture k's end; get_planes / read_planes give
+ * picture k, under OUT_HOST in `flags` also copied to the next slot of the host ring (get_host_planes), under
+ * OUT_RGBA also converted to the stream's RGBA picture (get_rgba / read_rgba) -- `flags` as for decode(); the two I/P
+ * sets and the two B sets hold what the fresh decoder's hold, and the next picture overwrites the same ones (every B
+ * picture the fresh decoder reconstructs in (j, k] is reconstructed: a later picture's absent macroblocks keep a set's
+ * content); last_picture gives k's type and temporal_reference.  So for a stream that begins with an I picture and
+ * whose pictures from j on code every macroblock, every later decode() gives what sequential decode() from the start
+ * gives at that point.
+ *
+ * Damaged input: the fresh decoder may never consume k, an earlier picture's walk having run across k's start code;
+ * status_out[i] is then 0 and the stream is left as the fresh decoder is after that decode() (its picture written to
+ * RGBA / the host ring as above).  Otherwise status_out[i] is PIC_DECODED.  n_present_out / error_out are those of the
+ * picture the state ends on.  All three may be NULL.
+ *
+ * Unchanged: streams not named (their parsed-ahead pictures may be dropped for record slots, as in decode_intra);
+ * resident bytes, sequence parameters and the decode_b option; stats, except that written bytes become resident and
+ * that upload is counted.  A named stream's parsed-ahead pictures are dropped.  Synchronous.  Returns n; -1 dead; -2 a
+ * request is invalid (stream out of range, without sequence header or named twice, picture not in the picture index,
+ * NULL arrays with n > 0) -- checked before any work, and then nothing changed. */
+long jsmpeg_b200_batch_seek_pictures(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
+                                     int flags, int32_t *status_out, int32_t *n_present_out, int32_t *error_out);
+
 void jsmpeg_b200_batch_get_stats(jsmpeg_b200_batch_t *b, jsmpeg_b200_stats_t *out);
 void jsmpeg_b200_batch_reset_stats(jsmpeg_b200_batch_t *b);
 

@@ -62,6 +62,7 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_decode_coefficients": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_decode_residuals": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_decode_accumulated": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "jsmpeg_b200_batch_seek_pictures": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, ctypes.c_int, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_get_stats": (None, [_VP, ctypes.POINTER(Stats)]),
     "jsmpeg_b200_batch_reset_stats": (None, [_VP]),
     "jsmpeg_b200_debug_parse_picture": (ctypes.c_int, [_VP, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int, ctypes.c_int,
@@ -135,6 +136,7 @@ class BatchDecoder:
         self.last_coefficients_info = []  # per request of the last decode_coefficients: {"n_present", "error"}
         self.last_residuals_info = []  # per request of the last decode_residuals: {"n_present", "error"}
         self.last_accumulated_info = []  # per request of the last decode_accumulated: {"status", "n_present", "error"}
+        self.last_seek_info = []  # per request of the last seek_pictures: {"status", "n_present", "error"}
         self.handle = self.lib.jsmpeg_b200_batch_create(n_streams, device, max_slots)
         err = self.lib.jsmpeg_b200_batch_last_error(self.handle)
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
@@ -434,6 +436,26 @@ class BatchDecoder:
         self.last_accumulated_info = [{"status": status[i], "n_present": n_present[i], "error": errors[i]}
                                       for i in range(n)]
         return maps
+
+    def seek_pictures(self, requests, flags=OUT_DEVICE):
+        """Move decode() of chosen streams to pictures listed by picture_index, in one call: `requests` is an iterable of
+        (stream, picture), each stream at most once.  Afterwards each named stream is where decode() is right after
+        consuming that picture (include/jsmpeg_b200.h): bit index, planes -- under `flags` (OUT_HOST, OUT_RGBA, as for
+        decode) also the host ring and RGBA -- reference sets and last_picture; the next decode() goes on from there.
+        Streams not named are left alone.  Returns the number of requests; last_seek_info gets {"status",
+        "n_present", "error"} per request (status 1: the picture was consumed; 0: the fresh decoder never reached it,
+        and the stream is where that decoder stopped)."""
+        reqs = [(int(s), int(p)) for s, p in requests]
+        n = len(reqs)
+        streams, pictures, n_present, errors = self._request_arrays(reqs)
+        status = (ctypes.c_int32 * max(n, 1))()
+        got = self.lib.jsmpeg_b200_batch_seek_pictures(self.handle, n, streams, pictures, int(flags), status, n_present, errors)
+        if got == -2:
+            raise ValueError("a request names a stream twice, or a picture that is not in the stream's picture index")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_seek_pictures failed")
+        self.last_seek_info = [{"status": status[i], "n_present": n_present[i], "error": errors[i]} for i in range(n)]
+        return got
 
     def _per_picture_views(self, reqs, shape, dtype):
         """Per (stream, picture) request a CUDA tensor of shape shape(mb_height, mb_width) and `dtype`, the views of one

@@ -756,6 +756,26 @@ ReconTask recon_task(const Batch *b, const Stream &s, int slot, uint8_t *cur, ui
 	return t;
 }
 
+// The stream's RGBA picture, made on first use: opaque white, like the canvas the reference creates
+// (canvas2d.js:24-29); the odd edge keeps it
+uint8_t *stream_rgba(Batch *b, Stream &s) {
+	if (!s.d_rgba.data()) {
+		s.d_rgba.reserve((size_t)s.width * s.height * 4);
+		CUDA_CHECK(cudaMemsetAsync(s.d_rgba.data(), 0xff, (size_t)s.width * s.height * 4, b->st_recon));
+	}
+	return s.d_rgba.data();
+}
+
+// The stream's two B-picture sets, made zeroed on first use (+ coded_width + 64: parse_sequence_header's slack)
+void reserve_b_sets(Batch *b, Stream &s) {
+	if (s.d_planes_b[0].data()) return;
+	const size_t bytes = (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64;
+	for (auto &pb : s.d_planes_b) {
+		pb.reserve(bytes);
+		CUDA_CHECK(cudaMemsetAsync(pb.data(), 0, bytes, b->st_recon));
+	}
+}
+
 // One round: parse ahead what is missing in one wave, then consume up to want[s] pictures per stream in decode()
 // order and queue their reconstruction.  Returns pictures consumed; `progress[s]` gets the per-stream count, `more[s]`
 // whether the stream may have further pictures.
@@ -841,25 +861,12 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			s.last_temporal = (uint64_t)e.pos + 5 < s.bb.length ? picture_header(s, e.pos).temporal_reference : 0;
 			if (e.info.status == PIC_DECODED) {
 				const bool is_b = e.info.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
-				uint8_t *rgba = nullptr;
-				if (flags & JSMPEG_B200_OUT_RGBA) {
-					if (!s.d_rgba.data()) {  // opaque white, like the canvas the reference creates (canvas2d.js:24-29): the odd edge keeps it
-						s.d_rgba.reserve((size_t)s.width * s.height * 4);
-						CUDA_CHECK(cudaMemsetAsync(s.d_rgba.data(), 0xff, (size_t)s.width * s.height * 4, b->st_recon));
-					}
-					rgba = s.d_rgba.data();
-				}
+				uint8_t *rgba = (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
 				ReconTask t;
 				if (is_b) {
 					// after the swaps `cur` holds the older and `1 - cur` the newer of the two most recent I/P pictures:
 					// the B picture's forward (past) and backward (future) reference.  It goes to a set of its own.
-					if (!s.d_planes_b[0].data()) {
-						const size_t bytes = (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64;
-						for (auto &pb : s.d_planes_b) {
-							pb.reserve(bytes);
-							CUDA_CHECK(cudaMemsetAsync(pb.data(), 0, bytes, b->st_recon));
-						}
-					}
+					reserve_b_sets(b, s);
 					t = recon_task(b, s, e.slot, s.d_planes_b[s.b_cur].data(), s.d_planes[s.cur].data(), s.d_planes[1 - s.cur].data(), rgba);
 					s.b_cur ^= 1;  // no reference: the I/P ping-pong stays as it is
 				} else {
@@ -1053,6 +1060,12 @@ struct Chain {
 	std::vector<int> slot;
 };
 
+// The picture decode() consumes after the one whose info is `e`: the first picture start code at or after where its
+// parse ended
+uint32_t next_picture(const Stream &s, const picture_info_t &e) {
+	return (uint32_t)(std::lower_bound(s.pics.begin(), s.pics.end(), (e.end_bit + 7) >> 3) - s.pics.begin());
+}
+
 // The requests in chain order (by stream, chain start and picture) and their chains, with n_sets 0 for a chain of one
 // picture and 2 (4 with a B picture requested) otherwise
 std::vector<Chain> make_chains(const Batch *b, const std::vector<PictureRequest> &req, std::vector<int> &order) {
@@ -1096,24 +1109,35 @@ struct ChainWork {
 	virtual ~ChainWork() = default;
 };
 
-// The schedule behind decode_pictures, decode_intra and decode_accumulated (DESIGN 3.7).  The chains' pictures
-// [first, last] are parsed in waves over consecutive positions of every chain, consumed on the host by decode()'s rule
-// (b_walk: B pictures go to the B walk, as decode_b; else they are skipped after their header) and handed to `work`
-// by depth (depth d: the d-th decoded picture of every chain of the wave).  Chains run in groups of at most a wave's
-// slots, each chain's sets (set_bytes each, zeroed first with zero_sets) within half of the free device memory, from
-// `pool` -- a request beyond the device is cut into groups, not refused.  The requests are valid (the caller checked
-// them); on return the work is queued on the reconstruct stream, and the infos are the consumed pictures'.
+// Where run_chains takes each chain's n_sets plane or map sets from: `set_bytes` each out of `buf`, zeroed first when
+// `zero`
+struct SetPool {
+	DeviceBuffer<uint8_t> &buf;
+	size_t set_bytes;
+	bool zero;
+};
+
+// The schedule behind decode_pictures, decode_intra, decode_accumulated and seek_pictures (DESIGN 3.7).  The chains'
+// pictures [first, last] are parsed in waves over consecutive positions of every chain, consumed on the host by
+// decode()'s rule (b_walk: B pictures go to the B walk, as decode_b; else they are skipped after their header) and
+// handed to `work` by depth (depth d: the d-th decoded picture of every chain of the wave).  Chains run in groups of at
+// most a wave's slots.  With a `pool`, each chain's sets come from it, a group's within half of the free device memory
+// -- a request beyond the device is cut into groups, not refused; without one, the caller has filled Chain::set.  The
+// requests are valid (the caller checked them); on return the work is queued on the reconstruct stream, and the infos
+// are the consumed pictures'.
 RequestInfo run_chains(Batch *b, const std::vector<PictureRequest> &req, const std::vector<int> &order,
-                       std::vector<Chain> &chains, bool b_walk, size_t set_bytes, DeviceBuffer<uint8_t> &pool,
-                       bool zero_sets, ChainWork &work) {
+                       std::vector<Chain> &chains, bool b_walk, const SetPool *pool, ChainWork &work) {
 	size_t n_tasks = 0;
 	for (const Chain &c : chains) n_tasks += c.info.size();
 	RequestInfo out((int)req.size());
 	free_slots_for(b, n_tasks);
 	const int wave_max = (int)b->free_slots.size();
-	size_t free_b = 0, total_b = 0;
-	CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-	const size_t max_sets = std::max<size_t>(4, ((size_t)(0.5 * (double)free_b) + pool.size()) / set_bytes);
+	size_t max_sets = SIZE_MAX;
+	if (pool) {
+		size_t free_b = 0, total_b = 0;
+		CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+		max_sets = std::max<size_t>(4, ((size_t)(0.5 * (double)free_b) + pool->buf.size()) / pool->set_bytes);
+	}
 	std::vector<std::pair<size_t, size_t>> groups;
 	size_t most_sets = 0;
 	for (size_t lo = 0; lo < chains.size();) {
@@ -1123,16 +1147,17 @@ RequestInfo run_chains(Batch *b, const std::vector<PictureRequest> &req, const s
 		most_sets = std::max(most_sets, sets);
 		lo = hi;
 	}
-	if (most_sets * set_bytes > pool.size()) {
-		if (pool.data()) CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-		pool.reserve(most_sets * set_bytes);
+	if (pool && most_sets * pool->set_bytes > pool->buf.size()) {
+		if (pool->buf.data()) CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+		pool->buf.reserve(most_sets * pool->set_bytes);
 	}
 	for (const auto &[glo, ghi] : groups) {
 		size_t sets = 0;
-		for (size_t c = glo; c < ghi; c++)
-			for (int k = 0; k < chains[c].n_sets; k++) chains[c].set[k] = pool.data() + set_bytes * sets++;
-		if (sets && zero_sets)  // (the previous group's copies are queued before)
-			CUDA_CHECK(cudaMemsetAsync(pool.data(), 0, set_bytes * sets, b->st_recon));
+		if (pool)
+			for (size_t c = glo; c < ghi; c++)
+				for (int k = 0; k < chains[c].n_sets; k++) chains[c].set[k] = pool->buf.data() + pool->set_bytes * sets++;
+		if (sets && pool->zero)  // (the previous group's copies are queued before)
+			CUDA_CHECK(cudaMemsetAsync(pool->buf.data(), 0, pool->set_bytes * sets, b->st_recon));
 		const uint32_t width = (uint32_t)std::max<size_t>(1, (size_t)wave_max / (ghi - glo));
 		for (uint32_t lo = 0;; lo += width) {
 			// ---- stage 1: positions [lo, lo + width) of every chain still consuming
@@ -1170,8 +1195,7 @@ RequestInfo run_chains(Batch *b, const std::vector<PictureRequest> &req, const s
 					const bool is_b = e.picture_type == 3;  // (only the B walk answers PIC_DECODED for one)
 					if (e.status == PIC_DECODED && (!is_b || k < ch.b_end))
 						work.picture(ch, s, ch.slot[k - ch.first], e, d++, q_lo, q_hi);
-					// the next picture: the first picture start code at or after where this one's parse ended
-					ch.next = (uint32_t)(std::lower_bound(s.pics.begin(), s.pics.end(), (e.end_bit + 7) >> 3) - s.pics.begin());
+					ch.next = next_picture(s, e);
 				}
 			}
 			// ---- stage 2, then the slots go back: the next wave's parse waits for ev_round
@@ -1256,7 +1280,8 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 		}
 	PlaneWork work(b, order, planes_dst, rgba_dst, rgba);
 	// (a fresh decoder's planes start zeroed, the B sets too)
-	const RequestInfo out = run_chains(b, req, order, chains, b->decode_b, set_bytes, b->d_chain_sets, true, work);
+	const SetPool pool{b->d_chain_sets, set_bytes, true};
+	const RequestInfo out = run_chains(b, req, order, chains, b->decode_b, &pool, work);
 	for (const Chain &c : chains)  // never consumed: planes 0 (a copied destination was not zeroed)
 		if (c.n_sets)
 			for (int q = c.req_lo; q < c.req_hi; q++)
@@ -1269,23 +1294,30 @@ void decode_chains(Batch *b, const std::vector<PictureRequest> &req, void *const
 	out.copy_out(status_out, n_present_out, error_out);
 }
 
-// The checks of a random-access call's requests, all before anything changes: the arrays are there; every request
-// names a stream with a sequence header and a picture of its `what` listing; its destination, and with `rgba` its image,
-// is 16-byte aligned (stage 2 stores 8 and 16 bytes at a time).  Fills `req` (with the chain starts) and returns true,
-// or returns false.
-bool check_requests(Batch *b, Listing what, int n, const int *streams, const uint32_t *pictures, void *const *dst,
-                    void *const *rgba_dst, bool rgba, std::vector<PictureRequest> &req) {
+// seek_pictures' chain start for entry `e` of the picture index: the index's, except that under decode_b an I picture
+// needs one reference in [j, k) -- the greatest I picture before it, or k itself where there is none -- so that the B
+// pictures after it (of an open GOP) are decoded from both their references (DESIGN 3.12)
+uint32_t seek_start(const Batch *b, const Stream &s, const IndexEntry &e) {
+	if (!b->decode_b || e.pic != e.chain_start) return e.chain_start;
+	for (uint32_t j = e.pic; j-- > 0;)
+		if (s.pics[j] >= s.seq_floor && picture_header(s, s.pics[j]).type == 1) return j;
+	return e.pic;
+}
+
+// The checks of a random-access call's requests that name no destination, all before anything changes: the arrays
+// are there; every request names a stream with a sequence header and a picture of its `what` listing.  Fills `req`
+// (with the chain starts) and returns true, or returns false.
+bool check_requests(Batch *b, Listing what, int n, const int *streams, const uint32_t *pictures,
+                    std::vector<PictureRequest> &req) {
 	use_device(b);
-	if (n < 0 || (n > 0 && (!streams || !pictures || !dst || (rgba && !rgba_dst)))) return false;
+	if (n < 0 || (n > 0 && (!streams || !pictures))) return false;
 	upload_all(b);
-	auto aligned = [](const void *p) { return p && ((uintptr_t)p & 15u) == 0; };
 	std::vector<std::vector<IndexEntry>> listed(b->streams.size());
 	std::vector<char> indexed(b->streams.size(), 0);
 	req.resize(n);
 	for (int i = 0; i < n; i++) {
 		const int si = streams[i];
-		if (si < 0 || si >= (int)b->streams.size() || !b->streams[si].has_seq || !aligned(dst[i])) return false;
-		if (rgba && !aligned(rgba_dst[i])) return false;
+		if (si < 0 || si >= (int)b->streams.size() || !b->streams[si].has_seq) return false;
 		if (!indexed[si]) {
 			listed[si] = list_pictures(b, b->streams[si], what);
 			indexed[si] = 1;
@@ -1295,6 +1327,18 @@ bool check_requests(Batch *b, Listing what, int n, const int *streams, const uin
 		if (e == listed[si].end() || e->pic != pictures[i]) return false;
 		req[i] = {si, pictures[i], e->chain_start};
 	}
+	return true;
+}
+
+// ... and of those that name one: besides, `dst` is there and every destination, and with `rgba` its image, is
+// 16-byte aligned (stage 2 stores 8 and 16 bytes at a time)
+bool check_requests(Batch *b, Listing what, int n, const int *streams, const uint32_t *pictures, void *const *dst,
+                    void *const *rgba_dst, bool rgba, std::vector<PictureRequest> &req) {
+	if (n > 0 && (!dst || (rgba && !rgba_dst))) return false;
+	if (!check_requests(b, what, n, streams, pictures, req)) return false;
+	auto aligned = [](const void *p) { return p && ((uintptr_t)p & 15u) == 0; };
+	for (int i = 0; i < n; i++)
+		if (!aligned(dst[i]) || (rgba && !aligned(rgba_dst[i]))) return false;
 	return true;
 }
 
@@ -1500,7 +1544,8 @@ void decode_accumulated(Batch *b, const std::vector<PictureRequest> &req, void *
 	}
 	MapWork work(b, order, acc_dst);
 	// (a scratch set is read only after the chain wrote it)
-	const RequestInfo out = run_chains(b, req, order, chains, false, set_bytes, b->d_map_sets, false, work);
+	const SetPool pool{b->d_map_sets, set_bytes, false};
+	const RequestInfo out = run_chains(b, req, order, chains, false, &pool, work);
 	for (int i = 0; i < (int)req.size(); i++)  // never consumed: every record untraced {0, 0, 0, -1}
 		if (out.status[i] != PIC_DECODED) {
 			const size_t n_rec = (size_t)b->streams[req[i].stream].coded_size * 3 / 2;
@@ -1534,6 +1579,105 @@ long batch_decode_accumulated(Batch *b, int n, const int *streams, const uint32_
 	}
 	if (n == 0) return 0;
 	decode_accumulated(b, req, acc_dst, status_out, n_present_out, error_out);
+	return n;
+}
+
+// ---- seek_pictures: move decode() of chosen streams to a listed picture, each from its seek chain start (DESIGN 3.12)
+
+// Each chain reconstructs into its stream's own sets (set[0..1] the I/P sets, set[2..3] the B sets) with decode()'s
+// rotation, one launch_reconstruct per depth.  The last picture a chain consumes -- picture k, or on damaged input the
+// picture whose walk ran across k -- is, when decoded, also written to the stream's RGBA under OUT_RGBA and copied to
+// the next slot of its host ring under OUT_HOST (copy_out_step).  No later launch of the call writes its set.
+struct SeekWork : ChainWork {
+	Batch *b;
+	int flags;
+	std::vector<uint8_t *> last;  // per stream: the set of the newest picture the call reconstructed (nullptr: none)
+	std::vector<ReconStep> steps;
+	SeekWork(Batch *b, int flags) : b(b), flags(flags), last(b->streams.size(), nullptr) {}
+	void picture(Chain &ch, const Stream &, int slot, const picture_info_t &e, size_t d, int, int) override {
+		Stream &s = b->streams[ch.stream];
+		const bool is_b = e.picture_type == 3;
+		const bool final = next_picture(s, e) > ch.last;
+		uint8_t *rgba = final && (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
+		const ReconTask t = is_b ? recon_task(b, s, slot, ch.set[2 + ch.b_cur], ch.set[ch.cur], ch.set[1 - ch.cur], rgba)
+		                         : recon_task(b, s, slot, ch.set[ch.cur], ch.set[1 - ch.cur], nullptr, rgba);
+		if (is_b) ch.b_cur ^= 1;
+		else ch.cur ^= 1;
+		last[ch.stream] = t.cur.y;
+		if (steps.size() <= d) steps.emplace_back();
+		steps[d].tasks.push_back(t);
+		if (final && (flags & JSMPEG_B200_OUT_HOST)) {
+			s.h_head = (s.h_head + 1) % HOST_RING;
+			steps[d].copy(s.h_planes[s.h_head].data(), t.cur.y, (size_t)s.coded_size * 3 / 2);
+		}
+	}
+	void depths() override {
+		for (ReconStep &r : steps) {
+			launch_reconstruct(r.tasks.data(), (int)r.tasks.size(), b->st_recon);
+			if (!r.dst.empty()) copy_out_step(b, r);
+		}
+		steps.clear();
+	}
+};
+
+// run_chains over the named streams' own plane sets, zeroed first, then the commit of what decode() observes: the bit
+// index, the set rotation, the newest picture, last_picture and the flushed look-ahead.  The requests are valid and
+// name distinct streams (the caller checked them).
+void seek_pictures(Batch *b, std::vector<PictureRequest> &req, int flags, int32_t *status_out, int32_t *n_present_out,
+                   int32_t *error_out) {
+	ensure_pool(b);
+	for (PictureRequest &r : req) r.from = seek_start(b, b->streams[r.stream], {r.pic, r.from});
+	std::vector<int> order;
+	std::vector<Chain> chains = make_chains(b, req, order);
+	// copies of earlier decode() calls (OUT_HOST) may still read the sets; the zeroing and the chains queue behind
+	// every earlier reconstruct launch on st_recon
+	CUDA_CHECK(cudaStreamSynchronize(b->st_copy));
+	for (Chain &c : chains) {
+		Stream &s = b->streams[c.stream];
+		flush_cache(b, s);
+		if (b->decode_b) reserve_b_sets(b, s);
+		uint8_t *sets[4] = {s.d_planes[0].data(), s.d_planes[1].data(), s.d_planes_b[0].data(), s.d_planes_b[1].data()};
+		for (int k = 0; k < 4; k++) {
+			c.set[k] = sets[k];
+			if (sets[k]) CUDA_CHECK(cudaMemsetAsync(sets[k], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
+		}
+		c.b_end = c.last + 1;  // every B picture the fresh decoder reconstructs: a set's content is decode() state
+	}
+	SeekWork work(b, flags);
+	RequestInfo out = run_chains(b, req, order, chains, b->decode_b, nullptr, work);
+	for (const Chain &c : chains) {
+		Stream &s = b->streams[c.stream];
+		uint32_t k = c.first;  // the last picture the chain consumed, by decode()'s rule over its infos
+		for (uint32_t next; (next = next_picture(s, c.info[k - c.first])) <= c.last;) k = next;
+		const picture_info_t &e = c.info[k - c.first];
+		s.bb.index = e.end_bit;
+		s.cur = c.cur;
+		s.b_cur = c.b_cur;
+		s.d_last = work.last[c.stream];
+		s.last_type = e.picture_type;
+		s.last_temporal = (uint64_t)s.pics[k] + 5 < s.bb.length ? picture_header(s, s.pics[k]).temporal_reference : 0;
+		const int i = order[c.req_lo];  // (one request per chain)
+		out.set(i, e);
+		if (k != c.last) out.status[i] = 0;
+	}
+	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+	CUDA_CHECK(cudaStreamSynchronize(b->st_copy));
+	b->recon_pending = false;
+	out.copy_out(status_out, n_present_out, error_out);
+}
+
+// seek_pictures' requests: decode_pictures' checks without destinations, and no stream named twice
+long batch_seek_pictures(Batch *b, int n, const int *streams, const uint32_t *pictures, int flags, int32_t *status_out,
+                         int32_t *n_present_out, int32_t *error_out) {
+	std::vector<PictureRequest> req;
+	if (!check_requests(b, Listing::Pictures, n, streams, pictures, req)) return -2;
+	std::vector<char> named(b->streams.size(), 0);
+	for (const PictureRequest &r : req) {
+		if (named[r.stream]) return -2;
+		named[r.stream] = 1;
+	}
+	if (n == 0) return 0;
+	seek_pictures(b, req, flags, status_out, n_present_out, error_out);
 	return n;
 }
 
@@ -1810,6 +1954,13 @@ long jsmpeg_b200_batch_decode_accumulated(jsmpeg_b200_batch_t *b, int n, const i
                                           int32_t *error_out) {
 	return guarded<long>(b, -1, [&] {
 		return batch_decode_accumulated(b, n, streams, pictures, acc_dst, status_out, n_present_out, error_out);
+	});
+}
+
+long jsmpeg_b200_batch_seek_pictures(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures, int flags,
+                                     int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
+	return guarded<long>(b, -1, [&] {
+		return batch_seek_pictures(b, n, streams, pictures, flags, status_out, n_present_out, error_out);
 	});
 }
 

@@ -78,6 +78,31 @@ def fresh_bytes(es, entry):
     return intra_model.fresh_bytes(es, {"byte_pos": entry["chain_start_pos"], "close": entry["close"]})
 
 
+def seek_start(es, entry, decode_b=False):
+    """The seek chain start of a listed picture (jsmpeg_b200_batch_seek_pictures): the index's chain start, except
+    that under decode_b an I picture needs one reference before it -- the greatest I picture j < k after the first
+    sequence header, or k itself where there is none -- so that the B pictures after k (of an open GOP) get both
+    their references."""
+    if not decode_b or entry["type"] != 1:
+        return entry["chain_start"]
+    floor = (intra_model.first_sequence_header(es)[1] + 7) >> 3
+    pics = picture_positions(es)
+    return next((j for j in range(entry["picture"] - 1, -1, -1) if pics[j] >= floor and picture_type(es, pics[j]) == 1),
+                entry["picture"])
+
+
+def seek_bytes(es, entry, decode_b=False):
+    """What the fresh decoder of a seek is fed: the first sequence header, then everything from the seek chain start
+    to the end of the buffer.  A position in it is the same position of `es` plus len(es) - len(seek_bytes(...))."""
+    start = picture_positions(es)[seek_start(es, entry, decode_b)]
+    return intra_model.fresh_bytes(es, {"byte_pos": start, "close": len(es) - 4})
+
+
+def picture_positions(es):
+    """Byte positions of the picture start codes (00 00 01 00) of `es`: picture k is the k-th."""
+    return [p for p in intra_model.prefixes(es) if p + 3 < len(es) and es[p + 3] == 0]
+
+
 def target_start_byte(es, entry):
     """Where picture k's header starts (the byte after its start code) inside fresh_bytes(es, entry)."""
     header = len(fresh_bytes(es, entry)) - (entry["close"] + 4 - entry["chain_start_pos"])
