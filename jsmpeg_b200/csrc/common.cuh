@@ -131,6 +131,7 @@ constexpr int PARSE_GROUPS = 8;
 struct ParseFork {
 	cudaStream_t side[PARSE_GROUPS];
 	cudaEvent_t fork, join[PARSE_GROUPS];
+	cudaEvent_t walked[PARSE_GROUPS];  // behind each group's walk, before its expand (launch_parse_pictures: after_walks)
 };
 // The walk kernels of stage 1a, in the order a wave launches them:
 //   WALK_LANES   I/P pictures: the lane-parallel walk (walk.cuh), or with JSMPEG_B200_WALK=serial the serial walk
@@ -141,10 +142,11 @@ enum WalkKind { WALK_LANES, WALK_SLICES, WALK_B, N_WALK_KINDS };
 constexpr int SLICE_WALK_MIN_SLICES = 4;
 // Stage 1 of n_tasks pictures of walk kernel `kind`: the walk + the expand, or with expand = false the walk alone
 // (macroblock records without coefficients).  A WALK_LANES wave with expand and `fork` is cut into size groups, a walk
-// + an expand launch per group; every other call is one group.  walk_done, unless nullptr, is recorded behind the first
-// group's walk.  Returns the number of kernels launched.
+// + an expand launch per group; every other call is one group.  after_walks, unless nullptr (it needs `fork`), is a stream
+// that is made to wait for every group's walk and for none of the expands: what is queued on it next finds the walks'
+// output, the picture infos among it, while stage 1b is still running.  Returns the number of kernels launched.
 int launch_parse_pictures(WalkKind kind, const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand,
-                          cudaStream_t stream, cudaEvent_t walk_done = nullptr, const ParseFork *fork = nullptr);
+                          cudaStream_t stream, const ParseFork *fork = nullptr, cudaStream_t after_walks = nullptr);
 // Stage 2 of n_tasks pictures, by kernel: I/P pictures, then I/P pictures with the planar -> RGBA conversion fused in
 // (tasks with `rgba`), then B pictures (tasks with `bwd`: prediction from two references), then B pictures with the
 // conversion; each kernel's tasks in their order.  `tasks_host` is read on the host at launch time: the table travels

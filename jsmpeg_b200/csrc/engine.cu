@@ -31,6 +31,7 @@
 #include <sched.h>
 
 #include <algorithm>
+#include <chrono>
 #include <cstring>
 #include <deque>
 #include <map>
@@ -122,9 +123,11 @@ struct jsmpeg_b200_batch_t {
 	PinnedBuffer<uint32_t> h_scan_counts, h_scan_pos;
 	DeviceBuffer<uint32_t> d_codes;  // empty until the first list is staged: the walks then search slice ends themselves
 	PinnedBuffer<uint32_t> h_codes;
-	cudaStream_t st_main = nullptr, st_recon = nullptr, st_copy = nullptr;  // uploads + scan + parse | reconstruct | copy-out
+	// uploads + scan + parse | reconstruct | copy-out | decode(): the infos' way to the host, behind the walks alone
+	cudaStream_t st_main = nullptr, st_recon = nullptr, st_copy = nullptr, st_info = nullptr;
 	cudaEvent_t ev_a = nullptr, ev_b = nullptr, ev_mid = nullptr, ev_step = nullptr, ev_round = nullptr, ev_copied[2] = {nullptr, nullptr};
 	cudaEvent_t ev_recon[2] = {nullptr, nullptr};  // around a round's reconstruct launches (timing)
+	cudaEvent_t ev_info = nullptr;  // decode(): the infos of a wave are on the host
 	// record slots
 	unsigned max_slots_req = 0;
 	int slot_mb = 0, n_slots = 0;
@@ -169,6 +172,14 @@ struct jsmpeg_b200_batch_t {
 	PinnedBuffer<AccTask> h_atasks;
 	DeviceBuffer<AccTask> d_atasks;
 	jsmpeg_b200_stats_t stats{};
+	// JSMPEG_B200_HOST_TRACE=1: decode() prints where the host's time of the call went (tools/time_stages.py), in ms:
+	// upload_all | planning the waves | building and queueing stage 1 | waiting for the infos | consuming them |
+	// queueing stage 2 | the closing synchronises; and `device`, from the tasks' upload to the later of the last expand
+	// and the last reconstruct launch
+	struct HostTrace {
+		bool on = false;
+		double upload = 0, plan = 0, stage1 = 0, infos = 0, consume = 0, stage2 = 0, close = 0, device = 0;
+	} trace;
 };
 
 namespace {
@@ -176,6 +187,14 @@ namespace {
 using Batch = jsmpeg_b200_batch_t;
 
 void use_device(Batch *b) { CUDA_CHECK(cudaSetDevice(b->device)); }
+
+// Adds the host time since `since` to `sum` (Batch::HostTrace) and restarts the clock
+using HostClock = std::chrono::steady_clock;
+void lap(double &sum, HostClock::time_point &since) {
+	const HostClock::time_point now = HostClock::now();
+	sum += std::chrono::duration<double, std::milli>(now - since).count();
+	since = now;
+}
 
 void mark_dead(Batch *b, const char *what) {
 	if (!b->dead) fprintf(stderr, "%s\njsmpeg_b200: decoder disabled (decode() returns false from now on)\n", what);
@@ -673,10 +692,13 @@ void free_slots_for(Batch *b, size_t need) {
 // within a kernel, longest first: a CTA's warps, and consecutive CTAs (which land on different SMs), then carry
 // similar amounts of work and the walk ends without a long tail.  The first kernel present runs on the main stream;
 // the others have walk kernels of their own (one warp per picture, latency-bound like every walk) and run beside it on
-// side streams, forked after the upload and joined before the infos are read.  On return the infos are on the host,
-// b->h_info[i] that of wave[i], and ev_a / ev_mid / ev_b bracket the wave and its lane-parallel walk.  Returns the
-// number of kernels launched.
-int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
+// side streams, forked after the upload and joined on the main stream, where ev_a / ev_b bracket the wave.  On return
+// the infos are on the host, b->h_info[i] that of wave[i].
+// early_infos = false: stage 1 is complete on return.  true (decode()): the infos, which the walks write, leave behind
+// the walks alone (ev_mid: every walk done) and the host returns with them while the expand of the biggest pictures is
+// still running; a reader of the coefficients waits for ev_b.
+// Returns the number of kernels launched.
+int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand, bool early_infos = false) {
 	const int n = (int)wave.size();
 	std::vector<int> order(n);
 	for (int i = 0; i < n; i++) order[i] = i;
@@ -708,18 +730,22 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand) {
 			st = b->st_side[n_side];
 			CUDA_CHECK(cudaStreamWaitEvent(st, b->ev_sfork, 0));
 		}
-		launches += launch_parse_pictures((WalkKind)kind, b->d_ptasks.data() + off, cnt[kind], b->slot_mb, expand, st,
-		                                  kind == WALK_LANES ? b->ev_mid : nullptr, &b->fork);
+		launches += launch_parse_pictures((WalkKind)kind, b->d_ptasks.data() + off, cnt[kind], b->slot_mb, expand, st, &b->fork,
+		                                  early_infos ? b->st_info : nullptr);
 		if (kind != primary) {
 			CUDA_CHECK(cudaEventRecord(b->ev_sjoin[n_side], st));
 			CUDA_CHECK(cudaStreamWaitEvent(b->st_main, b->ev_sjoin[n_side], 0));
 			n_side++;
 		}
 	}
-	CUDA_CHECK(cudaMemcpyAsync(b->h_info.data(), b->d_info.data(), n * sizeof(picture_info_t), cudaMemcpyDeviceToHost, b->st_main));
-	if (cnt[WALK_LANES] == 0) CUDA_CHECK(cudaEventRecord(b->ev_mid, b->st_main));  // (a wave without the lane-parallel walk)
+	cudaStream_t st_info = early_infos ? b->st_info : b->st_main;
+	if (early_infos) CUDA_CHECK(cudaEventRecord(b->ev_mid, st_info));
+	CUDA_CHECK(cudaMemcpyAsync(b->h_info.data(), b->d_info.data(), n * sizeof(picture_info_t), cudaMemcpyDeviceToHost, st_info));
+	if (early_infos) CUDA_CHECK(cudaEventRecord(b->ev_info, st_info));
 	CUDA_CHECK(cudaEventRecord(b->ev_b, b->st_main));
-	CUDA_CHECK(cudaEventSynchronize(b->ev_b));
+	HostClock::time_point t = HostClock::now();
+	CUDA_CHECK(cudaEventSynchronize(early_infos ? b->ev_info : b->ev_b));
+	lap(b->trace.infos, t);
 	return launches;
 }
 
@@ -781,6 +807,7 @@ void reserve_b_sets(Batch *b, Stream &s) {
 // whether the stream may have further pictures.
 long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &progress, std::vector<char> &more, int flags) {
 	const int S = (int)b->streams.size();
+	HostClock::time_point t = HostClock::now();
 	// ---- 1. plan the parse wave
 	std::vector<WaveItem> wave;
 	std::vector<size_t> fresh(S, 0);  // per stream: the cache index of its first picture in the wave
@@ -812,9 +839,14 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			s.cache.push_back(p);
 		}
 	}
-	// ---- 2. stage 1: the wave, every picture's info on the host before consumption starts
+	// ---- 2. stage 1: the wave, every picture's info on the host before consumption starts; the end of its expand goes
+	// on beside steps 3 and 4
+	lap(b->trace.plan, t);
 	if (!wave.empty()) {
-		b->stats.kernel_launches += parse_wave(b, wave, true);
+		const double infos = b->trace.infos;
+		b->stats.kernel_launches += parse_wave(b, wave, true, true);
+		lap(b->trace.stage1, t);
+		b->trace.stage1 -= b->trace.infos - infos;
 		for (size_t i = 0; i < wave.size(); i++) {  // a stream's pictures are in the wave in cache order
 			const int si = wave[i].stream;
 			Parsed &p = b->streams[si].cache[fresh[si]++];
@@ -824,11 +856,6 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 		}
 		b->stats.h2d_bytes += wave.size() * sizeof(ParseTask);
 		b->stats.d2h_bytes += wave.size() * sizeof(picture_info_t);
-		float ms = 0;
-		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_a, b->ev_b));
-		b->stats.parse_ms += ms;
-		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_a, b->ev_mid));
-		b->stats.walk_ms += ms;
 	}
 	// ---- 3. consume in decode() order; the j-th reconstructed picture of a stream goes to step j
 	long consumed = 0;
@@ -889,11 +916,16 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 				b->stats.algorithmic_bytes += planes + (e.info.picture_type == 2 ? planes : (is_b ? 2 * planes : 0)) +
 				                              (uint64_t)s.seq.mb_size * sizeof(mb_record_t) + (uint64_t)e.info.n_coded_blocks * sizeof(coef_record_t);
 			}
-			release_slot(b, e.slot);  // reused by the NEXT round's parse, which waits for this round's reconstruction (ev_round)
+			// reused by the NEXT round's parse, which waits for this round's reconstruction (ev_round) and is queued behind
+			// this round's expand on the main stream
+			release_slot(b, e.slot);
 		}
 	}
-	// ---- 4. reconstruction, one step after the other on the reconstruct stream
+	lap(b->trace.consume, t);
+	// ---- 4. reconstruction, one step after the other on the reconstruct stream, behind the wave's expand: the host has
+	// consumed the infos and queues the launches while the expand of the biggest pictures is still running
 	if (!steps.empty()) {
+		if (!wave.empty()) CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_b, 0));
 		CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
 		for (ReconStep &r : steps) {
 			// A launch overwrites, per stream, the plane set written two of that stream's pictures ago, i.e. by
@@ -908,17 +940,41 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 		CUDA_CHECK(cudaEventRecord(b->ev_recon[1], b->st_recon));
 		CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
 		b->recon_pending = true;
+	}
+	lap(b->trace.stage2, t);
+	// ---- 5. the round ends with its wave complete (a round that reconstructs nothing has not waited for its expand yet)
+	float ms = 0;
+	if (!steps.empty()) {
 		CUDA_CHECK(cudaEventSynchronize(b->ev_recon[1]));
-		float ms = 0;
 		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_recon[0], b->ev_recon[1]));
 		b->stats.recon_ms += ms;
 	}
+	if (!wave.empty()) {
+		CUDA_CHECK(cudaEventSynchronize(b->ev_b));
+		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_a, b->ev_b));  // (beside the reconstruction: the two overlap)
+		b->stats.parse_ms += ms;
+		CUDA_CHECK(cudaEventElapsedTime(&ms, b->ev_a, b->ev_mid));
+		b->stats.walk_ms += ms;
+		if (b->trace.on) {
+			float to_b = 0, to_recon = 0;
+			CUDA_CHECK(cudaEventElapsedTime(&to_b, b->ev_a, b->ev_b));
+			if (!steps.empty()) CUDA_CHECK(cudaEventElapsedTime(&to_recon, b->ev_a, b->ev_recon[1]));
+			b->trace.device += std::max(to_b, to_recon);
+		}
+	}
+	lap(b->trace.close, t);
 	return consumed;
 }
 
 long batch_decode(Batch *b, int n_pictures, int flags) {
 	use_device(b);
+	Batch::HostTrace &tr = b->trace;
+	const bool trace_on = tr.on;
+	tr = Batch::HostTrace{};
+	tr.on = trace_on;
+	HostClock::time_point t = HostClock::now();
 	upload_all(b);
+	lap(tr.upload, t);
 	ensure_pool(b);
 	const int S = (int)b->streams.size();
 	std::vector<int> remaining(S, n_pictures), want(S), progress(S);
@@ -945,10 +1001,15 @@ long batch_decode(Batch *b, int n_pictures, int flags) {
 		if (got == 0 && (!replanned || ++idle_rounds > 2)) break;
 		if (got) idle_rounds = 0;
 	}
+	t = HostClock::now();
 	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
 	CUDA_CHECK(cudaStreamSynchronize(b->st_copy));
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+	lap(tr.close, t);
 	b->recon_pending = false;
+	if (tr.on)
+		fprintf(stderr, "jsmpeg_b200 decode host_ms: upload=%.3f plan=%.3f stage1=%.3f infos=%.3f consume=%.3f stage2=%.3f close=%.3f device=%.3f\n",
+		        tr.upload, tr.plan, tr.stage1, tr.infos, tr.consume, tr.stage2, tr.close, tr.device);
 	return total;
 }
 
@@ -1761,20 +1822,23 @@ jsmpeg_b200_batch_t *jsmpeg_b200_batch_create(int n_streams, int device, unsigne
 	b->max_slots_req = max_slots;
 	b->decode_b = env_int("JSMPEG_B200_DECODE_B", 0) != 0;
 	b->slice_walk = env_int("JSMPEG_B200_SLICE_WALK", 0) != 0;
+	b->trace.on = env_int("JSMPEG_B200_HOST_TRACE", 0) != 0;
 	try {
 		use_device(b);
 		CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_main, cudaStreamNonBlocking));
 		CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_recon, cudaStreamNonBlocking));
+		CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_info, cudaStreamNonBlocking));
 		CUDA_CHECK(cudaStreamCreateWithFlags(&b->st_copy, cudaStreamNonBlocking));
 		for (auto &st : b->st_side) CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
 		cudaEvent_t *timed[] = {&b->ev_a, &b->ev_b, &b->ev_mid, &b->ev_recon[0], &b->ev_recon[1]};
 		for (auto e : timed) CUDA_CHECK(cudaEventCreate(e));
-		cudaEvent_t *untimed[] = {&b->ev_step, &b->ev_round, &b->ev_copied[0], &b->ev_copied[1], &b->ev_sfork, &b->ev_sjoin[0], &b->ev_sjoin[1]};
+		cudaEvent_t *untimed[] = {&b->ev_step, &b->ev_round, &b->ev_copied[0], &b->ev_copied[1], &b->ev_sfork, &b->ev_sjoin[0], &b->ev_sjoin[1], &b->ev_info};
 		for (auto e : untimed) CUDA_CHECK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
 		CUDA_CHECK(cudaEventCreateWithFlags(&b->fork.fork, cudaEventDisableTiming));
 		for (int i = 0; i < PARSE_GROUPS; i++) {
 			CUDA_CHECK(cudaStreamCreateWithFlags(&b->fork.side[i], cudaStreamNonBlocking));
 			CUDA_CHECK(cudaEventCreateWithFlags(&b->fork.join[i], cudaEventDisableTiming));
+			CUDA_CHECK(cudaEventCreateWithFlags(&b->fork.walked[i], cudaEventDisableTiming));
 		}
 	} catch (const std::exception &e) {
 		mark_dead(b, e.what());  // no usable device: a decoder that answers false, not a dead process
@@ -1789,12 +1853,13 @@ void jsmpeg_b200_batch_destroy(jsmpeg_b200_batch_t *b) {
 	(void)cudaDeviceSynchronize();
 	for (auto &s : b->streams) if (s.bb.bytes) kPinned.release(s.bb.bytes, kPinned.ctx);
 	for (auto e : {b->ev_a, b->ev_b, b->ev_mid, b->ev_recon[0], b->ev_recon[1], b->ev_step, b->ev_round, b->ev_copied[0],
-	               b->ev_copied[1], b->ev_sfork, b->ev_sjoin[0], b->ev_sjoin[1], b->fork.fork}) if (e) cudaEventDestroy(e);
+	               b->ev_copied[1], b->ev_sfork, b->ev_sjoin[0], b->ev_sjoin[1], b->fork.fork, b->ev_info}) if (e) cudaEventDestroy(e);
 	for (int i = 0; i < PARSE_GROUPS; i++) {
 		if (b->fork.join[i]) cudaEventDestroy(b->fork.join[i]);
+		if (b->fork.walked[i]) cudaEventDestroy(b->fork.walked[i]);
 		if (b->fork.side[i]) cudaStreamDestroy(b->fork.side[i]);
 	}
-	for (auto st : {b->st_main, b->st_recon, b->st_copy, b->st_side[0], b->st_side[1]}) if (st) cudaStreamDestroy(st);
+	for (auto st : {b->st_main, b->st_recon, b->st_copy, b->st_info, b->st_side[0], b->st_side[1]}) if (st) cudaStreamDestroy(st);
 	delete b;  // the buffers free themselves, after the synchronize above
 	(void)cudaGetLastError();
 }

@@ -206,7 +206,7 @@ static const uint16_t *ms_table_for_current_device() {
 }
 
 int launch_parse_pictures(WalkKind kind, const ParseTask *tasks, int n_tasks, int max_mb_size, bool expand,
-                          cudaStream_t stream, cudaEvent_t walk_done, const ParseFork *fork) {
+                          cudaStream_t stream, const ParseFork *fork, cudaStream_t after_walks) {
 	if (n_tasks <= 0) return 0;
 	const uint4 *ms = reinterpret_cast<const uint4 *>(ms_table_for_current_device());
 	const WalkKernel walk = walk_kernels()[kind];
@@ -225,7 +225,10 @@ int launch_parse_pictures(WalkKind kind, const ParseTask *tasks, int n_tasks, in
 		cudaStream_t st = g == 0 ? stream : fork->side[g];
 		if (g > 0) CUDA_CHECK(cudaStreamWaitEvent(st, fork->fork, 0));
 		walk.fn<<<(n + per_cta - 1) / per_cta, WALK_THREADS, walk.smem, st>>>(tasks + lo, n, ms);
-		if (g == 0 && walk_done) CUDA_CHECK(cudaEventRecord(walk_done, st));
+		if (after_walks) {
+			CUDA_CHECK(cudaEventRecord(fork->walked[g], st));
+			CUDA_CHECK(cudaStreamWaitEvent(after_walks, fork->walked[g], 0));
+		}
 		if (expand) launch_expand(tasks + lo, n, max_mb_size, st);
 		if (g > 0) {
 			CUDA_CHECK(cudaEventRecord(fork->join[g], st));

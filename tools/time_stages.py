@@ -2,6 +2,12 @@
 """GPU helper: per-stage device time of the batch decode on a bench-like workload.
 
     python tools/time_stages.py [streams] [pictures] [reps]
+
+parse (the tasks' upload to the end of the last expand) and recon (around the reconstruct launches) overlap.  Before each
+line the library prints where the host's time of the call went (JSMPEG_B200_HOST_TRACE: upload_all, planning, building
+and queueing stage 1, the wait for the infos, their consumption, queueing stage 2, the closing synchronises) and
+`device`, the span from the tasks' upload to the end of the later of expand and reconstruction; step - scan - device is
+what no device event covers.
 """
 import os
 import sys
@@ -10,6 +16,7 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
+os.environ.setdefault("JSMPEG_B200_HOST_TRACE", "1")
 import bench  # noqa: E402
 from jsmpeg_b200.batch import OUT_DEVICE, BatchDecoder  # noqa: E402
 
