@@ -133,11 +133,30 @@ int jsmpeg_b200_batch_stream_info(jsmpeg_b200_batch_t *b, int stream, int *width
  * searched for like the reference does (ts.js:155-189); a PID that a later PES header binds to
  * another stream id stops feeding this stream (ts.js:81-83).  Returns the number of
  * elementary-stream bytes appended (-1: the decoder is dead).  pts_out / offset_out (capacity n_max,
- * may be NULL) receive, per
- * PES packet in stream order, its PTS in 90 kHz ticks (0 if absent) and the byte offset of its
+ * may be NULL) receive, per PES packet in stream order (the first n_max of them; *n_pes counts all), its PTS in 90 kHz ticks (0 if absent) and the byte offset of its
  * payload in the stream's buffer -- the table Decoder.Base.write keeps (src/decoder.js:36-47). */
 long jsmpeg_b200_batch_write_ts(jsmpeg_b200_batch_t *b, int stream, const uint8_t *ts, size_t n_bytes, int stream_id,
                                 uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes);
+
+/* MPEG-TS of many streams in one call (live ingest: a chunk from each of many sources per tick).  Request i does
+ * exactly what jsmpeg_b200_batch_write_ts(b, streams[i], ts[i], n_bytes[i], stream_ids ? stream_ids[i] : 0xE0, ...)
+ * does: the same elementary-stream bytes appended, the same PES table, the same bytes left over for the stream's
+ * next TS write and the same PID bindings carried on, for any interleaving of write_ts and write_ts_many calls.
+ * All requests are demultiplexed in one pass on the GPU; the call's kernel launches and host synchronisations do
+ * not grow with n.  A stream may be named at most once per call.  Two requests may pass the same buffer (a
+ * multiplex of several video programs, each to its own stream by its stream id).  Streams not named are not touched.
+ *   appended_out[i] (may be NULL): ES bytes appended to streams[i] (write_ts's return value).
+ *   n_pes_out[i]    (may be NULL): PES starts of request i (write_ts's *n_pes), counted even where dropped below.
+ *   pts_out / offset_out (each may be NULL; n_max entries for the whole call): request 0's PES starts in stream
+ *   order, then request 1's, ...; 90 kHz PTS (0 if absent) and payload offset in the stream's buffer, as write_ts;
+ *   entries beyond n_max are dropped.
+ * Synchronous.  Returns the ES bytes appended over all requests; -1 dead; -2 a request is invalid (n < 0; streams,
+ * ts or n_bytes NULL with n > 0; a stream out of range or named twice; ts[i] NULL with n_bytes[i] > 0; the call's
+ * input plus the named streams' left-over bytes 4 GiB - 4 KiB or more) -- checked before any work, and then
+ * nothing changed. */
+long jsmpeg_b200_batch_write_ts_many(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint8_t *const *ts,
+                                     const size_t *n_bytes, const int *stream_ids, long *appended_out,
+                                     uint64_t *pts_out, uint32_t *offset_out, long n_max, int32_t *n_pes_out);
 
 /* MPEG program stream in (ISO 11172-1 system stream, .mpg / VCD .dat; ISO 13818-1 program stream, .vob),
  * demultiplexed on the GPU: the payload of every PES packet with stream id `stream_id` (0xE0..0xEF) is

@@ -216,12 +216,30 @@ struct AccTask {
 };
 void launch_accumulate(const AccTask *tasks, int n_tasks, uint32_t total_warps, cudaStream_t stream);
 
-// device MPEG-TS demux (tsdemux.cu)
+// device MPEG-TS demux of many requests in one pass (tsdemux.cu, tsdemux.cuh).  A call: ts_call_begin makes room for
+// n_req requests, `bytes` staged bytes and n_slots packet slots (max_req: the most requests a call of the batch can
+// have, which fixes the event key's width); the caller stages the bytes and h_req[0 .. n_req] (entry n_req: slot0 =
+// n_slots) and uploads them; ts_call_measure queues the grid, classify, bind and place scans and the D2H of the
+// per-request totals to h_out; once the caller has set every request's dst / es_base and uploaded h_req again,
+// ts_call_gather queues the copy of the payloads and the PES list (d_pes_*, in (request, offset) order).  Both
+// return the launches they queued.
+struct TsReq;
+struct TsReqOut;
 struct TsScratch;
+struct TsCall {
+	uint8_t *stage;
+	TsReq *h_req, *d_req;
+	TsReqOut *h_out;
+	uint32_t *d_pes_offset;
+	uint64_t *d_pes_pts;
+	uint32_t *h_pes_offset;
+	uint64_t *h_pes_pts;
+};
 TsScratch *ts_scratch_create();
 void ts_scratch_destroy(TsScratch *s);
-long ts_demux_measure(TsScratch *s, const uint8_t *ts_host, size_t ts_bytes, int stream_id, int16_t *bound, size_t *consumed, cudaStream_t st);
-int ts_demux_gather(TsScratch *s, uint8_t *es, uint32_t es_base, uint64_t *pts_out, uint32_t *offset_out, int n_max, cudaStream_t st);
+TsCall ts_call_begin(TsScratch *s, uint32_t n_req, size_t bytes, uint32_t n_slots, uint32_t max_req);
+uint32_t ts_call_measure(TsScratch *s, cudaStream_t st);
+uint32_t ts_call_gather(TsScratch *s, uint32_t pad, cudaStream_t st);
 
 // device MPEG program stream demux (psdemux.cu)
 struct PsScratch;

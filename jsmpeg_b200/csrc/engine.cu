@@ -42,6 +42,7 @@
 #include "bitbuffer.h"
 #include "buffers.h"
 #include "common.cuh"
+#include "tsdemux.cuh"
 #include "../../include/jsmpeg_b200.h"
 
 namespace {
@@ -93,7 +94,7 @@ struct Stream {
 	uint8_t *d_last = nullptr;
 	int last_type = 0, last_temporal = 0;  // picture_coding_type / temporal_reference of the last picture decode() consumed
 	DeviceBuffer<uint8_t> d_rgba;
-	std::vector<int16_t> ts_bound;     // device TS demux: the stream id every PID is bound to, 0 = none (ts.js pidsToStreamIds)
+	DeviceBuffer<int16_t> ts_bound;    // device TS demux: the stream id every PID is bound to, 0 = none (ts.js pidsToStreamIds)
 	std::vector<uint8_t> ts_leftover;  // ... and the bytes the last write_ts left over (ts.js leftoverBytes)
 	std::vector<uint8_t> ps_leftover;  // device PS demux: the bytes the last write_ps left over
 	bool ps_in_sync = false;           // ... and whether they continue the item chain (else: look for a pack header)
@@ -567,13 +568,15 @@ bool entry_stale(const Stream &s, const Parsed &e) {
 }
 
 // dst[i] <- src[i], size[i] bytes, in ONE batched copy call on `st` (cudaMemcpyBatchAsync, CUDA 12.8+); plain copies
-// where the driver has no batched copy
-void copy_batch(Batch *b, std::vector<void *> &dst, std::vector<void *> &src, std::vector<size_t> &size, cudaStream_t st) {
+// where the driver has no batched copy.  `order`: cudaMemcpySrcAccessOrderDuringApiCall for sources the caller may
+// change once the call returns (pageable memory)
+void copy_batch(Batch *b, std::vector<void *> &dst, std::vector<void *> &src, std::vector<size_t> &size, cudaStream_t st,
+                cudaMemcpySrcAccessOrder order = cudaMemcpySrcAccessOrderStream) {
 	const size_t n_copy = dst.size();
 	bool batched = false;
 	if (b->batch_copy_ok && n_copy > 1) {
 		cudaMemcpyAttributes attr{};
-		attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
+		attr.srcAccessOrder = order;
 		size_t attr_idx = 0, fail_idx = 0;
 		cudaError_t e = cudaMemcpyBatchAsync(dst.data(), src.data(), size.data(), n_copy, &attr, &attr_idx, 1, &fail_idx, st);
 		if (e == cudaSuccess) batched = true;
@@ -1774,7 +1777,7 @@ int env_int(const char *name, int fallback) {
 	return e && *e ? atoi(e) : fallback;
 }
 
-// The tail of a device demux (write_ts, write_ps): `total` ES bytes that gather(es_base) writes to the HBM
+// The tail of the program stream demux (write_ps): `total` ES bytes that gather(es_base) writes to the HBM
 // mirror at s.d_es + es_base are appended to the stream as if written with get_write_ptr / did_write.
 // gather returns the number of PES starts it listed in pts_out / offset_out (unordered).
 template <typename F>
@@ -1804,6 +1807,138 @@ long append_demuxed(Batch *b, Stream &s, uint32_t total, F &&gather, uint64_t *p
 		for (int i = 0; i < m; i++) { offset_out[i] = v[i].first; pts_out[i] = v[i].second; }
 	}
 	return total;
+}
+
+// jsmpeg_b200_batch_write_ts_many (include/jsmpeg_b200.h): request i appends to streams[i] what write_ts would.  One
+// pass for all requests (tsdemux.cu, DESIGN 3.3): one batched upload, the measure launches, one synchronize for the
+// totals; the host makes room in every stream (the write protocol, may expand or evict) and flushes its ordinary
+// writes; one gather launch, one batched copy back of the new ES bytes and the PES list, one synchronize.
+long ts_write_many(Batch *b, int n, const int *streams, const uint8_t *const *ts, const size_t *n_bytes, const int *stream_ids,
+                   long *appended_out, uint64_t *pts_out, uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
+	if (n < 0 || (n > 0 && (!streams || !ts || !n_bytes))) return -2;
+	const int S = (int)b->streams.size();
+	std::vector<char> named(S, 0);
+	uint64_t all = 0;
+	for (int i = 0; i < n; i++) {
+		if (streams[i] < 0 || streams[i] >= S || named[streams[i]] || (!ts[i] && n_bytes[i] > 0)) return -2;
+		named[streams[i]] = 1;
+		all += b->streams[streams[i]].ts_leftover.size() + (uint64_t)n_bytes[i];
+	}
+	if (all >= 0xfffff000ull) return -2;  // (positions are 32-bit; a header read may run a few bytes past a request)
+	for (int i = 0; i < n; i++) {
+		if (appended_out) appended_out[i] = 0;
+		if (n_pes_out) n_pes_out[i] = 0;
+	}
+	if (n == 0) return 0;
+	use_device(b);
+	if (!b->ts) b->ts.reset(ts_scratch_create());
+	// a request's bytes: what its stream's last write left over (a partial packet, a resync that wanted more data:
+	// ts.js:25-41), then the new ones; packet slots: one per 188 bytes
+	size_t staged = 0;
+	uint32_t slots = 0;
+	for (int i = 0; i < n; i++) {
+		const uint64_t len = b->streams[streams[i]].ts_leftover.size() + n_bytes[i];
+		if (len >= 188) { staged += len; slots += (uint32_t)(len / 188); }
+	}
+	std::vector<uint32_t> stop(n, 0), total(n, 0);
+	long appended = 0;
+	if (slots) {
+		const TsCall c = ts_call_begin(b->ts.get(), (uint32_t)n, staged, slots, (uint32_t)S);
+		std::vector<void *> dst, src;
+		std::vector<size_t> size;
+		uint32_t base = 0, slot = 0;
+		for (int i = 0; i < n; i++) {
+			Stream &s = b->streams[streams[i]];
+			if (!s.ts_bound.data()) {  // the stream's first TS write: no PID bound yet
+				s.ts_bound.reserve(8192);
+				CUDA_CHECK(cudaMemsetAsync(s.ts_bound.data(), 0, 8192 * sizeof(int16_t), b->st_main));
+			}
+			const uint32_t lo = (uint32_t)s.ts_leftover.size(), len = lo + (uint32_t)n_bytes[i];
+			const bool whole = len >= 188;  // (fewer bytes: not a packet yet, nothing to upload)
+			c.h_req[i] = TsReq{base, whole ? len : 0, slot, stream_ids ? stream_ids[i] : 0xE0, s.ts_bound.data(), nullptr, 0, 0};
+			if (!whole) continue;
+			if (lo) { dst.push_back(c.stage + base); src.push_back(s.ts_leftover.data()); size.push_back(lo); }
+			if (n_bytes[i]) { dst.push_back(c.stage + base + lo); src.push_back(const_cast<uint8_t *>(ts[i])); size.push_back(n_bytes[i]); }
+			base += len;
+			slot += len / 188;
+		}
+		c.h_req[n] = TsReq{base, 0, slot, 0, nullptr, nullptr, 0, 0};
+		dst.push_back(c.d_req);
+		src.push_back(c.h_req);
+		size.push_back((n + 1) * sizeof(TsReq));
+		copy_batch(b, dst, src, size, b->st_main, cudaMemcpySrcAccessOrderDuringApiCall);
+		b->stats.h2d_bytes += staged;
+		b->stats.kernel_launches += ts_call_measure(b->ts.get(), b->st_main);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		// room in every stream's host bit buffer and HBM mirror; its ordinary writes made resident first
+		dst.clear(), src.clear(), size.clear();
+		std::vector<uint8_t *> hdst(n, nullptr);
+		uint32_t n_pes = 0;
+		for (int i = 0; i < n; i++) {
+			stop[i] = c.h_out[i].stop;
+			total[i] = c.h_out[i].total;
+			n_pes = std::max(n_pes, c.h_out[i].pes_first + c.h_out[i].pes);
+			if (!total[i]) continue;
+			Stream &s = b->streams[streams[i]];
+			hdst[i] = static_cast<uint8_t *>(stream_get_write_ptr(b, s, total[i]));
+			reserve_device_es(b, s, s.bb.length + total[i]);
+			if (s.d_valid < s.bb.length) {
+				dst.push_back(s.d_es.data() + s.d_valid);
+				src.push_back(s.bb.bytes + s.d_valid);
+				size.push_back(s.bb.length - s.d_valid);
+				b->stats.h2d_bytes += s.bb.length - s.d_valid;
+				s.d_valid = s.bb.length;
+			}
+			c.h_req[i].dst = s.d_es.data() + s.bb.length;
+			c.h_req[i].es_base = s.bb.length;
+		}
+		dst.push_back(c.d_req);
+		src.push_back(c.h_req);
+		size.push_back((n + 1) * sizeof(TsReq));
+		copy_batch(b, dst, src, size, b->st_main);
+		b->stats.kernel_launches += ts_call_gather(b->ts.get(), ES_PAD, b->st_main);
+		// the host keeps a mirror of the ES (sequence header parse, EVICT bookkeeping): the new bytes come back
+		dst.clear(), src.clear(), size.clear();
+		for (int i = 0; i < n; i++) {
+			if (!total[i]) continue;
+			dst.push_back(hdst[i]);
+			src.push_back(c.h_req[i].dst);
+			size.push_back(total[i]);
+			b->stats.d2h_bytes += total[i];
+		}
+		if (n_pes && (pts_out || offset_out) && n_max > 0) {
+			dst.push_back(c.h_pes_offset), src.push_back(c.d_pes_offset), size.push_back(n_pes * sizeof(uint32_t));
+			dst.push_back(c.h_pes_pts), src.push_back(c.d_pes_pts), size.push_back(n_pes * sizeof(uint64_t));
+		}
+		if (!dst.empty()) copy_batch(b, dst, src, size, b->st_main);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		long listed = 0;
+		for (int i = 0; i < n; i++) {
+			if (!total[i]) continue;
+			Stream &s = b->streams[streams[i]];
+			stream_did_write(b, s, total[i]);
+			s.d_valid = s.bb.length;
+			appended += total[i];
+			if (appended_out) appended_out[i] = total[i];
+			if (n_pes_out) n_pes_out[i] = (int32_t)c.h_out[i].pes;
+			for (uint32_t k = 0; k < c.h_out[i].pes && listed < n_max; k++, listed++) {
+				if (pts_out) pts_out[listed] = c.h_pes_pts[c.h_out[i].pes_first + k];
+				if (offset_out) offset_out[listed] = c.h_pes_offset[c.h_out[i].pes_first + k];
+			}
+		}
+	}
+	// what the demuxer did not consume stays for the stream's next write
+	for (int i = 0; i < n; i++) {
+		std::vector<uint8_t> &lo = b->streams[streams[i]].ts_leftover;
+		const size_t k = stop[i];
+		if (k <= lo.size()) {
+			lo.erase(lo.begin(), lo.begin() + k);
+			lo.insert(lo.end(), ts[i], ts[i] + n_bytes[i]);
+		} else {
+			lo.assign(ts[i] + (k - lo.size()), ts[i] + n_bytes[i]);
+		}
+	}
+	return appended;
 }
 
 }  // namespace
@@ -2073,28 +2208,20 @@ long jsmpeg_b200_batch_write_ts(jsmpeg_b200_batch_t *b, int stream, const uint8_
                                 uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes) {
 	if (n_pes) *n_pes = 0;
 	return guarded<long>(b, -1, [&]() -> long {
-		use_device(b);
-		Stream &s = b->streams[stream];
-		if (!b->ts) b->ts.reset(ts_scratch_create());
-		if (s.ts_bound.empty()) s.ts_bound.assign(8192, 0);
-		// what the previous call left over comes first (a partial packet, a resync that wanted more data: ts.js:25-41)
-		const uint8_t *data = ts;
-		size_t n_data = n_bytes;
-		if (!s.ts_leftover.empty()) {
-			s.ts_leftover.insert(s.ts_leftover.end(), ts, ts + n_bytes);
-			data = s.ts_leftover.data();
-			n_data = s.ts_leftover.size();
-		}
-		size_t consumed = 0;
-		const long total = ts_demux_measure(b->ts.get(), data, n_data, stream_id, s.ts_bound.data(), &consumed, b->st_main);
-		std::vector<uint8_t> rest(data + consumed, data + n_data);  // (data may alias ts_leftover)
-		s.ts_leftover.swap(rest);
-		if (total <= 0) return total;
-		b->stats.kernel_launches += 7;
-		b->stats.h2d_bytes += n_data;
-		return append_demuxed(b, s, (uint32_t)total, [&](uint32_t es_base) {
-			return ts_demux_gather(b->ts.get(), s.d_es.data(), es_base, pts_out, offset_out, n_max, b->st_main);
-		}, pts_out, offset_out, n_max, n_pes);
+		int32_t count = 0;
+		const long r = ts_write_many(b, 1, &stream, &ts, &n_bytes, &stream_id, nullptr, pts_out && offset_out ? pts_out : nullptr,
+		                             pts_out && offset_out ? offset_out : nullptr, n_max, &count);
+		if (r == -2) throw std::runtime_error("jsmpeg_b200: write_ts: stream out of range, or a transport stream buffer of 4 GiB or more");
+		if (n_pes) *n_pes = count;
+		return r;
+	});
+}
+
+long jsmpeg_b200_batch_write_ts_many(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint8_t *const *ts,
+                                     const size_t *n_bytes, const int *stream_ids, long *appended_out, uint64_t *pts_out,
+                                     uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
+	return guarded<long>(b, -1, [&] {
+		return ts_write_many(b, n, streams, ts, n_bytes, stream_ids, appended_out, pts_out, offset_out, n_max, n_pes_out);
 	});
 }
 
