@@ -173,6 +173,27 @@ long jsmpeg_b200_batch_write_ts_many(jsmpeg_b200_batch_t *b, int n, const int *s
 long jsmpeg_b200_batch_write_ps(jsmpeg_b200_batch_t *b, int stream, const uint8_t *ps, size_t n_bytes, int stream_id,
                                 uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes);
 
+/* MPEG program streams of many streams in one call (a server or data loader reading a chunk of each of many .mpg /
+ * .vob files per tick).  Request i does exactly what jsmpeg_b200_batch_write_ps(b, streams[i], ps[i], n_bytes[i],
+ * stream_ids ? stream_ids[i] : 0xE0, ...) does: the same elementary-stream bytes appended, the same PES table, the
+ * same bytes left over and the same in-sync state carried to the stream's next PS write, for any interleaving of
+ * write_ps and write_ps_many calls.  All requests are demultiplexed in one pass on the GPU; the call's kernel
+ * launches and host synchronisations grow neither with n nor with the breaks in the input.  A stream may be named at
+ * most once per call.  Two requests may pass the same buffer (the 0xE0 and 0xE1 video streams of one .vob, each to
+ * its own stream).  Streams not named are not touched.
+ *   appended_out[i] (may be NULL): ES bytes appended to streams[i] (write_ps's return value).
+ *   n_pes_out[i]    (may be NULL): PES table entries of request i (write_ps's *n_pes), counted even where dropped below.
+ *   pts_out / offset_out (each may be NULL; n_max entries for the whole call): request 0's entries in stream order,
+ *   then request 1's, ...; 33-bit PTS in 90 kHz ticks and payload offset in the stream's buffer, as write_ps;
+ *   entries beyond n_max are dropped.
+ * Synchronous.  Returns the ES bytes appended over all requests; -1 dead; -2 a request is invalid (n < 0; streams,
+ * ps or n_bytes NULL with n > 0; a stream out of range or named twice; ps[i] NULL with n_bytes[i] > 0; a stream id
+ * outside 0xE0..0xEF; the call's input plus the named streams' left-over bytes 4 GiB - 4 KiB or more, each request
+ * rounded up to 16 bytes) -- checked before any work, and then nothing changed. */
+long jsmpeg_b200_batch_write_ps_many(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint8_t *const *ps,
+                                     const size_t *n_bytes, const int *stream_ids, long *appended_out,
+                                     uint64_t *pts_out, uint32_t *offset_out, long n_max, int32_t *n_pes_out);
+
 /* Make everything written so far resident in HBM and indexed (H2D copy of new bytes + start-code
  * scan).  Called implicitly by decode; exposed so that a benchmark can separate it.  Returns the
  * number of picture start codes currently indexed over all streams. */

@@ -44,6 +44,7 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_write_ts_many": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, ctypes.c_long, _VP]),
     "jsmpeg_b200_batch_write_ps": (ctypes.c_long, [_VP, ctypes.c_int, ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int,
                                                    _VP, _VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
+    "jsmpeg_b200_batch_write_ps_many": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, _VP, _VP, _VP, ctypes.c_long, _VP]),
     "jsmpeg_b200_batch_upload": (ctypes.c_long, [_VP]),
     "jsmpeg_b200_batch_rewind": (None, [_VP]),
     "jsmpeg_b200_batch_reset": (None, [_VP]),
@@ -223,14 +224,18 @@ class BatchDecoder:
             out.append((int(a), table))
         return out
 
+    @staticmethod
+    def _ps_pes_capacity(n_bytes):
+        """PES table entries a PS write of n_bytes can report: a table entry needs >= 12 bytes (6 + a 5-byte PTS + 1
+        payload byte); the call may also finish items of up to 65,541 bytes that an earlier call left over."""
+        return (n_bytes + 65541) // 12 + 1
+
     def write_ps(self, stream, ps_bytes, stream_id=0xE0):
         """MPEG program stream in (.mpg: ISO 11172-1, .vob: ISO 13818-1), demultiplexed on the GPU (any
         chunking, resyncs at the next pack header).  Returns (ES bytes appended, [(payload byte offset, pts
         seconds), ...] per PES packet of `stream_id` with a PTS in it)."""
         ps_bytes = bytes(ps_bytes)
-        # a table entry needs >= 12 bytes (6 + a 5-byte PTS + 1 payload byte); the call may also finish items
-        # of up to 65,541 bytes that an earlier call left over
-        n_max = (len(ps_bytes) + 65541) // 12 + 1
+        n_max = self._ps_pes_capacity(len(ps_bytes))
         pts = np.zeros(n_max, np.uint64)
         off = np.zeros(n_max, np.uint32)
         n = ctypes.c_int()
@@ -243,6 +248,38 @@ class BatchDecoder:
         table = [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
         self._pes[stream] += table
         return total, table
+
+    def write_ps_many(self, writes):
+        """MPEG program streams of many streams in one GPU pass: `writes` is an iterable of (stream, bytes) or (stream,
+        bytes, stream_id), each stream at most once.  Returns one (ES bytes appended, [(payload byte offset, pts
+        seconds), ...]) per write, what write_ps returns for it."""
+        writes = [(w[0], bytes(w[1]), w[2] if len(w) > 2 else 0xE0) for w in writes]
+        n = len(writes)
+        streams = np.array([w[0] for w in writes], np.int32)
+        bufs = [w[1] for w in writes]
+        ptrs = (ctypes.c_char_p * max(n, 1))(*bufs)
+        sizes = np.array([len(b) for b in bufs], np.uint64)
+        sids = np.array([w[2] for w in writes], np.int32)
+        appended = np.zeros(n, np.int64)
+        n_pes = np.zeros(n, np.int32)
+        n_max = sum(self._ps_pes_capacity(len(b)) for b in bufs)
+        pts = np.zeros(max(n_max, 1), np.uint64)
+        off = np.zeros(max(n_max, 1), np.uint32)
+        total = self.lib.jsmpeg_b200_batch_write_ps_many(self.handle, n, streams.ctypes.data, ctypes.addressof(ptrs),
+                                                         sizes.ctypes.data, sids.ctypes.data, appended.ctypes.data,
+                                                         pts.ctypes.data, off.ctypes.data, n_max, n_pes.ctypes.data)
+        if total == -2:
+            raise ValueError("write_ps_many: a stream out of range or named twice, a stream id outside 0xE0..0xEF, "
+                             "or 4 GiB of input or more")
+        if total < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ps_many failed")
+        out, k = [], 0
+        for (stream, _, _), a, m in zip(writes, appended, n_pes):
+            table = [(int(off[k + j]), float(pts[k + j]) / 90000.0) for j in range(m)]
+            k += m
+            self._pes[stream] += table
+            out.append((int(a), table))
+        return out
 
     def read_es(self, stream):
         """The stream's elementary stream as it is resident in HBM (test hook)."""

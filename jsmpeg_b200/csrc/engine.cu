@@ -42,6 +42,7 @@
 #include "bitbuffer.h"
 #include "buffers.h"
 #include "common.cuh"
+#include "psdemux.cuh"
 #include "tsdemux.cuh"
 #include "../../include/jsmpeg_b200.h"
 
@@ -1777,38 +1778,6 @@ int env_int(const char *name, int fallback) {
 	return e && *e ? atoi(e) : fallback;
 }
 
-// The tail of the program stream demux (write_ps): `total` ES bytes that gather(es_base) writes to the HBM
-// mirror at s.d_es + es_base are appended to the stream as if written with get_write_ptr / did_write.
-// gather returns the number of PES starts it listed in pts_out / offset_out (unordered).
-template <typename F>
-long append_demuxed(Batch *b, Stream &s, uint32_t total, F &&gather, uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes) {
-	// room in the host bit buffer (the reference's write protocol, may expand or evict) and in HBM
-	uint8_t *hdst = static_cast<uint8_t *>(stream_get_write_ptr(b, s, total));
-	reserve_device_es(b, s, s.bb.length + total);
-	if (s.d_valid < s.bb.length) {  // bytes written the ordinary way that are not resident yet
-		CUDA_CHECK(cudaMemcpyAsync(s.d_es.data() + s.d_valid, s.bb.bytes + s.d_valid, s.bb.length - s.d_valid, cudaMemcpyHostToDevice, b->st_main));
-		b->stats.h2d_bytes += s.bb.length - s.d_valid;
-		s.d_valid = s.bb.length;
-	}
-	const int count = gather(s.bb.length);
-	// the host keeps a mirror of the ES (sequence header parse, EVICT bookkeeping): copy the new bytes back
-	CUDA_CHECK(cudaMemcpyAsync(hdst, s.d_es.data() + s.bb.length, (size_t)total, cudaMemcpyDeviceToHost, b->st_main));
-	CUDA_CHECK(cudaMemsetAsync(s.d_es.data() + s.bb.length + total, 0, ES_PAD, b->st_main));
-	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-	b->stats.d2h_bytes += (uint64_t)total;
-	stream_did_write(b, s, total);
-	s.d_valid = s.bb.length;
-	if (n_pes) *n_pes = count;
-	if (pts_out && offset_out && count > 1) {  // the device appends PES starts unordered: sort by offset
-		const int m = std::min(count, n_max);
-		std::vector<std::pair<uint32_t, uint64_t>> v(m);
-		for (int i = 0; i < m; i++) v[i] = {offset_out[i], pts_out[i]};
-		std::sort(v.begin(), v.end());
-		for (int i = 0; i < m; i++) { offset_out[i] = v[i].first; pts_out[i] = v[i].second; }
-	}
-	return total;
-}
-
 // jsmpeg_b200_batch_write_ts_many (include/jsmpeg_b200.h): request i appends to streams[i] what write_ts would.  One
 // pass for all requests (tsdemux.cu, DESIGN 3.3): one batched upload, the measure launches, one synchronize for the
 // totals; the host makes room in every stream (the write protocol, may expand or evict) and flushes its ordinary
@@ -1937,6 +1906,135 @@ long ts_write_many(Batch *b, int n, const int *streams, const uint8_t *const *ts
 		} else {
 			lo.assign(ts[i] + (k - lo.size()), ts[i] + n_bytes[i]);
 		}
+	}
+	return appended;
+}
+
+// jsmpeg_b200_batch_write_ps_many (include/jsmpeg_b200.h): request i appends to streams[i] what write_ps would.  One
+// pass for all requests (psdemux.cu, DESIGN 3.5): one batched upload and the candidate search, one synchronize for the
+// candidate counts (they size the scratch and the doubling); the chain, place and totals launches, one synchronize for
+// the per-request results; the host makes room in every stream (the write protocol, may expand or evict) and flushes
+// its ordinary writes; one gather launch, one batched copy back of the new ES bytes and the PES list, one synchronize.
+long ps_write_many(Batch *b, int n, const int *streams, const uint8_t *const *ps, const size_t *n_bytes, const int *stream_ids,
+                   long *appended_out, uint64_t *pts_out, uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
+	if (n < 0 || (n > 0 && (!streams || !ps || !n_bytes))) return -2;
+	const int S = (int)b->streams.size();
+	std::vector<char> named(S, 0);
+	// a request's bytes: what its stream's last write left over (an unfinished item, or the tail that may begin a
+	// pack header), then the new ones; each at a 16-byte aligned offset (the candidate search reads 16-byte vectors)
+	uint64_t all = 0, staged = 0, left = 0;
+	for (int i = 0; i < n; i++) {
+		const int sid = stream_ids ? stream_ids[i] : 0xE0;
+		if (streams[i] < 0 || streams[i] >= S || named[streams[i]] || (!ps[i] && n_bytes[i] > 0) || sid < 0xE0 || sid > 0xEF) return -2;
+		named[streams[i]] = 1;
+		const uint64_t len = b->streams[streams[i]].ps_leftover.size() + (uint64_t)n_bytes[i];
+		left += b->streams[streams[i]].ps_leftover.size();
+		all += len;
+		staged += (len + 15) & ~15ull;
+	}
+	if (all >= 0xfffff000ull || staged >= 0xfffff000ull) return -2;  // (positions are 32-bit)
+	for (int i = 0; i < n; i++) {
+		if (appended_out) appended_out[i] = 0;
+		if (n_pes_out) n_pes_out[i] = 0;
+	}
+	if (staged == 0) return 0;  // no bytes anywhere (or no request): nothing changes
+	use_device(b);
+	if (!b->ps) b->ps.reset(ps_scratch_create());
+	PsCall c = ps_call_begin(b->ps.get(), (uint32_t)n, staged, left);
+	std::vector<void *> dst, src;
+	std::vector<size_t> size;
+	uint32_t base = 0;
+	size_t at_left = 0;
+	for (int i = 0; i < n; i++) {
+		Stream &s = b->streams[streams[i]];
+		const uint32_t lo = (uint32_t)s.ps_leftover.size(), len = lo + (uint32_t)n_bytes[i];
+		c.h_req[i] = PsReq{base, len, stream_ids ? stream_ids[i] : 0xE0, s.ps_in_sync ? 1u : 0u, nullptr, 0, 0};
+		// the left-over bytes go up from pinned memory: a left-over buffer is reallocated by nearly every call, and a
+		// pageable source whose pages come and go between batched copies faulted the copy on the H100 (DESIGN 3.5)
+		if (lo) {
+			memcpy(c.h_left + at_left, s.ps_leftover.data(), lo);
+			dst.push_back(c.stage + base), src.push_back(c.h_left + at_left), size.push_back(lo);
+			at_left += lo;
+		}
+		if (n_bytes[i]) { dst.push_back(c.stage + base + lo); src.push_back(const_cast<uint8_t *>(ps[i])); size.push_back(n_bytes[i]); }
+		base += (len + 15) & ~15u;
+	}
+	dst.push_back(c.d_req);
+	src.push_back(c.h_req);
+	size.push_back(n * sizeof(PsReq));
+	copy_batch(b, dst, src, size, b->st_main, cudaMemcpySrcAccessOrderDuringApiCall);
+	b->stats.h2d_bytes += all;
+	b->stats.kernel_launches += ps_call_candidates(b->ps.get(), b->st_main);
+	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+	b->stats.kernel_launches += ps_call_measure(b->ps.get(), &c, b->st_main);
+	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+	// room in every stream's host bit buffer and HBM mirror; its ordinary writes made resident first
+	dst.clear(), src.clear(), size.clear();
+	std::vector<uint8_t *> hdst(n, nullptr);
+	std::vector<uint32_t> total(n, 0);
+	uint32_t n_pes = 0;
+	for (int i = 0; i < n; i++) {
+		total[i] = c.h_out[i].total;
+		n_pes = std::max(n_pes, c.h_out[i].pes_first + c.h_out[i].pes);
+		if (!total[i]) continue;
+		Stream &s = b->streams[streams[i]];
+		hdst[i] = static_cast<uint8_t *>(stream_get_write_ptr(b, s, total[i]));
+		reserve_device_es(b, s, s.bb.length + total[i]);
+		if (s.d_valid < s.bb.length) {
+			dst.push_back(s.d_es.data() + s.d_valid);
+			src.push_back(s.bb.bytes + s.d_valid);
+			size.push_back(s.bb.length - s.d_valid);
+			b->stats.h2d_bytes += s.bb.length - s.d_valid;
+			s.d_valid = s.bb.length;
+		}
+		c.h_req[i].dst = s.d_es.data() + s.bb.length;
+		c.h_req[i].es_base = s.bb.length;
+	}
+	dst.push_back(c.d_req);
+	src.push_back(c.h_req);
+	size.push_back(n * sizeof(PsReq));
+	copy_batch(b, dst, src, size, b->st_main);
+	b->stats.kernel_launches += ps_call_gather(b->ps.get(), ES_PAD, b->st_main);
+	// the host keeps a mirror of the ES (sequence header parse, EVICT bookkeeping): the new bytes come back
+	dst.clear(), src.clear(), size.clear();
+	for (int i = 0; i < n; i++) {
+		if (!total[i]) continue;
+		dst.push_back(hdst[i]);
+		src.push_back(c.h_req[i].dst);
+		size.push_back(total[i]);
+		b->stats.d2h_bytes += total[i];
+	}
+	if (n_pes && (pts_out || offset_out) && n_max > 0) {
+		dst.push_back(c.h_pes_offset), src.push_back(c.d_pes_offset), size.push_back(n_pes * sizeof(uint32_t));
+		dst.push_back(c.h_pes_pts), src.push_back(c.d_pes_pts), size.push_back(n_pes * sizeof(uint64_t));
+	}
+	if (!dst.empty()) copy_batch(b, dst, src, size, b->st_main);
+	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+	long appended = 0, listed = 0;
+	for (int i = 0; i < n; i++) {
+		Stream &s = b->streams[streams[i]];
+		const PsReqOut &o = c.h_out[i];
+		if (total[i]) {
+			stream_did_write(b, s, total[i]);
+			s.d_valid = s.bb.length;
+			appended += total[i];
+			if (appended_out) appended_out[i] = total[i];
+			if (n_pes_out) n_pes_out[i] = (int32_t)o.pes;
+			for (uint32_t k = 0; k < o.pes && listed < n_max; k++, listed++) {
+				if (pts_out) pts_out[listed] = c.h_pes_pts[o.pes_first + k];
+				if (offset_out) offset_out[listed] = c.h_pes_offset[o.pes_first + k];
+			}
+		}
+		// what the demuxer did not consume stays for the stream's next write
+		std::vector<uint8_t> &lo = s.ps_leftover;
+		const size_t k = o.consumed;
+		if (k <= lo.size()) {
+			lo.erase(lo.begin(), lo.begin() + k);
+			lo.insert(lo.end(), ps[i], ps[i] + n_bytes[i]);
+		} else {
+			lo.assign(ps[i] + (k - lo.size()), ps[i] + n_bytes[i]);
+		}
+		s.ps_in_sync = o.in_sync != 0;
 	}
 	return appended;
 }
@@ -2230,29 +2328,20 @@ long jsmpeg_b200_batch_write_ps(jsmpeg_b200_batch_t *b, int stream, const uint8_
 	if (n_pes) *n_pes = 0;
 	return guarded<long>(b, -1, [&]() -> long {
 		if (stream_id < 0xE0 || stream_id > 0xEF) return -2;  // not a video stream id: the caller's mistake, nothing changes
-		use_device(b);
-		Stream &s = b->streams[stream];
-		if (!b->ps) b->ps.reset(ps_scratch_create());
-		// what the previous call left over comes first: an unfinished item, or the tail that may begin a pack header
-		const uint8_t *data = ps;
-		size_t n_data = n_bytes;
-		if (!s.ps_leftover.empty()) {
-			s.ps_leftover.insert(s.ps_leftover.end(), ps, ps + n_bytes);
-			data = s.ps_leftover.data();
-			n_data = s.ps_leftover.size();
-		}
-		size_t consumed = 0;
-		const long total = ps_demux_measure(b->ps.get(), data, n_data, stream_id, &s.ps_in_sync, &consumed, b->st_main);
-		std::vector<uint8_t> rest(data + consumed, data + n_data);  // (data may alias ps_leftover)
-		s.ps_leftover.swap(rest);
-		b->stats.h2d_bytes += n_data;
-		long r = total;
-		if (total > 0)
-			r = append_demuxed(b, s, (uint32_t)total, [&](uint32_t es_base) {
-				return ps_demux_gather(b->ps.get(), s.d_es.data(), es_base, pts_out, offset_out, n_max, b->st_main);
-			}, pts_out, offset_out, n_max, n_pes);
-		b->stats.kernel_launches += ps_demux_launches(b->ps.get());
+		int32_t count = 0;
+		const long r = ps_write_many(b, 1, &stream, &ps, &n_bytes, &stream_id, nullptr, pts_out && offset_out ? pts_out : nullptr,
+		                             pts_out && offset_out ? offset_out : nullptr, n_max, &count);
+		if (r == -2) throw std::runtime_error("jsmpeg_b200: write_ps: stream out of range, or a program stream buffer of 4 GiB or more");
+		if (n_pes) *n_pes = count;
 		return r;
+	});
+}
+
+long jsmpeg_b200_batch_write_ps_many(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint8_t *const *ps,
+                                     const size_t *n_bytes, const int *stream_ids, long *appended_out, uint64_t *pts_out,
+                                     uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
+	return guarded<long>(b, -1, [&] {
+		return ps_write_many(b, n, streams, ps, n_bytes, stream_ids, appended_out, pts_out, offset_out, n_max, n_pes_out);
 	});
 }
 

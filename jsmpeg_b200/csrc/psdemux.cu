@@ -1,26 +1,27 @@
-// psdemux.cu -- MPEG program stream demultiplexing on the device (ISO 11172-1 system streams, .mpg;
-// ISO 13818-1 program streams, .vob).  The item rules are in psdemux.cuh; the Python model is
-// tools/mini_ps.py; DESIGN section 3.5 has the why.
+// psdemux.cu -- MPEG program stream demultiplexing on the device, many streams in one pass (ISO 11172-1
+// system streams, .mpg; ISO 13818-1 program streams, .vob).  The item, link and place rules are in
+// psdemux.cuh; the Python model is tools/mini_ps.py; DESIGN section 3.5 has the why.
 //
-// Decomposition.  Where the items ARE is a chain of variable lengths: item k + 1 starts where item k
-// ends.  Walking it is ~6,000 dependent steps for a 12 MB clip of 2 KB packets, so it is resolved in
-// parallel over CANDIDATES instead:
-//   candidates  every 00 00 01 of the buffer (scan.cu's kernel), those with a code >= B9 kept, sorted;
-//               per candidate: its item length and its SUCCESSOR, the candidate at pos + len (binary
-//               search) -- or a terminal: END (exactly at the buffer end), INCOMPLETE (needs bytes of the
-//               next call), BREAK (no item where one should start); a terminal points to itself
-//   chain       pointer doubling J(k+1)(x) = Jk(Jk(x)), then marking from the head top down: S = {head},
-//               for k = K .. 0 add Jk(x) for every x in S.  What ends up marked is exactly what the head
-//               reaches, after 2 (K + 1) launches.  A BREAK restarts from the next valid pack header
-//               after it (a suffix minimum over the candidates), one round per break.
-//   classify    one thread per marked candidate: PES packet of the selected stream -> payload span, PTS
-//   place       exclusive scan of the payload lengths; one CTA copies one packet's payload to its place;
-//               PES starts with a PTS are appended to a list for the host's PTS table.
-#include <algorithm>
-
+// A call demultiplexes many requests (psdemux.cuh: a stream's left-over bytes and new bytes, each at its own
+// 16-byte aligned offset of one staging buffer).  Where the items ARE is a chain of variable lengths: item k + 1
+// starts where item k ends.  Walking it is ~6,000 dependent steps for a 12 MB clip of 2 KB packets, so it is
+// resolved in parallel over CANDIDATES instead:
+//   candidates  one thread per 16 staged bytes keeps every 00 00 01 that lies inside one request and has a code
+//               >= B9 and counts it for its request; one sort of the call-wide positions groups them by request
+//   link        per candidate: its SUCCESSOR, the candidate at pos + len of its request (binary search) -- or,
+//               after a break (no item where one should start), the request's next valid pack header (a
+//               suffix minimum over the candidates) -- or a terminal: END (exactly at the request's end),
+//               INCOMPLETE (needs bytes of the stream's next write), NOHEAD (no pack header left); a terminal
+//               points to itself.  Successors lie strictly later in the same request.
+//   chain       pointer doubling J(k+1)(x) = Jk(Jk(x)) up to the largest request's candidate count; one head per
+//               request; marking from all heads top down: S = {heads}, for k = K .. 0 add Jk(x) for every x in
+//               S.  What ends up marked is exactly what the heads reach; J_K(head) is the request's terminal.
+//   place       one thread per marked candidate: PES packet of the request's stream -> payload span, PTS; one
+//               exclusive scan of (payload length << 32 | PES table entry) over all candidates gives every payload
+//               its ES offset within its request and every entry its index in (request, offset) order; after the
+//               host has made room in the streams, one CTA per packet copies its payload to its stream.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
-#include <cub/device/device_select.cuh>
 
 #include "buffers.h"
 #include "common.cuh"
@@ -28,53 +29,67 @@
 
 namespace {
 
-constexpr uint32_t NONE = 0xffffffffu;
-constexpr uint64_t NONE_PTS = ~0ull;  // (a PTS has 33 bits)
-enum : uint32_t { T_LINK = 0, T_END = 1, T_INCOMPLETE = 2, T_BREAK = 3, T_NOHEAD = 4 };
-
-struct KeepCode {  // start-code prefixes that can begin an item (video ES has none of these)
-	const uint8_t *buf;
-	uint32_t n;
-	__device__ bool operator()(uint32_t p) const { return p + 3 >= n || buf[p + 3] >= 0xB9; }
-};
+constexpr uint32_t NONE = PS_NONE;
 
 struct MinOp {
 	__device__ uint32_t operator()(uint32_t a, uint32_t b) const { return a < b ? a : b; }
 };
 
-// first index with pos[index] >= want (m if none)
-__device__ uint32_t lower_bound(const uint32_t *__restrict__ pos, uint32_t m, uint32_t want) {
-	uint32_t lo = 0, hi = m;
+// the request owning staging byte g: the last one whose base is <= g; NONE if g lies in the padding behind it
+__device__ __forceinline__ uint32_t request_at(const PsReq *__restrict__ req, uint32_t n_req, uint32_t g) {
+	uint32_t lo = 0, hi = n_req;
 	while (lo < hi) {
 		const uint32_t mid = (lo + hi) >> 1;
-		if (pos[mid] < want) lo = mid + 1; else hi = mid;
+		if (req[mid].base <= g) lo = mid + 1; else hi = mid;
 	}
-	return lo;
+	return lo > 0 && g - req[lo - 1].base < req[lo - 1].n ? lo - 1 : NONE;
 }
 
-// What follows when the chain reaches byte t: the candidate there, or a terminal.
-__device__ uint2 follow(const uint8_t *__restrict__ buf, uint32_t n, const uint32_t *__restrict__ pos, uint32_t m, uint32_t t) {
-	if (t == n) return make_uint2(T_END, n);
-	const uint32_t j = lower_bound(pos, m, t);
-	if (j < m && pos[j] == t) return make_uint2(T_LINK, j);
-	// no candidate: only the head of a start-code prefix cut by the buffer end can still become an item
-	return make_uint2(ps_item_at(buf, n, t).kind == PS_NEED_MORE ? T_INCOMPLETE : T_BREAK, t);
+__device__ __forceinline__ PsCands cands_of(const PsReq &rq, const PsReqOut &o, const uint32_t *pos, const uint32_t *npr, uint32_t m) {
+	return PsCands{pos, npr, m, o.c0, o.c0 + o.count, rq.base};
 }
 
-// per candidate: successor (J0) and terminal record; rev[m - 1 - i] = i if a valid pack header starts there
-__global__ void ps_link_kernel(const uint8_t *__restrict__ buf, uint32_t n, const uint32_t *__restrict__ pos, uint32_t m,
-                               uint32_t *__restrict__ j0, uint2 *__restrict__ term, uint32_t *__restrict__ rev) {
+// candidates: a thread tests 16 staged byte positions (one 16-byte load plus a look-ahead word, as scan.cu does);
+// ctl[0] = candidates, ctl[1] = the largest request's count
+__global__ void ps_candidates_kernel(const uint8_t *__restrict__ stage, uint32_t staged, const PsReq *__restrict__ req, uint32_t n_req,
+                                     PsReqOut *__restrict__ out, uint32_t *__restrict__ sel, uint32_t *__restrict__ ctl) {
+	const uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) * 16u;
+	if (base >= staged) return;
+	const uint4 v = __ldg(reinterpret_cast<const uint4 *>(stage + base));
+	uint32_t w[5] = {v.x, v.y, v.z, v.w, 0u};
+	if (base + 16u < staged) w[4] = __ldg(reinterpret_cast<const uint32_t *>(stage + base + 16u));
+#pragma unroll
+	for (int i = 0; i < 16; i++) {
+		const uint32_t q = __funnelshift_r(w[i >> 2], w[(i >> 2) + 1], (i & 3) * 8);
+		if ((q & 0x00ffffffu) != 0x00010000u) continue;
+		const uint32_t g = base + i, r = request_at(req, n_req, g);
+		if (r == NONE || !ps_keep(stage + req[r].base, req[r].n, g - req[r].base)) continue;
+		sel[atomicAdd(ctl, 1u)] = g;
+		atomicMax(ctl + 1, atomicAdd(&out[r].count, 1u) + 1u);
+	}
+}
+
+// per candidate: rev[m - 1 - i] = i if a valid pack header starts there; per request: its first candidate
+__global__ void ps_pack_kernel(const uint8_t *__restrict__ stage, const PsReq *__restrict__ req, uint32_t n_req, const uint32_t *__restrict__ pos,
+                               uint32_t m, PsReqOut *__restrict__ out, uint32_t *__restrict__ rev) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < m) {
+		const uint32_t r = request_at(req, n_req, pos[i]);
+		rev[m - 1 - i] = ps_is_pack(stage + req[r].base, req[r].n, pos[i] - req[r].base) ? i : NONE;
+	}
+	if (i < n_req) out[i].c0 = ps_lower(pos, 0, m, req[i].base);
+}
+
+// per candidate: successor (J0) and terminal record
+__global__ void ps_link_kernel(const uint8_t *__restrict__ stage, const PsReq *__restrict__ req, uint32_t n_req, const PsReqOut *__restrict__ out,
+                               const uint32_t *__restrict__ pos, const uint32_t *__restrict__ npr, uint32_t m, uint32_t *__restrict__ j0,
+                               uint2 *__restrict__ term) {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= m) return;
-	const uint32_t p = pos[i];
-	const PsItem it = ps_item_at(buf, n, p);
-	uint2 r;
-	if (it.kind == PS_NEED_MORE) r = make_uint2(T_INCOMPLETE, p);
-	else if (it.kind == PS_BAD) r = make_uint2(T_BREAK, p);
-	else r = follow(buf, n, pos, m, p + it.len);
-	j0[i] = r.x == T_LINK ? r.y : i;
-	term[i] = r;
-	rev[m - 1 - i] = ps_is_pack(buf, n, p) ? i : NONE;
+	const uint32_t r = request_at(req, n_req, pos[i]);
+	const PsStep s = ps_link(stage + req[r].base, req[r].n, cands_of(req[r], out[r], pos, npr, m), i);
+	j0[i] = s.kind == PS_T_LINK ? s.next : i;
+	term[i] = make_uint2(s.kind, s.stop);
 }
 
 __global__ void ps_double_kernel(const uint32_t *__restrict__ jk, uint32_t *__restrict__ jk1, uint32_t m) {
@@ -82,263 +97,235 @@ __global__ void ps_double_kernel(const uint32_t *__restrict__ jk, uint32_t *__re
 	if (i < m) jk1[i] = jk[jk[i]];
 }
 
-// Head of a round (one thread).  ctl: [0] head, [1] terminal type, [2] stop position.  from == NONE: the chain
-// continues from the previous call at byte 0; otherwise it starts at the first valid pack header at or after `from`.
-__global__ void ps_head_kernel(const uint8_t *__restrict__ buf, uint32_t n, const uint32_t *__restrict__ pos, uint32_t m,
-                               const uint32_t *__restrict__ next_pack_rev, uint32_t from, uint32_t *__restrict__ ctl,
-                               uint8_t *__restrict__ marked) {
-	uint32_t head = NONE;
-	if (from == NONE) {
-		const uint2 r = follow(buf, n, pos, m, 0);
-		if (r.x == T_LINK) head = r.y;
-		else if (r.x == T_BREAK) from = 1;
-		else { ctl[0] = NONE; ctl[1] = r.x; ctl[2] = r.y; return; }
+// one thread per request: the head of its chain (marked), or its terminal if it has none
+__global__ void ps_head_kernel(const uint8_t *__restrict__ stage, const PsReq *__restrict__ req, uint32_t n_req, PsReqOut *__restrict__ out,
+                               const uint32_t *__restrict__ pos, const uint32_t *__restrict__ npr, uint32_t m, uint8_t *__restrict__ marked) {
+	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+	if (r >= n_req) return;
+	const PsStep s = ps_head(stage + req[r].base, req[r].n, cands_of(req[r], out[r], pos, npr, m), req[r].in_sync != 0);
+	if (s.kind == PS_T_LINK) {
+		out[r].head = s.next;
+		marked[s.next] = 1;
+	} else {
+		out[r].head = NONE;
+		out[r].kind = s.kind;
+		out[r].stop = s.stop;
 	}
-	if (head == NONE) {
-		const uint32_t i = lower_bound(pos, m, from);
-		if (i < m) head = next_pack_rev[m - 1 - i];
-	}
-	ctl[0] = head;
-	ctl[1] = T_NOHEAD;
-	ctl[2] = from;
-	if (head != NONE) marked[head] = 1;
 }
 
 // one level of the top-down marking.  A node marked during this launch may or may not pass its mark on:
-// either way only nodes the head reaches get marked, and every one of them is marked after level 0.
+// either way only nodes a head reaches get marked, and every one of them is marked after level 0.
 __global__ void ps_mark_kernel(const uint32_t *__restrict__ jk, uint32_t m, uint8_t *marked) {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i < m && marked[i]) marked[jk[i]] = 1;
 }
 
-__global__ void ps_end_kernel(const uint32_t *__restrict__ jtop, const uint2 *__restrict__ term, uint32_t *__restrict__ ctl) {
-	const uint32_t head = ctl[0];
-	if (head == NONE) return;
-	const uint2 r = term[jtop[head]];
-	ctl[1] = r.x;
-	ctl[2] = r.y;
-}
-
-// classify: payload span of every marked PES packet of `stream_id`
-__global__ void ps_classify_kernel(const uint8_t *__restrict__ buf, uint32_t n, const uint32_t *__restrict__ pos, uint32_t m,
-                                   const uint8_t *__restrict__ marked, int stream_id, uint32_t *__restrict__ src,
-                                   uint32_t *__restrict__ lens, uint64_t *__restrict__ pts) {
+// classify: place key, payload start (staging position) and PTS of every candidate; key[m] = 0 for the scan's total
+__global__ void ps_classify_kernel(const uint8_t *__restrict__ stage, const PsReq *__restrict__ req, uint32_t n_req,
+                                   const uint32_t *__restrict__ pos, uint32_t m, const uint8_t *__restrict__ marked,
+                                   uint64_t *__restrict__ key, uint32_t *__restrict__ src, uint64_t *__restrict__ pts) {
 	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= m) return;
-	uint32_t len = 0, start = 0;
-	uint64_t t = NONE_PTS;
-	const uint32_t p = pos[i];
-	if (marked[i] && p + 3 < n && buf[p + 3] == (uint32_t)stream_id) {
-		const PsItem it = ps_item_at(buf, n, p);
-		if (it.kind == PS_ITEM) {
-			const PsPayload pl = ps_payload(buf + p, it.len);
-			start = p + pl.start;
-			len = pl.len;
-			if (pl.has_pts && len) t = pl.pts;
-		}
+	if (i > m) return;
+	uint64_t k = 0;
+	if (i < m && marked[i]) {
+		const uint32_t r = request_at(req, n_req, pos[i]);
+		uint32_t start;
+		uint64_t t;
+		k = ps_place_key(stage + req[r].base, req[r].n, pos[i] - req[r].base, req[r].stream_id, &start, &t);
+		src[i] = req[r].base + start;
+		pts[i] = t;
 	}
-	src[i] = start;
-	lens[i] = len;
-	pts[i] = t;
+	key[i] = k;
 }
 
-// place: one CTA per candidate copies its payload; a PES start with a PTS is appended to the list
-__global__ void ps_gather_kernel(const uint8_t *__restrict__ buf, uint32_t m, const uint32_t *__restrict__ src,
-                                 const uint32_t *__restrict__ lens, const uint32_t *__restrict__ offsets,
-                                 const uint64_t *__restrict__ pts, uint8_t *__restrict__ es, uint32_t es_base,
-                                 uint32_t *__restrict__ pes_count, uint32_t *__restrict__ pes_offset, uint64_t *__restrict__ pes_pts) {
-	const uint32_t i = blockIdx.x;
-	const uint32_t len = lens[i];
-	if (len == 0) return;
-	const uint32_t off = offsets[i];
-	if (threadIdx.x == 0 && pts[i] != NONE_PTS) {
-		const uint32_t k = atomicAdd(pes_count, 1u);
-		pes_offset[k] = es_base + off;
-		pes_pts[k] = pts[i];
+// per request: its terminal, what it consumed, its ES bytes and PES table entries
+__global__ void ps_totals_kernel(const PsReq *__restrict__ req, uint32_t n_req, const uint32_t *__restrict__ jtop, const uint2 *__restrict__ term,
+                                 const uint64_t *__restrict__ scan, PsReqOut *__restrict__ out) {
+	const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+	if (r >= n_req) return;
+	PsReqOut o = out[r];
+	if (o.head != NONE) {
+		const uint2 t = term[jtop[o.head]];
+		o.kind = t.x;
+		o.stop = t.y;
 	}
-	const uint8_t *s = buf + src[i];
-	uint8_t *d = es + es_base + off;
+	ps_finish(o.kind, o.stop, req[r].n, &o.consumed, &o.in_sync);
+	const uint64_t a = scan[o.c0], b = scan[o.c0 + o.count];
+	o.total = (uint32_t)(b >> 32) - (uint32_t)(a >> 32);
+	o.pes = (uint32_t)b - (uint32_t)a;
+	o.pes_first = (uint32_t)a;
+	out[r] = o;
+}
+
+// place: CTA i < m copies candidate i's payload to its stream and lists its PES table entry; CTAs m + r then zero
+// the `pad` bytes behind request r's new ES bytes (the kernels read zeros there)
+__global__ void ps_gather_kernel(const uint8_t *__restrict__ stage, const PsReq *__restrict__ req, uint32_t n_req, const PsReqOut *__restrict__ out,
+                                 const uint32_t *__restrict__ pos, uint32_t m, const uint64_t *__restrict__ key, const uint32_t *__restrict__ src,
+                                 const uint64_t *__restrict__ pts, const uint64_t *__restrict__ scan, uint32_t pad,
+                                 uint32_t *__restrict__ pes_offset, uint64_t *__restrict__ pes_pts) {
+	const uint32_t i = blockIdx.x;
+	if (i >= m) {
+		const uint32_t r = i - m;
+		if (req[r].dst)
+			for (uint32_t k = threadIdx.x; k < pad; k += blockDim.x) req[r].dst[out[r].total + k] = 0;
+		return;
+	}
+	const uint64_t kk = key[i];
+	const uint32_t len = (uint32_t)(kk >> 32);
+	if (len == 0) return;
+	const uint32_t r = request_at(req, n_req, pos[i]);
+	if (!req[r].dst) return;
+	const uint64_t at = scan[i];
+	const uint32_t off = (uint32_t)(at >> 32) - (uint32_t)(scan[out[r].c0] >> 32);
+	if (threadIdx.x == 0 && (kk & 1)) {
+		pes_offset[(uint32_t)at] = req[r].es_base + off;
+		pes_pts[(uint32_t)at] = pts[i];
+	}
+	const uint8_t *s = stage + src[i];
+	uint8_t *d = req[r].dst + off;
 	for (uint32_t k = threadIdx.x; k < len; k += blockDim.x) d[k] = s[k];
 }
+
+constexpr int BLOCK = 256;
+int blocks(uint64_t threads) { return (int)std::max<uint64_t>((threads + BLOCK - 1) / BLOCK, 1); }
 
 }  // namespace
 
 struct PsScratch {
-	DeviceBuffer<uint8_t> buf, marked;
-	DeviceBuffer<uint32_t> scan_pos, scan_count, sel, sel_count, pos;
-	DeviceBuffer<ScanSpan> span;
+	DeviceBuffer<uint8_t> stage, marked;
+	DeviceBuffer<PsReq> req;
+	DeviceBuffer<PsReqOut> out;
+	PinnedBuffer<PsReq> h_req;
+	PinnedBuffer<PsReqOut> h_out;
+	PinnedBuffer<uint8_t> h_left;  // the requests' left-over bytes, staged for the upload
+	DeviceBuffer<uint32_t> ctl, sel, pos;
+	PinnedBuffer<uint32_t> h_ctl;
 	DeviceBuffer<uint32_t> jump;  // (levels + 1) x cap
 	DeviceBuffer<uint2> term;
-	DeviceBuffer<uint32_t> rev, next_pack_rev, ctl;
-	DeviceBuffer<uint32_t> src, lens, offsets;
-	DeviceBuffer<uint64_t> pts;
-	DeviceBuffer<uint32_t> pes_count, pes_offset;
+	DeviceBuffer<uint32_t> rev, next_pack_rev, src;
+	DeviceBuffer<uint64_t> key, scan, pts;
+	DeviceBuffer<uint32_t> pes_offset;
 	DeviceBuffer<uint64_t> pes_pts;
+	PinnedBuffer<uint32_t> h_pes_offset;
+	PinnedBuffer<uint64_t> h_pes_pts;
 	DeviceBuffer<uint8_t> temp;  // cub's temporary storage
 	size_t cap = 0;  // candidates the per-candidate arrays have room for
 	int levels = 0;
-	uint32_t m = 0, launches = 0;
+	uint32_t n_req = 0, staged = 0, m = 0;
 };
-
-// room for `need` bytes of cub's temporary storage
-static void *ps_temp(PsScratch &s, size_t need) {
-	s.temp.reserve(need);
-	return s.temp.data();
-}
-
-static void ps_reserve_scan(PsScratch &s, uint32_t n) {
-	if (n <= s.scan_pos.size()) return;
-	const uint32_t cap = n + n / 4 + 64;
-	s.scan_pos.reserve(cap);
-	s.sel.reserve(cap);
-}
-
-static void ps_reserve(PsScratch &s, size_t m) {
-	int levels = 1;
-	while ((size_t(1) << levels) < m) levels++;
-	if (m <= s.cap && levels <= s.levels) return;
-	const size_t cap = m + m / 4 + 64;
-	while ((size_t(1) << levels) < cap) levels++;
-	s.pos.reserve(cap);
-	s.jump.reserve((size_t)(levels + 1) * cap);
-	s.term.reserve(cap);
-	s.rev.reserve(cap);
-	s.next_pack_rev.reserve(cap);
-	s.marked.reserve(cap);
-	s.src.reserve(cap);
-	s.lens.reserve(cap + 1);
-	s.offsets.reserve(cap + 1);
-	s.pts.reserve(cap);
-	s.pes_offset.reserve(cap);
-	s.pes_pts.reserve(cap);
-	s.cap = cap;
-	s.levels = levels;
-}
 
 PsScratch *ps_scratch_create() { return new PsScratch(); }
 void ps_scratch_destroy(PsScratch *s) { delete s; }
 
-// Phase 1: upload, candidates, chain, classify, scan.  *in_sync in/out: does the buffer continue the chain of
-// the previous call at its first byte?  Returns the ES byte count; *consumed = the bytes of the buffer the
-// demuxer is done with (the rest is the caller's leftover).
-long ps_demux_measure(PsScratch *s, const uint8_t *host, size_t n_bytes, int stream_id, bool *in_sync, size_t *consumed, cudaStream_t st) {
-	*consumed = 0;
+static void *ps_temp(PsScratch *s, size_t bytes) {
+	if (bytes > s->temp.size()) s->temp.reserve(bytes + bytes / 4);
+	return s->temp.data();
+}
+
+static PsCall ps_call_view(PsScratch *s) {
+	return PsCall{s->stage.data(), s->h_left.data(), s->h_req.data(), s->req.data(), s->h_out.data(), s->pes_offset.data(),
+	              s->pes_pts.data(), s->h_pes_offset.data(), s->h_pes_pts.data()};
+}
+
+PsCall ps_call_begin(PsScratch *s, uint32_t n_req, size_t staged, size_t left) {
+	s->n_req = n_req;
+	s->staged = (uint32_t)staged;
 	s->m = 0;
-	s->launches = 0;
-	if (n_bytes == 0) return 0;
-	if (n_bytes > 0xfffff000ull) throw std::runtime_error("jsmpeg_b200: program stream buffer of 4 GiB or more");
-	const uint32_t n = (uint32_t)n_bytes;
-	// the scan reads 16-byte vectors and a look-ahead word
-	if (n_bytes + 32 > s->buf.size()) s->buf.reserve(n_bytes + n_bytes / 4 + 32);
-	s->span.reserve(1);
-	s->scan_count.reserve(1);
-	s->sel_count.reserve(1);
-	s->ctl.reserve(3);
-	s->pes_count.reserve(1);
-	CUDA_CHECK(cudaMemcpyAsync(s->buf.data(), host, n_bytes, cudaMemcpyHostToDevice, st));
-	CUDA_CHECK(cudaMemsetAsync(s->buf.data() + n_bytes, 0, 32, st));
-	const ScanSpan span{s->buf.data(), 0, n};
-	CUDA_CHECK(cudaMemcpyAsync(s->span.data(), &span, sizeof(span), cudaMemcpyHostToDevice, st));
-	// candidates: every 00 00 01 (a scan that ran out of room counts on: rescan with room for all)
-	ps_reserve_scan(*s, n / 256 + 1024);
-	uint32_t hits = 0;
-	for (;;) {
-		CUDA_CHECK(cudaMemsetAsync(s->scan_count.data(), 0, sizeof(uint32_t), st));
-		launch_scan_start_codes(s->span.data(), 1, n, s->scan_pos.data(), (uint32_t)s->scan_pos.size(), s->scan_count.data(), st);
-		s->launches++;
-		CUDA_CHECK(cudaMemcpyAsync(&hits, s->scan_count.data(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-		CUDA_CHECK(cudaStreamSynchronize(st));
-		if (hits <= s->scan_pos.size()) break;
-		ps_reserve_scan(*s, hits);
+	// (a 16-byte load at the last multiple of 16 and a look-ahead word behind it)
+	if (staged + 32 > s->stage.size()) s->stage.reserve(staged + staged / 4 + 32);
+	if (left > s->h_left.size()) s->h_left.reserve(left + left / 4);
+	if (n_req > s->req.size()) {
+		const size_t cap = n_req + n_req / 4 + 1;
+		s->req.reserve(cap);
+		s->h_req.reserve(cap);
+		s->out.reserve(cap);
+		s->h_out.reserve(cap);
 	}
-	ps_reserve(*s, hits);
-	uint32_t m = 0;
-	if (hits) {
-		const KeepCode keep{s->buf.data(), n};
-		size_t bytes = 0;
-		cub::DeviceSelect::If(nullptr, bytes, s->scan_pos.data(), s->sel.data(), s->sel_count.data(), (int)hits, keep, st);
-		cub::DeviceSelect::If(ps_temp(*s, bytes), bytes, s->scan_pos.data(), s->sel.data(), s->sel_count.data(), (int)hits, keep, st);
-		CUDA_CHECK(cudaMemcpyAsync(&m, s->sel_count.data(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-		CUDA_CHECK(cudaStreamSynchronize(st));
-		s->launches++;
+	s->ctl.reserve(2);
+	s->h_ctl.reserve(2);
+	// candidates lie >= 4 bytes apart (the byte behind 00 00 01 is >= B9, so no prefix starts there) except one
+	// cut by a request's end: room for every one the staged bytes can hold
+	const size_t most = staged / 4 + n_req + 1;
+	if (most > s->sel.size()) s->sel.reserve(most + most / 4);
+	return ps_call_view(s);
+}
+
+uint32_t ps_call_candidates(PsScratch *s, cudaStream_t st) {
+	CUDA_CHECK(cudaMemsetAsync(s->out.data(), 0, s->n_req * sizeof(PsReqOut), st));
+	CUDA_CHECK(cudaMemsetAsync(s->ctl.data(), 0, 2 * sizeof(uint32_t), st));
+	ps_candidates_kernel<<<blocks((s->staged + 15) / 16), BLOCK, 0, st>>>(s->stage.data(), s->staged, s->req.data(), s->n_req, s->out.data(),
+	                                                                      s->sel.data(), s->ctl.data());
+	CUDA_CHECK(cudaMemcpyAsync(s->h_ctl.data(), s->ctl.data(), 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+	return 1;
+}
+
+uint32_t ps_call_measure(PsScratch *s, PsCall *c, cudaStream_t st) {
+	const uint32_t n = s->n_req, m = s->h_ctl[0], most = s->h_ctl[1];
+	s->m = m;
+	// doubling levels: 2^levels >= the largest request's candidate count bounds every chain
+	int levels = 1;
+	while ((1u << levels) < most) levels++;
+	if (m > s->cap || levels > s->levels) {
+		const size_t cap = std::max<size_t>(m + m / 4 + 64, s->cap);
+		const int lv = std::max(levels + 1, s->levels);
+		s->pos.reserve(cap);
+		s->jump.reserve((size_t)(lv + 1) * cap);
+		s->term.reserve(cap);
+		s->rev.reserve(cap);
+		s->next_pack_rev.reserve(cap);
+		s->marked.reserve(cap);
+		s->src.reserve(cap);
+		s->pts.reserve(cap);
+		s->key.reserve(cap + 1);
+		s->scan.reserve(cap + 1);
+		s->pes_offset.reserve(cap);
+		s->pes_pts.reserve(cap);
+		s->h_pes_offset.reserve(cap);
+		s->h_pes_pts.reserve(cap);
+		s->cap = cap;
+		s->levels = lv;
+		*c = ps_call_view(s);
 	}
+	uint32_t launches = 0;
+	const uint8_t *stage = s->stage.data();
+	const PsReq *req = s->req.data();
+	PsReqOut *out = s->out.data();
+	const uint32_t *pos = s->pos.data(), *npr = s->next_pack_rev.data();
+	size_t bytes = 0;
 	if (m) {
 		int bits = 1;
-		while (bits < 32 && (1ull << bits) <= n) bits++;
-		size_t bytes = 0;
+		while (bits < 32 && (1ull << bits) <= s->staged) bits++;
 		cub::DeviceRadixSort::SortKeys(nullptr, bytes, s->sel.data(), s->pos.data(), (int)m, 0, bits, st);
-		cub::DeviceRadixSort::SortKeys(ps_temp(*s, bytes), bytes, s->sel.data(), s->pos.data(), (int)m, 0, bits, st);
-		s->launches++;
+		cub::DeviceRadixSort::SortKeys(ps_temp(s, bytes), bytes, s->sel.data(), s->pos.data(), (int)m, 0, bits, st);
+		launches++;
 	}
-	const int block = 256;
-	const int grid = (int)((m + block - 1) / block);
-	int levels = 1;
-	while ((1u << levels) < m) levels++;
-	uint32_t *jtop = s->jump.data() + (size_t)levels * s->cap;
+	ps_pack_kernel<<<blocks(std::max(m, n)), BLOCK, 0, st>>>(stage, req, n, pos, m, out, s->rev.data());
+	launches++;
 	if (m) {
-		ps_link_kernel<<<grid, block, 0, st>>>(s->buf.data(), n, s->pos.data(), m, s->jump.data(), s->term.data(), s->rev.data());
-		size_t bytes = 0;
+		bytes = 0;
 		cub::DeviceScan::InclusiveScan(nullptr, bytes, s->rev.data(), s->next_pack_rev.data(), MinOp(), (int)m, st);
-		cub::DeviceScan::InclusiveScan(ps_temp(*s, bytes), bytes, s->rev.data(), s->next_pack_rev.data(), MinOp(), (int)m, st);
-		for (int k = 0; k < levels; k++)
-			ps_double_kernel<<<grid, block, 0, st>>>(s->jump.data() + (size_t)k * s->cap, s->jump.data() + (size_t)(k + 1) * s->cap, m);
-		CUDA_CHECK(cudaMemsetAsync(s->marked.data(), 0, m, st));
-		s->launches += 2 + levels;
+		cub::DeviceScan::InclusiveScan(ps_temp(s, bytes), bytes, s->rev.data(), s->next_pack_rev.data(), MinOp(), (int)m, st);
+		launches++;
 	}
-	// the chain, one round per break
-	uint32_t from = *in_sync ? NONE : 0;
-	uint32_t ctl[3] = {NONE, T_NOHEAD, 0};
-	for (;;) {
-		ps_head_kernel<<<1, 1, 0, st>>>(s->buf.data(), n, s->pos.data(), m, s->next_pack_rev.data(), from, s->ctl.data(), s->marked.data());
-		if (m) {
-			for (int k = levels; k >= 0; k--) ps_mark_kernel<<<grid, block, 0, st>>>(s->jump.data() + (size_t)k * s->cap, m, s->marked.data());
-			ps_end_kernel<<<1, 1, 0, st>>>(jtop, s->term.data(), s->ctl.data());
-			s->launches += levels + 2;
-		}
-		s->launches++;
-		CUDA_CHECK(cudaMemcpyAsync(ctl, s->ctl.data(), sizeof(ctl), cudaMemcpyDeviceToHost, st));
-		CUDA_CHECK(cudaStreamSynchronize(st));
-		if (ctl[1] != T_BREAK) break;
-		from = ctl[2] + 1;
-	}
-	switch (ctl[1]) {
-		case T_END: *consumed = n; *in_sync = true; break;
-		case T_INCOMPLETE: *consumed = ctl[2]; *in_sync = true; break;
-		default:  // no valid pack header at or after ctl[2]: keep what could still begin one
-			*consumed = std::max<size_t>(ctl[2], n >= 4 ? n - 4 : 0);
-			*in_sync = false;
-	}
-	if (m == 0) return 0;
-	ps_classify_kernel<<<grid, block, 0, st>>>(s->buf.data(), n, s->pos.data(), m, s->marked.data(), stream_id, s->src.data(), s->lens.data(), s->pts.data());
-	CUDA_CHECK(cudaMemsetAsync(s->lens.data() + m, 0, sizeof(uint32_t), st));
-	size_t bytes = 0;
-	cub::DeviceScan::ExclusiveSum(nullptr, bytes, s->lens.data(), s->offsets.data(), (int)(m + 1), st);
-	cub::DeviceScan::ExclusiveSum(ps_temp(*s, bytes), bytes, s->lens.data(), s->offsets.data(), (int)(m + 1), st);
-	s->launches += 2;
-	uint32_t total = 0;
-	CUDA_CHECK(cudaMemcpyAsync(&total, s->offsets.data() + m, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-	CUDA_CHECK(cudaStreamSynchronize(st));
-	s->m = m;
-	return (long)total;
+	uint32_t *jump = s->jump.data();
+	ps_link_kernel<<<blocks(m), BLOCK, 0, st>>>(stage, req, n, out, pos, npr, m, jump, s->term.data());
+	for (int k = 0; k < levels; k++) ps_double_kernel<<<blocks(m), BLOCK, 0, st>>>(jump + (size_t)k * s->cap, jump + (size_t)(k + 1) * s->cap, m);
+	if (m) CUDA_CHECK(cudaMemsetAsync(s->marked.data(), 0, m, st));
+	ps_head_kernel<<<blocks(n), BLOCK, 0, st>>>(stage, req, n, out, pos, npr, m, s->marked.data());
+	for (int k = levels; k >= 0; k--) ps_mark_kernel<<<blocks(m), BLOCK, 0, st>>>(jump + (size_t)k * s->cap, m, s->marked.data());
+	ps_classify_kernel<<<blocks((uint64_t)m + 1), BLOCK, 0, st>>>(stage, req, n, pos, m, s->marked.data(), s->key.data(), s->src.data(), s->pts.data());
+	bytes = 0;
+	cub::DeviceScan::ExclusiveSum(nullptr, bytes, s->key.data(), s->scan.data(), (int)(m + 1), st);
+	cub::DeviceScan::ExclusiveSum(ps_temp(s, bytes), bytes, s->key.data(), s->scan.data(), (int)(m + 1), st);
+	ps_totals_kernel<<<blocks(n), BLOCK, 0, st>>>(req, n, jump + (size_t)levels * s->cap, s->term.data(), s->scan.data(), out);
+	launches += 2 * levels + 6;  // link, doubling, head, marking, classify, scan, totals (a cub algorithm counts as one)
+	CUDA_CHECK(cudaMemcpyAsync(s->h_out.data(), out, n * sizeof(PsReqOut), cudaMemcpyDeviceToHost, st));
+	return launches;
 }
 
-// Phase 2: gather into es[es_base ...]; returns the PES count, lists copied to the host arrays.
-int ps_demux_gather(PsScratch *s, uint8_t *es, uint32_t es_base, uint64_t *pts_out, uint32_t *offset_out, int n_max, cudaStream_t st) {
-	if (s->m == 0) return 0;
-	CUDA_CHECK(cudaMemsetAsync(s->pes_count.data(), 0, sizeof(uint32_t), st));
-	ps_gather_kernel<<<s->m, 128, 0, st>>>(s->buf.data(), s->m, s->src.data(), s->lens.data(), s->offsets.data(), s->pts.data(), es, es_base, s->pes_count.data(),
-	                                       s->pes_offset.data(), s->pes_pts.data());
-	s->launches++;
-	uint32_t count = 0;
-	CUDA_CHECK(cudaMemcpyAsync(&count, s->pes_count.data(), sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-	CUDA_CHECK(cudaStreamSynchronize(st));
-	if (pts_out && offset_out && n_max > 0) {
-		const uint32_t k = count < (uint32_t)n_max ? count : (uint32_t)n_max;
-		CUDA_CHECK(cudaMemcpyAsync(pts_out, s->pes_pts.data(), k * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-		CUDA_CHECK(cudaMemcpyAsync(offset_out, s->pes_offset.data(), k * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-		CUDA_CHECK(cudaStreamSynchronize(st));
-	}
-	return (int)count;
+uint32_t ps_call_gather(PsScratch *s, uint32_t pad, cudaStream_t st) {
+	const uint32_t n = s->n_req, m = s->m;
+	ps_gather_kernel<<<m + n, 128, 0, st>>>(s->stage.data(), s->req.data(), n, s->out.data(), s->pos.data(), m, s->key.data(), s->src.data(),
+	                                        s->pts.data(), s->scan.data(), pad, s->pes_offset.data(), s->pes_pts.data());
+	return 1;
 }
-
-uint32_t ps_demux_launches(const PsScratch *s) { return s->launches; }
