@@ -171,32 +171,26 @@ class BatchDecoder:
         ctypes.memmove(ptr, data, len(data))
         self.lib.jsmpeg_b200_batch_did_write(self.handle, stream, len(data))
 
-    @staticmethod
-    def _ts_pes_capacity(n_bytes):
-        """PES starts a TS write of n_bytes can report: one per packet of the bytes and of what the stream's last write
-        left over (up to 188 x 6 - 1 bytes of a pending resync)."""
-        return (n_bytes + 188 * 6 - 1) // 188 + 1
-
-    def write_ts(self, stream, ts_bytes, stream_id=0xE0):
-        """MPEG-TS in, demultiplexed on the GPU (any chunking, resyncs like src/ts.js).  Returns (ES bytes
-        appended, [(payload byte offset, pts seconds), ...] per PES packet of `stream_id` that starts in it)."""
-        ts_bytes = bytes(ts_bytes)
-        n_max = self._ts_pes_capacity(len(ts_bytes))
+    def _write_one(self, name, capacity, refused, stream, data, stream_id):
+        """write_ts / write_ps through the C call `name`, with room for capacity(len(data)) PES entries.  A -2 raises
+        ValueError(refused) where the format refuses a stream id, any other failure RuntimeError."""
+        data = bytes(data)
+        n_max = capacity(len(data))
         pts = np.zeros(n_max, np.uint64)
         off = np.zeros(n_max, np.uint32)
         n = ctypes.c_int()
-        total = self.lib.jsmpeg_b200_batch_write_ts(self.handle, stream, ts_bytes, len(ts_bytes), stream_id,
-                                                    pts.ctypes.data, off.ctypes.data, n_max, ctypes.byref(n))
+        total = getattr(self.lib, name)(self.handle, stream, data, len(data), stream_id, pts.ctypes.data, off.ctypes.data,
+                                        n_max, ctypes.byref(n))
+        if total == -2 and refused:
+            raise ValueError(refused.format(stream_id=stream_id))
         if total < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ts failed")
+            raise RuntimeError(self.last_error() or f"{name} failed")
         table = [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
         self._pes[stream] += table
         return total, table
 
-    def write_ts_many(self, writes):
-        """MPEG-TS of many streams in one GPU pass: `writes` is an iterable of (stream, bytes) or (stream, bytes,
-        stream_id), each stream at most once.  Returns one (ES bytes appended, [(payload byte offset, pts seconds),
-        ...]) per write, what write_ts returns for it."""
+    def _write_many(self, name, capacity, refused, writes):
+        """write_ts_many / write_ps_many through the C call `name`; a -2 raises ValueError(refused)."""
         writes = [(w[0], bytes(w[1]), w[2] if len(w) > 2 else 0xE0) for w in writes]
         n = len(writes)
         streams = np.array([w[0] for w in writes], np.int32)
@@ -206,16 +200,16 @@ class BatchDecoder:
         sids = np.array([w[2] for w in writes], np.int32)
         appended = np.zeros(n, np.int64)
         n_pes = np.zeros(n, np.int32)
-        n_max = sum(self._ts_pes_capacity(len(b)) for b in bufs)
+        n_max = sum(capacity(len(b)) for b in bufs)
         pts = np.zeros(max(n_max, 1), np.uint64)
         off = np.zeros(max(n_max, 1), np.uint32)
-        total = self.lib.jsmpeg_b200_batch_write_ts_many(self.handle, n, streams.ctypes.data, ctypes.addressof(ptrs),
-                                                         sizes.ctypes.data, sids.ctypes.data, appended.ctypes.data,
-                                                         pts.ctypes.data, off.ctypes.data, n_max, n_pes.ctypes.data)
+        total = getattr(self.lib, name)(self.handle, n, streams.ctypes.data, ctypes.addressof(ptrs), sizes.ctypes.data,
+                                        sids.ctypes.data, appended.ctypes.data, pts.ctypes.data, off.ctypes.data, n_max,
+                                        n_pes.ctypes.data)
         if total == -2:
-            raise ValueError("write_ts_many: a stream out of range or named twice, or 4 GiB of input or more")
+            raise ValueError(refused)
         if total < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ts_many failed")
+            raise RuntimeError(self.last_error() or f"{name} failed")
         out, k = [], 0
         for (stream, _, _), a, m in zip(writes, appended, n_pes):
             table = [(int(off[k + j]), float(pts[k + j]) / 90000.0) for j in range(m)]
@@ -223,6 +217,24 @@ class BatchDecoder:
             self._pes[stream] += table
             out.append((int(a), table))
         return out
+
+    @staticmethod
+    def _ts_pes_capacity(n_bytes):
+        """PES starts a TS write of n_bytes can report: one per packet of the bytes and of what the stream's last write
+        left over (up to 188 x 6 - 1 bytes of a pending resync)."""
+        return (n_bytes + 188 * 6 - 1) // 188 + 1
+
+    def write_ts(self, stream, ts_bytes, stream_id=0xE0):
+        """MPEG-TS in, demultiplexed on the GPU (any chunking, resyncs like src/ts.js).  Returns (ES bytes
+        appended, [(payload byte offset, pts seconds), ...] per PES packet of `stream_id` that starts in it)."""
+        return self._write_one("jsmpeg_b200_batch_write_ts", self._ts_pes_capacity, None, stream, ts_bytes, stream_id)
+
+    def write_ts_many(self, writes):
+        """MPEG-TS of many streams in one GPU pass: `writes` is an iterable of (stream, bytes) or (stream, bytes,
+        stream_id), each stream at most once.  Returns one (ES bytes appended, [(payload byte offset, pts seconds),
+        ...]) per write, what write_ts returns for it."""
+        return self._write_many("jsmpeg_b200_batch_write_ts_many", self._ts_pes_capacity,
+                                "write_ts_many: a stream out of range or named twice, or 4 GiB of input or more", writes)
 
     @staticmethod
     def _ps_pes_capacity(n_bytes):
@@ -234,52 +246,16 @@ class BatchDecoder:
         """MPEG program stream in (.mpg: ISO 11172-1, .vob: ISO 13818-1), demultiplexed on the GPU (any
         chunking, resyncs at the next pack header).  Returns (ES bytes appended, [(payload byte offset, pts
         seconds), ...] per PES packet of `stream_id` with a PTS in it)."""
-        ps_bytes = bytes(ps_bytes)
-        n_max = self._ps_pes_capacity(len(ps_bytes))
-        pts = np.zeros(n_max, np.uint64)
-        off = np.zeros(n_max, np.uint32)
-        n = ctypes.c_int()
-        total = self.lib.jsmpeg_b200_batch_write_ps(self.handle, stream, ps_bytes, len(ps_bytes), stream_id,
-                                                    pts.ctypes.data, off.ctypes.data, n_max, ctypes.byref(n))
-        if total == -2:
-            raise ValueError(f"stream_id {stream_id:#x} is not a video stream id (0xE0..0xEF)")
-        if total < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ps failed")
-        table = [(int(off[i]), float(pts[i]) / 90000.0) for i in range(n.value)]
-        self._pes[stream] += table
-        return total, table
+        return self._write_one("jsmpeg_b200_batch_write_ps", self._ps_pes_capacity,
+                               "stream_id {stream_id:#x} is not a video stream id (0xE0..0xEF)", stream, ps_bytes, stream_id)
 
     def write_ps_many(self, writes):
         """MPEG program streams of many streams in one GPU pass: `writes` is an iterable of (stream, bytes) or (stream,
         bytes, stream_id), each stream at most once.  Returns one (ES bytes appended, [(payload byte offset, pts
         seconds), ...]) per write, what write_ps returns for it."""
-        writes = [(w[0], bytes(w[1]), w[2] if len(w) > 2 else 0xE0) for w in writes]
-        n = len(writes)
-        streams = np.array([w[0] for w in writes], np.int32)
-        bufs = [w[1] for w in writes]
-        ptrs = (ctypes.c_char_p * max(n, 1))(*bufs)
-        sizes = np.array([len(b) for b in bufs], np.uint64)
-        sids = np.array([w[2] for w in writes], np.int32)
-        appended = np.zeros(n, np.int64)
-        n_pes = np.zeros(n, np.int32)
-        n_max = sum(self._ps_pes_capacity(len(b)) for b in bufs)
-        pts = np.zeros(max(n_max, 1), np.uint64)
-        off = np.zeros(max(n_max, 1), np.uint32)
-        total = self.lib.jsmpeg_b200_batch_write_ps_many(self.handle, n, streams.ctypes.data, ctypes.addressof(ptrs),
-                                                         sizes.ctypes.data, sids.ctypes.data, appended.ctypes.data,
-                                                         pts.ctypes.data, off.ctypes.data, n_max, n_pes.ctypes.data)
-        if total == -2:
-            raise ValueError("write_ps_many: a stream out of range or named twice, a stream id outside 0xE0..0xEF, "
-                             "or 4 GiB of input or more")
-        if total < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_write_ps_many failed")
-        out, k = [], 0
-        for (stream, _, _), a, m in zip(writes, appended, n_pes):
-            table = [(int(off[k + j]), float(pts[k + j]) / 90000.0) for j in range(m)]
-            k += m
-            self._pes[stream] += table
-            out.append((int(a), table))
-        return out
+        return self._write_many("jsmpeg_b200_batch_write_ps_many", self._ps_pes_capacity,
+                                "write_ps_many: a stream out of range or named twice, a stream id outside 0xE0..0xEF, "
+                                "or 4 GiB of input or more", writes)
 
     def read_es(self, stream):
         """The stream's elementary stream as it is resident in HBM (test hook)."""

@@ -215,56 +215,3 @@ struct AccTask {
 	int32_t mb_width, mb_height;
 };
 void launch_accumulate(const AccTask *tasks, int n_tasks, uint32_t total_warps, cudaStream_t stream);
-
-// device MPEG-TS demux of many requests in one pass (tsdemux.cu, tsdemux.cuh).  A call: ts_call_begin makes room for
-// n_req requests, `bytes` staged bytes and n_slots packet slots (max_req: the most requests a call of the batch can
-// have, which fixes the event key's width); the caller stages the bytes and h_req[0 .. n_req] (entry n_req: slot0 =
-// n_slots) and uploads them; ts_call_measure queues the grid, classify, bind and place scans and the D2H of the
-// per-request totals to h_out; once the caller has set every request's dst / es_base and uploaded h_req again,
-// ts_call_gather queues the copy of the payloads and the PES list (d_pes_*, in (request, offset) order).  Both
-// return the launches they queued.
-struct TsReq;
-struct TsReqOut;
-struct TsScratch;
-struct TsCall {
-	uint8_t *stage;
-	TsReq *h_req, *d_req;
-	TsReqOut *h_out;
-	uint32_t *d_pes_offset;
-	uint64_t *d_pes_pts;
-	uint32_t *h_pes_offset;
-	uint64_t *h_pes_pts;
-};
-TsScratch *ts_scratch_create();
-void ts_scratch_destroy(TsScratch *s);
-TsCall ts_call_begin(TsScratch *s, uint32_t n_req, size_t bytes, uint32_t n_slots, uint32_t max_req);
-uint32_t ts_call_measure(TsScratch *s, cudaStream_t st);
-uint32_t ts_call_gather(TsScratch *s, uint32_t pad, cudaStream_t st);
-
-// device MPEG program stream demux of many requests in one pass (psdemux.cu, psdemux.cuh).  A call: ps_call_begin
-// makes room for n_req requests, `staged` staged bytes (requests at 16-byte aligned offsets) and `left` left-over
-// bytes in pinned memory; the caller stages the bytes and h_req[0 .. n_req) and uploads them; ps_call_candidates queues the candidate search and the D2H of
-// its counts; once the caller has synchronised, ps_call_measure sizes the per-candidate scratch by them (which may
-// move the PES lists: *c is updated), queues sort, link, doubling, heads, marking, classify, place scan and totals
-// and the D2H of the per-request results to h_out; once the caller has set every request's dst / es_base and
-// uploaded h_req again, ps_call_gather queues the copy of the payloads and the PES list (d_pes_*, in (request,
-// offset) order).  The three return the launches they queued.
-struct PsReq;
-struct PsReqOut;
-struct PsScratch;
-struct PsCall {
-	uint8_t *stage;
-	uint8_t *h_left;  // pinned room for the requests' left-over bytes (`left` of ps_call_begin)
-	PsReq *h_req, *d_req;
-	PsReqOut *h_out;
-	uint32_t *d_pes_offset;
-	uint64_t *d_pes_pts;
-	uint32_t *h_pes_offset;
-	uint64_t *h_pes_pts;
-};
-PsScratch *ps_scratch_create();
-void ps_scratch_destroy(PsScratch *s);
-PsCall ps_call_begin(PsScratch *s, uint32_t n_req, size_t staged, size_t left);
-uint32_t ps_call_candidates(PsScratch *s, cudaStream_t st);
-uint32_t ps_call_measure(PsScratch *s, PsCall *c, cudaStream_t st);
-uint32_t ps_call_gather(PsScratch *s, uint32_t pad, cudaStream_t st);

@@ -42,6 +42,7 @@
 #include "bitbuffer.h"
 #include "buffers.h"
 #include "common.cuh"
+#include "demux.h"
 #include "psdemux.cuh"
 #include "tsdemux.cuh"
 #include "../../include/jsmpeg_b200.h"
@@ -154,8 +155,11 @@ struct jsmpeg_b200_batch_t {
 	uint64_t copy_steps = 0;  // reconstruct launches with a copy-out so far (event parity)
 	ParseFork fork{};
 	bool batch_copy_ok = true;
+	// write_ts_many / write_ps_many: each format's scratch and the per-call I/O (demux_many)
 	std::unique_ptr<TsScratch, ScratchDeleter> ts;
 	std::unique_ptr<PsScratch, ScratchDeleter> ps;
+	TsIo ts_io;
+	PsIo ps_io;
 	// decode_pictures / decode_intra: the forward plane set a chain of one picture names, zeroed and never written
 	// (DESIGN 3.6); and the pool of the other chains' plane sets, zeroed per chain group (DESIGN 3.7)
 	DeviceBuffer<uint8_t> d_intra_fwd;
@@ -1778,79 +1782,156 @@ int env_int(const char *name, int fallback) {
 	return e && *e ? atoi(e) : fallback;
 }
 
-// jsmpeg_b200_batch_write_ts_many (include/jsmpeg_b200.h): request i appends to streams[i] what write_ts would.  One
-// pass for all requests (tsdemux.cu, DESIGN 3.3): one batched upload, the measure launches, one synchronize for the
-// totals; the host makes room in every stream (the write protocol, may expand or evict) and flushes its ordinary
-// writes; one gather launch, one batched copy back of the new ES bytes and the PES list, one synchronize.
-long ts_write_many(Batch *b, int n, const int *streams, const uint8_t *const *ts, const size_t *n_bytes, const int *stream_ids,
-                   long *appended_out, uint64_t *pts_out, uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
-	if (n < 0 || (n > 0 && (!streams || !ts || !n_bytes))) return -2;
+// MPEG-TS in demux_many (tsdemux.cu, DESIGN 3.3): a request is staged only if it holds a whole packet, and owns one
+// packet slot per 188 bytes, numbered over the call; a stream's PID table is made on its first TS write.
+struct TsFormat {
+	using Req = TsReq;
+	using Out = TsReqOut;
+	Batch *b;
+	TsIo &io;
+	uint32_t slots = 0;  // of the requests staged so far
+	explicit TsFormat(Batch *b) : b(b), io(b->ts_io) {}
+
+	// a partial packet, a resync that wanted more data (ts.js:25-41)
+	static std::vector<uint8_t> &leftover(Stream &s) { return s.ts_leftover; }
+	static bool stream_id_ok(int) { return true; }
+	static bool fits(uint64_t all, uint64_t) { return all < 0xfffff000ull; }  // (positions are 32-bit; a header read may run a few bytes past a request)
+	static uint64_t room(uint64_t len) { return len >= 188 ? len : 0; }  // (fewer bytes: not a packet yet, nothing to upload)
+	TsReq request(Stream &s, uint32_t base, uint32_t len, int sid) {
+		if (!s.ts_bound.data()) {  // the stream's first TS write: no PID bound yet
+			s.ts_bound.reserve(8192);
+			CUDA_CHECK(cudaMemsetAsync(s.ts_bound.data(), 0, 8192 * sizeof(int16_t), b->st_main));
+		}
+		const TsReq r{base, (uint32_t)room(len), slots, sid, s.ts_bound.data(), nullptr, 0, 0};
+		slots += len / 188;
+		return r;
+	}
+	uint32_t rows(uint32_t n, uint32_t base) {  // entry n carries the call's slot count
+		io.h_req[n] = TsReq{base, 0, slots, 0, nullptr, nullptr, 0, 0};
+		return n + 1;
+	}
+	void begin(uint32_t n, uint32_t) {
+		if (!b->ts) b->ts.reset(ts_scratch_create());
+		ts_call_begin(b->ts.get(), io, n, slots, (uint32_t)b->streams.size());
+	}
+	uint32_t measure() {
+		const uint32_t launches = ts_call_measure(b->ts.get(), io, b->st_main);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		return launches;
+	}
+	uint32_t gather() { return ts_call_gather(b->ts.get(), io, ES_PAD, b->st_main); }
+	static uint32_t carry(Stream &, const TsReqOut &o) { return o.stop; }
+};
+
+// MPEG program streams in demux_many (psdemux.cu, DESIGN 3.5): every request is staged, at a 16-byte aligned offset
+// (the candidate search reads 16-byte vectors), with its stream's in-sync state; the candidate counts size the
+// rest of the measure step, so they come to the host first.
+struct PsFormat {
+	using Req = PsReq;
+	using Out = PsReqOut;
+	Batch *b;
+	PsIo &io;
+	explicit PsFormat(Batch *b) : b(b), io(b->ps_io) {}
+
+	// an unfinished item, or the tail that may begin a pack header
+	static std::vector<uint8_t> &leftover(Stream &s) { return s.ps_leftover; }
+	static bool stream_id_ok(int sid) { return sid >= 0xE0 && sid <= 0xEF; }
+	static bool fits(uint64_t all, uint64_t staged) { return all < 0xfffff000ull && staged < 0xfffff000ull; }  // (positions are 32-bit)
+	static uint64_t room(uint64_t len) { return (len + 15) & ~15ull; }
+	PsReq request(Stream &s, uint32_t base, uint32_t len, int sid) { return PsReq{base, len, sid, s.ps_in_sync ? 1u : 0u, nullptr, 0, 0}; }
+	uint32_t rows(uint32_t n, uint32_t) { return n; }
+	void begin(uint32_t n, uint32_t staged) {
+		if (!b->ps) b->ps.reset(ps_scratch_create());
+		ps_call_begin(b->ps.get(), n, staged);
+	}
+	uint32_t measure() {
+		uint32_t launches = ps_call_candidates(b->ps.get(), io, b->st_main);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		launches += ps_call_measure(b->ps.get(), io, b->st_main);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		return launches;
+	}
+	uint32_t gather() { return ps_call_gather(b->ps.get(), io, ES_PAD, b->st_main); }
+	static uint32_t carry(Stream &s, const PsReqOut &o) {  // bytes consumed; the stream's in-sync state after them
+		s.ps_in_sync = o.in_sync != 0;
+		return o.consumed;
+	}
+};
+
+// jsmpeg_b200_batch_write_ts_many / _write_ps_many (include/jsmpeg_b200.h): request i appends to streams[i] what the
+// format's one-request write would.  One pass for all requests (DESIGN 3.3): one batched upload of the staged bytes and
+// the request table; the format's measure launches and synchronisation(s) for the per-request results; the host makes
+// room in every stream (the write protocol, may expand or evict) and flushes its ordinary writes; one gather launch,
+// one batched copy back of the new ES bytes and the PES list, one synchronisation.  The format F (TsFormat, PsFormat)
+// says which requests are staged and where (room: a request's bytes in the staging buffer), fills their rows of the
+// request table and queues its steps.
+template <class F>
+long demux_many(Batch *b, int n, const int *streams, const uint8_t *const *data, const size_t *n_bytes, const int *stream_ids,
+                long *appended_out, uint64_t *pts_out, uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
+	if (n < 0 || (n > 0 && (!streams || !data || !n_bytes))) return -2;
 	const int S = (int)b->streams.size();
 	std::vector<char> named(S, 0);
-	uint64_t all = 0;
+	// a request's bytes: what its stream's last write left over, then the new ones
+	uint64_t all = 0, staged = 0, left = 0;
 	for (int i = 0; i < n; i++) {
-		if (streams[i] < 0 || streams[i] >= S || named[streams[i]] || (!ts[i] && n_bytes[i] > 0)) return -2;
+		if (streams[i] < 0 || streams[i] >= S || named[streams[i]] || (!data[i] && n_bytes[i] > 0) ||
+		    !F::stream_id_ok(stream_ids ? stream_ids[i] : 0xE0))
+			return -2;
 		named[streams[i]] = 1;
-		all += b->streams[streams[i]].ts_leftover.size() + (uint64_t)n_bytes[i];
+		const uint64_t lo = F::leftover(b->streams[streams[i]]).size();
+		all += lo + n_bytes[i];
+		staged += F::room(lo + n_bytes[i]);
+		left += lo;
 	}
-	if (all >= 0xfffff000ull) return -2;  // (positions are 32-bit; a header read may run a few bytes past a request)
+	if (!F::fits(all, staged)) return -2;
 	for (int i = 0; i < n; i++) {
 		if (appended_out) appended_out[i] = 0;
 		if (n_pes_out) n_pes_out[i] = 0;
 	}
-	if (n == 0) return 0;
-	use_device(b);
-	if (!b->ts) b->ts.reset(ts_scratch_create());
-	// a request's bytes: what its stream's last write left over (a partial packet, a resync that wanted more data:
-	// ts.js:25-41), then the new ones; packet slots: one per 188 bytes
-	size_t staged = 0;
-	uint32_t slots = 0;
-	for (int i = 0; i < n; i++) {
-		const uint64_t len = b->streams[streams[i]].ts_leftover.size() + n_bytes[i];
-		if (len >= 188) { staged += len; slots += (uint32_t)(len / 188); }
-	}
-	std::vector<uint32_t> stop(n, 0), total(n, 0);
+	std::vector<uint32_t> consumed(n, 0);
 	long appended = 0;
-	if (slots) {
-		const TsCall c = ts_call_begin(b->ts.get(), (uint32_t)n, staged, slots, (uint32_t)S);
+	if (staged) {  // (else no request has bytes to demultiplex: no GPU work)
+		use_device(b);
+		F f(b);
+		auto &io = f.io;
+		io.begin(n + 1, staged, left);  // (TS's table has an entry n)
 		std::vector<void *> dst, src;
 		std::vector<size_t> size;
-		uint32_t base = 0, slot = 0;
+		uint32_t base = 0;
+		size_t at_left = 0;
 		for (int i = 0; i < n; i++) {
 			Stream &s = b->streams[streams[i]];
-			if (!s.ts_bound.data()) {  // the stream's first TS write: no PID bound yet
-				s.ts_bound.reserve(8192);
-				CUDA_CHECK(cudaMemsetAsync(s.ts_bound.data(), 0, 8192 * sizeof(int16_t), b->st_main));
+			const std::vector<uint8_t> &lo = F::leftover(s);
+			const uint32_t len = (uint32_t)(lo.size() + n_bytes[i]), room = (uint32_t)F::room(len);
+			io.h_req[i] = f.request(s, base, len, stream_ids ? stream_ids[i] : 0xE0);
+			if (!room) continue;
+			// the left-over bytes go up from pinned memory: a left-over buffer is reallocated by nearly every call, and
+			// a pageable source whose pages come and go between batched copies faulted the copy on the H100 (DESIGN 3.3)
+			if (!lo.empty()) {
+				memcpy(io.h_left.data() + at_left, lo.data(), lo.size());
+				dst.push_back(io.stage.data() + base), src.push_back(io.h_left.data() + at_left), size.push_back(lo.size());
+				at_left += lo.size();
 			}
-			const uint32_t lo = (uint32_t)s.ts_leftover.size(), len = lo + (uint32_t)n_bytes[i];
-			const bool whole = len >= 188;  // (fewer bytes: not a packet yet, nothing to upload)
-			c.h_req[i] = TsReq{base, whole ? len : 0, slot, stream_ids ? stream_ids[i] : 0xE0, s.ts_bound.data(), nullptr, 0, 0};
-			if (!whole) continue;
-			if (lo) { dst.push_back(c.stage + base); src.push_back(s.ts_leftover.data()); size.push_back(lo); }
-			if (n_bytes[i]) { dst.push_back(c.stage + base + lo); src.push_back(const_cast<uint8_t *>(ts[i])); size.push_back(n_bytes[i]); }
-			base += len;
-			slot += len / 188;
+			if (n_bytes[i]) dst.push_back(io.stage.data() + base + lo.size()), src.push_back(const_cast<uint8_t *>(data[i])), size.push_back(n_bytes[i]);
+			b->stats.h2d_bytes += len;
+			base += room;
 		}
-		c.h_req[n] = TsReq{base, 0, slot, 0, nullptr, nullptr, 0, 0};
-		dst.push_back(c.d_req);
-		src.push_back(c.h_req);
-		size.push_back((n + 1) * sizeof(TsReq));
+		const uint32_t rows = f.rows(n, base);
+		f.begin(n, (uint32_t)staged);  // (the format's scratch: every allocation of the call before the upload is queued)
+		dst.push_back(io.req.data()), src.push_back(io.h_req.data()), size.push_back(rows * sizeof(typename F::Req));
 		copy_batch(b, dst, src, size, b->st_main, cudaMemcpySrcAccessOrderDuringApiCall);
-		b->stats.h2d_bytes += staged;
-		b->stats.kernel_launches += ts_call_measure(b->ts.get(), b->st_main);
-		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+		b->stats.kernel_launches += f.measure();
 		// room in every stream's host bit buffer and HBM mirror; its ordinary writes made resident first
 		dst.clear(), src.clear(), size.clear();
 		std::vector<uint8_t *> hdst(n, nullptr);
 		uint32_t n_pes = 0;
 		for (int i = 0; i < n; i++) {
-			stop[i] = c.h_out[i].stop;
-			total[i] = c.h_out[i].total;
-			n_pes = std::max(n_pes, c.h_out[i].pes_first + c.h_out[i].pes);
-			if (!total[i]) continue;
+			const typename F::Out &o = io.h_out[i];
+			n_pes = std::max(n_pes, o.pes_first + o.pes);
+			if (!o.total) continue;
 			Stream &s = b->streams[streams[i]];
-			hdst[i] = static_cast<uint8_t *>(stream_get_write_ptr(b, s, total[i]));
-			reserve_device_es(b, s, s.bb.length + total[i]);
+			hdst[i] = static_cast<uint8_t *>(stream_get_write_ptr(b, s, o.total));
+			reserve_device_es(b, s, s.bb.length + o.total);
 			if (s.d_valid < s.bb.length) {
 				dst.push_back(s.d_es.data() + s.d_valid);
 				src.push_back(s.bb.bytes + s.d_valid);
@@ -1858,185 +1939,72 @@ long ts_write_many(Batch *b, int n, const int *streams, const uint8_t *const *ts
 				b->stats.h2d_bytes += s.bb.length - s.d_valid;
 				s.d_valid = s.bb.length;
 			}
-			c.h_req[i].dst = s.d_es.data() + s.bb.length;
-			c.h_req[i].es_base = s.bb.length;
+			io.h_req[i].dst = s.d_es.data() + s.bb.length;
+			io.h_req[i].es_base = s.bb.length;
 		}
-		dst.push_back(c.d_req);
-		src.push_back(c.h_req);
-		size.push_back((n + 1) * sizeof(TsReq));
+		dst.push_back(io.req.data()), src.push_back(io.h_req.data()), size.push_back(rows * sizeof(typename F::Req));
 		copy_batch(b, dst, src, size, b->st_main);
-		b->stats.kernel_launches += ts_call_gather(b->ts.get(), ES_PAD, b->st_main);
+		b->stats.kernel_launches += f.gather();
 		// the host keeps a mirror of the ES (sequence header parse, EVICT bookkeeping): the new bytes come back
 		dst.clear(), src.clear(), size.clear();
 		for (int i = 0; i < n; i++) {
-			if (!total[i]) continue;
-			dst.push_back(hdst[i]);
-			src.push_back(c.h_req[i].dst);
-			size.push_back(total[i]);
-			b->stats.d2h_bytes += total[i];
+			const uint32_t total = io.h_out[i].total;
+			if (!total) continue;
+			dst.push_back(hdst[i]), src.push_back(io.h_req[i].dst), size.push_back(total);
+			b->stats.d2h_bytes += total;
 		}
 		if (n_pes && (pts_out || offset_out) && n_max > 0) {
-			dst.push_back(c.h_pes_offset), src.push_back(c.d_pes_offset), size.push_back(n_pes * sizeof(uint32_t));
-			dst.push_back(c.h_pes_pts), src.push_back(c.d_pes_pts), size.push_back(n_pes * sizeof(uint64_t));
+			dst.push_back(io.h_pes_offset.data()), src.push_back(io.pes_offset.data()), size.push_back(n_pes * sizeof(uint32_t));
+			dst.push_back(io.h_pes_pts.data()), src.push_back(io.pes_pts.data()), size.push_back(n_pes * sizeof(uint64_t));
 		}
 		if (!dst.empty()) copy_batch(b, dst, src, size, b->st_main);
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 		long listed = 0;
 		for (int i = 0; i < n; i++) {
-			if (!total[i]) continue;
 			Stream &s = b->streams[streams[i]];
-			stream_did_write(b, s, total[i]);
+			const typename F::Out &o = io.h_out[i];
+			consumed[i] = F::carry(s, o);
+			if (!o.total) continue;
+			stream_did_write(b, s, o.total);
 			s.d_valid = s.bb.length;
-			appended += total[i];
-			if (appended_out) appended_out[i] = total[i];
-			if (n_pes_out) n_pes_out[i] = (int32_t)c.h_out[i].pes;
-			for (uint32_t k = 0; k < c.h_out[i].pes && listed < n_max; k++, listed++) {
-				if (pts_out) pts_out[listed] = c.h_pes_pts[c.h_out[i].pes_first + k];
-				if (offset_out) offset_out[listed] = c.h_pes_offset[c.h_out[i].pes_first + k];
+			appended += o.total;
+			if (appended_out) appended_out[i] = o.total;
+			if (n_pes_out) n_pes_out[i] = (int32_t)o.pes;
+			for (uint32_t k = 0; k < o.pes && listed < n_max; k++, listed++) {
+				if (pts_out) pts_out[listed] = io.h_pes_pts[o.pes_first + k];
+				if (offset_out) offset_out[listed] = io.h_pes_offset[o.pes_first + k];
 			}
 		}
 	}
 	// what the demuxer did not consume stays for the stream's next write
 	for (int i = 0; i < n; i++) {
-		std::vector<uint8_t> &lo = b->streams[streams[i]].ts_leftover;
-		const size_t k = stop[i];
+		std::vector<uint8_t> &lo = F::leftover(b->streams[streams[i]]);
+		const size_t k = consumed[i];
 		if (k <= lo.size()) {
 			lo.erase(lo.begin(), lo.begin() + k);
-			lo.insert(lo.end(), ts[i], ts[i] + n_bytes[i]);
+			lo.insert(lo.end(), data[i], data[i] + n_bytes[i]);
 		} else {
-			lo.assign(ts[i] + (k - lo.size()), ts[i] + n_bytes[i]);
+			lo.assign(data[i] + (k - lo.size()), data[i] + n_bytes[i]);
 		}
 	}
 	return appended;
 }
 
-// jsmpeg_b200_batch_write_ps_many (include/jsmpeg_b200.h): request i appends to streams[i] what write_ps would.  One
-// pass for all requests (psdemux.cu, DESIGN 3.5): one batched upload and the candidate search, one synchronize for the
-// candidate counts (they size the scratch and the doubling); the chain, place and totals launches, one synchronize for
-// the per-request results; the host makes room in every stream (the write protocol, may expand or evict) and flushes
-// its ordinary writes; one gather launch, one batched copy back of the new ES bytes and the PES list, one synchronize.
-long ps_write_many(Batch *b, int n, const int *streams, const uint8_t *const *ps, const size_t *n_bytes, const int *stream_ids,
-                   long *appended_out, uint64_t *pts_out, uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
-	if (n < 0 || (n > 0 && (!streams || !ps || !n_bytes))) return -2;
-	const int S = (int)b->streams.size();
-	std::vector<char> named(S, 0);
-	// a request's bytes: what its stream's last write left over (an unfinished item, or the tail that may begin a
-	// pack header), then the new ones; each at a 16-byte aligned offset (the candidate search reads 16-byte vectors)
-	uint64_t all = 0, staged = 0, left = 0;
-	for (int i = 0; i < n; i++) {
-		const int sid = stream_ids ? stream_ids[i] : 0xE0;
-		if (streams[i] < 0 || streams[i] >= S || named[streams[i]] || (!ps[i] && n_bytes[i] > 0) || sid < 0xE0 || sid > 0xEF) return -2;
-		named[streams[i]] = 1;
-		const uint64_t len = b->streams[streams[i]].ps_leftover.size() + (uint64_t)n_bytes[i];
-		left += b->streams[streams[i]].ps_leftover.size();
-		all += len;
-		staged += (len + 15) & ~15ull;
-	}
-	if (all >= 0xfffff000ull || staged >= 0xfffff000ull) return -2;  // (positions are 32-bit)
-	for (int i = 0; i < n; i++) {
-		if (appended_out) appended_out[i] = 0;
-		if (n_pes_out) n_pes_out[i] = 0;
-	}
-	if (staged == 0) return 0;  // no bytes anywhere (or no request): nothing changes
-	use_device(b);
-	if (!b->ps) b->ps.reset(ps_scratch_create());
-	PsCall c = ps_call_begin(b->ps.get(), (uint32_t)n, staged, left);
-	std::vector<void *> dst, src;
-	std::vector<size_t> size;
-	uint32_t base = 0;
-	size_t at_left = 0;
-	for (int i = 0; i < n; i++) {
-		Stream &s = b->streams[streams[i]];
-		const uint32_t lo = (uint32_t)s.ps_leftover.size(), len = lo + (uint32_t)n_bytes[i];
-		c.h_req[i] = PsReq{base, len, stream_ids ? stream_ids[i] : 0xE0, s.ps_in_sync ? 1u : 0u, nullptr, 0, 0};
-		// the left-over bytes go up from pinned memory: a left-over buffer is reallocated by nearly every call, and a
-		// pageable source whose pages come and go between batched copies faulted the copy on the H100 (DESIGN 3.5)
-		if (lo) {
-			memcpy(c.h_left + at_left, s.ps_leftover.data(), lo);
-			dst.push_back(c.stage + base), src.push_back(c.h_left + at_left), size.push_back(lo);
-			at_left += lo;
-		}
-		if (n_bytes[i]) { dst.push_back(c.stage + base + lo); src.push_back(const_cast<uint8_t *>(ps[i])); size.push_back(n_bytes[i]); }
-		base += (len + 15) & ~15u;
-	}
-	dst.push_back(c.d_req);
-	src.push_back(c.h_req);
-	size.push_back(n * sizeof(PsReq));
-	copy_batch(b, dst, src, size, b->st_main, cudaMemcpySrcAccessOrderDuringApiCall);
-	b->stats.h2d_bytes += all;
-	b->stats.kernel_launches += ps_call_candidates(b->ps.get(), b->st_main);
-	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-	b->stats.kernel_launches += ps_call_measure(b->ps.get(), &c, b->st_main);
-	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-	// room in every stream's host bit buffer and HBM mirror; its ordinary writes made resident first
-	dst.clear(), src.clear(), size.clear();
-	std::vector<uint8_t *> hdst(n, nullptr);
-	std::vector<uint32_t> total(n, 0);
-	uint32_t n_pes = 0;
-	for (int i = 0; i < n; i++) {
-		total[i] = c.h_out[i].total;
-		n_pes = std::max(n_pes, c.h_out[i].pes_first + c.h_out[i].pes);
-		if (!total[i]) continue;
-		Stream &s = b->streams[streams[i]];
-		hdst[i] = static_cast<uint8_t *>(stream_get_write_ptr(b, s, total[i]));
-		reserve_device_es(b, s, s.bb.length + total[i]);
-		if (s.d_valid < s.bb.length) {
-			dst.push_back(s.d_es.data() + s.d_valid);
-			src.push_back(s.bb.bytes + s.d_valid);
-			size.push_back(s.bb.length - s.d_valid);
-			b->stats.h2d_bytes += s.bb.length - s.d_valid;
-			s.d_valid = s.bb.length;
-		}
-		c.h_req[i].dst = s.d_es.data() + s.bb.length;
-		c.h_req[i].es_base = s.bb.length;
-	}
-	dst.push_back(c.d_req);
-	src.push_back(c.h_req);
-	size.push_back(n * sizeof(PsReq));
-	copy_batch(b, dst, src, size, b->st_main);
-	b->stats.kernel_launches += ps_call_gather(b->ps.get(), ES_PAD, b->st_main);
-	// the host keeps a mirror of the ES (sequence header parse, EVICT bookkeeping): the new bytes come back
-	dst.clear(), src.clear(), size.clear();
-	for (int i = 0; i < n; i++) {
-		if (!total[i]) continue;
-		dst.push_back(hdst[i]);
-		src.push_back(c.h_req[i].dst);
-		size.push_back(total[i]);
-		b->stats.d2h_bytes += total[i];
-	}
-	if (n_pes && (pts_out || offset_out) && n_max > 0) {
-		dst.push_back(c.h_pes_offset), src.push_back(c.d_pes_offset), size.push_back(n_pes * sizeof(uint32_t));
-		dst.push_back(c.h_pes_pts), src.push_back(c.d_pes_pts), size.push_back(n_pes * sizeof(uint64_t));
-	}
-	if (!dst.empty()) copy_batch(b, dst, src, size, b->st_main);
-	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-	long appended = 0, listed = 0;
-	for (int i = 0; i < n; i++) {
-		Stream &s = b->streams[streams[i]];
-		const PsReqOut &o = c.h_out[i];
-		if (total[i]) {
-			stream_did_write(b, s, total[i]);
-			s.d_valid = s.bb.length;
-			appended += total[i];
-			if (appended_out) appended_out[i] = total[i];
-			if (n_pes_out) n_pes_out[i] = (int32_t)o.pes;
-			for (uint32_t k = 0; k < o.pes && listed < n_max; k++, listed++) {
-				if (pts_out) pts_out[listed] = c.h_pes_pts[o.pes_first + k];
-				if (offset_out) offset_out[listed] = c.h_pes_offset[o.pes_first + k];
-			}
-		}
-		// what the demuxer did not consume stays for the stream's next write
-		std::vector<uint8_t> &lo = s.ps_leftover;
-		const size_t k = o.consumed;
-		if (k <= lo.size()) {
-			lo.erase(lo.begin(), lo.begin() + k);
-			lo.insert(lo.end(), ps[i], ps[i] + n_bytes[i]);
-		} else {
-			lo.assign(ps[i] + (k - lo.size()), ps[i] + n_bytes[i]);
-		}
-		s.ps_in_sync = o.in_sync != 0;
-	}
-	return appended;
+// jsmpeg_b200_batch_write_ts / _write_ps: one request of demux_many.  A stream id the format does not take is refused
+// before anything changes; any other refusal (a stream out of range, 4 GiB or more) is a runtime error, `what` its message.
+template <class F>
+long write_one(Batch *b, int stream, const uint8_t *data, size_t n_bytes, int stream_id, uint64_t *pts_out, uint32_t *offset_out,
+               int n_max, int *n_pes, const char *what) {
+	if (n_pes) *n_pes = 0;
+	return guarded<long>(b, -1, [&]() -> long {
+		if (!F::stream_id_ok(stream_id)) return -2;
+		int32_t count = 0;
+		const long r = demux_many<F>(b, 1, &stream, &data, &n_bytes, &stream_id, nullptr, pts_out && offset_out ? pts_out : nullptr,
+		                             pts_out && offset_out ? offset_out : nullptr, n_max, &count);
+		if (r == -2) throw std::runtime_error(what);
+		if (n_pes) *n_pes = count;
+		return r;
+	});
 }
 
 }  // namespace
@@ -2304,44 +2272,29 @@ int jsmpeg_b200_batch_read_planes(jsmpeg_b200_batch_t *b, int stream, void *y, v
 
 long jsmpeg_b200_batch_write_ts(jsmpeg_b200_batch_t *b, int stream, const uint8_t *ts, size_t n_bytes, int stream_id,
                                 uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes) {
-	if (n_pes) *n_pes = 0;
-	return guarded<long>(b, -1, [&]() -> long {
-		int32_t count = 0;
-		const long r = ts_write_many(b, 1, &stream, &ts, &n_bytes, &stream_id, nullptr, pts_out && offset_out ? pts_out : nullptr,
-		                             pts_out && offset_out ? offset_out : nullptr, n_max, &count);
-		if (r == -2) throw std::runtime_error("jsmpeg_b200: write_ts: stream out of range, or a transport stream buffer of 4 GiB or more");
-		if (n_pes) *n_pes = count;
-		return r;
-	});
+	return write_one<TsFormat>(b, stream, ts, n_bytes, stream_id, pts_out, offset_out, n_max, n_pes,
+	                           "jsmpeg_b200: write_ts: stream out of range, or a transport stream buffer of 4 GiB or more");
 }
 
 long jsmpeg_b200_batch_write_ts_many(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint8_t *const *ts,
                                      const size_t *n_bytes, const int *stream_ids, long *appended_out, uint64_t *pts_out,
                                      uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
 	return guarded<long>(b, -1, [&] {
-		return ts_write_many(b, n, streams, ts, n_bytes, stream_ids, appended_out, pts_out, offset_out, n_max, n_pes_out);
+		return demux_many<TsFormat>(b, n, streams, ts, n_bytes, stream_ids, appended_out, pts_out, offset_out, n_max, n_pes_out);
 	});
 }
 
 long jsmpeg_b200_batch_write_ps(jsmpeg_b200_batch_t *b, int stream, const uint8_t *ps, size_t n_bytes, int stream_id,
                                 uint64_t *pts_out, uint32_t *offset_out, int n_max, int *n_pes) {
-	if (n_pes) *n_pes = 0;
-	return guarded<long>(b, -1, [&]() -> long {
-		if (stream_id < 0xE0 || stream_id > 0xEF) return -2;  // not a video stream id: the caller's mistake, nothing changes
-		int32_t count = 0;
-		const long r = ps_write_many(b, 1, &stream, &ps, &n_bytes, &stream_id, nullptr, pts_out && offset_out ? pts_out : nullptr,
-		                             pts_out && offset_out ? offset_out : nullptr, n_max, &count);
-		if (r == -2) throw std::runtime_error("jsmpeg_b200: write_ps: stream out of range, or a program stream buffer of 4 GiB or more");
-		if (n_pes) *n_pes = count;
-		return r;
-	});
+	return write_one<PsFormat>(b, stream, ps, n_bytes, stream_id, pts_out, offset_out, n_max, n_pes,
+	                           "jsmpeg_b200: write_ps: stream out of range, or a program stream buffer of 4 GiB or more");
 }
 
 long jsmpeg_b200_batch_write_ps_many(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint8_t *const *ps,
                                      const size_t *n_bytes, const int *stream_ids, long *appended_out, uint64_t *pts_out,
                                      uint32_t *offset_out, long n_max, int32_t *n_pes_out) {
 	return guarded<long>(b, -1, [&] {
-		return ps_write_many(b, n, streams, ps, n_bytes, stream_ids, appended_out, pts_out, offset_out, n_max, n_pes_out);
+		return demux_many<PsFormat>(b, n, streams, ps, n_bytes, stream_ids, appended_out, pts_out, offset_out, n_max, n_pes_out);
 	});
 }
 

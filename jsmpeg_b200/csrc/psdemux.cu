@@ -23,8 +23,8 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
-#include "buffers.h"
 #include "common.cuh"
+#include "demux.h"
 #include "psdemux.cuh"
 
 namespace {
@@ -192,23 +192,13 @@ int blocks(uint64_t threads) { return (int)std::max<uint64_t>((threads + BLOCK -
 }  // namespace
 
 struct PsScratch {
-	DeviceBuffer<uint8_t> stage, marked;
-	DeviceBuffer<PsReq> req;
-	DeviceBuffer<PsReqOut> out;
-	PinnedBuffer<PsReq> h_req;
-	PinnedBuffer<PsReqOut> h_out;
-	PinnedBuffer<uint8_t> h_left;  // the requests' left-over bytes, staged for the upload
+	DeviceBuffer<uint8_t> marked;
 	DeviceBuffer<uint32_t> ctl, sel, pos;
 	PinnedBuffer<uint32_t> h_ctl;
 	DeviceBuffer<uint32_t> jump;  // (levels + 1) x cap
 	DeviceBuffer<uint2> term;
 	DeviceBuffer<uint32_t> rev, next_pack_rev, src;
 	DeviceBuffer<uint64_t> key, scan, pts;
-	DeviceBuffer<uint32_t> pes_offset;
-	DeviceBuffer<uint64_t> pes_pts;
-	PinnedBuffer<uint32_t> h_pes_offset;
-	PinnedBuffer<uint64_t> h_pes_pts;
-	DeviceBuffer<uint8_t> temp;  // cub's temporary storage
 	size_t cap = 0;  // candidates the per-candidate arrays have room for
 	int levels = 0;
 	uint32_t n_req = 0, staged = 0, m = 0;
@@ -217,49 +207,28 @@ struct PsScratch {
 PsScratch *ps_scratch_create() { return new PsScratch(); }
 void ps_scratch_destroy(PsScratch *s) { delete s; }
 
-static void *ps_temp(PsScratch *s, size_t bytes) {
-	if (bytes > s->temp.size()) s->temp.reserve(bytes + bytes / 4);
-	return s->temp.data();
-}
-
-static PsCall ps_call_view(PsScratch *s) {
-	return PsCall{s->stage.data(), s->h_left.data(), s->h_req.data(), s->req.data(), s->h_out.data(), s->pes_offset.data(),
-	              s->pes_pts.data(), s->h_pes_offset.data(), s->h_pes_pts.data()};
-}
-
-PsCall ps_call_begin(PsScratch *s, uint32_t n_req, size_t staged, size_t left) {
+void ps_call_begin(PsScratch *s, uint32_t n_req, uint32_t staged) {
 	s->n_req = n_req;
-	s->staged = (uint32_t)staged;
+	s->staged = staged;
 	s->m = 0;
-	// (a 16-byte load at the last multiple of 16 and a look-ahead word behind it)
-	if (staged + 32 > s->stage.size()) s->stage.reserve(staged + staged / 4 + 32);
-	if (left > s->h_left.size()) s->h_left.reserve(left + left / 4);
-	if (n_req > s->req.size()) {
-		const size_t cap = n_req + n_req / 4 + 1;
-		s->req.reserve(cap);
-		s->h_req.reserve(cap);
-		s->out.reserve(cap);
-		s->h_out.reserve(cap);
-	}
 	s->ctl.reserve(2);
 	s->h_ctl.reserve(2);
 	// candidates lie >= 4 bytes apart (the byte behind 00 00 01 is >= B9, so no prefix starts there) except one
 	// cut by a request's end: room for every one the staged bytes can hold
 	const size_t most = staged / 4 + n_req + 1;
 	if (most > s->sel.size()) s->sel.reserve(most + most / 4);
-	return ps_call_view(s);
 }
 
-uint32_t ps_call_candidates(PsScratch *s, cudaStream_t st) {
-	CUDA_CHECK(cudaMemsetAsync(s->out.data(), 0, s->n_req * sizeof(PsReqOut), st));
+uint32_t ps_call_candidates(PsScratch *s, PsIo &io, cudaStream_t st) {
+	CUDA_CHECK(cudaMemsetAsync(io.out.data(), 0, s->n_req * sizeof(PsReqOut), st));
 	CUDA_CHECK(cudaMemsetAsync(s->ctl.data(), 0, 2 * sizeof(uint32_t), st));
-	ps_candidates_kernel<<<blocks((s->staged + 15) / 16), BLOCK, 0, st>>>(s->stage.data(), s->staged, s->req.data(), s->n_req, s->out.data(),
+	ps_candidates_kernel<<<blocks((s->staged + 15) / 16), BLOCK, 0, st>>>(io.stage.data(), s->staged, io.req.data(), s->n_req, io.out.data(),
 	                                                                      s->sel.data(), s->ctl.data());
 	CUDA_CHECK(cudaMemcpyAsync(s->h_ctl.data(), s->ctl.data(), 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 	return 1;
 }
 
-uint32_t ps_call_measure(PsScratch *s, PsCall *c, cudaStream_t st) {
+uint32_t ps_call_measure(PsScratch *s, PsIo &io, cudaStream_t st) {
 	const uint32_t n = s->n_req, m = s->h_ctl[0], most = s->h_ctl[1];
 	s->m = m;
 	// doubling levels: 2^levels >= the largest request's candidate count bounds every chain
@@ -278,25 +247,21 @@ uint32_t ps_call_measure(PsScratch *s, PsCall *c, cudaStream_t st) {
 		s->pts.reserve(cap);
 		s->key.reserve(cap + 1);
 		s->scan.reserve(cap + 1);
-		s->pes_offset.reserve(cap);
-		s->pes_pts.reserve(cap);
-		s->h_pes_offset.reserve(cap);
-		s->h_pes_pts.reserve(cap);
 		s->cap = cap;
 		s->levels = lv;
-		*c = ps_call_view(s);
 	}
+	io.reserve_pes(m);  // (a PES table entry per candidate at most)
 	uint32_t launches = 0;
-	const uint8_t *stage = s->stage.data();
-	const PsReq *req = s->req.data();
-	PsReqOut *out = s->out.data();
+	const uint8_t *stage = io.stage.data();
+	const PsReq *req = io.req.data();
+	PsReqOut *out = io.out.data();
 	const uint32_t *pos = s->pos.data(), *npr = s->next_pack_rev.data();
 	size_t bytes = 0;
 	if (m) {
 		int bits = 1;
 		while (bits < 32 && (1ull << bits) <= s->staged) bits++;
 		cub::DeviceRadixSort::SortKeys(nullptr, bytes, s->sel.data(), s->pos.data(), (int)m, 0, bits, st);
-		cub::DeviceRadixSort::SortKeys(ps_temp(s, bytes), bytes, s->sel.data(), s->pos.data(), (int)m, 0, bits, st);
+		cub::DeviceRadixSort::SortKeys(io.temp_storage(bytes), bytes, s->sel.data(), s->pos.data(), (int)m, 0, bits, st);
 		launches++;
 	}
 	ps_pack_kernel<<<blocks(std::max(m, n)), BLOCK, 0, st>>>(stage, req, n, pos, m, out, s->rev.data());
@@ -304,7 +269,7 @@ uint32_t ps_call_measure(PsScratch *s, PsCall *c, cudaStream_t st) {
 	if (m) {
 		bytes = 0;
 		cub::DeviceScan::InclusiveScan(nullptr, bytes, s->rev.data(), s->next_pack_rev.data(), MinOp(), (int)m, st);
-		cub::DeviceScan::InclusiveScan(ps_temp(s, bytes), bytes, s->rev.data(), s->next_pack_rev.data(), MinOp(), (int)m, st);
+		cub::DeviceScan::InclusiveScan(io.temp_storage(bytes), bytes, s->rev.data(), s->next_pack_rev.data(), MinOp(), (int)m, st);
 		launches++;
 	}
 	uint32_t *jump = s->jump.data();
@@ -316,16 +281,16 @@ uint32_t ps_call_measure(PsScratch *s, PsCall *c, cudaStream_t st) {
 	ps_classify_kernel<<<blocks((uint64_t)m + 1), BLOCK, 0, st>>>(stage, req, n, pos, m, s->marked.data(), s->key.data(), s->src.data(), s->pts.data());
 	bytes = 0;
 	cub::DeviceScan::ExclusiveSum(nullptr, bytes, s->key.data(), s->scan.data(), (int)(m + 1), st);
-	cub::DeviceScan::ExclusiveSum(ps_temp(s, bytes), bytes, s->key.data(), s->scan.data(), (int)(m + 1), st);
+	cub::DeviceScan::ExclusiveSum(io.temp_storage(bytes), bytes, s->key.data(), s->scan.data(), (int)(m + 1), st);
 	ps_totals_kernel<<<blocks(n), BLOCK, 0, st>>>(req, n, jump + (size_t)levels * s->cap, s->term.data(), s->scan.data(), out);
 	launches += 2 * levels + 6;  // link, doubling, head, marking, classify, scan, totals (a cub algorithm counts as one)
-	CUDA_CHECK(cudaMemcpyAsync(s->h_out.data(), out, n * sizeof(PsReqOut), cudaMemcpyDeviceToHost, st));
+	CUDA_CHECK(cudaMemcpyAsync(io.h_out.data(), out, n * sizeof(PsReqOut), cudaMemcpyDeviceToHost, st));
 	return launches;
 }
 
-uint32_t ps_call_gather(PsScratch *s, uint32_t pad, cudaStream_t st) {
+uint32_t ps_call_gather(PsScratch *s, PsIo &io, uint32_t pad, cudaStream_t st) {
 	const uint32_t n = s->n_req, m = s->m;
-	ps_gather_kernel<<<m + n, 128, 0, st>>>(s->stage.data(), s->req.data(), n, s->out.data(), s->pos.data(), m, s->key.data(), s->src.data(),
-	                                        s->pts.data(), s->scan.data(), pad, s->pes_offset.data(), s->pes_pts.data());
+	ps_gather_kernel<<<m + n, 128, 0, st>>>(io.stage.data(), io.req.data(), n, io.out.data(), s->pos.data(), m, s->key.data(), s->src.data(),
+	                                        s->pts.data(), s->scan.data(), pad, io.pes_offset.data(), io.pes_pts.data());
 	return 1;
 }

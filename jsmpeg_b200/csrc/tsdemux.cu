@@ -31,8 +31,8 @@
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
-#include "buffers.h"
 #include "common.cuh"
+#include "demux.h"
 #include "tsdemux.cuh"
 
 namespace {
@@ -197,22 +197,12 @@ int blocks(uint64_t threads) { return (int)((threads + BLOCK - 1) / BLOCK); }
 }  // namespace
 
 struct TsScratch {
-	DeviceBuffer<uint8_t> stage;
-	DeviceBuffer<TsReq> req;
-	DeviceBuffer<TsReqOut> out;
-	PinnedBuffer<TsReq> h_req;
-	PinnedBuffer<TsReqOut> h_out;
 	DeviceBuffer<uint32_t> grid;
 	DeviceBuffer<TsPacketInfo> info;
 	DeviceBuffer<TsPacketUse> use;
 	DeviceBuffer<uint64_t> pts, lenpes, scan;
 	DeviceBuffer<uint64_t> ev_key, ev_key2;
 	DeviceBuffer<uint32_t> ev_val, ev_val2;
-	DeviceBuffer<uint32_t> pes_offset;
-	DeviceBuffer<uint64_t> pes_pts;
-	PinnedBuffer<uint32_t> h_pes_offset;
-	PinnedBuffer<uint64_t> h_pes_pts;
-	DeviceBuffer<uint8_t> temp;  // cub's temporary storage
 	uint32_t n_req = 0, n_slots = 0;
 	int key_bits = 0;
 };
@@ -220,21 +210,14 @@ struct TsScratch {
 TsScratch *ts_scratch_create() { return new TsScratch(); }
 void ts_scratch_destroy(TsScratch *s) { delete s; }
 
-TsCall ts_call_begin(TsScratch *s, uint32_t n_req, size_t bytes, uint32_t n_slots, uint32_t max_req) {
+void ts_call_begin(TsScratch *s, TsIo &io, uint32_t n_req, uint32_t n_slots, uint32_t max_req) {
+	const uint32_t m = n_slots;
 	s->n_req = n_req;
 	s->n_slots = n_slots;
 	s->key_bits = TS_PID_BITS + TS_SLOT_BITS;
 	while (s->key_bits < 64 && (1ull << (s->key_bits - TS_PID_BITS - TS_SLOT_BITS)) < max_req) s->key_bits++;
-	if (bytes > s->stage.size()) s->stage.reserve(bytes + bytes / 4);
-	if (n_req + 1 > s->req.size()) {
-		const size_t cap = n_req + 1 + n_req / 4;
-		s->req.reserve(cap);
-		s->h_req.reserve(cap);
-		s->out.reserve(cap);
-		s->h_out.reserve(cap);
-	}
-	if (n_slots + 1 > s->grid.size()) {
-		const size_t cap = n_slots + 1 + n_slots / 4 + 8;
+	if (m + 1 > s->grid.size()) {
+		const size_t cap = m + 1 + m / 4 + 8;
 		s->grid.reserve(cap);
 		s->info.reserve(cap);
 		s->use.reserve(cap);
@@ -245,47 +228,37 @@ TsCall ts_call_begin(TsScratch *s, uint32_t n_req, size_t bytes, uint32_t n_slot
 		s->ev_key2.reserve(cap);
 		s->ev_val.reserve(cap);
 		s->ev_val2.reserve(cap);
-		s->pes_offset.reserve(cap);
-		s->pes_pts.reserve(cap);
-		s->h_pes_offset.reserve(cap);
-		s->h_pes_pts.reserve(cap);
 	}
-	return TsCall{s->stage.data(), s->h_req.data(), s->req.data(), s->h_out.data(), s->pes_offset.data(), s->pes_pts.data(),
-	              s->h_pes_offset.data(), s->h_pes_pts.data()};
+	io.reserve_pes(m);  // (a PES start per packet at most)
 }
 
-static void *ts_temp(TsScratch *s, size_t bytes) {
-	if (bytes > s->temp.size()) s->temp.reserve(bytes + bytes / 4);
-	return s->temp.data();
-}
-
-uint32_t ts_call_measure(TsScratch *s, cudaStream_t st) {
+uint32_t ts_call_measure(TsScratch *s, TsIo &io, cudaStream_t st) {
 	const uint32_t n = s->n_req, m = s->n_slots;
-	CUDA_CHECK(cudaMemsetAsync(s->out.data(), 0, n * sizeof(TsReqOut), st));
-	ts_check_grid_kernel<<<blocks(m), BLOCK, 0, st>>>(s->stage.data(), s->req.data(), n, s->out.data());
-	ts_walk_grid_kernel<<<blocks((uint64_t)n * 32), BLOCK, 0, st>>>(s->stage.data(), s->req.data(), n, s->grid.data(), s->out.data());
-	ts_classify_kernel<<<blocks(m), BLOCK, 0, st>>>(s->stage.data(), s->req.data(), n, s->grid.data(), s->out.data(), s->info.data(),
+	CUDA_CHECK(cudaMemsetAsync(io.out.data(), 0, n * sizeof(TsReqOut), st));
+	ts_check_grid_kernel<<<blocks(m), BLOCK, 0, st>>>(io.stage.data(), io.req.data(), n, io.out.data());
+	ts_walk_grid_kernel<<<blocks((uint64_t)n * 32), BLOCK, 0, st>>>(io.stage.data(), io.req.data(), n, s->grid.data(), io.out.data());
+	ts_classify_kernel<<<blocks(m), BLOCK, 0, st>>>(io.stage.data(), io.req.data(), n, s->grid.data(), io.out.data(), s->info.data(),
 	                                                 s->pts.data(), s->ev_key.data(), s->ev_val.data());
 	size_t bytes = 0;
 	cub::DeviceRadixSort::SortPairs(nullptr, bytes, s->ev_key.data(), s->ev_key2.data(), s->ev_val.data(), s->ev_val2.data(), (int)m, 0,
 	                                s->key_bits, st);
-	cub::DeviceRadixSort::SortPairs(ts_temp(s, bytes), bytes, s->ev_key.data(), s->ev_key2.data(), s->ev_val.data(), s->ev_val2.data(),
-	                                (int)m, 0, s->key_bits, st);
-	ts_bind_kernel<<<blocks((uint64_t)m + 1), BLOCK, 0, st>>>(s->req.data(), n, s->info.data(), s->ev_key2.data(), s->ev_val2.data(),
+	cub::DeviceRadixSort::SortPairs(io.temp_storage(bytes), bytes, s->ev_key.data(), s->ev_key2.data(), s->ev_val.data(),
+	                                s->ev_val2.data(), (int)m, 0, s->key_bits, st);
+	ts_bind_kernel<<<blocks((uint64_t)m + 1), BLOCK, 0, st>>>(io.req.data(), n, s->info.data(), s->ev_key2.data(), s->ev_val2.data(),
 	                                                          s->use.data(), s->lenpes.data());
-	ts_carry_kernel<<<blocks(m), BLOCK, 0, st>>>(s->req.data(), n, s->ev_key2.data(), s->ev_val2.data());
+	ts_carry_kernel<<<blocks(m), BLOCK, 0, st>>>(io.req.data(), n, s->ev_key2.data(), s->ev_val2.data());
 	bytes = 0;
 	cub::DeviceScan::ExclusiveSum(nullptr, bytes, s->lenpes.data(), s->scan.data(), (int)(m + 1), st);
-	cub::DeviceScan::ExclusiveSum(ts_temp(s, bytes), bytes, s->lenpes.data(), s->scan.data(), (int)(m + 1), st);
-	ts_totals_kernel<<<blocks(n), BLOCK, 0, st>>>(s->req.data(), n, s->scan.data(), s->out.data());
-	CUDA_CHECK(cudaMemcpyAsync(s->h_out.data(), s->out.data(), n * sizeof(TsReqOut), cudaMemcpyDeviceToHost, st));
+	cub::DeviceScan::ExclusiveSum(io.temp_storage(bytes), bytes, s->lenpes.data(), s->scan.data(), (int)(m + 1), st);
+	ts_totals_kernel<<<blocks(n), BLOCK, 0, st>>>(io.req.data(), n, s->scan.data(), io.out.data());
+	CUDA_CHECK(cudaMemcpyAsync(io.h_out.data(), io.out.data(), n * sizeof(TsReqOut), cudaMemcpyDeviceToHost, st));
 	return 8;  // (a cub algorithm counts as one launch)
 }
 
-uint32_t ts_call_gather(TsScratch *s, uint32_t pad, cudaStream_t st) {
+uint32_t ts_call_gather(TsScratch *s, TsIo &io, uint32_t pad, cudaStream_t st) {
 	const uint32_t n = s->n_req, m = s->n_slots;
-	ts_gather_kernel<<<blocks(((uint64_t)m + n) * 32), BLOCK, 0, st>>>(s->stage.data(), s->req.data(), n, s->grid.data(), s->out.data(),
+	ts_gather_kernel<<<blocks(((uint64_t)m + n) * 32), BLOCK, 0, st>>>(io.stage.data(), io.req.data(), n, s->grid.data(), io.out.data(),
 	                                                                    s->use.data(), s->scan.data(), s->pts.data(), pad,
-	                                                                    s->pes_offset.data(), s->pes_pts.data());
+	                                                                    io.pes_offset.data(), io.pes_pts.data());
 	return 1;
 }

@@ -29,7 +29,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-# host synchronisations per call of the PS path (csrc/engine.cu ps_write_many) by design, not counted: the candidate
+# host synchronisations per call of the PS path (csrc/engine.cu demux_many) by design, not counted: the candidate
 # counts, the per-request results, then the copy back.  A stream whose HBM mirror or the per-candidate scratch grows
 # adds one; the timed passes start from a reset batch whose mirrors and scratch mostly have room already.
 SYNCS_PER_CALL_NOMINAL = 3

@@ -27,7 +27,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-# host synchronisations per call of the TS path (csrc/engine.cu ts_write_many): the totals, then the copy back.  A
+# host synchronisations per call of the TS path (csrc/engine.cu demux_many): the totals, then the copy back.  A
 # stream whose HBM mirror grows adds one (reserve_device_es); the timed passes start from a reset batch whose mirrors
 # already have room.
 SYNCS_PER_CALL = 2
