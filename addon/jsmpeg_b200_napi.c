@@ -147,6 +147,31 @@ static napi_value js_planes(napi_env env, napi_callback_info info) {
 	return out;
 }
 
+/* Extension: setExportMacroblocks(decoder, on) switches the decoder's "macroblocks" option; macroblocks(decoder) is a
+ * zero-copy Uint8Array over the pinned macroblock entries (16 bytes per macroblock, raster order, the layout of
+ * jsmpeg_b200_macroblock_t) of the picture the last decode() rendered -- valid until the next decode(), like the
+ * planes; undefined before the sequence header. */
+static napi_value js_set_export_macroblocks(napi_env env, napi_callback_info info) {
+	napi_value argv[2];
+	uint32_t on = 0;
+	mpeg1_decoder_t *d = decoder_arg(env, info, 2, argv);
+	if (!d) return NULL;
+	napi_get_value_uint32(env, argv[1], &on);
+	jsmpeg_b200_decoder_set_option(d, "macroblocks", (int)on);
+	return NULL;
+}
+static napi_value js_macroblocks(napi_env env, napi_callback_info info) {
+	napi_value argv[1];
+	mpeg1_decoder_t *d = decoder_arg(env, info, 1, argv);
+	void *entries;
+	size_t n;
+	if (!d) return NULL;
+	entries = jsmpeg_b200_decoder_get_macroblocks(d);
+	if (!entries) return NULL;
+	n = (size_t)((mpeg1_decoder_get_width(d) + 15) / 16) * (size_t)((mpeg1_decoder_get_height(d) + 15) / 16) * 16;
+	return plane_view(env, entries, n);
+}
+
 static napi_value init(napi_env env, napi_value exports) {
 	static const struct { const char *name; napi_callback fn; } table[] = {
 		{"create", js_create}, {"destroy", js_destroy}, {"write", js_write},
@@ -155,6 +180,7 @@ static napi_value init(napi_env env, napi_value exports) {
 		{"getCodedSize", js_get_coded_size}, {"getWidth", js_get_width}, {"getHeight", js_get_height},
 		{"decode", js_decode}, {"planes", js_planes},
 		{"setDecodeB", js_set_decode_b}, {"lastPictureType", js_last_picture_type},
+		{"setExportMacroblocks", js_set_export_macroblocks}, {"macroblocks", js_macroblocks},
 	};
 	for (size_t i = 0; i < sizeof(table) / sizeof(table[0]); i++) {
 		napi_value fn;

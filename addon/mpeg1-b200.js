@@ -24,6 +24,10 @@ var MPEG1B200 = function(options) {
 	// ... and with displayOrder an I/P picture is held back (a copy: the planes are borrowed until the next
 	// decode) until the next I/P picture arrives; flush() renders the last one
 	this.displayOrder = !!(options.decodeBPictures && options.displayOrder);
+	// extension: with exportMacroblocks, macroblocks() gives the macroblock types and motion vectors of the picture the
+	// last decode() rendered (motion detection, overlays) without walking the picture a second time
+	this.exportMacroblocks = !!options.exportMacroblocks;
+	if (this.exportMacroblocks) { native.setExportMacroblocks(this.decoder, 1); }
 	this.held = null;
 	this.decodeFirstFrame = options.decodeFirstFrame !== false;
 	this.hasSequenceHeader = false;
@@ -83,6 +87,12 @@ MPEG1B200.prototype.decode = function() {
 		this.onDecodeCallback(this, JSMpeg.Now() - startTime);
 	}
 	return true;
+};
+
+// Uint8Array of 16 bytes per macroblock in raster order (include/jsmpeg_b200.h: jsmpeg_b200_macroblock_t), borrowed
+// until the next decode(); null without exportMacroblocks or before the sequence header
+MPEG1B200.prototype.macroblocks = function() {
+	return this.exportMacroblocks ? (native.macroblocks(this.decoder) || null) : null;
 };
 
 MPEG1B200.prototype.flush = function() {

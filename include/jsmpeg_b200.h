@@ -77,6 +77,8 @@ typedef struct jsmpeg_b200_batch_t jsmpeg_b200_batch_t;
 #define JSMPEG_B200_OUT_DEVICE 0 /* planes stay in HBM (jsmpeg_b200_batch_get_planes)           */
 #define JSMPEG_B200_OUT_HOST   1 /* every decoded picture is also copied to pinned host memory  */
 #define JSMPEG_B200_OUT_RGBA   2 /* run the fused planar->RGBA epilogue (canvas2d.js:53-122)    */
+#define JSMPEG_B200_OUT_MACROBLOCKS 4 /* every reconstructed picture's macroblock entries beside its planes
+                                       * (jsmpeg_b200_batch_get_macroblocks, below decode_macroblocks)  */
 
 typedef struct jsmpeg_b200_stats_t {
 	uint64_t pictures;            /* decode() == true count                                     */
@@ -86,7 +88,7 @@ typedef struct jsmpeg_b200_stats_t {
 	uint64_t algorithmic_bytes;   /* stage-2 bytes: records + planes written + planes referenced */
 	uint64_t es_bytes;            /* bitstream bytes consumed by stage 1                        */
 	uint64_t h2d_bytes, d2h_bytes;
-	uint64_t kernel_launches;     /* scan + parse + reconstruct (+ rgba) launches               */
+	uint64_t kernel_launches;     /* scan + parse + reconstruct (+ rgba, + macroblock export) launches */
 	uint64_t recon_launches;
 	double parse_ms, recon_ms, scan_ms; /* CUDA-event device time on the launching stream       */
 	uint64_t parse_errors;        /* pictures whose slice walk hit an invalid code              */
@@ -320,6 +322,32 @@ long jsmpeg_b200_batch_macroblock_index(jsmpeg_b200_batch_t *b, int stream, uint
 long jsmpeg_b200_batch_decode_macroblocks(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
                                           void *const *mb_dst, int32_t *n_present_out, int32_t *error_out);
 
+/* MACROBLOCK DATA OF THE PLAYBACK PATH (live analytics on the pictures decode() plays: motion detection, intra share as
+ * a shot-cut cue, motion overlays): with JSMPEG_B200_OUT_MACROBLOCKS in the flags of jsmpeg_b200_batch_decode or
+ * jsmpeg_b200_batch_seek_pictures (combined freely with OUT_HOST / OUT_RGBA), every picture the call reconstructs gets
+ * its macroblock entries beside its planes, from the walk decode() reconstructs it from: no second walk.
+ *
+ * A stream's ENTRIES are mb_height * mb_width jsmpeg_b200_macroblock_t in raster order, in the layout and conversion of
+ * decode_macroblocks.  After a call with the flag they are the entries of the picture get_planes gives, whenever a call
+ * with the flag reconstructed that picture; for a picture decode() reconstructs (PIC_DECODED: I and P pictures, B
+ * pictures under decode_b) they equal byte for byte what decode_macroblocks writes for the same picture k -- on damaged
+ * streams too, both reading the records of the walk that starts at k's start code.  A call that reconstructs nothing
+ * for a stream leaves its entries as they were, like its planes.  A call WITHOUT the flag writes no entries: after it
+ * the entries may describe an older picture than the planes.  Entries not yet written by a call with the flag are 0,
+ * and again after jsmpeg_b200_batch_reset.  seek_pictures with the flag: the entries of the picture the stream's state
+ * ends on (picture k, or under status 0 the picture the fresh decoder ended on; 0 where that decoder reconstructed
+ * nothing).
+ *
+ * Each returns 0, or non-zero for a dead batch, a stream out of range or one without a sequence header. */
+/* Device pointer to the entries; valid until the next decode / seek, like get_planes. */
+int jsmpeg_b200_batch_get_macroblocks(jsmpeg_b200_batch_t *b, int stream, void **entries);
+/* Synchronous copy of the entries into caller memory (mb_height * mb_width * 16 bytes), like read_planes. */
+int jsmpeg_b200_batch_read_macroblocks(jsmpeg_b200_batch_t *b, int stream, void *dst);
+/* Host pointer (pinned) to the entries of the picture get_host_planes gives: under OUT_HOST | OUT_MACROBLOCKS every
+ * reconstructed picture's entries go to the slot of the host ring that receives its planes, so the planes and entries of
+ * one slot always belong together. */
+int jsmpeg_b200_batch_get_host_macroblocks(jsmpeg_b200_batch_t *b, int stream, void **entries);
+
 /* COEFFICIENTS (DC images for shot-boundary detection and thumbnails, residual-energy and texture features,
  * DCT-domain learning): each block's 64 dequantised DCT coefficients of chosen pictures of any streams, as the
  * inverse transform consumes them -- no pixels and no reference pictures, so every request of a call is one wave of
@@ -489,9 +517,14 @@ long jsmpeg_b200_debug_read_es(jsmpeg_b200_batch_t *b, int stream, void *dst, si
 const char *jsmpeg_b200_decoder_last_error(mpeg1_decoder_t *self);
 
 /* jsmpeg_b200_batch_set_option / jsmpeg_b200_batch_last_picture for a decoder of the reference ABI (which has no
- * option call): "decode_b" switches the B-picture extension on, "lookahead" sets the pictures parsed ahead. */
+ * option call): "decode_b" switches the B-picture extension on, "lookahead" sets the pictures parsed ahead.  The
+ * decoder's own option "macroblocks" (default 0): with 1, mpeg1_decoder_decode decodes with JSMPEG_B200_OUT_MACROBLOCKS
+ * and jsmpeg_b200_decoder_get_macroblocks returns the entries of the picture it rendered (what get_y_ptr shows). */
 int jsmpeg_b200_decoder_set_option(mpeg1_decoder_t *self, const char *name, int value);
 int jsmpeg_b200_decoder_last_picture(mpeg1_decoder_t *self, int *picture_type, int *temporal_reference);
+/* HOST-visible (pinned) mb_height * mb_width jsmpeg_b200_macroblock_t (jsmpeg_b200_batch_get_host_macroblocks);
+ * borrowed until the next decode; NULL before the sequence header or when the decoder is dead. */
+void *jsmpeg_b200_decoder_get_macroblocks(mpeg1_decoder_t *self);
 
 /* CUDA device for decoders created through the reference ABI from now on (the reference ABI has no
  * device argument; the JS/Python class passes its `device` option here). */

@@ -10,6 +10,7 @@ import numpy as np
 OUT_DEVICE = 0
 OUT_HOST = 1
 OUT_RGBA = 2
+OUT_MACROBLOCKS = 4  # every reconstructed picture's macroblock entries beside its planes (device_macroblocks)
 
 
 class Stats(ctypes.Structure):
@@ -54,6 +55,9 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_get_rgba": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
     "jsmpeg_b200_batch_read_planes": (ctypes.c_int, [_VP, ctypes.c_int, _VP, _VP, _VP]),
     "jsmpeg_b200_batch_read_rgba": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
+    "jsmpeg_b200_batch_get_macroblocks": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
+    "jsmpeg_b200_batch_read_macroblocks": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
+    "jsmpeg_b200_batch_get_host_macroblocks": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
     "jsmpeg_b200_batch_last_picture": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_batch_intra_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
@@ -77,6 +81,7 @@ _BATCH_ABI = {
     "jsmpeg_b200_decoder_last_error": (ctypes.c_char_p, [_VP]),
     "jsmpeg_b200_decoder_set_option": (ctypes.c_int, [_VP, ctypes.c_char_p, ctypes.c_int]),
     "jsmpeg_b200_decoder_last_picture": (ctypes.c_int, [_VP, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
+    "jsmpeg_b200_decoder_get_macroblocks": (_VP, [_VP]),
     "jsmpeg_b200_bind_host_to_device": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_version": (ctypes.c_char_p, []),
 }
@@ -317,6 +322,45 @@ class BatchDecoder:
             return np.ctypeslib.as_array(ctypes.cast(p, ctypes.POINTER(ctypes.c_uint8)), shape=(size,))
 
         return view(y, n), view(cr, n >> 2), view(cb, n >> 2)
+
+    def _entries_shape(self, stream):
+        """(mb_height, mb_width, 16) of the stream's macroblock entries; ValueError unless the stream is in range and
+        has a sequence header."""
+        info = self._request_stream_info(stream)
+        return (info["height"] + 15) // 16, (info["width"] + 15) // 16, MACROBLOCK_BYTES
+
+    def _entries_ptr(self, fn, stream):
+        ptr = _VP()
+        if fn(self.handle, stream, ctypes.byref(ptr)) != 0:
+            raise RuntimeError(self.last_error() or f"{fn.__name__} failed")
+        return ptr.value
+
+    def device_macroblocks(self, stream):
+        """The stream's macroblock entries (decode / seek_pictures with OUT_MACROBLOCKS, include/jsmpeg_b200.h): a
+        torch.uint8 CUDA view [mb_height, mb_width, 16] of the library's buffer beside the planes of the picture
+        device_planes gives (see macroblocks_view).  Borrowed: valid until the next decode / seek; clone to keep it."""
+        import torch
+        shape = self._entries_shape(stream)
+        ptr = self._entries_ptr(self.lib.jsmpeg_b200_batch_get_macroblocks, stream)
+
+        class _Entries:  # (zero copy: torch wraps memory that exposes __cuda_array_interface__)
+            __cuda_array_interface__ = {"data": (ptr, False), "shape": shape, "typestr": "|u1", "version": 2}
+
+        return torch.as_tensor(_Entries(), device=torch.device("cuda", self.device))
+
+    def read_macroblocks(self, stream):
+        """A numpy copy [mb_height, mb_width, 16] of the entries device_macroblocks views (synchronous)."""
+        out = np.empty(self._entries_shape(stream), np.uint8)
+        if self.lib.jsmpeg_b200_batch_read_macroblocks(self.handle, stream, out.ctypes.data) != 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_read_macroblocks failed")
+        return out
+
+    def host_macroblocks(self, stream):
+        """Under OUT_HOST | OUT_MACROBLOCKS: a numpy view [mb_height, mb_width, 16] of the pinned entries of the
+        picture host_planes gives (the same host-ring slot).  Borrowed like host_planes."""
+        shape = self._entries_shape(stream)
+        ptr = self._entries_ptr(self.lib.jsmpeg_b200_batch_get_host_macroblocks, stream)
+        return np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ctypes.c_uint8)), shape=shape)
 
     def read_rgba(self, stream):
         info = self.stream_info(stream)

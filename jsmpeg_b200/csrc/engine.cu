@@ -95,6 +95,11 @@ struct Stream {
 	int b_cur = 0;
 	uint8_t *d_last = nullptr;
 	int last_type = 0, last_temporal = 0;  // picture_coding_type / temporal_reference of the last picture decode() consumed
+	// macroblock entries (OUT_MACROBLOCKS, DESIGN 3.13): one buffer beside each plane set (d_mb[i] beside d_planes[i],
+	// d_mb_b[i] beside d_planes_b[i]) and one per host-ring slot, made zeroed on first use (reserve_entries).  A picture's
+	// entries go where its planes go, so every ordering rule of the planes covers them.
+	DeviceBuffer<uint8_t> d_mb[2], d_mb_b[2];
+	PinnedBuffer<uint8_t> h_mb[HOST_RING];
 	DeviceBuffer<uint8_t> d_rgba;
 	DeviceBuffer<int16_t> ts_bound;    // device TS demux: the stream id every PID is bound to, 0 = none (ts.js pidsToStreamIds)
 	std::vector<uint8_t> ts_leftover;  // ... and the bytes the last write_ts left over (ts.js leftoverBytes)
@@ -167,6 +172,9 @@ struct jsmpeg_b200_batch_t {
 	// decode_macroblocks: the export tasks of a wave (DESIGN 3.8)
 	PinnedBuffer<MbExportTask> h_xtasks;
 	DeviceBuffer<MbExportTask> d_xtasks;
+	// decode() and seek_pictures under OUT_MACROBLOCKS: the export tasks of a round's (a wave's) steps (DESIGN 3.13)
+	PinnedBuffer<MbExportTask> h_etasks;
+	DeviceBuffer<MbExportTask> d_etasks;
 	// decode_coefficients: the coefficient export tasks of a wave (DESIGN 3.9)
 	PinnedBuffer<CoefExportTask> h_ctasks;
 	DeviceBuffer<CoefExportTask> d_ctasks;
@@ -591,10 +599,13 @@ void copy_batch(Batch *b, std::vector<void *> &dst, std::vector<void *> &src, st
 		for (size_t i = 0; i < n_copy; i++) CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], size[i], cudaMemcpyDefault, st));
 }
 
-// The reconstruct tasks of one step of decode() (or one depth of decode_chains), queued by launch_reconstruct; and
-// the copies of its pictures that follow them
+// The reconstruct tasks of one step of decode() (or one depth of decode_chains), queued by launch_reconstruct; the
+// export of their macroblock entries (OUT_MACROBLOCKS: `entries`, one launch of export_macroblocks_kernel over
+// `entry_mb` macroblocks); and the copies of its pictures that follow them
 struct ReconStep {
 	std::vector<ReconTask> tasks;
+	std::vector<MbExportTask> entries;
+	uint32_t entry_mb = 0;
 	std::vector<void *> dst, src;
 	std::vector<size_t> size;
 	void copy(void *to, void *from, size_t n) {
@@ -602,7 +613,40 @@ struct ReconStep {
 		src.push_back(from);
 		size.push_back(n);
 	}
+	// the entries of task t's picture (picture_coding_type `type`) into `to`
+	void entry(const ReconTask &t, int type, void *to) {
+		entries.push_back(MbExportTask{t.hdr, to, entry_mb, t.mb_size, type, 0});
+		entry_mb += (uint32_t)t.mb_size;
+	}
 };
+
+// OUT_MACROBLOCKS: the export tasks of all `steps` go up in one copy on the reconstruct stream; returns where each step's
+// tasks begin in the device table.  The previous upload's readers are done before the pinned table is written again:
+// decode_round ends with its reconstruction complete, and run_chains' next wave waits for ev_round.
+std::vector<const MbExportTask *> upload_entry_tasks(Batch *b, const std::vector<ReconStep> &steps) {
+	size_t n = 0;
+	for (const ReconStep &r : steps) n += r.entries.size();
+	if (n > b->d_etasks.size()) {
+		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+		b->h_etasks.reserve(n);
+		b->d_etasks.reserve(n);
+	}
+	std::vector<const MbExportTask *> at;
+	size_t m = 0;
+	for (const ReconStep &r : steps) {
+		at.push_back(b->d_etasks.data() + m);
+		for (const MbExportTask &t : r.entries) b->h_etasks[m++] = t;
+	}
+	if (m) CUDA_CHECK(cudaMemcpyAsync(b->d_etasks.data(), b->h_etasks.data(), m * sizeof(MbExportTask), cudaMemcpyHostToDevice, b->st_recon));
+	return at;
+}
+
+// The step's export launch, queued behind its reconstruct launch (`tasks`: upload_entry_tasks); returns the launches
+int launch_step_entries(Batch *b, const ReconStep &r, const MbExportTask *tasks) {
+	if (r.entries.empty()) return 0;
+	launch_export_macroblocks(tasks, (int)r.entries.size(), r.entry_mb, b->st_recon);
+	return 1;
+}
 
 // The copy-out of one step's pictures (OUT_HOST) on the copy stream, behind the step's launches
 void copy_out_step(Batch *b, ReconStep &r) {
@@ -810,6 +854,30 @@ void reserve_b_sets(Batch *b, Stream &s) {
 	}
 }
 
+// The stream's entry buffers (OUT_MACROBLOCKS), made on first use: every plane set's, zeroed on the reconstruct stream,
+// and every host-ring slot's
+void reserve_entries(Batch *b, Stream &s) {
+	if (s.d_mb[0].data()) return;
+	const size_t bytes = (size_t)s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t);
+	for (DeviceBuffer<uint8_t> *e : {&s.d_mb[0], &s.d_mb[1], &s.d_mb_b[0], &s.d_mb_b[1]}) {
+		e->reserve(bytes);
+		CUDA_CHECK(cudaMemsetAsync(e->data(), 0, bytes, b->st_recon));
+	}
+	for (auto &h : s.h_mb) {
+		h.reserve(bytes);
+		memset(h.data(), 0, bytes);
+	}
+}
+
+// The entry buffer beside plane set `set`, one of the stream's four (reserve_entries made them)
+uint8_t *set_entries(const Stream &s, const uint8_t *set) {
+	for (int i = 0; i < 2; i++) {
+		if (set == s.d_planes[i].data()) return s.d_mb[i].data();
+		if (set == s.d_planes_b[i].data()) return s.d_mb_b[i].data();
+	}
+	throw std::logic_error("jsmpeg_b200: a plane set without an entry buffer");
+}
+
 // One round: parse ahead what is missing in one wave, then consume up to want[s] pictures per stream in decode()
 // order and queue their reconstruction.  Returns pictures consumed; `progress[s]` gets the per-stream count, `more[s]`
 // whether the stream may have further pictures.
@@ -912,10 +980,21 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 				const uint64_t planes = (uint64_t)s.coded_size * 3 / 2;
 				if (steps.size() <= step) steps.emplace_back();
 				steps[step].tasks.push_back(t);
+				uint8_t *entries = nullptr;
+				if (flags & JSMPEG_B200_OUT_MACROBLOCKS) {  // beside the planes, in the set's entry buffer
+					reserve_entries(b, s);
+					entries = set_entries(s, t.cur.y);
+					steps[step].entry(t, e.info.picture_type, entries);
+				}
 				if (flags & JSMPEG_B200_OUT_HOST) {  // into the next slot of the stream's host ring
 					s.h_head = (s.h_head + 1) % HOST_RING;
 					steps[step].copy(s.h_planes[s.h_head].data(), t.cur.y, planes);
 					b->stats.d2h_bytes += planes;
+					if (entries) {
+						const size_t n = (size_t)s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t);
+						steps[step].copy(s.h_mb[s.h_head].data(), entries, n);
+						b->stats.d2h_bytes += n;
+					}
 				}
 				step++;
 				b->stats.pictures_decoded++;
@@ -933,16 +1012,21 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 	// ---- 4. reconstruction, one step after the other on the reconstruct stream, behind the wave's expand: the host has
 	// consumed the infos and queues the launches while the expand of the biggest pictures is still running
 	if (!steps.empty()) {
+		std::vector<const MbExportTask *> entry_tasks;
+		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) entry_tasks = upload_entry_tasks(b, steps);  // (outside recon_ms)
 		if (!wave.empty()) CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_b, 0));
 		CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
-		for (ReconStep &r : steps) {
+		for (size_t i = 0; i < steps.size(); i++) {
+			ReconStep &r = steps[i];
 			// A launch overwrites, per stream, the plane set written two of that stream's pictures ago, i.e. by
 			// a launch at least two copy-out launches back: the copy-out recorded two launches ago must be done
-			// (the copy stream is in order, so that covers every earlier one).
+			// (the copy stream is in order, so that covers every earlier one).  The same holds for the set's entries.
 			if ((flags & JSMPEG_B200_OUT_HOST) && b->copy_steps >= 2)
 				CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_copied[b->copy_steps & 1], 0));
 			b->stats.kernel_launches += launch_reconstruct(r.tasks.data(), (int)r.tasks.size(), b->st_recon);
 			b->stats.recon_launches++;
+			// the step's records are final here (st_recon waited for ev_b) and stay until the next round's parse (ev_round)
+			if (!entry_tasks.empty()) b->stats.kernel_launches += launch_step_entries(b, r, entry_tasks[i]);
 			if (flags & JSMPEG_B200_OUT_HOST) copy_out_step(b, r);  // while the next step reconstructs
 		}
 		CUDA_CHECK(cudaEventRecord(b->ev_recon[1], b->st_recon));
@@ -1654,9 +1738,11 @@ long batch_decode_accumulated(Batch *b, int n, const int *streams, const uint32_
 // ---- seek_pictures: move decode() of chosen streams to a listed picture, each from its seek chain start (DESIGN 3.12)
 
 // Each chain reconstructs into its stream's own sets (set[0..1] the I/P sets, set[2..3] the B sets) with decode()'s
-// rotation, one launch_reconstruct per depth.  The last picture a chain consumes -- picture k, or on damaged input the
-// picture whose walk ran across k -- is, when decoded, also written to the stream's RGBA under OUT_RGBA and copied to
-// the next slot of its host ring under OUT_HOST (copy_out_step).  No later launch of the call writes its set.
+// rotation, one launch_reconstruct per depth, and under OUT_MACROBLOCKS one export launch per depth into the sets'
+// entry buffers.  The last picture a chain consumes -- picture k, or on damaged input the picture whose walk ran across
+// k -- is, when decoded, also written to the stream's RGBA under OUT_RGBA and copied (with its entries under
+// OUT_MACROBLOCKS) to the next slot of its host ring under OUT_HOST (copy_out_step).  No later launch of the call
+// writes its set.
 struct SeekWork : ChainWork {
 	Batch *b;
 	int flags;
@@ -1675,15 +1761,21 @@ struct SeekWork : ChainWork {
 		last[ch.stream] = t.cur.y;
 		if (steps.size() <= d) steps.emplace_back();
 		steps[d].tasks.push_back(t);
+		uint8_t *entries = (flags & JSMPEG_B200_OUT_MACROBLOCKS) ? set_entries(s, t.cur.y) : nullptr;
+		if (entries) steps[d].entry(t, e.picture_type, entries);
 		if (final && (flags & JSMPEG_B200_OUT_HOST)) {
 			s.h_head = (s.h_head + 1) % HOST_RING;
 			steps[d].copy(s.h_planes[s.h_head].data(), t.cur.y, (size_t)s.coded_size * 3 / 2);
+			if (entries) steps[d].copy(s.h_mb[s.h_head].data(), entries, (size_t)s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t));
 		}
 	}
 	void depths() override {
-		for (ReconStep &r : steps) {
-			launch_reconstruct(r.tasks.data(), (int)r.tasks.size(), b->st_recon);
-			if (!r.dst.empty()) copy_out_step(b, r);
+		std::vector<const MbExportTask *> entry_tasks;
+		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) entry_tasks = upload_entry_tasks(b, steps);
+		for (size_t i = 0; i < steps.size(); i++) {
+			launch_reconstruct(steps[i].tasks.data(), (int)steps[i].tasks.size(), b->st_recon);
+			if (!entry_tasks.empty()) launch_step_entries(b, steps[i], entry_tasks[i]);
+			if (!steps[i].dst.empty()) copy_out_step(b, steps[i]);
 		}
 		steps.clear();
 	}
@@ -1709,6 +1801,11 @@ void seek_pictures(Batch *b, std::vector<PictureRequest> &req, int flags, int32_
 		for (int k = 0; k < 4; k++) {
 			c.set[k] = sets[k];
 			if (sets[k]) CUDA_CHECK(cudaMemsetAsync(sets[k], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
+		}
+		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) {  // the fresh decoder's entries, like its planes: 0 until written
+			reserve_entries(b, s);
+			for (DeviceBuffer<uint8_t> *e : {&s.d_mb[0], &s.d_mb[1], &s.d_mb_b[0], &s.d_mb_b[1]})
+				CUDA_CHECK(cudaMemsetAsync(e->data(), 0, e->size(), b->st_recon));
 		}
 		c.b_end = c.last + 1;  // every B picture the fresh decoder reconstructs: a set's content is decode() state
 	}
@@ -2151,6 +2248,11 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 				for (auto &p : s.d_planes) CUDA_CHECK(cudaMemsetAsync(p.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_main));
 				for (auto &p : s.d_planes_b) if (p.data()) CUDA_CHECK(cudaMemsetAsync(p.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_main));
 			}
+			if (s.d_mb[0].data()) {  // (made after the sequence header, by a call with OUT_MACROBLOCKS)
+				for (DeviceBuffer<uint8_t> *e : {&s.d_mb[0], &s.d_mb[1], &s.d_mb_b[0], &s.d_mb_b[1]})
+					CUDA_CHECK(cudaMemsetAsync(e->data(), 0, e->size(), b->st_main));
+				for (auto &h : s.h_mb) memset(h.data(), 0, h.size());
+			}
 		}
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 	});
@@ -2308,6 +2410,47 @@ int jsmpeg_b200_batch_read_rgba(jsmpeg_b200_batch_t *b, int stream, void *rgba) 
 	});
 }
 
+// The stream whose entries the three *_macroblocks calls hand out, its entry buffers made (nullptr: out of range or
+// no sequence header yet)
+static Stream *entries_stream(Batch *b, int stream) {
+	if (stream < 0 || stream >= (int)b->streams.size() || !b->streams[stream].has_seq) return nullptr;
+	Stream &s = b->streams[stream];
+	if (!s.d_mb[0].data()) {
+		use_device(b);
+		reserve_entries(b, s);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+	}
+	return &s;
+}
+
+int jsmpeg_b200_batch_get_macroblocks(jsmpeg_b200_batch_t *b, int stream, void **entries) {
+	return guarded<int>(b, -1, [&] {
+		const Stream *s = entries_stream(b, stream);
+		if (!s) return -1;
+		if (entries) *entries = set_entries(*s, latest_planes(*s).y);
+		return 0;
+	});
+}
+
+int jsmpeg_b200_batch_read_macroblocks(jsmpeg_b200_batch_t *b, int stream, void *dst) {
+	return guarded<int>(b, -1, [&] {
+		const Stream *s = entries_stream(b, stream);
+		if (!s) return -1;
+		if (dst) CUDA_CHECK(cudaMemcpy(dst, set_entries(*s, latest_planes(*s).y), (size_t)s->seq.mb_size * sizeof(jsmpeg_b200_macroblock_t),
+		                               cudaMemcpyDeviceToHost));
+		return 0;
+	});
+}
+
+int jsmpeg_b200_batch_get_host_macroblocks(jsmpeg_b200_batch_t *b, int stream, void **entries) {
+	return guarded<int>(b, -1, [&] {
+		const Stream *s = entries_stream(b, stream);
+		if (!s) return -1;
+		if (entries) *entries = s->h_mb[s->h_head < 0 ? 0 : s->h_head].data();
+		return 0;
+	});
+}
+
 int jsmpeg_b200_batch_last_picture(jsmpeg_b200_batch_t *b, int stream, int *picture_type, int *temporal_reference) {
 	const Stream &s = b->streams[stream];
 	if (picture_type) *picture_type = s.last_type;
@@ -2323,6 +2466,7 @@ void jsmpeg_b200_batch_reset_stats(jsmpeg_b200_batch_t *b) { b->stats = jsmpeg_b
 
 struct mpeg1_decoder_t {
 	jsmpeg_b200_batch_t *b;
+	bool macroblocks = false;  // the "macroblocks" option: decode() also copies the picture's entries to the host
 };
 
 // Host placement.  The pinned bit buffers and plane rings of a decoder are touched by the host threads
@@ -2391,7 +2535,15 @@ void mpeg1_decoder_destroy(mpeg1_decoder_t *self) {
 
 const char *jsmpeg_b200_decoder_last_error(mpeg1_decoder_t *self) { return self ? jsmpeg_b200_batch_last_error(self->b) : nullptr; }
 int jsmpeg_b200_decoder_set_option(mpeg1_decoder_t *self, const char *name, int value) {
+	if (self && name && !strcmp(name, "macroblocks")) {
+		self->macroblocks = value != 0;
+		return 0;
+	}
 	return self ? jsmpeg_b200_batch_set_option(self->b, name, value) : -1;
+}
+void *jsmpeg_b200_decoder_get_macroblocks(mpeg1_decoder_t *self) {
+	void *p = nullptr;
+	return self && jsmpeg_b200_batch_get_host_macroblocks(self->b, 0, &p) == 0 ? p : nullptr;
 }
 int jsmpeg_b200_decoder_last_picture(mpeg1_decoder_t *self, int *picture_type, int *temporal_reference) {
 	return self ? jsmpeg_b200_batch_last_picture(self->b, 0, picture_type, temporal_reference) : -1;
@@ -2420,7 +2572,7 @@ void *mpeg1_decoder_get_cb_ptr(mpeg1_decoder_t *self) { return host_plane(self, 
 
 bool mpeg1_decoder_decode(mpeg1_decoder_t *self) {
 	if (!self->b->streams[0].has_seq) return false;
-	return jsmpeg_b200_batch_decode(self->b, 1, JSMPEG_B200_OUT_HOST) > 0;
+	return jsmpeg_b200_batch_decode(self->b, 1, JSMPEG_B200_OUT_HOST | (self->macroblocks ? JSMPEG_B200_OUT_MACROBLOCKS : 0)) > 0;
 }
 
 // ================================================================================================

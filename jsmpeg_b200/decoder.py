@@ -7,7 +7,9 @@
                    (+ our extensions `device`: CUDA device index; `decodeBPictures`: decode B pictures, which
                    the reference skips (src/mpeg1.js:181-184), in coded order -- `lastPicture()` tells type and
                    temporal_reference; with `displayOrder` the destination gets them in DISPLAY order: an I/P
-                   picture is held back (a copy) until the next I/P picture arrives, `flush()` renders the last)
+                   picture is held back (a copy) until the next I/P picture arrives, `flush()` renders the last;
+                   `exportMacroblocks`: `macroblocks()` gives the macroblock types and motion vectors of the
+                   picture the last decode() rendered)
     connect(destination) / destroy()
     bufferGetIndex() / bufferSetIndex(i) / bufferWrite(buffers)
     write(pts, buffers) / seek(time) / decode() -> bool
@@ -73,6 +75,11 @@ class MPEG1Video:
                 raise ValueError("decodeBPictures: this library has no B-picture extension")
             self.functions.jsmpeg_b200_decoder_set_option(self.decoder, b"decode_b", 1)
             self.displayOrder = bool(options.get("displayOrder"))
+        self.exportMacroblocks = bool(options.get("exportMacroblocks"))
+        if self.exportMacroblocks:
+            if not hasattr(self.functions, "jsmpeg_b200_decoder_get_macroblocks"):
+                raise ValueError("exportMacroblocks: this library has no macroblock export")
+            self.functions.jsmpeg_b200_decoder_set_option(self.decoder, b"macroblocks", 1)
 
     # ---- src/decoder.js:19-35 / src/mpeg1-wasm.js:32-50
     def destroy(self):
@@ -198,6 +205,17 @@ class MPEG1Video:
         return (view(f.mpeg1_decoder_get_y_ptr(self.decoder), n),
                 view(f.mpeg1_decoder_get_cr_ptr(self.decoder), n >> 2),
                 view(f.mpeg1_decoder_get_cb_ptr(self.decoder), n >> 2))
+
+    def macroblocks(self):
+        """exportMacroblocks (extension): a zero-copy uint8 view [mb_height, mb_width, 16] of the macroblock entries
+        (include/jsmpeg_b200.h: jsmpeg_b200_macroblock_t; jsmpeg_b200.batch.macroblocks_view names the fields) of the
+        picture the last decode() rendered -- borrowed like planes(); None without the option or before the sequence
+        header."""
+        ptr = self.functions.jsmpeg_b200_decoder_get_macroblocks(self.decoder) if self.exportMacroblocks else None
+        if not ptr:
+            return None
+        shape = ((self.height + 15) // 16, (self.width + 15) // 16, 16)
+        return np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ctypes.c_uint8)), shape=shape)
 
     # ---- src/decoder.js:77-106
     def advanceDecodedTime(self, seconds):
