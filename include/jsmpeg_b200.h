@@ -79,6 +79,8 @@ typedef struct jsmpeg_b200_batch_t jsmpeg_b200_batch_t;
 #define JSMPEG_B200_OUT_RGBA   2 /* run the fused planar->RGBA epilogue (canvas2d.js:53-122)    */
 #define JSMPEG_B200_OUT_MACROBLOCKS 4 /* every reconstructed picture's macroblock entries beside its planes
                                        * (jsmpeg_b200_batch_get_macroblocks, below decode_macroblocks)  */
+#define JSMPEG_B200_OUT_ACCUMULATED (1 << 3) /* = 8: every reconstructed I/P picture's accumulated map beside its planes
+                                       * (jsmpeg_b200_batch_get_accumulated, below decode_accumulated) */
 
 typedef struct jsmpeg_b200_stats_t {
 	uint64_t pictures;            /* decode() == true count                                     */
@@ -88,7 +90,7 @@ typedef struct jsmpeg_b200_stats_t {
 	uint64_t algorithmic_bytes;   /* stage-2 bytes: records + planes written + planes referenced */
 	uint64_t es_bytes;            /* bitstream bytes consumed by stage 1                        */
 	uint64_t h2d_bytes, d2h_bytes;
-	uint64_t kernel_launches;     /* scan + parse + reconstruct (+ rgba, + macroblock export) launches */
+	uint64_t kernel_launches;     /* scan + parse + reconstruct (+ rgba, + macroblock export, + accumulate) launches */
 	uint64_t recon_launches;
 	double parse_ms, recon_ms, scan_ms; /* CUDA-event device time on the launching stream       */
 	uint64_t parse_errors;        /* pictures whose slice walk hit an invalid code              */
@@ -455,6 +457,43 @@ typedef struct jsmpeg_b200_accumulated_t {
 long jsmpeg_b200_batch_decode_accumulated(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
                                           void *const *acc_dst, int32_t *status_out, int32_t *n_present_out,
                                           int32_t *error_out);
+
+/* ACCUMULATED MAPS OF THE PLAYBACK PATH (live compressed-domain models on the pictures decode() plays: camera walls,
+ * stream moderation, action recognition on ingest): with JSMPEG_B200_OUT_ACCUMULATED in the flags of
+ * jsmpeg_b200_batch_decode or jsmpeg_b200_batch_seek_pictures (combined freely with OUT_HOST, OUT_RGBA and
+ * OUT_MACROBLOCKS), every I or P picture the call reconstructs (PIC_DECODED, type 1 or 2) gets the map of
+ * decode_accumulated beside its planes, from the records decode() reconstructs it from: no second walk, and one depth
+ * step per picture instead of the whole chain.
+ *
+ * A stream has one MAP per I/P plane set: coded_size * 3 / 2 jsmpeg_b200_accumulated_t in decode_accumulated's layout.
+ * The map of a reconstructed I/P picture is one step of decode_accumulated's rule from its own records, its own
+ * residual and `prev`, the map beside the forward set it was predicted from.  `prev` counts as absent (predicted samples
+ * untraced, intra samples back 0) unless a call with the flag wrote it for the picture that set holds: a reconstruct
+ * without the flag, jsmpeg_b200_batch_reset, a seek without the flag and a stream that starts on a P picture break the
+ * trace, which then stays untraced up to the next I picture.  B pictures (decode_b) get no map and leave both maps as
+ * they are.
+ *
+ * So for a picture k that decode() reconstructs under the flag, after every reference picture from the last I picture
+ * through k was also reconstructed under the flag, the map is decode_accumulated's fold over exactly the I/P pictures
+ * decode() reconstructed from that I picture, with the records and residuals decode_macroblocks / decode_residuals
+ * give for them -- on every clean stream byte for byte decode_accumulated of k.  After seek_pictures with the flag it is
+ * decode_accumulated of k for an I/P picture k, or of the newer reference for a B picture k, wherever the seek's fresh
+ * decoder and decode_accumulated's chain consume the same I/P pictures: every clean stream, and with decode_b off
+ * always.  More than 32,767 reference pictures without an I picture (decode_accumulated refuses such a chain) are not
+ * covered: `back` is int16 and wraps.
+ *
+ * Nothing else decode() observes changes: planes, RGBA, host ring, entries, bit index, last_picture and the stats, but
+ * kernel_launches, which counts one accumulate launch per reconstruct step with an I/P picture.  The maps are not
+ * copied to the host ring.  They are made on first use (2 x coded_size * 12 bytes per stream).
+ *
+ * Both calls give the map of the stream's NEWEST I/P picture -- the picture get_planes gives unless the last picture
+ * was a B picture (last_picture tells).  A map no call with the flag wrote for that picture reads as all untraced
+ * {0, 0, 0, -1}, so does every map before the first call with the flag.  Each returns 0, or non-zero for a dead batch,
+ * a stream out of range or one without a sequence header. */
+/* Device pointer to the map; valid until the next decode / seek, like get_planes. */
+int jsmpeg_b200_batch_get_accumulated(jsmpeg_b200_batch_t *b, int stream, void **map);
+/* Synchronous copy of the map into caller memory (coded_size * 12 bytes), like read_planes. */
+int jsmpeg_b200_batch_read_accumulated(jsmpeg_b200_batch_t *b, int stream, void *dst);
 
 /* SEEK (players, video walls, clip loaders): move decode() of chosen streams to a chosen picture each, and play on from
  * there with decode() -- OUT_HOST, OUT_RGBA and the host ring as usual -- without stepping the other streams.  The

@@ -11,6 +11,7 @@ OUT_DEVICE = 0
 OUT_HOST = 1
 OUT_RGBA = 2
 OUT_MACROBLOCKS = 4  # every reconstructed picture's macroblock entries beside its planes (device_macroblocks)
+OUT_ACCUMULATED = 8  # every reconstructed I/P picture's accumulated map beside its planes (device_accumulated)
 
 
 class Stats(ctypes.Structure):
@@ -58,6 +59,8 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_get_macroblocks": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
     "jsmpeg_b200_batch_read_macroblocks": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
     "jsmpeg_b200_batch_get_host_macroblocks": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
+    "jsmpeg_b200_batch_get_accumulated": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
+    "jsmpeg_b200_batch_read_accumulated": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
     "jsmpeg_b200_batch_last_picture": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_batch_intra_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
@@ -361,6 +364,32 @@ class BatchDecoder:
         shape = self._entries_shape(stream)
         ptr = self._entries_ptr(self.lib.jsmpeg_b200_batch_get_host_macroblocks, stream)
         return np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ctypes.c_uint8)), shape=shape)
+
+    def _map_shape(self, stream):
+        """(coded_size * 3 // 2, 4) of the stream's accumulated map; ValueError unless the stream is in range and has a
+        sequence header."""
+        return self._request_stream_info(stream)["coded_size"] * 3 // 2, 4
+
+    def device_accumulated(self, stream):
+        """The accumulated map of the stream's newest I/P picture (decode / seek_pictures with OUT_ACCUMULATED,
+        include/jsmpeg_b200.h): a torch.int16 CUDA view [coded_size * 3 // 2, 4] of the library's map (see
+        accumulated_view), all untraced where no call with the flag wrote it.  Borrowed: valid until the next decode /
+        seek; clone to keep it."""
+        import torch
+        shape = self._map_shape(stream)
+        ptr = self._entries_ptr(self.lib.jsmpeg_b200_batch_get_accumulated, stream)
+
+        class _Map:  # (zero copy, as device_macroblocks)
+            __cuda_array_interface__ = {"data": (ptr, False), "shape": shape, "typestr": "<i2", "version": 2}
+
+        return torch.as_tensor(_Map(), device=torch.device("cuda", self.device))
+
+    def read_accumulated(self, stream):
+        """A numpy copy int16 [coded_size * 3 // 2, 4] of the map device_accumulated views (synchronous)."""
+        out = np.empty(self._map_shape(stream), np.int16)
+        if self.lib.jsmpeg_b200_batch_read_accumulated(self.handle, stream, out.ctypes.data) != 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_read_accumulated failed")
+        return out
 
     def read_rgba(self, stream):
         info = self.stream_info(stream)

@@ -100,6 +100,11 @@ struct Stream {
 	// entries go where its planes go, so every ordering rule of the planes covers them.
 	DeviceBuffer<uint8_t> d_mb[2], d_mb_b[2];
 	PinnedBuffer<uint8_t> h_mb[HOST_RING];
+	// accumulated maps (OUT_ACCUMULATED, DESIGN 3.14): d_acc[i] beside d_planes[i], made on first use (reserve_maps);
+	// acc_written[i]: a call with the flag wrote d_acc[i] for the picture d_planes[i] holds now.  An unwritten map is
+	// never read as a trace's previous map.
+	DeviceBuffer<uint2> d_acc[2];
+	bool acc_written[2] = {false, false};
 	DeviceBuffer<uint8_t> d_rgba;
 	DeviceBuffer<int16_t> ts_bound;    // device TS demux: the stream id every PID is bound to, 0 = none (ts.js pidsToStreamIds)
 	std::vector<uint8_t> ts_leftover;  // ... and the bytes the last write_ts left over (ts.js leftoverBytes)
@@ -183,6 +188,7 @@ struct jsmpeg_b200_batch_t {
 	DeviceBuffer<ResExportTask> d_rtasks;
 	// decode_accumulated: the pool of the chains' two scratch map sets, and the tasks of a wave's depths (DESIGN 3.11)
 	DeviceBuffer<uint8_t> d_map_sets;
+	// (and under OUT_ACCUMULATED, the accumulate tasks of a decode() round's or a seek wave's steps, DESIGN 3.14)
 	PinnedBuffer<AccTask> h_atasks;
 	DeviceBuffer<AccTask> d_atasks;
 	jsmpeg_b200_stats_t stats{};
@@ -601,11 +607,14 @@ void copy_batch(Batch *b, std::vector<void *> &dst, std::vector<void *> &src, st
 
 // The reconstruct tasks of one step of decode() (or one depth of decode_chains), queued by launch_reconstruct; the
 // export of their macroblock entries (OUT_MACROBLOCKS: `entries`, one launch of export_macroblocks_kernel over
-// `entry_mb` macroblocks); and the copies of its pictures that follow them
+// `entry_mb` macroblocks); the accumulated maps of its I/P pictures (OUT_ACCUMULATED: `maps`, one launch of
+// accumulate_kernel over `map_warps` warps); and the copies of its pictures that follow them
 struct ReconStep {
 	std::vector<ReconTask> tasks;
 	std::vector<MbExportTask> entries;
 	uint32_t entry_mb = 0;
+	std::vector<AccTask> maps;
+	uint32_t map_warps = 0;
 	std::vector<void *> dst, src;
 	std::vector<size_t> size;
 	void copy(void *to, void *from, size_t n) {
@@ -618,33 +627,60 @@ struct ReconStep {
 		entries.push_back(MbExportTask{t.hdr, to, entry_mb, t.mb_size, type, 0});
 		entry_mb += (uint32_t)t.mb_size;
 	}
+	// the map of task t's I/P picture into `to`, one depth step from `prev` (nullptr: no previous map)
+	void map(const ReconTask &t, const uint2 *prev, uint2 *to) {
+		maps.push_back(AccTask{t.hdr, t.coef, t.compact, prev, to, map_warps, t.mb_width, t.mb_size / t.mb_width});
+		map_warps += res_export_warps(t.mb_size);
+	}
 };
 
-// OUT_MACROBLOCKS: the export tasks of all `steps` go up in one copy on the reconstruct stream; returns where each step's
-// tasks begin in the device table.  The previous upload's readers are done before the pinned table is written again:
-// decode_round ends with its reconstruction complete, and run_chains' next wave waits for ev_round.
-std::vector<const MbExportTask *> upload_entry_tasks(Batch *b, const std::vector<ReconStep> &steps) {
+// The tasks `list` of all `steps` (ReconStep::entries, ReconStep::maps) go up in one copy on the reconstruct stream,
+// through the pinned table `h` into `d`; returns where each step's tasks begin in `d`.  The previous upload's readers are
+// done before the pinned table is written again: decode_round ends with its reconstruction complete, and run_chains'
+// next wave waits for ev_round.
+template <typename T>
+std::vector<const T *> upload_step_tasks(Batch *b, const std::vector<ReconStep> &steps, std::vector<T> ReconStep::*list,
+                                         PinnedBuffer<T> &h, DeviceBuffer<T> &d) {
 	size_t n = 0;
-	for (const ReconStep &r : steps) n += r.entries.size();
-	if (n > b->d_etasks.size()) {
+	for (const ReconStep &r : steps) n += (r.*list).size();
+	if (n > d.size()) {
 		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-		b->h_etasks.reserve(n);
-		b->d_etasks.reserve(n);
+		h.reserve(n);
+		d.reserve(n);
 	}
-	std::vector<const MbExportTask *> at;
+	std::vector<const T *> at;
 	size_t m = 0;
 	for (const ReconStep &r : steps) {
-		at.push_back(b->d_etasks.data() + m);
-		for (const MbExportTask &t : r.entries) b->h_etasks[m++] = t;
+		at.push_back(d.data() + m);
+		for (const T &t : r.*list) h[m++] = t;
 	}
-	if (m) CUDA_CHECK(cudaMemcpyAsync(b->d_etasks.data(), b->h_etasks.data(), m * sizeof(MbExportTask), cudaMemcpyHostToDevice, b->st_recon));
+	if (m) CUDA_CHECK(cudaMemcpyAsync(d.data(), h.data(), m * sizeof(T), cudaMemcpyHostToDevice, b->st_recon));
 	return at;
+}
+
+// OUT_MACROBLOCKS: the export tasks of all `steps` (upload_step_tasks)
+std::vector<const MbExportTask *> upload_entry_tasks(Batch *b, const std::vector<ReconStep> &steps) {
+	return upload_step_tasks(b, steps, &ReconStep::entries, b->h_etasks, b->d_etasks);
+}
+
+// OUT_ACCUMULATED: the accumulate tasks of all `steps` (upload_step_tasks), in decode_accumulated's table: that call
+// ends with its launches complete
+std::vector<const AccTask *> upload_map_tasks(Batch *b, const std::vector<ReconStep> &steps) {
+	return upload_step_tasks(b, steps, &ReconStep::maps, b->h_atasks, b->d_atasks);
 }
 
 // The step's export launch, queued behind its reconstruct launch (`tasks`: upload_entry_tasks); returns the launches
 int launch_step_entries(Batch *b, const ReconStep &r, const MbExportTask *tasks) {
 	if (r.entries.empty()) return 0;
 	launch_export_macroblocks(tasks, (int)r.entries.size(), r.entry_mb, b->st_recon);
+	return 1;
+}
+
+// The step's accumulate launch, queued behind its reconstruct launch (`tasks`: upload_map_tasks); returns the launches.
+// A map the step reads as `prev` was written by an earlier step, on the same stream.
+int launch_step_maps(Batch *b, const ReconStep &r, const AccTask *tasks) {
+	if (r.maps.empty()) return 0;
+	launch_accumulate(tasks, (int)r.maps.size(), r.map_warps, b->st_recon);
 	return 1;
 }
 
@@ -878,6 +914,27 @@ uint8_t *set_entries(const Stream &s, const uint8_t *set) {
 	throw std::logic_error("jsmpeg_b200: a plane set without an entry buffer");
 }
 
+// The stream's two maps (OUT_ACCUMULATED), made on first use, unwritten: nothing reads them before a call with the flag
+// writes them, or get / read_accumulated fills them untraced (fill_untraced)
+void reserve_maps(Stream &s) {
+	if (s.d_acc[0].data()) return;
+	for (auto &m : s.d_acc) m.reserve((size_t)s.coded_size * 3 / 2);
+	s.acc_written[0] = s.acc_written[1] = false;
+}
+
+// Which of the two maps is beside I/P plane set `set`
+int set_map(const Stream &s, const uint8_t *set) {
+	for (int i = 0; i < 2; i++)
+		if (set == s.d_planes[i].data()) return i;
+	throw std::logic_error("jsmpeg_b200: an I/P plane set without a map");
+}
+
+// Every record of `n_rec` from `map` untraced {0, 0, 0, -1}, on `st`
+void fill_untraced(uint2 *map, size_t n_rec, cudaStream_t st) {
+	CUDA_CHECK(cudaMemsetAsync(map, 0, n_rec * 8, st));
+	CUDA_CHECK(cudaMemset2DAsync(reinterpret_cast<uint8_t *>(map) + 6, 8, 0xff, 2, n_rec, st));
+}
+
 // One round: parse ahead what is missing in one wave, then consume up to want[s] pictures per stream in decode()
 // order and queue their reconstruction.  Returns pictures consumed; `progress[s]` gets the per-stream count, `more[s]`
 // whether the stream may have further pictures.
@@ -986,6 +1043,16 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 					entries = set_entries(s, t.cur.y);
 					steps[step].entry(t, e.info.picture_type, entries);
 				}
+				if (!is_b) {  // the map beside the set, one depth step from the map beside the forward set
+					const int set = 1 - s.cur;  // (swapped above)
+					if (flags & JSMPEG_B200_OUT_ACCUMULATED) {
+						reserve_maps(s);
+						steps[step].map(t, s.acc_written[1 - set] ? s.d_acc[1 - set].data() : nullptr, s.d_acc[set].data());
+						s.acc_written[set] = true;
+					} else {
+						s.acc_written[set] = false;  // the set's new picture has no map
+					}
+				}
 				if (flags & JSMPEG_B200_OUT_HOST) {  // into the next slot of the stream's host ring
 					s.h_head = (s.h_head + 1) % HOST_RING;
 					steps[step].copy(s.h_planes[s.h_head].data(), t.cur.y, planes);
@@ -1013,7 +1080,9 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 	// consumed the infos and queues the launches while the expand of the biggest pictures is still running
 	if (!steps.empty()) {
 		std::vector<const MbExportTask *> entry_tasks;
+		std::vector<const AccTask *> map_tasks;
 		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) entry_tasks = upload_entry_tasks(b, steps);  // (outside recon_ms)
+		if (flags & JSMPEG_B200_OUT_ACCUMULATED) map_tasks = upload_map_tasks(b, steps);
 		if (!wave.empty()) CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_b, 0));
 		CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
 		for (size_t i = 0; i < steps.size(); i++) {
@@ -1027,6 +1096,8 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			b->stats.recon_launches++;
 			// the step's records are final here (st_recon waited for ev_b) and stay until the next round's parse (ev_round)
 			if (!entry_tasks.empty()) b->stats.kernel_launches += launch_step_entries(b, r, entry_tasks[i]);
+			// (the maps stay in HBM: no copy-out reads them)
+			if (!map_tasks.empty()) b->stats.kernel_launches += launch_step_maps(b, r, map_tasks[i]);
 			if (flags & JSMPEG_B200_OUT_HOST) copy_out_step(b, r);  // while the next step reconstructs
 		}
 		CUDA_CHECK(cudaEventRecord(b->ev_recon[1], b->st_recon));
@@ -1700,11 +1771,8 @@ void decode_accumulated(Batch *b, const std::vector<PictureRequest> &req, void *
 	const SetPool pool{b->d_map_sets, set_bytes, false};
 	const RequestInfo out = run_chains(b, req, order, chains, false, &pool, work);
 	for (int i = 0; i < (int)req.size(); i++)  // never consumed: every record untraced {0, 0, 0, -1}
-		if (out.status[i] != PIC_DECODED) {
-			const size_t n_rec = (size_t)b->streams[req[i].stream].coded_size * 3 / 2;
-			CUDA_CHECK(cudaMemsetAsync(acc_dst[i], 0, n_rec * 8, b->st_recon));
-			CUDA_CHECK(cudaMemset2DAsync(static_cast<uint8_t *>(acc_dst[i]) + 6, 8, 0xff, 2, n_rec, b->st_recon));
-		}
+		if (out.status[i] != PIC_DECODED)
+			fill_untraced(static_cast<uint2 *>(acc_dst[i]), (size_t)b->streams[req[i].stream].coded_size * 3 / 2, b->st_recon);
 	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
 	b->recon_pending = false;
 	out.copy_out(status_out, n_present_out, error_out);
@@ -1763,6 +1831,11 @@ struct SeekWork : ChainWork {
 		steps[d].tasks.push_back(t);
 		uint8_t *entries = (flags & JSMPEG_B200_OUT_MACROBLOCKS) ? set_entries(s, t.cur.y) : nullptr;
 		if (entries) steps[d].entry(t, e.picture_type, entries);
+		if (!is_b && (flags & JSMPEG_B200_OUT_ACCUMULATED)) {  // as decode_round, over the stream's own sets
+			const int set = set_map(s, t.cur.y);
+			steps[d].map(t, s.acc_written[1 - set] ? s.d_acc[1 - set].data() : nullptr, s.d_acc[set].data());
+			s.acc_written[set] = true;
+		}
 		if (final && (flags & JSMPEG_B200_OUT_HOST)) {
 			s.h_head = (s.h_head + 1) % HOST_RING;
 			steps[d].copy(s.h_planes[s.h_head].data(), t.cur.y, (size_t)s.coded_size * 3 / 2);
@@ -1771,10 +1844,13 @@ struct SeekWork : ChainWork {
 	}
 	void depths() override {
 		std::vector<const MbExportTask *> entry_tasks;
+		std::vector<const AccTask *> map_tasks;
 		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) entry_tasks = upload_entry_tasks(b, steps);
+		if (flags & JSMPEG_B200_OUT_ACCUMULATED) map_tasks = upload_map_tasks(b, steps);
 		for (size_t i = 0; i < steps.size(); i++) {
 			launch_reconstruct(steps[i].tasks.data(), (int)steps[i].tasks.size(), b->st_recon);
 			if (!entry_tasks.empty()) launch_step_entries(b, steps[i], entry_tasks[i]);
+			if (!map_tasks.empty()) launch_step_maps(b, steps[i], map_tasks[i]);
 			if (!steps[i].dst.empty()) copy_out_step(b, steps[i]);
 		}
 		steps.clear();
@@ -1807,6 +1883,8 @@ void seek_pictures(Batch *b, std::vector<PictureRequest> &req, int flags, int32_
 			for (DeviceBuffer<uint8_t> *e : {&s.d_mb[0], &s.d_mb[1], &s.d_mb_b[0], &s.d_mb_b[1]})
 				CUDA_CHECK(cudaMemsetAsync(e->data(), 0, e->size(), b->st_recon));
 		}
+		if (flags & JSMPEG_B200_OUT_ACCUMULATED) reserve_maps(s);
+		s.acc_written[0] = s.acc_written[1] = false;  // the fresh decoder's sets hold no picture yet
 		c.b_end = c.last + 1;  // every B picture the fresh decoder reconstructs: a set's content is decode() state
 	}
 	SeekWork work(b, flags);
@@ -2253,6 +2331,7 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 					CUDA_CHECK(cudaMemsetAsync(e->data(), 0, e->size(), b->st_main));
 				for (auto &h : s.h_mb) memset(h.data(), 0, h.size());
 			}
+			s.acc_written[0] = s.acc_written[1] = false;  // (zeroed sets: no picture, no map)
 		}
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 	});
@@ -2447,6 +2526,40 @@ int jsmpeg_b200_batch_get_host_macroblocks(jsmpeg_b200_batch_t *b, int stream, v
 		const Stream *s = entries_stream(b, stream);
 		if (!s) return -1;
 		if (entries) *entries = s->h_mb[s->h_head < 0 ? 0 : s->h_head].data();
+		return 0;
+	});
+}
+
+// The map get / read_accumulated hand out: the one beside the set of the stream's newest I/P picture, made on first use
+// and filled untraced unless a call with the flag wrote it for that picture (nullptr: stream out of range or no
+// sequence header yet)
+static uint2 *newest_map(Batch *b, int stream) {
+	if (stream < 0 || stream >= (int)b->streams.size() || !b->streams[stream].has_seq) return nullptr;
+	Stream &s = b->streams[stream];
+	use_device(b);
+	reserve_maps(s);
+	const int set = 1 - s.cur;
+	if (!s.acc_written[set]) {  // (the earlier calls have synchronised their streams)
+		fill_untraced(s.d_acc[set].data(), s.d_acc[set].size(), b->st_recon);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+	}
+	return s.d_acc[set].data();
+}
+
+int jsmpeg_b200_batch_get_accumulated(jsmpeg_b200_batch_t *b, int stream, void **map) {
+	return guarded<int>(b, -1, [&] {
+		uint2 *m = newest_map(b, stream);
+		if (!m) return -1;
+		if (map) *map = m;
+		return 0;
+	});
+}
+
+int jsmpeg_b200_batch_read_accumulated(jsmpeg_b200_batch_t *b, int stream, void *dst) {
+	return guarded<int>(b, -1, [&] {
+		const uint2 *m = newest_map(b, stream);
+		if (!m) return -1;
+		if (dst) CUDA_CHECK(cudaMemcpy(dst, m, (size_t)b->streams[stream].coded_size * 3 / 2 * sizeof(uint2), cudaMemcpyDeviceToHost));
 		return 0;
 	});
 }

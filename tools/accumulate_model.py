@@ -3,7 +3,8 @@
 A map is int16 [coded_size * 3 // 2, 4] in the planes' layout (Y | Cr | Cb): per sample (dx, dy, residual, back), back
 -1 for an untraced sample.  step() is one depth: the map of reference picture p_m from that of p_(m-1), p_m's records
 and residual; oracle_chain() folds it over a chain.  The chain's pictures are those the oracle's decode() reconstructs,
-with B pictures off, when fed chain_model.fresh_bytes() of the requested picture (oracle_chain).
+with B pictures off, when fed chain_model.fresh_bytes() of the requested picture (oracle_chain).  sequential() is the
+map decode() keeps under OUT_ACCUMULATED: the same step, folded over the I/P pictures decode() reconstructs.
 """
 from __future__ import annotations
 
@@ -87,15 +88,18 @@ def untraced(mb_width, mb_height):
     return m
 
 
-def oracle_decode(lib, es, stop=None):
-    """The oracle (B pictures off) fed `es`: [(start byte, picture_info, records, coefficient plane, planes)] of every
-    picture its decode() consumes, up to the one whose header starts at byte `stop`."""
+def oracle_decode(lib, es, stop=None, decode_b=False, index=None):
+    """The oracle (B pictures off, or on with `decode_b`) fed `es`: [(start byte, picture_info, records, coefficient
+    plane, planes)] of every picture its decode() consumes, up to the one whose header starts at byte `stop`; with
+    `index`, from that bit index on (set_index right after the write)."""
     from jsmpeg_b200 import decoder
 
     import helpers
-    lib.oracle_set_decode_b(0)
+    lib.oracle_set_decode_b(int(decode_b))
     d = decoder.MPEG1Video({"decodeFirstFrame": False}, lib=lib)
     d.write(0.0, [es])
+    if index is not None:
+        d.bufferSetIndex(index)
     seq = lib.oracle_seq_params(d.decoder)
     mb, mbw = seq.contents.mb_size, seq.contents.mb_width
     cs = mb * 256
@@ -114,6 +118,7 @@ def oracle_decode(lib, es, stop=None):
         if stop is not None and info.start_byte >= stop:
             break
     d.destroy()
+    lib.oracle_set_decode_b(0)
     return out, mbw, mb // mbw
 
 
@@ -136,3 +141,17 @@ def oracle_chain(lib, es, entry, rest=False):
                 return info.status, info.n_present, info.error, untraced(mbw, mbh)
             return info.status, info.n_present, info.error, prev
     return 0, 0, 0, untraced(mbw, mbh)
+
+
+def sequential(lib, es, decode_b=False, index=None):
+    """The maps decode() with OUT_ACCUMULATED keeps for `es` (include/jsmpeg_b200.h): [(start byte, picture_info, map)]
+    per I/P picture the oracle's decode() reconstructs (B pictures as `decode_b` says; from bit index `index` when
+    given), each one step from the map of the I/P picture reconstructed before it -- none for the first, so a start on
+    a P picture leaves its predicted samples untraced up to the next I picture.  B pictures get no map."""
+    got, mbw, mbh = oracle_decode(lib, es, decode_b=decode_b, index=index)
+    out, prev = [], None
+    for start, info, rec, coef, _ in got:
+        if info.status == 1 and info.picture_type in (1, 2):
+            prev = depth(prev, rec, coef, mbw, mbh)
+            out.append((start, info, prev))
+    return out
