@@ -81,6 +81,8 @@ typedef struct jsmpeg_b200_batch_t jsmpeg_b200_batch_t;
                                        * (jsmpeg_b200_batch_get_macroblocks, below decode_macroblocks)  */
 #define JSMPEG_B200_OUT_ACCUMULATED (1 << 3) /* = 8: every reconstructed I/P picture's accumulated map beside its planes
                                        * (jsmpeg_b200_batch_get_accumulated, below decode_accumulated) */
+#define JSMPEG_B200_OUT_RESIDUALS (0x10) /* = 16 = bit 4: the residual of the picture get_planes gives
+                                       * (jsmpeg_b200_batch_get_residuals, below the accumulated maps) */
 
 typedef struct jsmpeg_b200_stats_t {
 	uint64_t pictures;            /* decode() == true count                                     */
@@ -90,7 +92,11 @@ typedef struct jsmpeg_b200_stats_t {
 	uint64_t algorithmic_bytes;   /* stage-2 bytes: records + planes written + planes referenced */
 	uint64_t es_bytes;            /* bitstream bytes consumed by stage 1                        */
 	uint64_t h2d_bytes, d2h_bytes;
-	uint64_t kernel_launches;     /* scan + parse + reconstruct (+ rgba, + macroblock export, + accumulate) launches */
+	uint64_t kernel_launches;     /* scan + parse + reconstruct (+ rgba, + macroblock export, + accumulate) launches;
+	                               * OUT_RESIDUALS adds none, but a step's reconstruct kernel with a residual task is
+	                               * cut into launches of its RES variant's capacity (72 plain, 56 RGBA, 63 B, 51 B + RGBA
+	                               * tasks, against 80, 60, 64, 48): a step with more tasks of one kernel than the
+	                               * smaller of the two may take a different number of launches */
 	uint64_t recon_launches;
 	double parse_ms, recon_ms, scan_ms; /* CUDA-event device time on the launching stream       */
 	uint64_t parse_errors;        /* pictures whose slice walk hit an invalid code              */
@@ -494,6 +500,36 @@ long jsmpeg_b200_batch_decode_accumulated(jsmpeg_b200_batch_t *b, int n, const i
 int jsmpeg_b200_batch_get_accumulated(jsmpeg_b200_batch_t *b, int stream, void **map);
 /* Synchronous copy of the map into caller memory (coded_size * 12 bytes), like read_planes. */
 int jsmpeg_b200_batch_read_accumulated(jsmpeg_b200_batch_t *b, int stream, void *dst);
+
+/* RESIDUAL OF THE PLAYBACK PATH (live compressed-domain models -- I frames, motion vectors and residuals -- on the
+ * pictures decode() plays): with JSMPEG_B200_OUT_RESIDUALS in the flags of jsmpeg_b200_batch_decode or
+ * jsmpeg_b200_batch_seek_pictures (combined freely with OUT_HOST, OUT_RGBA, OUT_MACROBLOCKS and OUT_ACCUMULATED), the
+ * reconstruct kernel also stores the pixel-domain residual it adds to the prediction: no second walk and no second
+ * transform.
+ *
+ * A stream has one RESIDUAL: coded_size * 3 / 2 int16 in decode_residuals' layout (Y at 0, Cr at coded_size, Cb at
+ * coded_size * 5 / 4, in samples), in device memory made zeroed on first use (coded_size * 3 bytes).  After a call
+ * with the flag it is the residual of the picture get_planes gives, whenever a call with the flag reconstructed that
+ * picture; for a picture decode() reconstructs (PIC_DECODED: I and P pictures, B pictures under decode_b) it equals byte
+ * for byte what decode_residuals writes for the same picture k -- on damaged streams too, both reading the records of
+ * the walk that starts at k's start code.  The rules are those of the entries (OUT_MACROBLOCKS): a call that
+ * reconstructs nothing for a stream leaves its residual as it was; a call WITHOUT the flag writes none, so afterwards
+ * the residual may describe an older picture than the planes; a residual no call with the flag wrote is 0, and again
+ * after jsmpeg_b200_batch_reset (rewind leaves it, like the planes); seek_pictures with the flag: the residual of the
+ * picture the stream's state ends on (picture k, or under status 0 the picture the fresh decoder ended on; 0 where
+ * that decoder reconstructed nothing).
+ *
+ * Only the stream's newest picture's residual can be observed, so decode(n) with the flag stores it only for the last
+ * picture each stream reconstructs in each of its rounds; a consumer that wants every picture's residual calls
+ * decode(1) with the flag.  The residual is not copied to the host ring: at coded_size * 3 bytes per picture its
+ * consumer is a model on the same GPU.  Nothing else decode() observes changes: planes, RGBA, host ring, entries, maps,
+ * bit index, last_picture and the stats, but kernel_launches as described there.
+ *
+ * Each returns 0, or non-zero for a dead batch, a stream out of range or one without a sequence header. */
+/* Device pointer to the residual; valid until the next decode / seek, like get_planes. */
+int jsmpeg_b200_batch_get_residuals(jsmpeg_b200_batch_t *b, int stream, void **res);
+/* Synchronous copy of the residual into caller memory (coded_size * 3 bytes), like read_planes. */
+int jsmpeg_b200_batch_read_residuals(jsmpeg_b200_batch_t *b, int stream, void *dst);
 
 /* SEEK (players, video walls, clip loaders): move decode() of chosen streams to a chosen picture each, and play on from
  * there with decode() -- OUT_HOST, OUT_RGBA and the host ring as usual -- without stepping the other streams.  The

@@ -12,6 +12,7 @@ OUT_HOST = 1
 OUT_RGBA = 2
 OUT_MACROBLOCKS = 4  # every reconstructed picture's macroblock entries beside its planes (device_macroblocks)
 OUT_ACCUMULATED = 8  # every reconstructed I/P picture's accumulated map beside its planes (device_accumulated)
+OUT_RESIDUALS = 16  # the residual of the picture the planes hold, stored by stage 2 (device_residuals)
 
 
 class Stats(ctypes.Structure):
@@ -61,6 +62,8 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_get_host_macroblocks": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
     "jsmpeg_b200_batch_get_accumulated": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
     "jsmpeg_b200_batch_read_accumulated": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
+    "jsmpeg_b200_batch_get_residuals": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
+    "jsmpeg_b200_batch_read_residuals": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
     "jsmpeg_b200_batch_last_picture": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_batch_intra_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
@@ -389,6 +392,32 @@ class BatchDecoder:
         out = np.empty(self._map_shape(stream), np.int16)
         if self.lib.jsmpeg_b200_batch_read_accumulated(self.handle, stream, out.ctypes.data) != 0:
             raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_read_accumulated failed")
+        return out
+
+    def _residuals_shape(self, stream):
+        """(coded_size * 3 // 2,) of the stream's residual; ValueError unless the stream is in range and has a sequence
+        header."""
+        return (self._request_stream_info(stream)["coded_size"] * 3 // 2,)
+
+    def device_residuals(self, stream):
+        """The residual of the picture device_planes gives (decode / seek_pictures with OUT_RESIDUALS,
+        include/jsmpeg_b200.h): a torch.int16 CUDA view [coded_size * 3 // 2] of the library's buffer in
+        decode_residuals' layout (planes_view splits it into Y, Cr, Cb), 0 where no call with the flag wrote it.
+        Borrowed: valid until the next decode / seek; clone to keep it."""
+        import torch
+        shape = self._residuals_shape(stream)
+        ptr = self._entries_ptr(self.lib.jsmpeg_b200_batch_get_residuals, stream)
+
+        class _Residual:  # (zero copy, as device_macroblocks)
+            __cuda_array_interface__ = {"data": (ptr, False), "shape": shape, "typestr": "<i2", "version": 2}
+
+        return torch.as_tensor(_Residual(), device=torch.device("cuda", self.device))
+
+    def read_residuals(self, stream):
+        """A numpy copy int16 [coded_size * 3 // 2] of the residual device_residuals views (synchronous)."""
+        out = np.empty(self._residuals_shape(stream), np.int16)
+        if self.lib.jsmpeg_b200_batch_read_residuals(self.handle, stream, out.ctypes.data) != 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_read_residuals failed")
         return out
 
     def read_rgba(self, stream):

@@ -113,6 +113,7 @@ struct ReconTask {
 	uint8_t *rgba;  // optional fused epilogue target (display size, RGBA8888) or nullptr
 	int32_t width, height;
 	PlaneSet bwd;   // B picture (the opt-in extension): the newer of the two most recent I/P pictures
+	int16_t *res;   // OUT_RESIDUALS: the picture's residual, coded_size * 3 / 2 int16 in the planes' layout, or nullptr
 };
 
 // kernel launchers (defined in scan.cu / parse.cu / recon.cu)
@@ -150,7 +151,9 @@ int launch_parse_pictures(WalkKind kind, const ParseTask *tasks, int n_tasks, in
 // Stage 2 of n_tasks pictures, by kernel: I/P pictures, then I/P pictures with the planar -> RGBA conversion fused in
 // (tasks with `rgba`), then B pictures (tasks with `bwd`: prediction from two references), then B pictures with the
 // conversion; each kernel's tasks in their order.  `tasks_host` is read on the host at launch time: the table travels
-// in the kernel parameters.  Returns the number of kernels launched.
+// in the kernel parameters.  When any task of a kernel has `res`, all that kernel's tasks go to its RES variant, which
+// also stores the residual of every task with `res` (the others ride along with none).  Returns the number of kernels
+// launched.
 int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
 
 // Macroblock export (macroblocks.cu): request i converts the records of one picture (`mb_size` of them at `src`, a

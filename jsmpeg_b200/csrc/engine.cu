@@ -105,6 +105,9 @@ struct Stream {
 	// never read as a trace's previous map.
 	DeviceBuffer<uint2> d_acc[2];
 	bool acc_written[2] = {false, false};
+	// residual (OUT_RESIDUALS, DESIGN 3.15): that of the newest picture a call with the flag reconstructed, stored by
+	// stage 2 (ReconTask::res); made zeroed on first use (reserve_residuals)
+	DeviceBuffer<int16_t> d_res;
 	DeviceBuffer<uint8_t> d_rgba;
 	DeviceBuffer<int16_t> ts_bound;    // device TS demux: the stream id every PID is bound to, 0 = none (ts.js pidsToStreamIds)
 	std::vector<uint8_t> ts_leftover;  // ... and the bytes the last write_ts left over (ts.js leftoverBytes)
@@ -922,6 +925,15 @@ void reserve_maps(Stream &s) {
 	s.acc_written[0] = s.acc_written[1] = false;
 }
 
+// The stream's residual (OUT_RESIDUALS), made zeroed on the reconstruct stream on first use
+int16_t *reserve_residuals(Batch *b, Stream &s) {
+	if (!s.d_res.data()) {
+		s.d_res.reserve((size_t)s.coded_size * 3 / 2);
+		CUDA_CHECK(cudaMemsetAsync(s.d_res.data(), 0, s.d_res.size() * sizeof(int16_t), b->st_recon));
+	}
+	return s.d_res.data();
+}
+
 // Which of the two maps is beside I/P plane set `set`
 int set_map(const Stream &s, const uint8_t *set) {
 	for (int i = 0; i < 2; i++)
@@ -1074,6 +1086,9 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			// this round's expand on the main stream
 			release_slot(b, e.slot);
 		}
+		// OUT_RESIDUALS: the stream's last reconstructed picture of the round (the newest task of its last step) stores its
+		// residual; the earlier ones of the round could not be observed
+		if ((flags & JSMPEG_B200_OUT_RESIDUALS) && step > 0) steps[step - 1].tasks.back().res = reserve_residuals(b, s);
 	}
 	lap(b->trace.consume, t);
 	// ---- 4. reconstruction, one step after the other on the reconstruct stream, behind the wave's expand: the host has
@@ -1816,7 +1831,9 @@ struct SeekWork : ChainWork {
 	int flags;
 	std::vector<uint8_t *> last;  // per stream: the set of the newest picture the call reconstructed (nullptr: none)
 	std::vector<ReconStep> steps;
-	SeekWork(Batch *b, int flags) : b(b), flags(flags), last(b->streams.size(), nullptr) {}
+	// OUT_RESIDUALS: per stream, its newest picture of the wave as (depth, task index), depth -1: none yet
+	std::vector<std::pair<int, int>> newest;
+	SeekWork(Batch *b, int flags) : b(b), flags(flags), last(b->streams.size(), nullptr), newest(b->streams.size(), {-1, 0}) {}
 	void picture(Chain &ch, const Stream &, int slot, const picture_info_t &e, size_t d, int, int) override {
 		Stream &s = b->streams[ch.stream];
 		const bool is_b = e.picture_type == 3;
@@ -1829,6 +1846,7 @@ struct SeekWork : ChainWork {
 		last[ch.stream] = t.cur.y;
 		if (steps.size() <= d) steps.emplace_back();
 		steps[d].tasks.push_back(t);
+		newest[ch.stream] = {(int)d, (int)steps[d].tasks.size() - 1};
 		uint8_t *entries = (flags & JSMPEG_B200_OUT_MACROBLOCKS) ? set_entries(s, t.cur.y) : nullptr;
 		if (entries) steps[d].entry(t, e.picture_type, entries);
 		if (!is_b && (flags & JSMPEG_B200_OUT_ACCUMULATED)) {  // as decode_round, over the stream's own sets
@@ -1847,6 +1865,11 @@ struct SeekWork : ChainWork {
 		std::vector<const AccTask *> map_tasks;
 		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) entry_tasks = upload_entry_tasks(b, steps);
 		if (flags & JSMPEG_B200_OUT_ACCUMULATED) map_tasks = upload_map_tasks(b, steps);
+		for (size_t si = 0; si < newest.size(); si++) {  // as decode_round: each stream's newest picture of the wave
+			if ((flags & JSMPEG_B200_OUT_RESIDUALS) && newest[si].first >= 0)
+				steps[newest[si].first].tasks[newest[si].second].res = b->streams[si].d_res.data();  // (seek_pictures made it)
+			newest[si].first = -1;
+		}
 		for (size_t i = 0; i < steps.size(); i++) {
 			launch_reconstruct(steps[i].tasks.data(), (int)steps[i].tasks.size(), b->st_recon);
 			if (!entry_tasks.empty()) launch_step_entries(b, steps[i], entry_tasks[i]);
@@ -1885,6 +1908,10 @@ void seek_pictures(Batch *b, std::vector<PictureRequest> &req, int flags, int32_
 		}
 		if (flags & JSMPEG_B200_OUT_ACCUMULATED) reserve_maps(s);
 		s.acc_written[0] = s.acc_written[1] = false;  // the fresh decoder's sets hold no picture yet
+		if (flags & JSMPEG_B200_OUT_RESIDUALS) {  // 0 unless the chain reconstructs a picture, like the entries
+			reserve_residuals(b, s);
+			CUDA_CHECK(cudaMemsetAsync(s.d_res.data(), 0, s.d_res.size() * sizeof(int16_t), b->st_recon));
+		}
 		c.b_end = c.last + 1;  // every B picture the fresh decoder reconstructs: a set's content is decode() state
 	}
 	SeekWork work(b, flags);
@@ -2332,6 +2359,7 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 				for (auto &h : s.h_mb) memset(h.data(), 0, h.size());
 			}
 			s.acc_written[0] = s.acc_written[1] = false;  // (zeroed sets: no picture, no map)
+			if (s.d_res.data()) CUDA_CHECK(cudaMemsetAsync(s.d_res.data(), 0, s.d_res.size() * sizeof(int16_t), b->st_main));
 		}
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
 	});
@@ -2526,6 +2554,37 @@ int jsmpeg_b200_batch_get_host_macroblocks(jsmpeg_b200_batch_t *b, int stream, v
 		const Stream *s = entries_stream(b, stream);
 		if (!s) return -1;
 		if (entries) *entries = s->h_mb[s->h_head < 0 ? 0 : s->h_head].data();
+		return 0;
+	});
+}
+
+// The residual get / read_residuals hand out, made zeroed on first use (nullptr: stream out of range or no sequence
+// header yet)
+static int16_t *stream_residuals(Batch *b, int stream) {
+	if (stream < 0 || stream >= (int)b->streams.size() || !b->streams[stream].has_seq) return nullptr;
+	Stream &s = b->streams[stream];
+	use_device(b);
+	if (!s.d_res.data()) {
+		reserve_residuals(b, s);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+	}
+	return s.d_res.data();
+}
+
+int jsmpeg_b200_batch_get_residuals(jsmpeg_b200_batch_t *b, int stream, void **res) {
+	return guarded<int>(b, -1, [&] {
+		int16_t *r = stream_residuals(b, stream);
+		if (!r) return -1;
+		if (res) *res = r;
+		return 0;
+	});
+}
+
+int jsmpeg_b200_batch_read_residuals(jsmpeg_b200_batch_t *b, int stream, void *dst) {
+	return guarded<int>(b, -1, [&] {
+		int16_t *r = stream_residuals(b, stream);
+		if (!r) return -1;
+		if (dst) CUDA_CHECK(cudaMemcpy(dst, r, b->streams[stream].d_res.size() * sizeof(int16_t), cudaMemcpyDeviceToHost));
 		return 0;
 	});
 }

@@ -90,6 +90,56 @@ reconstruct_rgba_b_kernel(const __grid_constant__ ReconRgbaParamsB params) {
 	reconstruct_rgba_block<true>(params.p, params.out[blockIdx.z], blockIdx.z, blockIdx.y, blockIdx.x * RGBA_MBS, threadIdx.x, stage, chroma);
 }
 
+// OUT_RESIDUALS (DESIGN 3.15): the four kernels above, each block also storing its residual (reconstruct_at<..., RES>),
+// with the tables of ReconResParamsT (recon.cuh)
+constexpr int MAX_TASKS_RES = 72;         // (72 * (48 + 8) B) + 8 < 4 KB
+constexpr int MAX_TASKS_RGBA_RES = 56;    // (56 * (48 + 8 + 16) B) + 8 < 4 KB
+constexpr int MAX_TASKS_B_RES = 63;       // (63 * (56 + 8) B) + 8 < 4 KB
+constexpr int MAX_TASKS_RGBA_B_RES = 51;  // (51 * (56 + 8 + 16) B) + 8 < 4 KB
+using ReconResParams = ReconResParamsT<CompactTask, MAX_TASKS_RES>;
+using ReconResParamsB = ReconResParamsT<CompactTaskB, MAX_TASKS_B_RES>;
+struct ReconRgbaResParams {
+	ReconResParamsT<CompactTask, MAX_TASKS_RGBA_RES> p;
+	RgbaTarget out[MAX_TASKS_RGBA_RES];
+};
+struct ReconRgbaResParamsB {
+	ReconResParamsT<CompactTaskB, MAX_TASKS_RGBA_B_RES> p;
+	RgbaTarget out[MAX_TASKS_RGBA_B_RES];
+};
+static_assert(sizeof(ReconResParams) <= 4096 && sizeof(ReconResParamsB) <= 4096 && sizeof(ReconRgbaResParams) <= 4096 &&
+              sizeof(ReconRgbaResParamsB) <= 4096, "kernel parameters");
+
+__global__ void __launch_bounds__(THREADS, JSMPEG_RECON_MIN_CTAS)
+reconstruct_res_kernel(const __grid_constant__ ReconResParams params) {
+	__shared__ __align__(16) uint8_t stage[(THREADS / 32) * WARP_STAGE];
+	reconstruct_block<false, true>(params, blockIdx.y, blockIdx.x * THREADS, threadIdx.x, stage);
+}
+
+__global__ void __launch_bounds__(RGBA_THREADS)
+reconstruct_rgba_res_kernel(const __grid_constant__ ReconRgbaResParams params) {
+	__shared__ __align__(16) uint8_t stage[(RGBA_THREADS / 32) * WARP_STAGE];
+	__shared__ __align__(16) uint8_t chroma[2][8][RGBA_MBS * 8];
+	reconstruct_rgba_block<false, true>(params.p, params.out[blockIdx.z], blockIdx.z, blockIdx.y, blockIdx.x * RGBA_MBS, threadIdx.x, stage, chroma);
+}
+
+// (at 5 resident CTAs, 96 registers, the B variant's residual store spills -- reconstruct_b_kernel spills there too, on
+// its per-tap path; at 4, 128 registers, it does not)
+#ifndef JSMPEG_RECON_RES_B_MIN_CTAS
+#define JSMPEG_RECON_RES_B_MIN_CTAS 4
+#endif
+__global__ void __launch_bounds__(THREADS, JSMPEG_RECON_RES_B_MIN_CTAS)
+reconstruct_res_b_kernel(const __grid_constant__ ReconResParamsB params) {
+	__shared__ __align__(16) uint8_t stage[(THREADS / 32) * WARP_STAGE];
+	reconstruct_block<true, true>(params, blockIdx.y, blockIdx.x * THREADS, threadIdx.x, stage);
+}
+
+__global__ void __launch_bounds__(RGBA_THREADS)
+reconstruct_rgba_res_b_kernel(const __grid_constant__ ReconRgbaResParamsB params) {
+	__shared__ __align__(16) uint8_t stage[(RGBA_THREADS / 32) * WARP_STAGE];
+	__shared__ __align__(16) uint8_t chroma[2][8][RGBA_MBS * 8];
+	reconstruct_rgba_block<true, true>(params.p, params.out[blockIdx.z], blockIdx.z, blockIdx.y, blockIdx.x * RGBA_MBS, threadIdx.x, stage, chroma);
+}
+
 void fill_task(CompactTask &c, const ReconTask &t) {
 	c.hdr = t.hdr;
 	c.coef = t.coef;
@@ -103,9 +153,9 @@ void fill_task(CompactTask &c, const ReconTask &t) {
 }
 
 // One kernel's tasks, cut into launches of at most `per`: B = the kernel takes `bwd`, RGBA = it takes the fused
-// conversion's target.  The plain kernels' grid covers the largest picture's block slots, the RGBA kernels' its
-// macroblock rows and columns.
-template <bool B, bool RGBA, class Params>
+// conversion's target, RES = it takes the residual destinations.  The plain kernels' grid covers the largest picture's
+// block slots, the RGBA kernels' its macroblock rows and columns.
+template <bool B, bool RGBA, bool RES = false, class Params>
 int launch_kernel(void (*kernel)(Params), int per, const std::vector<const ReconTask *> &tasks, cudaStream_t stream) {
 	int launches = 0;
 	for (size_t first = 0; first < tasks.size(); first += per, launches++) {
@@ -118,6 +168,7 @@ int launch_kernel(void (*kernel)(Params), int per, const std::vector<const Recon
 			fill_task(table.t[i], t);
 			if constexpr (B) table.t[i].bwd = t.bwd.y;
 			if constexpr (RGBA) p.out[i] = RgbaTarget{t.rgba, t.width, t.height};
+			if constexpr (RES) table.res[i] = t.res;
 			max_slots = std::max(max_slots, t.mb_size * 6);
 			max_w = std::max(max_w, t.mb_width);
 			max_h = std::max(max_h, t.mb_size / t.mb_width);
@@ -133,14 +184,21 @@ int launch_kernel(void (*kernel)(Params), int per, const std::vector<const Recon
 
 int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream) {
 	std::vector<const ReconTask *> by_kernel[4];  // I/P, I/P + RGBA, B, B + RGBA
+	bool res[4] = {false, false, false, false};   // some task of the kernel has a residual destination: its RES variant
 	for (int i = 0; i < n_tasks; i++) {
 		const ReconTask &t = tasks_host[i];
-		by_kernel[(t.bwd.y ? 2 : 0) + (t.rgba ? 1 : 0)].push_back(&t);
+		const int k = (t.bwd.y ? 2 : 0) + (t.rgba ? 1 : 0);
+		by_kernel[k].push_back(&t);
+		res[k] = res[k] || t.res;
 	}
 	// (one statement per kernel: the launch order is the order above)
-	int launches = launch_kernel<false, false>(reconstruct_kernel, MAX_TASKS, by_kernel[0], stream);
-	launches += launch_kernel<false, true>(reconstruct_rgba_kernel, MAX_TASKS_RGBA, by_kernel[1], stream);
-	launches += launch_kernel<true, false>(reconstruct_b_kernel, MAX_TASKS_B, by_kernel[2], stream);
-	launches += launch_kernel<true, true>(reconstruct_rgba_b_kernel, MAX_TASKS_RGBA_B, by_kernel[3], stream);
+	int launches = res[0] ? launch_kernel<false, false, true>(reconstruct_res_kernel, MAX_TASKS_RES, by_kernel[0], stream)
+	                      : launch_kernel<false, false>(reconstruct_kernel, MAX_TASKS, by_kernel[0], stream);
+	launches += res[1] ? launch_kernel<false, true, true>(reconstruct_rgba_res_kernel, MAX_TASKS_RGBA_RES, by_kernel[1], stream)
+	                   : launch_kernel<false, true>(reconstruct_rgba_kernel, MAX_TASKS_RGBA, by_kernel[1], stream);
+	launches += res[2] ? launch_kernel<true, false, true>(reconstruct_res_b_kernel, MAX_TASKS_B_RES, by_kernel[2], stream)
+	                   : launch_kernel<true, false>(reconstruct_b_kernel, MAX_TASKS_B, by_kernel[2], stream);
+	launches += res[3] ? launch_kernel<true, true, true>(reconstruct_rgba_res_b_kernel, MAX_TASKS_RGBA_B_RES, by_kernel[3], stream)
+	                   : launch_kernel<true, true>(reconstruct_rgba_b_kernel, MAX_TASKS_RGBA_B, by_kernel[3], stream);
 	return launches;
 }

@@ -51,6 +51,15 @@ struct ReconParamsB {
 	int32_t n_tasks;
 };
 
+// OUT_RESIDUALS (DESIGN 3.15): a RES kernel's table is the plain one plus a parallel res[] (nullptr: no residual for
+// that task), so CompactTask keeps its 48 bytes and a launch carries fewer tasks than the plain kernel's
+template <class TASK, int N>
+struct ReconResParamsT {
+	TASK t[N];
+	int32_t n_tasks;
+	int16_t *res[N];
+};
+
 #ifndef JSMPEG_WALK_EMU
 __device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ uint32_t umulhi_u32(uint32_t a, uint32_t b) { return __umulhi(a, b); }
@@ -244,6 +253,23 @@ __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)_
 static inline uint32_t smem_u32(const void *) { return 0; }
 #endif
 
+// OUT_RESIDUALS (DESIGN 3.15): the block's residual v[] into the residual plane at `dst` (the block's origin, in the
+// plane's stride), each row as 8 packed int16 in one streaming 16-byte store (export_residuals_kernel's packing;
+// |r| <= 14,314 fits int16).  Nothing in the call reads it back.
+__device__ __forceinline__ void store_residual_row(int16_t *dst, uint4 o) {
+#ifndef JSMPEG_WALK_EMU
+	__stcs(reinterpret_cast<uint4 *>(dst), o);
+#else
+	memcpy(dst, &o, 16);
+#endif
+}
+__device__ __forceinline__ void store_residual(int16_t *dst, int stride, const int (&v)[64]) {
+#pragma unroll
+	for (int r = 0; r < 8; r++)
+		store_residual_row(dst + r * stride, make_uint4(__byte_perm(v[r * 8 + 0], v[r * 8 + 1], 0x5410), __byte_perm(v[r * 8 + 2], v[r * 8 + 3], 0x5410),
+		                                                __byte_perm(v[r * 8 + 4], v[r * 8 + 5], 0x5410), __byte_perm(v[r * 8 + 6], v[r * 8 + 7], 0x5410)));
+}
+
 // One 8x8 block: slot first_slot + tid of picture `ty` of the launch (see above); `stage` = the CTA's
 // staging area (one WARP_STAGE per warp), tid = the thread's index in the CTA.
 // WARP-CONVERGENT: the 32 lanes of a warp call it together (collectives inside).
@@ -264,7 +290,9 @@ static inline uint32_t smem_u32(const void *) { return 0; }
 // the samples it keeps).
 // BIDIR (B pictures, PARAMS = ReconParamsB): the record's MBF_MOTION_* bits say which of t.fwd / t.bwd a predicted
 // block uses; everything up to the prediction is the same code.
-template <bool KEEP, bool BIDIR = false, class PARAMS>
+// RES (OUT_RESIDUALS, PARAMS with `res`: ReconResParamsT above): a task whose params.res[ty] is not nullptr also
+// gets each in-picture block's residual v[] there (store_residual): zeros for a macroblock that is not present.
+template <bool KEEP, bool BIDIR = false, bool RES = false, class PARAMS>
 __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int mb_row, int mb_col, int b, bool in_picture,
                                                int lane, uint8_t *wstage, uint2 (&rows)[8]) {
 	const auto &t = params.t[ty];
@@ -405,6 +433,12 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		for (int r = 0; r < 8; r++) rows[r] = *reinterpret_cast<const uint2 *>(dst + r * stride);
 	};
 	if (!present) {
+		if constexpr (RES) {
+			if (params.res[ty] && in_picture) {  // (a uniform branch: the CTA's blocks belong to one task)
+#pragma unroll
+				for (int r = 0; r < 8; r++) store_residual_row(params.res[ty] + plane_off + origin + r * stride, make_uint4(0u, 0u, 0u, 0u));
+			}
+		}
 		if (KEEP && in_picture) reload_rows();
 		return;
 	}
@@ -470,6 +504,9 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		}
 #pragma unroll
 		for (int i = 0; i < 64; i++) v[i] = dc;
+	}
+	if constexpr (RES) {
+		if (params.res[ty]) store_residual(params.res[ty] + plane_off + origin, stride, v);
 	}
 
 	if (intra) {
@@ -572,7 +609,7 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 // The plain kernel's numbering: slot first_slot + tid of picture `ty`; `stage` = the CTA's staging area (one
 // WARP_STAGE per warp).  The 32 lanes of a warp hold 32 horizontally adjacent blocks of one plane row:
 // [luma top 2W | luma bottom 2W | Cb W | Cr W] per macroblock row.
-template <bool BIDIR = false, class PARAMS>
+template <bool BIDIR = false, bool RES = false, class PARAMS>
 __device__ __forceinline__ void reconstruct_block(const PARAMS &params, int ty, int first_slot, int tid, uint8_t *stage) {
 	const auto &t = params.t[ty];
 	const int W = t.mb_width;
@@ -594,7 +631,7 @@ __device__ __forceinline__ void reconstruct_block(const PARAMS &params, int ty, 
 		b = 4 + second;  // block 4 -> Cb plane, block 5 -> Cr plane (mpeg1.js:829-834, SURVEY Q8)
 	}
 	uint2 unused[8];
-	reconstruct_at<false, BIDIR>(params, ty, mb_row, mb_col, b, in_picture, tid & 31, stage + (tid >> 5) * WARP_STAGE, unused);
+	reconstruct_at<false, BIDIR, RES>(params, ty, mb_row, mb_col, b, in_picture, tid & 31, stage + (tid >> 5) * WARP_STAGE, unused);
 }
 
 #ifndef JSMPEG_WALK_EMU  // (a CTA-wide barrier: outside what the one-warp host emulation runs)
@@ -621,7 +658,7 @@ __device__ __forceinline__ uint32_t rgba_px(int y, int r, int g, int b) {
 	return c(y + r) | (c(y - g) << 8) | (c(y + b) << 16) | 0xff000000u;
 }
 
-template <bool BIDIR = false, class PARAMS>
+template <bool BIDIR = false, bool RES = false, class PARAMS>
 __device__ __forceinline__ void reconstruct_rgba_block(const PARAMS &params, const RgbaTarget &out, int ty, int mb_row, int first_mb_col,
                                                        int tid, uint8_t *stage, uint8_t (*chroma)[8][RGBA_MBS * 8]) {
 	const auto &t = params.t[ty];
@@ -636,7 +673,7 @@ __device__ __forceinline__ void reconstruct_rgba_block(const PARAMS &params, con
 	uint2 rows[8];
 #pragma unroll
 	for (int r = 0; r < 8; r++) rows[r] = make_uint2(0u, 0u);
-	reconstruct_at<true, BIDIR>(params, ty, mb_row, in_picture ? mb_col : 0, b, in_picture, lane, stage + warp * WARP_STAGE, rows);
+	reconstruct_at<true, BIDIR, RES>(params, ty, mb_row, in_picture ? mb_col : 0, b, in_picture, lane, stage + warp * WARP_STAGE, rows);
 	if (warp == 2) {
 		// plane 0 = Cb (block 4), plane 1 = Cr (block 5)
 #pragma unroll
