@@ -10,7 +10,9 @@ compiled reference and the CUDA path can be compared bit for bit on them:
   * macroblock_stuffing, macroblock_escape, long skipped runs in P pictures
   * every I and P macroblock type, quantiser changes, all coded_block_pattern values
   * forward_f_code 1..7, full_pel_forward_vector, all four half-pel parities, vector wrap-around,
-    always keeping the whole 17x17 / 9x9 reference footprint inside the coded planes (SURVEY Q11)
+    by default keeping the whole 17x17 / 9x9 reference footprint inside the coded planes (SURVEY Q11);
+    Knobs.vectors opens the rest of the vector domain: the f_code's whole range, footprints that wrap
+    from one row into the next, and taps outside the plane
   * intra DC sizes 0..8, DC-only blocks, the (0,1) first-coefficient form, long runs, index 63,
     escapes in the one- and two-byte forms, positive and negative
   * custom intra / non-intra quantiser matrices, extension and user data after the picture header,
@@ -105,6 +107,14 @@ class Knobs:
         self.b_skip_prob = 0.2
         self.b_intra_prob = 0.08
         self.b_f_codes = (1, 2, 3)
+        # Where motion vectors point (SURVEY Q11: prediction by flat index, a tap outside the plane zeroes its sample):
+        #   "inside"   small vectors (at most 24 half-pel) whose 17x17 / 9x9 footprints stay inside the 2-D planes
+        #   "wide"     the whole [-16f, 16f - 1] range of the picture's f_code, footprints inside the 2-D planes
+        #   "wrap"     footprints that cross the left or right edge with every tap's flat index inside its plane
+        #   "outside"  at least one tap outside its plane: mostly near misses, some far out
+        #   "mixed"    one of the four per macroblock
+        # "inside" draws exactly what it always drew: the streams of the committed cases stay byte-identical.
+        self.vectors = "inside"
         self.__dict__.update(kw)
 
 
@@ -256,17 +266,102 @@ class SynthStream:
         return target
 
     def pick_vector(self, mb_col, mb_row, f, full_pel):
-        """A predictor value (in the units the bitstream carries) whose luma AND chroma footprints
-        stay inside the coded planes."""
+        """A predictor value (in the units the bitstream carries) in the vector domain of Knobs.vectors; for "inside"
+        one whose luma AND chroma footprints stay inside the coded planes."""
         rng = self.rng
         lo, hi = -16 * f, 16 * f - 1
         scale = 2 if full_pel else 1
+        mode = self.k.vectors
+        if mode == "mixed":
+            mode = ("inside", "wide", "wrap", "outside")[int(rng.integers(0, 4))]
+        if mode != "inside":
+            return self._pick_in_domain(mode, mb_col, mb_row, lo, hi, scale)
         for _ in range(50):
             vx = int(rng.integers(max(lo, -24), min(hi, 24) + 1))
             vy = int(rng.integers(max(lo, -24), min(hi, 24) + 1))
             if self.footprint_inside(mb_col, mb_row, vx * scale, vy * scale):
                 return vx, vy
         return 0, 0
+
+    def _pick_in_domain(self, mode, mb_col, mb_row, lo, hi, scale):
+        """A predictor of domain "wide", "wrap" or "outside" (Knobs.vectors) for macroblock (mb_col, mb_row): targets
+        drawn around the plane edges the domain needs, kept when the predictor is representable and the domain's rule
+        holds."""
+        rng = self.rng
+        cw, ch = self.mbw * 16, self.mbh * 16
+        x_here, y_here = mb_col * 16, mb_row * 16
+
+        def unit(m):  # a half-pel target -> the predictor value that gives it, or None when out of range
+            v = m // scale
+            return v if lo <= v <= hi else None
+
+        def spread(here, size):  # a luma half-pel component anywhere the f_code reaches
+            return int(rng.integers(lo, hi + 1)) * scale if rng.random() < 0.3 else \
+                2 * (int(rng.integers(-here, size - here - 16 + 1))) + int(rng.integers(0, 2))
+
+        def edge(here, size, reach):  # a component that puts the footprint's first sample around an edge of one axis
+            at = int(rng.integers(-reach, 1)) if rng.random() < 0.5 else size - 16 + int(rng.integers(0, reach + 1))
+            return 2 * (at - here) + int(rng.integers(-1, 2))
+
+        for _ in range(60):
+            if mode == "wide":
+                mx, my, rule = spread(x_here, cw), spread(y_here, ch), "inside"
+            elif mode == "wrap":
+                mx = edge(x_here, cw, 17 if rng.random() < 0.8 else 40)
+                my = spread(y_here, ch) if rng.random() < 0.5 else 2 * int(rng.integers(-2, 3)) + int(rng.integers(0, 2))
+                rule = "wrap"
+            else:
+                kind, rule = rng.random(), "out"
+                if kind < 0.45:    # a row just past the top or bottom edge (the half-pel row, one row, chroma alone)
+                    mx = 2 * int(rng.integers(-3, 4)) + int(rng.integers(-1, 2))
+                    my = edge(y_here, ch, 2)
+                elif kind < 0.7:   # a column just past the left or right edge in the first or last rows
+                    mx = edge(x_here, cw, 2)
+                    my = edge(y_here, ch, 1) if rng.random() < 0.6 else \
+                        2 * int(rng.integers(-2, 3)) + int(rng.integers(-1, 2))
+                elif kind < 0.85:  # the chroma taps out, the luma ones inside (a wrap a row further for luma)
+                    mx = edge(x_here, cw, 40)
+                    my = 2 * int(rng.integers(-3, 4)) + int(rng.integers(-1, 2))
+                    rule = "chroma_out"
+                else:              # anywhere in the f_code's range
+                    mx, my = int(rng.integers(lo, hi + 1)) * scale, int(rng.integers(lo, hi + 1)) * scale
+            vx, vy = unit(mx), unit(my)
+            if vx is not None and vy is not None and self._obeys(rule, mb_col, mb_row, vx * scale, vy * scale):
+                return vx, vy
+        # a macroblock too far from the edges the domain needs: a "wide" vector instead
+        return self._pick_in_domain("wide", mb_col, mb_row, lo, hi, scale) if mode != "wide" else (0, 0)
+
+    def _obeys(self, rule, mb_col, mb_row, mx, my):
+        """Whether vector (mx, my) (luma half-pel units) at macroblock (mb_col, mb_row) follows `rule`: "inside" (both
+        footprints inside the 2-D planes), "wrap" (every flat-index tap inside, a footprint across the left or right
+        edge), "out" (some tap outside its plane) or "chroma_out" (the luma taps inside, some chroma tap outside)"""
+        if rule == "inside":
+            return self.footprint_inside(mb_col, mb_row, mx, my)
+        if rule == "wrap":
+            return self.flat_inside(mb_col, mb_row, mx, my) and not self.footprint_inside(mb_col, mb_row, mx, my)
+        if rule == "out":
+            return not self.flat_inside(mb_col, mb_row, mx, my)
+        return self.flat_inside(mb_col, mb_row, mx, my, "luma") and not self.flat_inside(mb_col, mb_row, mx, my, "chroma")
+
+    def flat_inside(self, mb_col, mb_row, mx, my, planes="both"):
+        """Vector (mx, my) in luma half-pel units at macroblock (mb_col, mb_row): every tap of the luma and of the chroma
+        prediction ("luma" / "chroma": of that one), addressed by flat index (a sample past a row's end is the next
+        row's first, mpeg1.js:479, 567), lies inside its plane."""
+        def plane(px, stride, size, h, v):
+            first = (mb_row * px + (v >> 1)) * stride + mb_col * px + (h >> 1)
+            return first >= 0 and first + (px - 1) * stride + px - 1 + (v & 1) * stride + (h & 1) < size
+        cw = self.mbw * 16
+        ysize = cw * self.mbh * 16
+        luma = planes == "chroma" or plane(16, cw, ysize, mx, my)
+        return luma and (planes == "luma" or plane(8, cw // 2, ysize // 4, int(mx / 2), int(my / 2)))
+
+    def skip_keeps_domain(self, mb_col, mb_row, mx, my):
+        """Whether a skipped B macroblock may repeat vector (mx, my) (luma half-pel units) under Knobs.vectors"""
+        if self.k.vectors in ("inside", "wide"):
+            return self.footprint_inside(mb_col, mb_row, mx, my)
+        if self.k.vectors == "wrap":
+            return self.flat_inside(mb_col, mb_row, mx, my)
+        return True
 
     def footprint_inside(self, mb_col, mb_row, mx, my):
         """Vector (mx, my) in luma half-pel units at macroblock (mb_col, mb_row): the luma and the chroma
@@ -404,9 +499,9 @@ class SynthStream:
                 want = int(min(rng.integers(1, self.k.max_skip + 1), last_mb - mb))
                 while skipped < want:
                     r2, c2 = divmod(mb + skipped, mbw)
-                    if last[0] and not self.footprint_inside(c2, r2, pf[0] * sf, pf[1] * sf):
+                    if last[0] and not self.skip_keeps_domain(c2, r2, pf[0] * sf, pf[1] * sf):
                         break
-                    if last[1] and not self.footprint_inside(c2, r2, pb[0] * sb, pb[1] * sb):
+                    if last[1] and not self.skip_keeps_domain(c2, r2, pb[0] * sb, pb[1] * sb):
                         break
                     skipped += 1
                 mb += skipped
@@ -547,8 +642,35 @@ B_CASES = {
 }
 
 
+# Streams over the whole motion-vector domain (Knobs.vectors), I/P and I/P/B, every macroblock of every picture coded
+# (no slice gaps).  The compiled reference decodes the I/P ones whose taps all lie inside the planes ("wide", "wrap"):
+# tests/golden/reference/decodes.json holds its decodes of them.
+VECTOR_CASES = {
+    "vec_wide_720p": dict(knobs=dict(width=1280, height=720, pictures=4, gop=4, slices="rows", f_codes=(4, 5, 6, 7),
+                                     full_pel_prob=0.3, vectors="wide"), seed=31),
+    "vec_wide_1080p": dict(knobs=dict(width=1920, height=1080, pictures=3, gop=3, slices="one", f_codes=(5, 6, 7),
+                                      full_pel_prob=0.3, vectors="wide"), seed=32),
+    "vec_wrap": dict(knobs=dict(width=176, height=144, pictures=6, gop=3, slices="rows", f_codes=(2, 3, 4, 5),
+                                full_pel_prob=0.3, vectors="wrap"), seed=33),
+    "vec_outside": dict(knobs=dict(width=112, height=80, pictures=6, gop=3, slices="random", f_codes=(1, 2, 3, 5, 7),
+                                   full_pel_prob=0.3, vectors="outside"), seed=34),
+    "vec_mixed": dict(knobs=dict(width=160, height=96, pictures=6, gop=3, slices="one", f_codes=(2, 3, 4, 6),
+                                 full_pel_prob=0.3, vectors="mixed"), seed=35),
+    "vec_wide_b": dict(knobs=dict(width=1280, height=720, pictures=7, gop=2, slices="rows", b_frames=2, f_codes=(4, 6),
+                                  b_f_codes=(5, 7), full_pel_prob=0.3, vectors="wide"), seed=36),
+    "vec_wrap_b": dict(knobs=dict(width=176, height=144, pictures=10, gop=2, slices="rows", b_frames=2,
+                                  f_codes=(2, 3, 4), b_f_codes=(3, 4, 5), full_pel_prob=0.3, b_skip_prob=0.35,
+                                  vectors="wrap"), seed=37),
+    "vec_outside_b": dict(knobs=dict(width=112, height=80, pictures=10, gop=2, slices="random", b_frames=2,
+                                     f_codes=(1, 3, 7), b_f_codes=(2, 4, 6), full_pel_prob=0.3, b_skip_prob=0.35,
+                                     vectors="outside"), seed=38),
+    "vec_mixed_b": dict(knobs=dict(width=160, height=96, pictures=10, gop=2, slices="one", b_frames=3, f_codes=(2, 4),
+                                   b_f_codes=(3, 5), full_pel_prob=0.3, b_skip_prob=0.35, vectors="mixed"), seed=39),
+}
+
+
 def make_case(name):
-    spec = CASES[name] if name in CASES else B_CASES[name]
+    spec = CASES[name] if name in CASES else (B_CASES[name] if name in B_CASES else VECTOR_CASES[name])
     return SynthStream(Knobs(**spec["knobs"]), spec["seed"]).generate()
 
 
