@@ -65,6 +65,24 @@ struct Parsed {
 	picture_info_t info;
 };
 
+// One plane set of a stream in HBM and what stage 2 writes beside it: the macroblock entries of its picture
+// (OUT_MACROBLOCKS, DESIGN 3.13) and, on the I/P sets, its accumulated map (OUT_ACCUMULATED, DESIGN 3.14).  A picture's
+// entries and map go where its planes go, so every ordering rule of the planes covers them.
+struct StreamSet {
+	DeviceBuffer<uint8_t> planes;
+	DeviceBuffer<uint8_t> entries;  // made zeroed on first use (reserve_entries)
+	DeviceBuffer<uint2> map;        // made on first use (reserve_maps)
+	// a call with the flag wrote `map` for the picture `planes` holds now; an unwritten map is never read as a trace's
+	// previous map
+	bool map_written = false;
+};
+
+// One slot of a stream's host ring (OUT_HOST): a picture's planes and, under OUT_MACROBLOCKS, its entries (made zeroed on
+// first use, reserve_entries)
+struct HostSlot {
+	PinnedBuffer<uint8_t> planes, entries;
+};
+
 struct Stream {
 	bitbuffer::Buffer bb;  // host bit buffer (pinned) -- src/wasm/buffer.c
 	// sequence header
@@ -84,27 +102,15 @@ struct Stream {
 	uint32_t scanned = 0;        // every prefix with pos + 2 < scanned is in `codes`
 	uint32_t scan_from = 0;      // the span a pending scan covers starts here
 	bool scan_pending = false;
-	// planes: two sets in HBM (ping-pong like mpeg1.js:221-246), a host ring for OUT_HOST
-	DeviceBuffer<uint8_t> d_planes[2];
-	int cur = 0;  // set written by the next I/P picture; forward = 1 - cur
-	PinnedBuffer<uint8_t> h_planes[HOST_RING];
+	// plane sets: 0 and 1 the I/P ping-pong (mpeg1.js:221-246); 2 and 3 the B-picture extension's ("decode_b"), made on
+	// the first B picture and written in turn -- a B picture is no reference, the ping-pong is untouched by it
+	StreamSet sets[4];
+	int cur = 0;    // I/P set written by the next I/P picture; forward = 1 - cur
+	int b_cur = 0;  // set 2 + b_cur is written by the next B picture
+	int last = 1;   // the set holding the most recently decoded picture (none yet: forward)
+	HostSlot ring[HOST_RING];
 	int h_head = -1;
-	// B-picture extension ("decode_b"): two more sets in HBM, written in turn -- a B picture is no reference, the
-	// ping-pong above is untouched by it; d_last = the set holding the most recently decoded picture
-	DeviceBuffer<uint8_t> d_planes_b[2];
-	int b_cur = 0;
-	uint8_t *d_last = nullptr;
 	int last_type = 0, last_temporal = 0;  // picture_coding_type / temporal_reference of the last picture decode() consumed
-	// macroblock entries (OUT_MACROBLOCKS, DESIGN 3.13): one buffer beside each plane set (d_mb[i] beside d_planes[i],
-	// d_mb_b[i] beside d_planes_b[i]) and one per host-ring slot, made zeroed on first use (reserve_entries).  A picture's
-	// entries go where its planes go, so every ordering rule of the planes covers them.
-	DeviceBuffer<uint8_t> d_mb[2], d_mb_b[2];
-	PinnedBuffer<uint8_t> h_mb[HOST_RING];
-	// accumulated maps (OUT_ACCUMULATED, DESIGN 3.14): d_acc[i] beside d_planes[i], made on first use (reserve_maps);
-	// acc_written[i]: a call with the flag wrote d_acc[i] for the picture d_planes[i] holds now.  An unwritten map is
-	// never read as a trace's previous map.
-	DeviceBuffer<uint2> d_acc[2];
-	bool acc_written[2] = {false, false};
 	// residual (OUT_RESIDUALS, DESIGN 3.15): that of the newest picture a call with the flag reconstructed, stored by
 	// stage 2 (ReconTask::res); made zeroed on first use (reserve_residuals)
 	DeviceBuffer<int16_t> d_res;
@@ -305,6 +311,14 @@ const uint8_t kDefaultIntraQ[64] = {8, 16, 19, 22, 26, 27, 29, 34, 16, 16, 22, 2
                                     22, 26, 27, 29, 32, 35, 40, 48, 26, 27, 29, 32, 35, 40, 48, 58,
                                     26, 27, 29, 34, 38, 46, 56, 69, 27, 29, 35, 38, 46, 56, 69, 83};
 
+// The planes of `set`, made zeroed on `st` (JS typed arrays start zeroed).  + coded_width + 64: stage 2's row loads may
+// touch (never use) up to one row past a plane set's end.
+void make_planes(const Stream &s, StreamSet &set, cudaStream_t st) {
+	const size_t bytes = (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64;
+	set.planes.reserve(bytes);
+	CUDA_CHECK(cudaMemsetAsync(set.planes.data(), 0, bytes, st));
+}
+
 // src/mpeg1.js:78-153 decodeSequenceHeader + initBuffers (first header only, mpeg1.c:812-819)
 void parse_sequence_header(Batch *b, Stream &s, uint32_t bit_index) {
 	HostBits hb{s.bb.bytes, s.bb.length, bit_index};
@@ -332,14 +346,10 @@ void parse_sequence_header(Batch *b, Stream &s, uint32_t bit_index) {
 	const size_t plane_bytes = (size_t)s.coded_size * 3 / 2;
 	s.d_seq.reserve(1);
 	CUDA_CHECK(cudaMemcpyAsync(s.d_seq.data(), &s.seq, sizeof(SeqParams), cudaMemcpyHostToDevice, b->st_main));
-	for (auto &p : s.d_planes) {
-		// + coded_width + 64: stage 2's row loads may touch (never use) up to one row past a plane set's end
-		p.reserve(plane_bytes + s.seq.coded_width + 64);
-		CUDA_CHECK(cudaMemsetAsync(p.data(), 0, plane_bytes + s.seq.coded_width + 64, b->st_main));  // JS typed arrays start zeroed
-	}
-	for (auto &p : s.h_planes) {
-		p.reserve(plane_bytes);
-		memset(p.data(), 0, plane_bytes);
+	for (int i = 0; i < 2; i++) make_planes(s, s.sets[i], b->st_main);  // the I/P sets
+	for (HostSlot &h : s.ring) {
+		h.planes.reserve(plane_bytes);
+		memset(h.planes.data(), 0, plane_bytes);
 	}
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));  // s.seq is read by the async copy
 }
@@ -608,10 +618,32 @@ void copy_batch(Batch *b, std::vector<void *> &dst, std::vector<void *> &src, st
 		for (size_t i = 0; i < n_copy; i++) CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], size[i], cudaMemcpyDefault, st));
 }
 
-// The reconstruct tasks of one step of decode() (or one depth of decode_chains), queued by launch_reconstruct; the
-// export of their macroblock entries (OUT_MACROBLOCKS: `entries`, one launch of export_macroblocks_kernel over
-// `entry_mb` macroblocks); the accumulated maps of its I/P pictures (OUT_ACCUMULATED: `maps`, one launch of
-// accumulate_kernel over `map_warps` warps); and the copies of its pictures that follow them
+// What stage 1 left in record `slot`, as its readers (stage 2, the coefficient export) take it: the macroblock records,
+// the dense coefficient records and the compact coefficient plane
+struct SlotRecords {
+	const mb_record_t *hdr;
+	const int16_t *coef;
+	const coef_record_t *compact;
+};
+SlotRecords slot_records(const Batch *b, int slot) {
+	return {b->d_hdr.data() + (size_t)slot * b->slot_mb, b->d_coef.data() + (size_t)slot * b->slot_mb * MB_COEF_INT16,
+	        compact_plane(b->d_stage.data() + (size_t)slot * stage_entries_for(b->slot_mb) * 4)};  // (stage 1b wrote it: parse_task)
+}
+
+// Room for `n` tasks in the pinned task table `h` and its device copy `d`; the reads of the device copy queued on
+// `reader` finish before it is reallocated
+template <typename T>
+void reserve_tasks(PinnedBuffer<T> &h, DeviceBuffer<T> &d, size_t n, cudaStream_t reader) {
+	if (n <= d.size()) return;
+	CUDA_CHECK(cudaStreamSynchronize(reader));
+	h.reserve(n);
+	d.reserve(n);
+}
+
+// One step of stage 2 (run_steps): the reconstruct tasks of one step of decode() (or one depth of run_chains), queued
+// by launch_reconstruct; the export of their macroblock entries (OUT_MACROBLOCKS: `entries`, one launch of
+// export_macroblocks_kernel over `entry_mb` macroblocks); accumulated maps (OUT_ACCUMULATED, decode_accumulated:
+// `maps`, one launch of accumulate_kernel over `map_warps` warps); and the copies of its pictures that follow them
 struct ReconStep {
 	std::vector<ReconTask> tasks;
 	std::vector<MbExportTask> entries;
@@ -630,27 +662,24 @@ struct ReconStep {
 		entries.push_back(MbExportTask{t.hdr, to, entry_mb, t.mb_size, type, 0});
 		entry_mb += (uint32_t)t.mb_size;
 	}
-	// the map of task t's I/P picture into `to`, one depth step from `prev` (nullptr: no previous map)
-	void map(const ReconTask &t, const uint2 *prev, uint2 *to) {
-		maps.push_back(AccTask{t.hdr, t.coef, t.compact, prev, to, map_warps, t.mb_width, t.mb_size / t.mb_width});
-		map_warps += res_export_warps(t.mb_size);
+	// the map of the I/P picture whose records are `sr` (of a stream with sequence parameters `seq`) into `to`, one depth
+	// step from `prev` (nullptr: no previous map)
+	void map(const SlotRecords &sr, const SeqParams &seq, const uint2 *prev, uint2 *to) {
+		maps.push_back(AccTask{sr.hdr, sr.coef, sr.compact, prev, to, map_warps, seq.mb_width, seq.mb_height});
+		map_warps += res_export_warps(seq.mb_size);
 	}
 };
 
 // The tasks `list` of all `steps` (ReconStep::entries, ReconStep::maps) go up in one copy on the reconstruct stream,
 // through the pinned table `h` into `d`; returns where each step's tasks begin in `d`.  The previous upload's readers are
-// done before the pinned table is written again: decode_round ends with its reconstruction complete, and run_chains'
+// done before the pinned table is written again: every call ends with its reconstruction complete, and run_chains'
 // next wave waits for ev_round.
 template <typename T>
 std::vector<const T *> upload_step_tasks(Batch *b, const std::vector<ReconStep> &steps, std::vector<T> ReconStep::*list,
                                          PinnedBuffer<T> &h, DeviceBuffer<T> &d) {
 	size_t n = 0;
 	for (const ReconStep &r : steps) n += (r.*list).size();
-	if (n > d.size()) {
-		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-		h.reserve(n);
-		d.reserve(n);
-	}
+	reserve_tasks(h, d, n, b->st_recon);
 	std::vector<const T *> at;
 	size_t m = 0;
 	for (const ReconStep &r : steps) {
@@ -661,32 +690,6 @@ std::vector<const T *> upload_step_tasks(Batch *b, const std::vector<ReconStep> 
 	return at;
 }
 
-// OUT_MACROBLOCKS: the export tasks of all `steps` (upload_step_tasks)
-std::vector<const MbExportTask *> upload_entry_tasks(Batch *b, const std::vector<ReconStep> &steps) {
-	return upload_step_tasks(b, steps, &ReconStep::entries, b->h_etasks, b->d_etasks);
-}
-
-// OUT_ACCUMULATED: the accumulate tasks of all `steps` (upload_step_tasks), in decode_accumulated's table: that call
-// ends with its launches complete
-std::vector<const AccTask *> upload_map_tasks(Batch *b, const std::vector<ReconStep> &steps) {
-	return upload_step_tasks(b, steps, &ReconStep::maps, b->h_atasks, b->d_atasks);
-}
-
-// The step's export launch, queued behind its reconstruct launch (`tasks`: upload_entry_tasks); returns the launches
-int launch_step_entries(Batch *b, const ReconStep &r, const MbExportTask *tasks) {
-	if (r.entries.empty()) return 0;
-	launch_export_macroblocks(tasks, (int)r.entries.size(), r.entry_mb, b->st_recon);
-	return 1;
-}
-
-// The step's accumulate launch, queued behind its reconstruct launch (`tasks`: upload_map_tasks); returns the launches.
-// A map the step reads as `prev` was written by an earlier step, on the same stream.
-int launch_step_maps(Batch *b, const ReconStep &r, const AccTask *tasks) {
-	if (r.maps.empty()) return 0;
-	launch_accumulate(tasks, (int)r.maps.size(), r.map_warps, b->st_recon);
-	return 1;
-}
-
 // The copy-out of one step's pictures (OUT_HOST) on the copy stream, behind the step's launches
 void copy_out_step(Batch *b, ReconStep &r) {
 	CUDA_CHECK(cudaEventRecord(b->ev_step, b->st_recon));
@@ -694,6 +697,43 @@ void copy_out_step(Batch *b, ReconStep &r) {
 	copy_batch(b, r.dst, r.src, r.size, b->st_copy);  // all pictures of the step leave in one batched copy call
 	CUDA_CHECK(cudaEventRecord(b->ev_copied[b->copy_steps & 1], b->st_copy));
 	b->copy_steps++;
+}
+
+// Stage 2 of decode_round and of a run_chains wave: `steps`, one after the other on the reconstruct stream.  Every step's
+// export and accumulate tasks go up in one copy per table (upload_step_tasks, before ev_recon[0]); then, behind the
+// latest stage-1 wave (ev_b: the records are final; where the host waited for the wave, an ordering already met) and
+// between ev_recon[0] and ev_recon[1] (decode()'s recon_ms), each step's reconstruct, export and accumulate launch,
+// those it has tasks for, and its copies: with `copy_out` on the copy stream (copy_out_step), else on the reconstruct
+// stream.  The record slots stay until ev_round.  Returns the kernels launched.
+int run_steps(Batch *b, std::vector<ReconStep> &steps, bool copy_out) {
+	const std::vector<const MbExportTask *> entries = upload_step_tasks(b, steps, &ReconStep::entries, b->h_etasks, b->d_etasks);
+	const std::vector<const AccTask *> maps = upload_step_tasks(b, steps, &ReconStep::maps, b->h_atasks, b->d_atasks);
+	CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_b, 0));
+	CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
+	int launches = 0;
+	for (size_t i = 0; i < steps.size(); i++) {
+		ReconStep &r = steps[i];
+		// A launch overwrites, per stream, the plane set written two of that stream's pictures ago, i.e. by a launch
+		// at least two copy-out launches back: the copy-out recorded two launches ago must be done (the copy stream is
+		// in order, so that covers every earlier one).  The same holds for the set's entries.
+		if (copy_out && b->copy_steps >= 2) CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_copied[b->copy_steps & 1], 0));
+		if (!r.tasks.empty()) launches += launch_reconstruct(r.tasks.data(), (int)r.tasks.size(), b->st_recon);
+		if (!r.entries.empty()) {
+			launch_export_macroblocks(entries[i], (int)r.entries.size(), r.entry_mb, b->st_recon);
+			launches++;
+		}
+		if (!r.maps.empty()) {  // (a map a step reads as `prev` was written by an earlier step)
+			launch_accumulate(maps[i], (int)r.maps.size(), r.map_warps, b->st_recon);
+			launches++;
+		}
+		if (r.dst.empty()) continue;
+		if (copy_out) copy_out_step(b, r);  // while the next step reconstructs
+		else copy_batch(b, r.dst, r.src, r.size, b->st_recon);
+	}
+	CUDA_CHECK(cudaEventRecord(b->ev_recon[1], b->st_recon));
+	CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
+	b->recon_pending = true;
+	return launches;
 }
 
 // The header of the picture whose start code is at byte `pos` (ISO 11172-2 2.4.2.5); fields whose bytes are not in the
@@ -840,18 +880,6 @@ int parse_wave(Batch *b, const std::vector<WaveItem> &wave, bool expand, bool ea
 	return launches;
 }
 
-// What stage 1 left in record `slot`, as its readers (stage 2, the coefficient export) take it: the macroblock records,
-// the dense coefficient records and the compact coefficient plane
-struct SlotRecords {
-	const mb_record_t *hdr;
-	const int16_t *coef;
-	const coef_record_t *compact;
-};
-SlotRecords slot_records(const Batch *b, int slot) {
-	return {b->d_hdr.data() + (size_t)slot * b->slot_mb, b->d_coef.data() + (size_t)slot * b->slot_mb * MB_COEF_INT16,
-	        compact_plane(b->d_stage.data() + (size_t)slot * stage_entries_for(b->slot_mb) * 4)};  // (stage 1b wrote it: parse_task)
-}
-
 // The reconstruct task of a picture of `s` whose records are in `slot`: written into the plane set at `cur`, predicted
 // from `fwd` (and, for a B picture, `bwd`), with the fused RGBA conversion into `rgba` unless that is nullptr
 ReconTask recon_task(const Batch *b, const Stream &s, int slot, uint8_t *cur, uint8_t *fwd, uint8_t *bwd, uint8_t *rgba) {
@@ -883,46 +911,35 @@ uint8_t *stream_rgba(Batch *b, Stream &s) {
 	return s.d_rgba.data();
 }
 
-// The stream's two B-picture sets, made zeroed on first use (+ coded_width + 64: parse_sequence_header's slack)
+// The stream's two B-picture sets, made zeroed on first use
 void reserve_b_sets(Batch *b, Stream &s) {
-	if (s.d_planes_b[0].data()) return;
-	const size_t bytes = (size_t)s.coded_size * 3 / 2 + s.seq.coded_width + 64;
-	for (auto &pb : s.d_planes_b) {
-		pb.reserve(bytes);
-		CUDA_CHECK(cudaMemsetAsync(pb.data(), 0, bytes, b->st_recon));
-	}
+	if (s.sets[2].planes.data()) return;
+	for (int i = 2; i < 4; i++) make_planes(s, s.sets[i], b->st_recon);
 }
 
 // The stream's entry buffers (OUT_MACROBLOCKS), made on first use: every plane set's, zeroed on the reconstruct stream,
 // and every host-ring slot's
 void reserve_entries(Batch *b, Stream &s) {
-	if (s.d_mb[0].data()) return;
+	if (s.sets[0].entries.data()) return;
 	const size_t bytes = (size_t)s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t);
-	for (DeviceBuffer<uint8_t> *e : {&s.d_mb[0], &s.d_mb[1], &s.d_mb_b[0], &s.d_mb_b[1]}) {
-		e->reserve(bytes);
-		CUDA_CHECK(cudaMemsetAsync(e->data(), 0, bytes, b->st_recon));
+	for (StreamSet &set : s.sets) {
+		set.entries.reserve(bytes);
+		CUDA_CHECK(cudaMemsetAsync(set.entries.data(), 0, bytes, b->st_recon));
 	}
-	for (auto &h : s.h_mb) {
-		h.reserve(bytes);
-		memset(h.data(), 0, bytes);
+	for (HostSlot &h : s.ring) {
+		h.entries.reserve(bytes);
+		memset(h.entries.data(), 0, bytes);
 	}
 }
 
-// The entry buffer beside plane set `set`, one of the stream's four (reserve_entries made them)
-uint8_t *set_entries(const Stream &s, const uint8_t *set) {
-	for (int i = 0; i < 2; i++) {
-		if (set == s.d_planes[i].data()) return s.d_mb[i].data();
-		if (set == s.d_planes_b[i].data()) return s.d_mb_b[i].data();
-	}
-	throw std::logic_error("jsmpeg_b200: a plane set without an entry buffer");
-}
-
-// The stream's two maps (OUT_ACCUMULATED), made on first use, unwritten: nothing reads them before a call with the flag
-// writes them, or get / read_accumulated fills them untraced (fill_untraced)
+// The maps of the stream's two I/P sets (OUT_ACCUMULATED), made on first use, unwritten: nothing reads them before a
+// call with the flag writes them, or get / read_accumulated fills them untraced (fill_untraced)
 void reserve_maps(Stream &s) {
-	if (s.d_acc[0].data()) return;
-	for (auto &m : s.d_acc) m.reserve((size_t)s.coded_size * 3 / 2);
-	s.acc_written[0] = s.acc_written[1] = false;
+	if (s.sets[0].map.data()) return;
+	for (int i = 0; i < 2; i++) {
+		s.sets[i].map.reserve((size_t)s.coded_size * 3 / 2);
+		s.sets[i].map_written = false;
+	}
 }
 
 // The stream's residual (OUT_RESIDUALS), made zeroed on the reconstruct stream on first use
@@ -934,11 +951,66 @@ int16_t *reserve_residuals(Batch *b, Stream &s) {
 	return s.d_res.data();
 }
 
-// Which of the two maps is beside I/P plane set `set`
-int set_map(const Stream &s, const uint8_t *set) {
-	for (int i = 0; i < 2; i++)
-		if (set == s.d_planes[i].data()) return i;
-	throw std::logic_error("jsmpeg_b200: an I/P plane set without a map");
+// Where a task is in a list of steps: steps[step].tasks[task]; step -1: nowhere
+struct TaskAt {
+	int step = -1, task = 0;
+};
+
+// Picture `e` of stream `s`, records in `slot`, consumed by decode() or by a seek, reconstructed by step `step` of
+// `steps` into the stream's own sets with decode()'s rotation; `visible`: the call leaves it in get_planes (decode():
+// every picture it consumes, a seek: each chain's last).  Beside its planes go, under OUT_MACROBLOCKS, its entries and,
+// for an I/P picture, under OUT_ACCUMULATED its map (else the set's map no longer matches it); the visible picture also
+// goes to the stream's RGBA under OUT_RGBA and, under OUT_HOST, with its entries to the next slot of its host ring.
+// `newest` gets where its task is (OUT_RESIDUALS: the caller's newest picture stores its residual).  Returns the bytes
+// its copies bring to the host.
+uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, size_t step, int slot, const picture_info_t &e,
+                         int flags, bool visible, TaskAt &newest) {
+	const bool is_b = e.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
+	uint8_t *rgba = visible && (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
+	ReconTask t;
+	if (is_b) {
+		// `cur` holds the older and `1 - cur` the newer of the two most recent I/P pictures: the B picture's forward
+		// (past) and backward (future) reference.  It goes to a set of its own.
+		reserve_b_sets(b, s);
+		s.last = 2 + s.b_cur;
+		t = recon_task(b, s, slot, s.sets[s.last].planes.data(), s.sets[s.cur].planes.data(), s.sets[1 - s.cur].planes.data(), rgba);
+		s.b_cur ^= 1;  // no reference: the I/P ping-pong stays as it is
+	} else {
+		s.last = s.cur;
+		t = recon_task(b, s, slot, s.sets[s.cur].planes.data(), s.sets[1 - s.cur].planes.data(), nullptr, rgba);
+		s.cur ^= 1;  // mpeg1.js:221-246: the picture just decoded becomes `forward`
+	}
+	StreamSet &set = s.sets[s.last];
+	if (steps.size() <= step) steps.emplace_back();
+	ReconStep &r = steps[step];
+	r.tasks.push_back(t);
+	newest = {(int)step, (int)r.tasks.size() - 1};
+	if (flags & JSMPEG_B200_OUT_MACROBLOCKS) {
+		reserve_entries(b, s);
+		r.entry(t, e.picture_type, set.entries.data());
+	}
+	if (!is_b) {  // the map beside the set, one depth step from the map beside the forward set
+		if (flags & JSMPEG_B200_OUT_ACCUMULATED) {
+			reserve_maps(s);
+			const StreamSet &fwd = s.sets[s.cur];  // (swapped above)
+			r.map(slot_records(b, slot), s.seq, fwd.map_written ? fwd.map.data() : nullptr, set.map.data());
+		}
+		set.map_written = (flags & JSMPEG_B200_OUT_ACCUMULATED) != 0;
+	}
+	uint64_t host_bytes = 0;
+	if (visible && (flags & JSMPEG_B200_OUT_HOST)) {
+		s.h_head = (s.h_head + 1) % HOST_RING;
+		HostSlot &h = s.ring[s.h_head];
+		const size_t planes = (size_t)s.coded_size * 3 / 2;
+		r.copy(h.planes.data(), t.cur.y, planes);
+		host_bytes += planes;
+		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) {
+			const size_t n = (size_t)s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t);
+			r.copy(h.entries.data(), set.entries.data(), n);
+			host_bytes += n;
+		}
+	}
+	return host_bytes;
 }
 
 // Every record of `n_rec` from `map` untraced {0, 0, 0, -1}, on `st`
@@ -1009,6 +1081,7 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 		if (!more[si]) continue;
 		Stream &s = b->streams[si];
 		size_t step = 0;
+		TaskAt newest;
 		while (progress[si] < want[si]) {
 			const uint32_t from_byte = (s.bb.index + 7) >> 3;
 			auto it = std::lower_bound(s.pics.begin(), s.pics.end(), from_byte);
@@ -1032,50 +1105,9 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			// (0 unless both of its bytes are in the buffer)
 			s.last_temporal = (uint64_t)e.pos + 5 < s.bb.length ? picture_header(s, e.pos).temporal_reference : 0;
 			if (e.info.status == PIC_DECODED) {
-				const bool is_b = e.info.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
-				uint8_t *rgba = (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
-				ReconTask t;
-				if (is_b) {
-					// after the swaps `cur` holds the older and `1 - cur` the newer of the two most recent I/P pictures:
-					// the B picture's forward (past) and backward (future) reference.  It goes to a set of its own.
-					reserve_b_sets(b, s);
-					t = recon_task(b, s, e.slot, s.d_planes_b[s.b_cur].data(), s.d_planes[s.cur].data(), s.d_planes[1 - s.cur].data(), rgba);
-					s.b_cur ^= 1;  // no reference: the I/P ping-pong stays as it is
-				} else {
-					t = recon_task(b, s, e.slot, s.d_planes[s.cur].data(), s.d_planes[1 - s.cur].data(), nullptr, rgba);
-					s.cur ^= 1;  // mpeg1.js:221-246: the picture just decoded becomes `forward`
-				}
-				s.d_last = t.cur.y;
+				b->stats.d2h_bytes += consume_picture(b, s, steps, step++, e.slot, e.info, flags, true, newest);
+				const bool is_b = e.info.picture_type == 3;
 				const uint64_t planes = (uint64_t)s.coded_size * 3 / 2;
-				if (steps.size() <= step) steps.emplace_back();
-				steps[step].tasks.push_back(t);
-				uint8_t *entries = nullptr;
-				if (flags & JSMPEG_B200_OUT_MACROBLOCKS) {  // beside the planes, in the set's entry buffer
-					reserve_entries(b, s);
-					entries = set_entries(s, t.cur.y);
-					steps[step].entry(t, e.info.picture_type, entries);
-				}
-				if (!is_b) {  // the map beside the set, one depth step from the map beside the forward set
-					const int set = 1 - s.cur;  // (swapped above)
-					if (flags & JSMPEG_B200_OUT_ACCUMULATED) {
-						reserve_maps(s);
-						steps[step].map(t, s.acc_written[1 - set] ? s.d_acc[1 - set].data() : nullptr, s.d_acc[set].data());
-						s.acc_written[set] = true;
-					} else {
-						s.acc_written[set] = false;  // the set's new picture has no map
-					}
-				}
-				if (flags & JSMPEG_B200_OUT_HOST) {  // into the next slot of the stream's host ring
-					s.h_head = (s.h_head + 1) % HOST_RING;
-					steps[step].copy(s.h_planes[s.h_head].data(), t.cur.y, planes);
-					b->stats.d2h_bytes += planes;
-					if (entries) {
-						const size_t n = (size_t)s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t);
-						steps[step].copy(s.h_mb[s.h_head].data(), entries, n);
-						b->stats.d2h_bytes += n;
-					}
-				}
-				step++;
 				b->stats.pictures_decoded++;
 				b->stats.coded_blocks += e.info.n_coded_blocks;
 				b->stats.macroblocks += e.info.n_present;
@@ -1086,38 +1118,17 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			// this round's expand on the main stream
 			release_slot(b, e.slot);
 		}
-		// OUT_RESIDUALS: the stream's last reconstructed picture of the round (the newest task of its last step) stores its
-		// residual; the earlier ones of the round could not be observed
-		if ((flags & JSMPEG_B200_OUT_RESIDUALS) && step > 0) steps[step - 1].tasks.back().res = reserve_residuals(b, s);
+		// OUT_RESIDUALS: the stream's last reconstructed picture of the round stores its residual; the earlier ones of the
+		// round could not be observed
+		if ((flags & JSMPEG_B200_OUT_RESIDUALS) && newest.step >= 0)
+			steps[newest.step].tasks[newest.task].res = reserve_residuals(b, s);
 	}
 	lap(b->trace.consume, t);
-	// ---- 4. reconstruction, one step after the other on the reconstruct stream, behind the wave's expand: the host has
-	// consumed the infos and queues the launches while the expand of the biggest pictures is still running
+	// ---- 4. reconstruction, behind the wave's expand: the host has consumed the infos and queues the launches while the
+	// expand of the biggest pictures is still running.  Every step reconstructs.
 	if (!steps.empty()) {
-		std::vector<const MbExportTask *> entry_tasks;
-		std::vector<const AccTask *> map_tasks;
-		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) entry_tasks = upload_entry_tasks(b, steps);  // (outside recon_ms)
-		if (flags & JSMPEG_B200_OUT_ACCUMULATED) map_tasks = upload_map_tasks(b, steps);
-		if (!wave.empty()) CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_b, 0));
-		CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
-		for (size_t i = 0; i < steps.size(); i++) {
-			ReconStep &r = steps[i];
-			// A launch overwrites, per stream, the plane set written two of that stream's pictures ago, i.e. by
-			// a launch at least two copy-out launches back: the copy-out recorded two launches ago must be done
-			// (the copy stream is in order, so that covers every earlier one).  The same holds for the set's entries.
-			if ((flags & JSMPEG_B200_OUT_HOST) && b->copy_steps >= 2)
-				CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_copied[b->copy_steps & 1], 0));
-			b->stats.kernel_launches += launch_reconstruct(r.tasks.data(), (int)r.tasks.size(), b->st_recon);
-			b->stats.recon_launches++;
-			// the step's records are final here (st_recon waited for ev_b) and stay until the next round's parse (ev_round)
-			if (!entry_tasks.empty()) b->stats.kernel_launches += launch_step_entries(b, r, entry_tasks[i]);
-			// (the maps stay in HBM: no copy-out reads them)
-			if (!map_tasks.empty()) b->stats.kernel_launches += launch_step_maps(b, r, map_tasks[i]);
-			if (flags & JSMPEG_B200_OUT_HOST) copy_out_step(b, r);  // while the next step reconstructs
-		}
-		CUDA_CHECK(cudaEventRecord(b->ev_recon[1], b->st_recon));
-		CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
-		b->recon_pending = true;
+		b->stats.kernel_launches += run_steps(b, steps, (flags & JSMPEG_B200_OUT_HOST) != 0);
+		b->stats.recon_launches += steps.size();
 	}
 	lap(b->trace.stage2, t);
 	// ---- 5. the round ends with its wave complete (a round that reconstructs nothing has not waited for its expand yet)
@@ -1291,7 +1302,7 @@ struct Chain {
 	int req_lo, req_hi;    // its requests: order[req_lo .. req_hi)
 	int req_next;          // the first of them not consumed yet
 	int n_sets;            // sets from the caller's pool: 0 (a leaf: its one picture goes to its destination), 2, 4
-	uint8_t *set[4];
+	uint8_t *set[4];       // (seek_pictures: none, its chains use their streams' sets)
 	int cur, b_cur;        // as Stream::cur / b_cur
 	const uint2 *map;      // decode_accumulated: the map of the newest reference picture (nullptr: none yet)
 	uint32_t next;         // the picture decode() consumes next; beyond `last`: the chain is done
@@ -1343,7 +1354,7 @@ struct ChainWork {
 	// picture e of chain `ch` (stream s) is consumed and decoded, the d-th of its chain in this wave: records in `slot`,
 	// named by requests order[q_lo .. q_hi)
 	virtual void picture(Chain &ch, const Stream &s, int slot, const picture_info_t &e, size_t d, int q_lo, int q_hi) = 0;
-	// the wave's depths, one after the other on the reconstruct stream
+	// the wave's depths, one after the other on the reconstruct stream (run_steps)
 	virtual void depths() = 0;
 	virtual ~ChainWork() = default;
 };
@@ -1361,7 +1372,7 @@ struct SetPool {
 // decode()'s rule (b_walk: B pictures go to the B walk, as decode_b; else they are skipped after their header) and
 // handed to `work` by depth (depth d: the d-th decoded picture of every chain of the wave).  Chains run in groups of at
 // most a wave's slots.  With a `pool`, each chain's sets come from it, a group's within half of the free device memory
-// -- a request beyond the device is cut into groups, not refused; without one, the caller has filled Chain::set.  The
+// -- a request beyond the device is cut into groups, not refused; without one, `work` uses sets of its own.  The
 // requests are valid (the caller checked them); on return the work is queued on the reconstruct stream, and the infos
 // are the consumed pictures'.
 RequestInfo run_chains(Batch *b, const std::vector<PictureRequest> &req, const std::vector<int> &order,
@@ -1437,10 +1448,8 @@ RequestInfo run_chains(Batch *b, const std::vector<PictureRequest> &req, const s
 					ch.next = next_picture(s, e);
 				}
 			}
-			// ---- stage 2, then the slots go back: the next wave's parse waits for ev_round
+			// ---- stage 2 (run_steps), then the slots go back: the next wave's parse waits for ev_round
 			work.depths();
-			CUDA_CHECK(cudaEventRecord(b->ev_round, b->st_recon));
-			b->recon_pending = true;
 			for (const WaveItem &w : wave) release_slot(b, w.slot);
 		}
 	}
@@ -1481,10 +1490,7 @@ struct PlaneWork : ChainWork {
 	}
 	// (a set is overwritten two references later, by a later launch on the same stream)
 	void depths() override {
-		for (ReconStep &dp : steps) {
-			launch_reconstruct(dp.tasks.data(), (int)dp.tasks.size(), b->st_recon);
-			if (!dp.dst.empty()) copy_batch(b, dp.dst, dp.src, dp.size, b->st_recon);
-		}
+		run_steps(b, steps, false);
 		steps.clear();
 	}
 };
@@ -1613,21 +1619,9 @@ void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *
 	for (int i = 0; i < n; i++)
 		uniq_of[i] = std::lower_bound(uniq.begin(), uniq.end(), std::make_pair(req[i].stream, req[i].pic)) - uniq.begin();
 	free_slots_for(b, uniq.size());
-	if (dst && (size_t)n > b->d_xtasks.size()) {
-		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-		b->h_xtasks.reserve(n);
-		b->d_xtasks.reserve(n);
-	}
-	if (coef_dst && (size_t)n > b->d_ctasks.size()) {
-		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-		b->h_ctasks.reserve(n);
-		b->d_ctasks.reserve(n);
-	}
-	if (res_dst && (size_t)n > b->d_rtasks.size()) {
-		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
-		b->h_rtasks.reserve(n);
-		b->d_rtasks.reserve(n);
-	}
+	if (dst) reserve_tasks(b->h_xtasks, b->d_xtasks, n, b->st_main);
+	if (coef_dst) reserve_tasks(b->h_ctasks, b->d_ctasks, n, b->st_main);
+	if (res_dst) reserve_tasks(b->h_rtasks, b->d_rtasks, n, b->st_main);
 	const size_t wave_max = b->free_slots.size();
 	RequestInfo out(n);
 	for (size_t lo = 0; lo < uniq.size(); lo += wave_max) {
@@ -1718,8 +1712,7 @@ struct MapWork : ChainWork {
 	Batch *b;
 	const std::vector<int> &order;
 	void *const *acc_dst;
-	std::vector<std::vector<AccTask>> tasks;  // per depth
-	std::vector<ReconStep> copies;           // per depth: its copy lists (no reconstruct task)
+	std::vector<ReconStep> steps;  // per depth: its maps and copies, no reconstruct task
 	MapWork(Batch *b, const std::vector<int> &order, void *const *acc_dst) : b(b), order(order), acc_dst(acc_dst) {}
 	void picture(Chain &ch, const Stream &s, int slot, const picture_info_t &, size_t d, int q_lo, int q_hi) override {
 		uint2 *out;
@@ -1729,37 +1722,14 @@ struct MapWork : ChainWork {
 			out = reinterpret_cast<uint2 *>(ch.set[ch.cur]);
 			ch.cur ^= 1;
 		}
-		const SlotRecords sr = slot_records(b, slot);
-		if (tasks.size() <= d) {
-			tasks.emplace_back();
-			copies.emplace_back();
-		}
-		tasks[d].push_back(AccTask{sr.hdr, sr.coef, sr.compact, ch.map, out, 0, s.seq.mb_width, s.seq.mb_height});
+		if (steps.size() <= d) steps.emplace_back();
+		steps[d].map(slot_records(b, slot), s.seq, ch.map, out);
 		ch.map = out;
-		for (int q = q_lo + 1; q < q_hi; q++) copies[d].copy(acc_dst[order[q]], out, (size_t)s.coded_size * 12);
+		for (int q = q_lo + 1; q < q_hi; q++) steps[d].copy(acc_dst[order[q]], out, (size_t)s.coded_size * 12);
 	}
-	// every depth's tasks in one upload (the previous wave's launches have read theirs: parse_wave waited for ev_round)
 	void depths() override {
-		size_t m = 0;
-		for (auto &dt : tasks) {
-			uint32_t warps = 0;
-			for (AccTask &t : dt) {
-				t.first = warps;
-				warps += res_export_warps(t.mb_width * t.mb_height);
-				b->h_atasks[m++] = t;
-			}
-		}
-		CUDA_CHECK(cudaMemcpyAsync(b->d_atasks.data(), b->h_atasks.data(), m * sizeof(AccTask), cudaMemcpyHostToDevice, b->st_recon));
-		size_t off = 0;
-		for (size_t d = 0; d < tasks.size(); d++) {
-			const AccTask &last = tasks[d].back();
-			launch_accumulate(b->d_atasks.data() + off, (int)tasks[d].size(), last.first + res_export_warps(last.mb_width * last.mb_height),
-			                  b->st_recon);
-			off += tasks[d].size();
-			if (!copies[d].dst.empty()) copy_batch(b, copies[d].dst, copies[d].src, copies[d].size, b->st_recon);
-		}
-		tasks.clear();
-		copies.clear();
+		run_steps(b, steps, false);
+		steps.clear();
 	}
 };
 
@@ -1770,16 +1740,10 @@ void decode_accumulated(Batch *b, const std::vector<PictureRequest> &req, void *
 	ensure_pool(b);
 	std::vector<int> order;
 	std::vector<Chain> chains = make_chains(b, req, order);
-	size_t set_bytes = 0, n_tasks = 0;
+	size_t set_bytes = 0;
 	for (Chain &c : chains) {
 		c.n_sets = c.n_sets ? 2 : 0;  // (no B picture is requested)
 		set_bytes = std::max(set_bytes, ((size_t)b->streams[c.stream].coded_size * 12 + 255) & ~(size_t)255);
-		n_tasks += c.info.size();
-	}
-	if (n_tasks > b->d_atasks.size()) {  // (a wave's tasks are at most the chains' pictures)
-		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
-		b->h_atasks.reserve(n_tasks);
-		b->d_atasks.reserve(n_tasks);
 	}
 	MapWork work(b, order, acc_dst);
 	// (a scratch set is read only after the chain wrote it)
@@ -1820,69 +1784,33 @@ long batch_decode_accumulated(Batch *b, int n, const int *streams, const uint32_
 
 // ---- seek_pictures: move decode() of chosen streams to a listed picture, each from its seek chain start (DESIGN 3.12)
 
-// Each chain reconstructs into its stream's own sets (set[0..1] the I/P sets, set[2..3] the B sets) with decode()'s
-// rotation, one launch_reconstruct per depth, and under OUT_MACROBLOCKS one export launch per depth into the sets'
-// entry buffers.  The last picture a chain consumes -- picture k, or on damaged input the picture whose walk ran across
-// k -- is, when decoded, also written to the stream's RGBA under OUT_RGBA and copied (with its entries under
-// OUT_MACROBLOCKS) to the next slot of its host ring under OUT_HOST (copy_out_step).  No later launch of the call
-// writes its set.
+// Each chain is consumed by decode()'s consume_picture into its stream's own sets, with the stream's rotation.  The last
+// picture a chain consumes -- picture k, or on damaged input the picture whose walk ran across k -- is the visible one.
+// No later launch of the call writes its set.
 struct SeekWork : ChainWork {
 	Batch *b;
 	int flags;
-	std::vector<uint8_t *> last;  // per stream: the set of the newest picture the call reconstructed (nullptr: none)
 	std::vector<ReconStep> steps;
-	// OUT_RESIDUALS: per stream, its newest picture of the wave as (depth, task index), depth -1: none yet
-	std::vector<std::pair<int, int>> newest;
-	SeekWork(Batch *b, int flags) : b(b), flags(flags), last(b->streams.size(), nullptr), newest(b->streams.size(), {-1, 0}) {}
+	std::vector<TaskAt> newest;  // per stream: its newest picture of the wave (OUT_RESIDUALS)
+	SeekWork(Batch *b, int flags) : b(b), flags(flags), newest(b->streams.size()) {}
 	void picture(Chain &ch, const Stream &, int slot, const picture_info_t &e, size_t d, int, int) override {
 		Stream &s = b->streams[ch.stream];
-		const bool is_b = e.picture_type == 3;
-		const bool final = next_picture(s, e) > ch.last;
-		uint8_t *rgba = final && (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
-		const ReconTask t = is_b ? recon_task(b, s, slot, ch.set[2 + ch.b_cur], ch.set[ch.cur], ch.set[1 - ch.cur], rgba)
-		                         : recon_task(b, s, slot, ch.set[ch.cur], ch.set[1 - ch.cur], nullptr, rgba);
-		if (is_b) ch.b_cur ^= 1;
-		else ch.cur ^= 1;
-		last[ch.stream] = t.cur.y;
-		if (steps.size() <= d) steps.emplace_back();
-		steps[d].tasks.push_back(t);
-		newest[ch.stream] = {(int)d, (int)steps[d].tasks.size() - 1};
-		uint8_t *entries = (flags & JSMPEG_B200_OUT_MACROBLOCKS) ? set_entries(s, t.cur.y) : nullptr;
-		if (entries) steps[d].entry(t, e.picture_type, entries);
-		if (!is_b && (flags & JSMPEG_B200_OUT_ACCUMULATED)) {  // as decode_round, over the stream's own sets
-			const int set = set_map(s, t.cur.y);
-			steps[d].map(t, s.acc_written[1 - set] ? s.d_acc[1 - set].data() : nullptr, s.d_acc[set].data());
-			s.acc_written[set] = true;
-		}
-		if (final && (flags & JSMPEG_B200_OUT_HOST)) {
-			s.h_head = (s.h_head + 1) % HOST_RING;
-			steps[d].copy(s.h_planes[s.h_head].data(), t.cur.y, (size_t)s.coded_size * 3 / 2);
-			if (entries) steps[d].copy(s.h_mb[s.h_head].data(), entries, (size_t)s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t));
-		}
+		consume_picture(b, s, steps, d, slot, e, flags, next_picture(s, e) > ch.last, newest[ch.stream]);  // (no stats)
 	}
 	void depths() override {
-		std::vector<const MbExportTask *> entry_tasks;
-		std::vector<const AccTask *> map_tasks;
-		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) entry_tasks = upload_entry_tasks(b, steps);
-		if (flags & JSMPEG_B200_OUT_ACCUMULATED) map_tasks = upload_map_tasks(b, steps);
 		for (size_t si = 0; si < newest.size(); si++) {  // as decode_round: each stream's newest picture of the wave
-			if ((flags & JSMPEG_B200_OUT_RESIDUALS) && newest[si].first >= 0)
-				steps[newest[si].first].tasks[newest[si].second].res = b->streams[si].d_res.data();  // (seek_pictures made it)
-			newest[si].first = -1;
+			if ((flags & JSMPEG_B200_OUT_RESIDUALS) && newest[si].step >= 0)
+				steps[newest[si].step].tasks[newest[si].task].res = reserve_residuals(b, b->streams[si]);
+			newest[si] = {};
 		}
-		for (size_t i = 0; i < steps.size(); i++) {
-			launch_reconstruct(steps[i].tasks.data(), (int)steps[i].tasks.size(), b->st_recon);
-			if (!entry_tasks.empty()) launch_step_entries(b, steps[i], entry_tasks[i]);
-			if (!map_tasks.empty()) launch_step_maps(b, steps[i], map_tasks[i]);
-			if (!steps[i].dst.empty()) copy_out_step(b, steps[i]);
-		}
+		run_steps(b, steps, (flags & JSMPEG_B200_OUT_HOST) != 0);
 		steps.clear();
 	}
 };
 
-// run_chains over the named streams' own plane sets, zeroed first, then the commit of what decode() observes: the bit
-// index, the set rotation, the newest picture, last_picture and the flushed look-ahead.  The requests are valid and
-// name distinct streams (the caller checked them).
+// run_chains over the named streams' own plane sets, zeroed first with the rotation started over, then the commit of
+// what else decode() observes: the bit index, last_picture and the flushed look-ahead.  The requests are valid and name
+// distinct streams (the caller checked them).
 void seek_pictures(Batch *b, std::vector<PictureRequest> &req, int flags, int32_t *status_out, int32_t *n_present_out,
                    int32_t *error_out) {
 	ensure_pool(b);
@@ -1896,18 +1824,16 @@ void seek_pictures(Batch *b, std::vector<PictureRequest> &req, int flags, int32_
 		Stream &s = b->streams[c.stream];
 		flush_cache(b, s);
 		if (b->decode_b) reserve_b_sets(b, s);
-		uint8_t *sets[4] = {s.d_planes[0].data(), s.d_planes[1].data(), s.d_planes_b[0].data(), s.d_planes_b[1].data()};
-		for (int k = 0; k < 4; k++) {
-			c.set[k] = sets[k];
-			if (sets[k]) CUDA_CHECK(cudaMemsetAsync(sets[k], 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
-		}
-		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) {  // the fresh decoder's entries, like its planes: 0 until written
-			reserve_entries(b, s);
-			for (DeviceBuffer<uint8_t> *e : {&s.d_mb[0], &s.d_mb[1], &s.d_mb_b[0], &s.d_mb_b[1]})
-				CUDA_CHECK(cudaMemsetAsync(e->data(), 0, e->size(), b->st_recon));
-		}
+		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) reserve_entries(b, s);
 		if (flags & JSMPEG_B200_OUT_ACCUMULATED) reserve_maps(s);
-		s.acc_written[0] = s.acc_written[1] = false;  // the fresh decoder's sets hold no picture yet
+		for (StreamSet &set : s.sets) {  // the fresh decoder's sets: zeroed planes, entries 0 until written, no map
+			if (set.planes.data()) CUDA_CHECK(cudaMemsetAsync(set.planes.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_recon));
+			if (flags & JSMPEG_B200_OUT_MACROBLOCKS)
+				CUDA_CHECK(cudaMemsetAsync(set.entries.data(), 0, set.entries.size(), b->st_recon));
+			set.map_written = false;
+		}
+		s.cur = s.b_cur = 0;
+		s.last = 1;
 		if (flags & JSMPEG_B200_OUT_RESIDUALS) {  // 0 unless the chain reconstructs a picture, like the entries
 			reserve_residuals(b, s);
 			CUDA_CHECK(cudaMemsetAsync(s.d_res.data(), 0, s.d_res.size() * sizeof(int16_t), b->st_recon));
@@ -1922,9 +1848,6 @@ void seek_pictures(Batch *b, std::vector<PictureRequest> &req, int flags, int32_
 		for (uint32_t next; (next = next_picture(s, c.info[k - c.first])) <= c.last;) k = next;
 		const picture_info_t &e = c.info[k - c.first];
 		s.bb.index = e.end_bit;
-		s.cur = c.cur;
-		s.b_cur = c.b_cur;
-		s.d_last = work.last[c.stream];
 		s.last_type = e.picture_type;
 		s.last_temporal = (uint64_t)s.pics[k] + 5 < s.bb.length ? picture_header(s, s.pics[k]).temporal_reference : 0;
 		const int i = order[c.req_lo];  // (one request per chain)
@@ -1977,7 +1900,7 @@ long write_index(Batch *b, int stream, Listing what, uint32_t *picture_out, uint
 
 // The planes of the stream's most recent picture: `forward` (mpeg1.c:841-851); with the B-picture extension it may be a
 // B picture's own set
-PlaneSet latest_planes(const Stream &s) { return plane_set(s, s.d_last ? s.d_last : s.d_planes[1 - s.cur].data()); }
+PlaneSet latest_planes(const Stream &s) { return plane_set(s, s.sets[s.last].planes.data()); }
 
 int env_int(const char *name, int fallback) {
 	const char *e = getenv(name);
@@ -2343,22 +2266,18 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 			forget_index(b, s);
 			s.bb.length = 0;
 			s.bb.index = 0;
-			s.cur = 0;
-			s.b_cur = 0;
-			s.d_last = nullptr;
+			s.cur = s.b_cur = 0;
+			s.last = 1;
 			s.last_type = s.last_temporal = 0;
 			s.h_head = -1;
 			s.seq_floor = 0;
-			if (s.has_seq) {
-				for (auto &p : s.d_planes) CUDA_CHECK(cudaMemsetAsync(p.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_main));
-				for (auto &p : s.d_planes_b) if (p.data()) CUDA_CHECK(cudaMemsetAsync(p.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_main));
+			for (StreamSet &set : s.sets) {  // (zeroed sets: no picture, no map)
+				if (set.planes.data()) CUDA_CHECK(cudaMemsetAsync(set.planes.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_main));
+				if (set.entries.data()) CUDA_CHECK(cudaMemsetAsync(set.entries.data(), 0, set.entries.size(), b->st_main));
+				set.map_written = false;
 			}
-			if (s.d_mb[0].data()) {  // (made after the sequence header, by a call with OUT_MACROBLOCKS)
-				for (DeviceBuffer<uint8_t> *e : {&s.d_mb[0], &s.d_mb[1], &s.d_mb_b[0], &s.d_mb_b[1]})
-					CUDA_CHECK(cudaMemsetAsync(e->data(), 0, e->size(), b->st_main));
-				for (auto &h : s.h_mb) memset(h.data(), 0, h.size());
-			}
-			s.acc_written[0] = s.acc_written[1] = false;  // (zeroed sets: no picture, no map)
+			for (HostSlot &h : s.ring)
+				if (h.entries.data()) memset(h.entries.data(), 0, h.entries.size());
 			if (s.d_res.data()) CUDA_CHECK(cudaMemsetAsync(s.d_res.data(), 0, s.d_res.size() * sizeof(int16_t), b->st_main));
 		}
 		CUDA_CHECK(cudaStreamSynchronize(b->st_main));
@@ -2452,7 +2371,7 @@ int jsmpeg_b200_batch_get_planes(jsmpeg_b200_batch_t *b, int stream, void **y, v
 int jsmpeg_b200_batch_get_host_planes(jsmpeg_b200_batch_t *b, int stream, void **y, void **cr, void **cb) {
 	const Stream &s = b->streams[stream];
 	if (!s.has_seq) return -1;
-	PlaneSet p = plane_set(s, s.h_planes[s.h_head < 0 ? 0 : s.h_head].data());
+	PlaneSet p = plane_set(s, s.ring[s.h_head < 0 ? 0 : s.h_head].planes.data());
 	if (y) *y = p.y;
 	if (cr) *cr = p.cr;
 	if (cb) *cb = p.cb;
@@ -2522,7 +2441,7 @@ int jsmpeg_b200_batch_read_rgba(jsmpeg_b200_batch_t *b, int stream, void *rgba) 
 static Stream *entries_stream(Batch *b, int stream) {
 	if (stream < 0 || stream >= (int)b->streams.size() || !b->streams[stream].has_seq) return nullptr;
 	Stream &s = b->streams[stream];
-	if (!s.d_mb[0].data()) {
+	if (!s.sets[0].entries.data()) {
 		use_device(b);
 		reserve_entries(b, s);
 		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
@@ -2534,7 +2453,7 @@ int jsmpeg_b200_batch_get_macroblocks(jsmpeg_b200_batch_t *b, int stream, void *
 	return guarded<int>(b, -1, [&] {
 		const Stream *s = entries_stream(b, stream);
 		if (!s) return -1;
-		if (entries) *entries = set_entries(*s, latest_planes(*s).y);
+		if (entries) *entries = s->sets[s->last].entries.data();
 		return 0;
 	});
 }
@@ -2543,7 +2462,7 @@ int jsmpeg_b200_batch_read_macroblocks(jsmpeg_b200_batch_t *b, int stream, void 
 	return guarded<int>(b, -1, [&] {
 		const Stream *s = entries_stream(b, stream);
 		if (!s) return -1;
-		if (dst) CUDA_CHECK(cudaMemcpy(dst, set_entries(*s, latest_planes(*s).y), (size_t)s->seq.mb_size * sizeof(jsmpeg_b200_macroblock_t),
+		if (dst) CUDA_CHECK(cudaMemcpy(dst, s->sets[s->last].entries.data(), (size_t)s->seq.mb_size * sizeof(jsmpeg_b200_macroblock_t),
 		                               cudaMemcpyDeviceToHost));
 		return 0;
 	});
@@ -2553,7 +2472,7 @@ int jsmpeg_b200_batch_get_host_macroblocks(jsmpeg_b200_batch_t *b, int stream, v
 	return guarded<int>(b, -1, [&] {
 		const Stream *s = entries_stream(b, stream);
 		if (!s) return -1;
-		if (entries) *entries = s->h_mb[s->h_head < 0 ? 0 : s->h_head].data();
+		if (entries) *entries = s->ring[s->h_head < 0 ? 0 : s->h_head].entries.data();
 		return 0;
 	});
 }
@@ -2597,12 +2516,12 @@ static uint2 *newest_map(Batch *b, int stream) {
 	Stream &s = b->streams[stream];
 	use_device(b);
 	reserve_maps(s);
-	const int set = 1 - s.cur;
-	if (!s.acc_written[set]) {  // (the earlier calls have synchronised their streams)
-		fill_untraced(s.d_acc[set].data(), s.d_acc[set].size(), b->st_recon);
+	StreamSet &set = s.sets[1 - s.cur];
+	if (!set.map_written) {  // (the earlier calls have synchronised their streams)
+		fill_untraced(set.map.data(), set.map.size(), b->st_recon);
 		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
 	}
-	return s.d_acc[set].data();
+	return set.map.data();
 }
 
 int jsmpeg_b200_batch_get_accumulated(jsmpeg_b200_batch_t *b, int stream, void **map) {

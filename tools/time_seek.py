@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Seeking decode() (BatchDecoder.seek_pictures) against the other ways to reach the same pictures.
 
-    python tools/time_seek.py [--reps 5] [--long-frames 600] [--seeks 50] [--out FILE]
+    python tools/time_seek.py [--reps 5] [--long-frames 600] [--seeks 50] [--flags 0] [--out FILE]
 
 (a) the bench's 64 distinct 1080p x 60-picture clips: every stream seeks to a seeded random listed P picture k (with
     16 listed pictures after it) in one call, then decode(16).  Timed: the seek alone; the seek + decode(16);
@@ -10,9 +10,10 @@
     set_index to the chain start j, then decode() k - j + 1 times (all 64 one after the other).
 (b) one 1080p stream of `long_frames` pictures: `seeks` seeded seeks to listed pictures, one call each, against
     set_index to the chain start and sequential decode() up to the picture, for each of them.
-Every call returns after a device synchronise, so a host clock around it measures it.  Best of `reps` after a warm-up
-round.  One more seek of (a) runs under torch.profiler for the stage split (tools/time_pictures.py).  The card's name
-and power limit are read in the same process.
+Every seek passes `flags` (jsmpeg_b200.batch's OUT_* bits; default 0, OUT_DEVICE).  Every call returns after a device
+synchronise, so a host clock around it measures it.  Best of `reps` after a warm-up round.  One more seek of (a) runs
+under torch.profiler for the stage split (tools/time_pictures.py).  The card's name and power limit are read in the
+same process.
 """
 from __future__ import annotations
 
@@ -35,6 +36,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--long-frames", type=int, default=600)
     ap.add_argument("--seeks", type=int, default=50)
+    ap.add_argument("--flags", type=int, default=0, help="OUT_* bits of every seek, e.g. 5 = OUT_HOST | OUT_MACROBLOCKS")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
 
@@ -42,7 +44,7 @@ def main():
     import gen_streams
     from jsmpeg_b200.batch import OUT_DEVICE, BatchDecoder
 
-    result = {"card": card(), "reps": args.reps}
+    result = {"card": card(), "reps": args.reps, "flags": args.flags}
     rng = random.Random(2026)
 
     # (a) 64 clips, one seek each, then 16 pictures
@@ -59,7 +61,7 @@ def main():
     following = [(s, p) for s, (_, _, after) in enumerate(targets) for p in after]
 
     def seek_and_play():
-        assert bd.seek_pictures(seeks) == len(seeks)
+        assert bd.seek_pictures(seeks, args.flags) == len(seeks)
         assert bd.decode(16, OUT_DEVICE) == 16 * len(seeks)
 
     singles = []
@@ -75,12 +77,12 @@ def main():
 
     leg_a = {"streams": len(clips), "clip": f"{bench.WIDTH}x{bench.HEIGHT}x{bench.PICTURES}",
              "chain_pictures": sum(k - j + 1 for k, j, _ in targets),
-             "seek": timed(lambda: bd.seek_pictures(seeks), args.reps),
+             "seek": timed(lambda: bd.seek_pictures(seeks, args.flags), args.reps),
              "seek_then_decode_16": timed(seek_and_play, args.reps),
              "decode_pictures_same_64": timed(lambda: bd.decode_pictures(seeks), args.reps),
              "decode_pictures_same_1024": dict(timed(lambda: bd.decode_pictures(following), args.reps), pictures=len(following)),
              "set_index_and_decode_per_stream": timed(without_the_call, args.reps)}
-    leg_a["seek"]["split"] = stage_split(lambda: bd.seek_pictures(seeks))
+    leg_a["seek"]["split"] = stage_split(lambda: bd.seek_pictures(seeks, args.flags))
     for one, _ in singles:
         one.close()
     bd.close()
@@ -96,7 +98,7 @@ def main():
 
     def seek_each():
         for e in picks:
-            assert bd.seek_pictures([(0, e["picture"])]) == 1
+            assert bd.seek_pictures([(0, e["picture"])], args.flags) == 1
 
     def sequential_each():
         for e in picks:
