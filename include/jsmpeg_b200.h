@@ -520,8 +520,8 @@ int jsmpeg_b200_batch_read_accumulated(jsmpeg_b200_batch_t *b, int stream, void 
  * that decoder reconstructed nothing).
  *
  * Only the stream's newest picture's residual can be observed, so decode(n) with the flag stores it only for the last
- * picture each stream reconstructs in each of its rounds; a consumer that wants every picture's residual calls
- * decode(1) with the flag.  The residual is not copied to the host ring: at coded_size * 3 bytes per picture its
+ * picture each stream reconstructs in each of its rounds; a consumer that wants every picture's residual gives
+ * jsmpeg_b200_batch_decode_frames residual destinations (below).  The residual is not copied to the host ring: at coded_size * 3 bytes per picture its
  * consumer is a model on the same GPU.  Nothing else decode() observes changes: planes, RGBA, host ring, entries, maps,
  * bit index, last_picture and the stats, but kernel_launches as described there.
  *
@@ -530,6 +530,50 @@ int jsmpeg_b200_batch_read_accumulated(jsmpeg_b200_batch_t *b, int stream, void 
 int jsmpeg_b200_batch_get_residuals(jsmpeg_b200_batch_t *b, int stream, void **res);
 /* Synchronous copy of the residual into caller memory (coded_size * 3 bytes), like read_planes. */
 int jsmpeg_b200_batch_read_residuals(jsmpeg_b200_batch_t *b, int stream, void *dst);
+
+/* EVERY PICTURE OF decode(n) (clip loaders for training, video walls, compressed-domain models): decode(n) reconstructs
+ * up to n pictures of every stream, but afterwards only the last one of each can be seen.  decode_frames does exactly
+ * what jsmpeg_b200_batch_decode(b, n_pictures, flags) does and returns the same value, and also gives each picture it
+ * reconstructs a destination of its own in caller device memory, written by stage 2 beside the planes: no copy-out per
+ * picture and no decode(1) loop.
+ *
+ * FRAME j of stream s is the j-th picture the call reconstructs for s (PIC_DECODED: I and P pictures, B pictures under
+ * decode_b), in consumption (coded) order; a skipped picture has none, although decode() returns true for it.
+ * n_frames_out[s] (<= n_pictures) counts them.  Each destination array has one pointer per stream to device memory,
+ * 16-byte aligned; frame j is at
+ *   planes_dst[s] + j * coded_size * 3 / 2 bytes: what read_planes gives right after the decode() that consumed the
+ *       picture (Y | Cr | Cb) -- on damaged streams too, where absent macroblocks keep the plane set's older content;
+ *   rgba_dst[s] + j * width * height * 4 bytes: what read_rgba gives after that decode() had it run with OUT_RGBA (the
+ *       odd edge opaque white);
+ *   res_dst[s] + j * coded_size * 3 / 2 int16: byte for byte what decode_residuals writes for the picture (the residual
+ *       OUT_RESIDUALS stores);
+ *   mb_dst[s] + j * mb_size jsmpeg_b200_macroblock_t: byte for byte what decode_macroblocks writes for it.
+ * Any of the four arrays may be NULL, and so may any entry of them: the stream then gets no frames of that kind.  Memory
+ * past frame n_frames_out[s] - 1 is left untouched.  info_out (NULL: none) has n_streams * n_pictures entries, stream
+ * s's frame j at s * n_pictures + j; n_frames_out (NULL: none) has n_streams.
+ *
+ * Per 1080p frame (1920 x 1088 coded, 120 x 68 macroblocks): planes 3,133,440 bytes, RGBA 8,294,400, residual 6,266,880,
+ * macroblock entries 130,560 -- so 64 streams x 60 planar frames take about 12 GB.
+ *
+ * Everything decode() observes afterwards is what decode() leaves: planes, RGBA, host ring, entries, maps, residual,
+ * bit index, last_picture and the stats, but kernel_launches (a step's reconstruct kernel with a frame is cut into
+ * launches of its FRAME variant's capacity: 63 plain, 51 RGBA, 56 B, 46 B + RGBA tasks).  The flags keep their meaning
+ * for decode()'s own buffers: with OUT_RGBA and an RGBA frame the stream's RGBA ends as its last frame, with
+ * OUT_RESIDUALS and a residual frame the stream's residual ends as its last frame's; an RGBA frame without OUT_RGBA
+ * leaves get_rgba as it was.
+ *
+ * Synchronous.  Returns what decode() returns; -1 for a dead batch; -2, before any work and with nothing changed, when
+ * n_pictures < 0 or a destination is not 16-byte aligned. */
+typedef struct jsmpeg_b200_frame_t {
+	uint32_t byte_pos;          /* the picture's start code in the stream's buffer (the index calls' byte_pos) */
+	int16_t picture_type;       /* 1 I, 2 P, 3 B (decode_b) */
+	int16_t temporal_reference; /* as jsmpeg_b200_batch_last_picture */
+	int32_t n_present, error;   /* picture_info_t.n_present / .error, as decode_pictures reports them */
+} jsmpeg_b200_frame_t;          /* 16 bytes */
+
+long jsmpeg_b200_batch_decode_frames(jsmpeg_b200_batch_t *b, int n_pictures, int flags, void *const *planes_dst,
+                                     void *const *rgba_dst, void *const *res_dst, void *const *mb_dst,
+                                     jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out);
 
 /* SEEK (players, video walls, clip loaders): move decode() of chosen streams to a chosen picture each, and play on from
  * there with decode() -- OUT_HOST, OUT_RGBA and the host ring as usual -- without stepping the other streams.  The

@@ -31,6 +31,12 @@ class Stats(ctypes.Structure):
         return {name: getattr(self, name) for name, _ in self._fields_}
 
 
+class Frame(ctypes.Structure):
+    """jsmpeg_b200_frame_t: what decode_frames reports per frame (16 bytes)."""
+    _fields_ = [("byte_pos", ctypes.c_uint32), ("picture_type", ctypes.c_int16), ("temporal_reference", ctypes.c_int16),
+                ("n_present", ctypes.c_int32), ("error", ctypes.c_int32)]
+
+
 _VP = ctypes.c_void_p
 _BATCH_ABI = {
     "jsmpeg_b200_batch_create": (_VP, [ctypes.c_int, ctypes.c_int, ctypes.c_uint]),
@@ -64,6 +70,8 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_read_accumulated": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
     "jsmpeg_b200_batch_get_residuals": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(_VP)]),
     "jsmpeg_b200_batch_read_residuals": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
+    "jsmpeg_b200_batch_decode_frames": (ctypes.c_long, [_VP, ctypes.c_int, ctypes.c_int, _VP, _VP, _VP, _VP,
+                                                        ctypes.POINTER(Frame), _VP]),
     "jsmpeg_b200_batch_last_picture": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_batch_intra_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
@@ -150,6 +158,7 @@ class BatchDecoder:
         self.last_residuals_info = []  # per request of the last decode_residuals: {"n_present", "error"}
         self.last_accumulated_info = []  # per request of the last decode_accumulated: {"status", "n_present", "error"}
         self.last_seek_info = []  # per request of the last seek_pictures: {"status", "n_present", "error"}
+        self.last_frames_batch = {}  # per kind of the last decode_frames: its [S, n, ...] tensor when the streams share one geometry
         self.handle = self.lib.jsmpeg_b200_batch_create(n_streams, device, max_slots)
         err = self.lib.jsmpeg_b200_batch_last_error(self.handle)
         if err:  # no usable CUDA device: the C ABI answers "false" for ever; the Python host says so loudly
@@ -301,6 +310,70 @@ class BatchDecoder:
 
     def decode(self, n_pictures=1, flags=OUT_DEVICE):
         return self.lib.jsmpeg_b200_batch_decode(self.handle, n_pictures, flags)
+
+    _FRAME_KINDS = ("planes", "rgba", "residuals", "macroblocks")
+
+    def decode_frames(self, n_pictures, flags=OUT_DEVICE, planes=True, rgba=False, residuals=False, macroblocks=False):
+        """decode(n_pictures, flags) that also hands back every picture it reconstructs (include/jsmpeg_b200.h,
+        jsmpeg_b200_batch_decode_frames): frame j of a stream is the j-th picture the call reconstructs for it (I and P,
+        and B under decode_b; skipped pictures have none), in coded order.  Returns per stream a dict with "n_frames",
+        "info" (per frame {"byte_pos", "type", "temporal_reference", "n_present", "error", "pts"}, pts as in
+        intra_index) and each kind asked for, a CUDA tensor cut to n_frames: "planes" uint8 [F, coded_size * 3 // 2]
+        (see planes_view), "rgba" uint8 [F, height, width, 4], "residuals" int16 [F, coded_size * 3 // 2],
+        "macroblocks" uint8 [F, mb_height, mb_width, 16] (see macroblocks_view); None for a stream without a sequence
+        header.  When every stream has one and all share one geometry, each kind is allocated as one [S, n_pictures,
+        ...] tensor (last_frames_batch[kind]; RGBA only where a stream's n_pictures images are a multiple of 16 bytes) and
+        the per-stream tensors are views of it: a clip batch without a gather."""
+        import torch
+        n = int(n_pictures)
+        if n < 0:
+            raise ValueError("n_pictures must be >= 0")
+        dev = torch.device("cuda", self.device)
+        infos = [self.stream_info(s) for s in range(self.n_streams)]
+        want = {"planes": planes, "rgba": rgba, "residuals": residuals, "macroblocks": macroblocks}
+
+        def shape(kind, info):
+            cs, w, h = info["coded_size"], info["width"], info["height"]
+            return {"planes": (cs * 3 // 2,), "rgba": (h, w, 4), "residuals": (cs * 3 // 2,),
+                    "macroblocks": ((h + 15) // 16, (w + 15) // 16, MACROBLOCK_BYTES)}[kind]
+
+        dtype = {"planes": torch.uint8, "rgba": torch.uint8, "residuals": torch.int16, "macroblocks": torch.uint8}
+        geometries = {(i["width"], i["height"]) for i in infos}
+        shared = all(i["has_sequence_header"] for i in infos) and len(geometries) == 1
+        full, self.last_frames_batch = {}, {}
+        for kind in self._FRAME_KINDS:
+            if not want[kind]:
+                continue
+            slab = n * int(np.prod(shape(kind, infos[0]))) * dtype[kind].itemsize
+            if shared and slab % 16 == 0:  # (every stream's frame 0 16-byte aligned)
+                self.last_frames_batch[kind] = t = torch.empty((self.n_streams, n, *shape(kind, infos[0])), dtype=dtype[kind], device=dev)
+                full[kind] = list(t.unbind(0))
+            else:  # (torch's allocations are 512-byte aligned)
+                full[kind] = [torch.empty((n, *shape(kind, i)), dtype=dtype[kind], device=dev) if i["has_sequence_header"] else None
+                              for i in infos]
+        S = max(self.n_streams, 1)
+        dst = {kind: (_VP * S)(*[t.data_ptr() if t is not None and n else None for t in full[kind]]) for kind in full}
+        info_out = (Frame * max(self.n_streams * n, 1))()
+        n_frames = (ctypes.c_int32 * S)()
+        if full:
+            torch.cuda.current_stream(dev).synchronize()  # the allocations are the caller's stream's; the call uses its own
+        got = self.lib.jsmpeg_b200_batch_decode_frames(self.handle, n, int(flags), dst.get("planes"), dst.get("rgba"),
+                                                       dst.get("residuals"), dst.get("macroblocks"), info_out, n_frames)
+        if got == -2:
+            raise ValueError("decode_frames refused its arguments")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_frames failed")
+        out = []
+        for s in range(self.n_streams):
+            f = n_frames[s]
+            rows = [info_out[s * n + j] for j in range(f)]
+            d = {"n_frames": f, "info": [{"byte_pos": r.byte_pos, "type": r.picture_type, "temporal_reference": r.temporal_reference,
+                                          "n_present": r.n_present, "error": r.error, "pts": self._pts(s, r.byte_pos)} for r in rows]}
+            for kind in full:
+                t = full[kind][s]
+                d[kind] = None if t is None else t[:f]
+            out.append(d)
+        return out
 
     def device_planes(self, stream):
         y, cr, cb = _VP(), _VP(), _VP()

@@ -114,6 +114,7 @@ struct ReconTask {
 	int32_t width, height;
 	PlaneSet bwd;   // B picture (the opt-in extension): the newer of the two most recent I/P pictures
 	int16_t *res;   // OUT_RESIDUALS: the picture's residual, coded_size * 3 / 2 int16 in the planes' layout, or nullptr
+	uint8_t *frame; // decode_frames: a second copy of the picture's planes (coded_size * 3 / 2 bytes), or nullptr
 };
 
 // kernel launchers (defined in scan.cu / parse.cu / recon.cu)
@@ -152,8 +153,9 @@ int launch_parse_pictures(WalkKind kind, const ParseTask *tasks, int n_tasks, in
 // (tasks with `rgba`), then B pictures (tasks with `bwd`: prediction from two references), then B pictures with the
 // conversion; each kernel's tasks in their order.  `tasks_host` is read on the host at launch time: the table travels
 // in the kernel parameters.  When any task of a kernel has `res`, all that kernel's tasks go to its RES variant, which
-// also stores the residual of every task with `res` (the others ride along with none).  Returns the number of kernels
-// launched.
+// also stores the residual of every task with `res` (the others ride along with none); when any has `frame`, they go to
+// its FRAME variant instead, which stores both the residual and the planar frame of every task that has one.  Returns
+// the number of kernels launched.
 int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream);
 
 // Macroblock export (macroblocks.cu): request i converts the records of one picture (`mb_size` of them at `src`, a

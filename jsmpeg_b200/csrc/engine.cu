@@ -956,17 +956,30 @@ struct TaskAt {
 	int step = -1, task = 0;
 };
 
+// decode_frames (DESIGN 3.16): where one stream's frames go -- each destination nullptr or the stream's frame 0 in device
+// memory, `info` its row of the caller's info_out on the host -- and how many the call has given it so far
+struct FrameCursor {
+	uint8_t *planes = nullptr, *rgba = nullptr, *mb = nullptr;
+	int16_t *res = nullptr;
+	jsmpeg_b200_frame_t *info = nullptr;
+	int n = 0;
+};
+
 // Picture `e` of stream `s`, records in `slot`, consumed by decode() or by a seek, reconstructed by step `step` of
 // `steps` into the stream's own sets with decode()'s rotation; `visible`: the call leaves it in get_planes (decode():
 // every picture it consumes, a seek: each chain's last).  Beside its planes go, under OUT_MACROBLOCKS, its entries and,
 // for an I/P picture, under OUT_ACCUMULATED its map (else the set's map no longer matches it); the visible picture also
 // goes to the stream's RGBA under OUT_RGBA and, under OUT_HOST, with its entries to the next slot of its host ring.
-// `newest` gets where its task is (OUT_RESIDUALS: the caller's newest picture stores its residual).  Returns the bytes
-// its copies bring to the host.
+// `newest` gets where its task is (OUT_RESIDUALS: the caller's newest picture stores its residual).  With a `frame`
+// cursor (decode_frames) the picture is the stream's next frame: stage 2 also stores its planes, and its RGBA and
+// residual go to that frame instead of the stream's own, and its entries are also exported there.  Returns the bytes its
+// copies bring to the host.
 uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, size_t step, int slot, const picture_info_t &e,
-                         int flags, bool visible, TaskAt &newest) {
+                         int flags, bool visible, TaskAt &newest, FrameCursor *frame = nullptr) {
 	const bool is_b = e.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
-	uint8_t *rgba = visible && (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
+	const size_t j = frame ? (size_t)frame->n++ : 0, planes = (size_t)s.coded_size * 3 / 2;
+	uint8_t *rgba = frame && frame->rgba ? frame->rgba + j * s.width * s.height * 4
+	                : visible && (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
 	ReconTask t;
 	if (is_b) {
 		// `cur` holds the older and `1 - cur` the newer of the two most recent I/P pictures: the B picture's forward
@@ -980,6 +993,8 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 		t = recon_task(b, s, slot, s.sets[s.cur].planes.data(), s.sets[1 - s.cur].planes.data(), nullptr, rgba);
 		s.cur ^= 1;  // mpeg1.js:221-246: the picture just decoded becomes `forward`
 	}
+	if (frame && frame->planes) t.frame = frame->planes + j * planes;
+	if (frame && frame->res) t.res = frame->res + j * planes;
 	StreamSet &set = s.sets[s.last];
 	if (steps.size() <= step) steps.emplace_back();
 	ReconStep &r = steps[step];
@@ -989,6 +1004,7 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 		reserve_entries(b, s);
 		r.entry(t, e.picture_type, set.entries.data());
 	}
+	if (frame && frame->mb) r.entry(t, e.picture_type, frame->mb + j * s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t));
 	if (!is_b) {  // the map beside the set, one depth step from the map beside the forward set
 		if (flags & JSMPEG_B200_OUT_ACCUMULATED) {
 			reserve_maps(s);
@@ -1001,7 +1017,6 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 	if (visible && (flags & JSMPEG_B200_OUT_HOST)) {
 		s.h_head = (s.h_head + 1) % HOST_RING;
 		HostSlot &h = s.ring[s.h_head];
-		const size_t planes = (size_t)s.coded_size * 3 / 2;
 		r.copy(h.planes.data(), t.cur.y, planes);
 		host_bytes += planes;
 		if (flags & JSMPEG_B200_OUT_MACROBLOCKS) {
@@ -1021,8 +1036,10 @@ void fill_untraced(uint2 *map, size_t n_rec, cudaStream_t st) {
 
 // One round: parse ahead what is missing in one wave, then consume up to want[s] pictures per stream in decode()
 // order and queue their reconstruction.  Returns pictures consumed; `progress[s]` gets the per-stream count, `more[s]`
-// whether the stream may have further pictures.
-long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &progress, std::vector<char> &more, int flags) {
+// whether the stream may have further pictures.  `frames` (decode_frames): per stream, the cursor its reconstructed
+// pictures go to as frames.
+long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &progress, std::vector<char> &more, int flags,
+                  std::vector<FrameCursor> *frames) {
 	const int S = (int)b->streams.size();
 	HostClock::time_point t = HostClock::now();
 	// ---- 1. plan the parse wave
@@ -1080,6 +1097,7 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 	for (int si = 0; si < S; si++) {
 		if (!more[si]) continue;
 		Stream &s = b->streams[si];
+		FrameCursor *frame = frames ? &(*frames)[si] : nullptr;
 		size_t step = 0;
 		TaskAt newest;
 		while (progress[si] < want[si]) {
@@ -1105,7 +1123,10 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			// (0 unless both of its bytes are in the buffer)
 			s.last_temporal = (uint64_t)e.pos + 5 < s.bb.length ? picture_header(s, e.pos).temporal_reference : 0;
 			if (e.info.status == PIC_DECODED) {
-				b->stats.d2h_bytes += consume_picture(b, s, steps, step++, e.slot, e.info, flags, true, newest);
+				b->stats.d2h_bytes += consume_picture(b, s, steps, step++, e.slot, e.info, flags, true, newest, frame);
+				if (frame && frame->info)
+					frame->info[frame->n - 1] = jsmpeg_b200_frame_t{e.pos, (int16_t)e.info.picture_type, (int16_t)s.last_temporal,
+					                                                 e.info.n_present, e.info.error};
 				const bool is_b = e.info.picture_type == 3;
 				const uint64_t planes = (uint64_t)s.coded_size * 3 / 2;
 				b->stats.pictures_decoded++;
@@ -1119,8 +1140,8 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			release_slot(b, e.slot);
 		}
 		// OUT_RESIDUALS: the stream's last reconstructed picture of the round stores its residual; the earlier ones of the
-		// round could not be observed
-		if ((flags & JSMPEG_B200_OUT_RESIDUALS) && newest.step >= 0)
+		// round could not be observed.  (With residual frames the last one is copied at the end of the call: finish_frames.)
+		if ((flags & JSMPEG_B200_OUT_RESIDUALS) && newest.step >= 0 && !(frame && frame->res))
 			steps[newest.step].tasks[newest.task].res = reserve_residuals(b, s);
 	}
 	lap(b->trace.consume, t);
@@ -1155,7 +1176,37 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 	return consumed;
 }
 
-long batch_decode(Batch *b, int n_pictures, int flags) {
+// decode_frames, once the rounds are queued: the odd edge of every RGBA frame opaque white (the epilogue never writes
+// it), then the last RGBA frame into the stream's RGBA under OUT_RGBA and the last residual frame into its residual under
+// OUT_RESIDUALS, in one batched copy; all on the reconstruct stream, behind the frames' stage 2
+void finish_frames(Batch *b, const std::vector<FrameCursor> &frames, int flags) {
+	std::vector<void *> dst, src;
+	std::vector<size_t> size;
+	for (size_t si = 0; si < frames.size(); si++) {
+		const FrameCursor &f = frames[si];
+		Stream &s = b->streams[si];
+		if (f.n == 0) continue;
+		if (f.rgba) {
+			const size_t row = (size_t)s.width * 4, image = row * s.height;
+			if (s.width & 1) CUDA_CHECK(cudaMemset2DAsync(f.rgba + row - 4, row, 0xff, 4, (size_t)f.n * s.height, b->st_recon));
+			if (s.height & 1) CUDA_CHECK(cudaMemset2DAsync(f.rgba + image - row, image, 0xff, row, f.n, b->st_recon));
+			if (flags & JSMPEG_B200_OUT_RGBA) {
+				dst.push_back(stream_rgba(b, s));
+				src.push_back(f.rgba + (f.n - 1) * image);
+				size.push_back(image);
+			}
+		}
+		if (f.res && (flags & JSMPEG_B200_OUT_RESIDUALS)) {
+			const size_t planes = (size_t)s.coded_size * 3 / 2;
+			dst.push_back(reserve_residuals(b, s));
+			src.push_back(f.res + (f.n - 1) * planes);
+			size.push_back(planes * sizeof(int16_t));
+		}
+	}
+	if (!dst.empty()) copy_batch(b, dst, src, size, b->st_recon);
+}
+
+long batch_decode(Batch *b, int n_pictures, int flags, std::vector<FrameCursor> *frames = nullptr) {
 	use_device(b);
 	Batch::HostTrace &tr = b->trace;
 	const bool trace_on = tr.on;
@@ -1180,7 +1231,7 @@ long batch_decode(Batch *b, int n_pictures, int flags) {
 		const int per_stream = std::max(1, (int)(b->free_slots.size() + cached) / active);
 		for (int i = 0; i < S; i++)
 			want[i] = (more[i] && b->streams[i].has_seq) ? std::min(remaining[i], per_stream) : 0;
-		const long got = decode_round(b, want, progress, more, flags);
+		const long got = decode_round(b, want, progress, more, flags, frames);
 		total += got;
 		bool replanned = false;
 		for (int i = 0; i < S; i++) {
@@ -1191,6 +1242,7 @@ long batch_decode(Batch *b, int n_pictures, int flags) {
 		if (got) idle_rounds = 0;
 	}
 	t = HostClock::now();
+	if (frames) finish_frames(b, *frames, flags);
 	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
 	CUDA_CHECK(cudaStreamSynchronize(b->st_copy));
 	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
@@ -2286,6 +2338,33 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 
 long jsmpeg_b200_batch_decode(jsmpeg_b200_batch_t *b, int n_pictures, int flags) {
 	return guarded<long>(b, 0, [&] { return batch_decode(b, n_pictures, flags); });
+}
+
+long jsmpeg_b200_batch_decode_frames(jsmpeg_b200_batch_t *b, int n_pictures, int flags, void *const *planes_dst,
+                                     void *const *rgba_dst, void *const *res_dst, void *const *mb_dst,
+                                     jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out) {
+	return guarded<long>(b, -1, [&]() -> long {
+		const size_t S = b->streams.size();
+		// every given destination 16-byte aligned (stage 2 stores 8 and 16 bytes at a time), checked before any work
+		auto aligned = [&](void *const *dst) {
+			for (size_t si = 0; dst && si < S; si++)
+				if ((uintptr_t)dst[si] & 15u) return false;
+			return true;
+		};
+		if (n_pictures < 0 || !aligned(planes_dst) || !aligned(rgba_dst) || !aligned(res_dst) || !aligned(mb_dst)) return -2;
+		std::vector<FrameCursor> frames(S);
+		for (size_t si = 0; si < S; si++) {
+			FrameCursor &f = frames[si];
+			if (planes_dst) f.planes = static_cast<uint8_t *>(planes_dst[si]);
+			if (rgba_dst) f.rgba = static_cast<uint8_t *>(rgba_dst[si]);
+			if (res_dst) f.res = static_cast<int16_t *>(res_dst[si]);
+			if (mb_dst) f.mb = static_cast<uint8_t *>(mb_dst[si]);
+			if (info_out) f.info = info_out + si * (size_t)n_pictures;
+		}
+		const long got = batch_decode(b, n_pictures, flags, &frames);
+		for (size_t si = 0; n_frames_out && si < S; si++) n_frames_out[si] = frames[si].n;
+		return got;
+	});
 }
 
 long jsmpeg_b200_batch_intra_index(jsmpeg_b200_batch_t *b, int stream, uint32_t *picture_out, uint32_t *byte_pos_out,

@@ -140,6 +140,56 @@ reconstruct_rgba_res_b_kernel(const __grid_constant__ ReconRgbaResParamsB params
 	reconstruct_rgba_block<true, true>(params.p, params.out[blockIdx.z], blockIdx.z, blockIdx.y, blockIdx.x * RGBA_MBS, threadIdx.x, stage, chroma);
 }
 
+// decode_frames (DESIGN 3.16): the four RES kernels, each block also storing its output rows to the task's planar frame
+// (reconstruct_at<..., FRAME>), with the tables of ReconFrameParamsT (recon.cuh)
+constexpr int MAX_TASKS_FRAME = 63;         // (63 * (48 + 8 + 8) B) + 8 < 4 KB
+constexpr int MAX_TASKS_RGBA_FRAME = 51;    // (51 * (48 + 8 + 8 + 16) B) + 8 < 4 KB
+constexpr int MAX_TASKS_B_FRAME = 56;       // (56 * (56 + 8 + 8) B) + 8 < 4 KB
+constexpr int MAX_TASKS_RGBA_B_FRAME = 46;  // (46 * (56 + 8 + 8 + 16) B) + 8 < 4 KB
+using ReconFrameParams = ReconFrameParamsT<CompactTask, MAX_TASKS_FRAME>;
+using ReconFrameParamsB = ReconFrameParamsT<CompactTaskB, MAX_TASKS_B_FRAME>;
+struct ReconRgbaFrameParams {
+	ReconFrameParamsT<CompactTask, MAX_TASKS_RGBA_FRAME> p;
+	RgbaTarget out[MAX_TASKS_RGBA_FRAME];
+};
+struct ReconRgbaFrameParamsB {
+	ReconFrameParamsT<CompactTaskB, MAX_TASKS_RGBA_B_FRAME> p;
+	RgbaTarget out[MAX_TASKS_RGBA_B_FRAME];
+};
+static_assert(sizeof(ReconFrameParams) <= 4096 && sizeof(ReconFrameParamsB) <= 4096 && sizeof(ReconRgbaFrameParams) <= 4096 &&
+              sizeof(ReconRgbaFrameParamsB) <= 4096, "kernel parameters");
+
+// (at 5 resident CTAs, 96 registers, the I/P variant spills 36 bytes; at 4, 126 registers, it does not.  The B variant
+// uses 128 registers at 4, like reconstruct_res_b_kernel, and does not spill.)
+#ifndef JSMPEG_RECON_FRAME_MIN_CTAS
+#define JSMPEG_RECON_FRAME_MIN_CTAS 4
+#endif
+__global__ void __launch_bounds__(THREADS, JSMPEG_RECON_FRAME_MIN_CTAS)
+reconstruct_frame_kernel(const __grid_constant__ ReconFrameParams params) {
+	__shared__ __align__(16) uint8_t stage[(THREADS / 32) * WARP_STAGE];
+	reconstruct_block<false, true, true>(params, blockIdx.y, blockIdx.x * THREADS, threadIdx.x, stage);
+}
+
+__global__ void __launch_bounds__(RGBA_THREADS)
+reconstruct_rgba_frame_kernel(const __grid_constant__ ReconRgbaFrameParams params) {
+	__shared__ __align__(16) uint8_t stage[(RGBA_THREADS / 32) * WARP_STAGE];
+	__shared__ __align__(16) uint8_t chroma[2][8][RGBA_MBS * 8];
+	reconstruct_rgba_block<false, true, true>(params.p, params.out[blockIdx.z], blockIdx.z, blockIdx.y, blockIdx.x * RGBA_MBS, threadIdx.x, stage, chroma);
+}
+
+__global__ void __launch_bounds__(THREADS, JSMPEG_RECON_FRAME_MIN_CTAS)
+reconstruct_frame_b_kernel(const __grid_constant__ ReconFrameParamsB params) {
+	__shared__ __align__(16) uint8_t stage[(THREADS / 32) * WARP_STAGE];
+	reconstruct_block<true, true, true>(params, blockIdx.y, blockIdx.x * THREADS, threadIdx.x, stage);
+}
+
+__global__ void __launch_bounds__(RGBA_THREADS)
+reconstruct_rgba_frame_b_kernel(const __grid_constant__ ReconRgbaFrameParamsB params) {
+	__shared__ __align__(16) uint8_t stage[(RGBA_THREADS / 32) * WARP_STAGE];
+	__shared__ __align__(16) uint8_t chroma[2][8][RGBA_MBS * 8];
+	reconstruct_rgba_block<true, true, true>(params.p, params.out[blockIdx.z], blockIdx.z, blockIdx.y, blockIdx.x * RGBA_MBS, threadIdx.x, stage, chroma);
+}
+
 void fill_task(CompactTask &c, const ReconTask &t) {
 	c.hdr = t.hdr;
 	c.coef = t.coef;
@@ -153,9 +203,9 @@ void fill_task(CompactTask &c, const ReconTask &t) {
 }
 
 // One kernel's tasks, cut into launches of at most `per`: B = the kernel takes `bwd`, RGBA = it takes the fused
-// conversion's target, RES = it takes the residual destinations.  The plain kernels' grid covers the largest picture's
-// block slots, the RGBA kernels' its macroblock rows and columns.
-template <bool B, bool RGBA, bool RES = false, class Params>
+// conversion's target, RES = it takes the residual destinations, FRAME = also the planar frames.  The plain kernels'
+// grid covers the largest picture's block slots, the RGBA kernels' its macroblock rows and columns.
+template <bool B, bool RGBA, bool RES = false, bool FRAME = false, class Params>
 int launch_kernel(void (*kernel)(Params), int per, const std::vector<const ReconTask *> &tasks, cudaStream_t stream) {
 	int launches = 0;
 	for (size_t first = 0; first < tasks.size(); first += per, launches++) {
@@ -169,6 +219,7 @@ int launch_kernel(void (*kernel)(Params), int per, const std::vector<const Recon
 			if constexpr (B) table.t[i].bwd = t.bwd.y;
 			if constexpr (RGBA) p.out[i] = RgbaTarget{t.rgba, t.width, t.height};
 			if constexpr (RES) table.res[i] = t.res;
+			if constexpr (FRAME) table.frame[i] = t.frame;
 			max_slots = std::max(max_slots, t.mb_size * 6);
 			max_w = std::max(max_w, t.mb_width);
 			max_h = std::max(max_h, t.mb_size / t.mb_width);
@@ -185,20 +236,26 @@ int launch_kernel(void (*kernel)(Params), int per, const std::vector<const Recon
 int launch_reconstruct(const ReconTask *tasks_host, int n_tasks, cudaStream_t stream) {
 	std::vector<const ReconTask *> by_kernel[4];  // I/P, I/P + RGBA, B, B + RGBA
 	bool res[4] = {false, false, false, false};   // some task of the kernel has a residual destination: its RES variant
+	bool frame[4] = {false, false, false, false}; // some task of the kernel has a planar frame: its FRAME variant
 	for (int i = 0; i < n_tasks; i++) {
 		const ReconTask &t = tasks_host[i];
 		const int k = (t.bwd.y ? 2 : 0) + (t.rgba ? 1 : 0);
 		by_kernel[k].push_back(&t);
 		res[k] = res[k] || t.res;
+		frame[k] = frame[k] || t.frame;
 	}
 	// (one statement per kernel: the launch order is the order above)
-	int launches = res[0] ? launch_kernel<false, false, true>(reconstruct_res_kernel, MAX_TASKS_RES, by_kernel[0], stream)
-	                      : launch_kernel<false, false>(reconstruct_kernel, MAX_TASKS, by_kernel[0], stream);
-	launches += res[1] ? launch_kernel<false, true, true>(reconstruct_rgba_res_kernel, MAX_TASKS_RGBA_RES, by_kernel[1], stream)
-	                   : launch_kernel<false, true>(reconstruct_rgba_kernel, MAX_TASKS_RGBA, by_kernel[1], stream);
-	launches += res[2] ? launch_kernel<true, false, true>(reconstruct_res_b_kernel, MAX_TASKS_B_RES, by_kernel[2], stream)
-	                   : launch_kernel<true, false>(reconstruct_b_kernel, MAX_TASKS_B, by_kernel[2], stream);
-	launches += res[3] ? launch_kernel<true, true, true>(reconstruct_rgba_res_b_kernel, MAX_TASKS_RGBA_B_RES, by_kernel[3], stream)
-	                   : launch_kernel<true, true>(reconstruct_rgba_b_kernel, MAX_TASKS_RGBA_B, by_kernel[3], stream);
+	int launches = frame[0] ? launch_kernel<false, false, true, true>(reconstruct_frame_kernel, MAX_TASKS_FRAME, by_kernel[0], stream)
+	             : res[0]   ? launch_kernel<false, false, true>(reconstruct_res_kernel, MAX_TASKS_RES, by_kernel[0], stream)
+	                        : launch_kernel<false, false>(reconstruct_kernel, MAX_TASKS, by_kernel[0], stream);
+	launches += frame[1] ? launch_kernel<false, true, true, true>(reconstruct_rgba_frame_kernel, MAX_TASKS_RGBA_FRAME, by_kernel[1], stream)
+	          : res[1]   ? launch_kernel<false, true, true>(reconstruct_rgba_res_kernel, MAX_TASKS_RGBA_RES, by_kernel[1], stream)
+	                     : launch_kernel<false, true>(reconstruct_rgba_kernel, MAX_TASKS_RGBA, by_kernel[1], stream);
+	launches += frame[2] ? launch_kernel<true, false, true, true>(reconstruct_frame_b_kernel, MAX_TASKS_B_FRAME, by_kernel[2], stream)
+	          : res[2]   ? launch_kernel<true, false, true>(reconstruct_res_b_kernel, MAX_TASKS_B_RES, by_kernel[2], stream)
+	                     : launch_kernel<true, false>(reconstruct_b_kernel, MAX_TASKS_B, by_kernel[2], stream);
+	launches += frame[3] ? launch_kernel<true, true, true, true>(reconstruct_rgba_frame_b_kernel, MAX_TASKS_RGBA_B_FRAME, by_kernel[3], stream)
+	          : res[3]   ? launch_kernel<true, true, true>(reconstruct_rgba_res_b_kernel, MAX_TASKS_RGBA_B_RES, by_kernel[3], stream)
+	                     : launch_kernel<true, true>(reconstruct_rgba_b_kernel, MAX_TASKS_RGBA_B, by_kernel[3], stream);
 	return launches;
 }

@@ -60,6 +60,16 @@ struct ReconResParamsT {
 	int16_t *res[N];
 };
 
+// decode_frames (DESIGN 3.16): a FRAME kernel's table is the RES one plus a parallel frame[] (nullptr: no planar frame for
+// that task); either pointer of a task may be nullptr
+template <class TASK, int N>
+struct ReconFrameParamsT {
+	TASK t[N];
+	int32_t n_tasks;
+	int16_t *res[N];
+	uint8_t *frame[N];
+};
+
 #ifndef JSMPEG_WALK_EMU
 __device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ uint32_t umulhi_u32(uint32_t a, uint32_t b) { return __umulhi(a, b); }
@@ -263,6 +273,15 @@ __device__ __forceinline__ void store_residual_row(int16_t *dst, uint4 o) {
 	memcpy(dst, &o, 16);
 #endif
 }
+// decode_frames (DESIGN 3.16): one packed output row of a block into the planar frame, a streaming 8-byte store
+// (nothing in the call reads it back)
+__device__ __forceinline__ void store_frame_row(uint8_t *dst, uint2 o) {
+#ifndef JSMPEG_WALK_EMU
+	__stcs(reinterpret_cast<uint2 *>(dst), o);
+#else
+	memcpy(dst, &o, 8);
+#endif
+}
 __device__ __forceinline__ void store_residual(int16_t *dst, int stride, const int (&v)[64]) {
 #pragma unroll
 	for (int r = 0; r < 8; r++)
@@ -292,7 +311,10 @@ __device__ __forceinline__ void store_residual(int16_t *dst, int stride, const i
 // block uses; everything up to the prediction is the same code.
 // RES (OUT_RESIDUALS, PARAMS with `res`: ReconResParamsT above): a task whose params.res[ty] is not nullptr also
 // gets each in-picture block's residual v[] there (store_residual): zeros for a macroblock that is not present.
-template <bool KEEP, bool BIDIR = false, bool RES = false, class PARAMS>
+// FRAME (decode_frames, PARAMS with `res` and `frame`: ReconFrameParamsT above): a task whose params.frame[ty] is not
+// nullptr also gets each in-picture block's eight output rows there, in the planes' layout: for a macroblock that is
+// not present, the rows the plane set keeps.  The rows are collected as under KEEP.
+template <bool KEEP, bool BIDIR = false, bool RES = false, bool FRAME = false, class PARAMS>
 __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int mb_row, int mb_col, int b, bool in_picture,
                                                int lane, uint8_t *wstage, uint2 (&rows)[8]) {
 	const auto &t = params.t[ty];
@@ -428,9 +450,18 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 #endif
 	}
 	uint8_t *dst = t.cur + plane_off + origin;
-	auto reload_rows = [&]() {  // what is in the plane now (rare paths of the RGBA variant)
+	constexpr bool ROWS = KEEP || FRAME;  // the output rows go back in `rows`
+	auto reload_rows = [&]() {  // what is in the plane now (rare paths of the RGBA and FRAME variants)
 #pragma unroll
 		for (int r = 0; r < 8; r++) rows[r] = *reinterpret_cast<const uint2 *>(dst + r * stride);
+	};
+	auto store_frame = [&]() {  // FRAME: the rows into the planar frame (a uniform branch, as RES's)
+		if constexpr (FRAME) {
+			if (params.frame[ty] && in_picture) {
+#pragma unroll
+				for (int r = 0; r < 8; r++) store_frame_row(params.frame[ty] + plane_off + origin + r * stride, rows[r]);
+			}
+		}
 	};
 	if (!present) {
 		if constexpr (RES) {
@@ -439,7 +470,8 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 				for (int r = 0; r < 8; r++) store_residual_row(params.res[ty] + plane_off + origin + r * stride, make_uint4(0u, 0u, 0u, 0u));
 			}
 		}
-		if (KEEP && in_picture) reload_rows();
+		if (ROWS && in_picture) reload_rows();
+		store_frame();
 		return;
 	}
 
@@ -516,8 +548,9 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 			out.x = pack_sat_u8x4(v[r * 8 + 0], v[r * 8 + 1], v[r * 8 + 2], v[r * 8 + 3]);
 			out.y = pack_sat_u8x4(v[r * 8 + 4], v[r * 8 + 5], v[r * 8 + 6], v[r * 8 + 7]);
 			*reinterpret_cast<uint2 *>(dst + r * stride) = out;
-			if (KEEP) rows[r] = out;
+			if (ROWS) rows[r] = out;
 		}
+		store_frame();
 		return;
 	}
 
@@ -528,7 +561,8 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		if ((!use_f || inside) && (!use_b || inside_b)) {
 			const uint32_t fw = (use_f && oh) ? (ov ? 0x01010101u : 0x00000202u) : ((use_f && ov) ? 0x00020002u : 0x00000004u);
 			const uint32_t bw = ohb ? (ovb ? 0x01010101u : 0x00000202u) : (ovb ? 0x00020002u : 0x00000004u);
-			predict_rows_b<KEEP>(splane, fsrc, fw, use_f, bplane, src_b, bw, use_b, stride, v, dst, rows);
+			predict_rows_b<ROWS>(splane, fsrc, fw, use_f, bplane, src_b, bw, use_b, stride, v, dst, rows);
+			store_frame();
 			return;
 		}
 		// a vector leaves its plane: per-tap bounds check, any outside tap zeroes that prediction's sample (SURVEY Q11)
@@ -554,7 +588,8 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 			out.y = add_sat4(p[1], rr[4], rr[5], rr[6], rr[7]);
 			*reinterpret_cast<uint2 *>(dst + r * stride) = out;
 		}
-		if (KEEP) reload_rows();
+		if (ROWS) reload_rows();
+		store_frame();
 		return;
 	}
 
@@ -562,8 +597,9 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 	if (inside) {
 		// tap weights of this lane: bytes (wA, wB, wC, wD)
 		const uint32_t weights = oh ? (ov ? 0x01010101u : 0x00000202u) : (ov ? 0x00020002u : 0x00000004u);
-		if (warp_halfpel) predict_rows<false, KEEP>(splane, src, stride, weights, v, dst, rows);
-		else predict_rows<true, KEEP>(splane, src, stride, weights, v, dst, rows);
+		if (warp_halfpel) predict_rows<false, ROWS>(splane, src, stride, weights, v, dst, rows);
+		else predict_rows<true, ROWS>(splane, src, stride, weights, v, dst, rows);
+		store_frame();
 		return;
 	}
 	// vector leaves the plane: per-tap bounds check, any outside tap zeroes the sample (SURVEY Q11)
@@ -603,13 +639,14 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 		}
 		*reinterpret_cast<uint2 *>(dst + r * stride) = out;
 	}
-	if (KEEP) reload_rows();
+	if (ROWS) reload_rows();
+	store_frame();
 }
 
 // The plain kernel's numbering: slot first_slot + tid of picture `ty`; `stage` = the CTA's staging area (one
 // WARP_STAGE per warp).  The 32 lanes of a warp hold 32 horizontally adjacent blocks of one plane row:
 // [luma top 2W | luma bottom 2W | Cb W | Cr W] per macroblock row.
-template <bool BIDIR = false, bool RES = false, class PARAMS>
+template <bool BIDIR = false, bool RES = false, bool FRAME = false, class PARAMS>
 __device__ __forceinline__ void reconstruct_block(const PARAMS &params, int ty, int first_slot, int tid, uint8_t *stage) {
 	const auto &t = params.t[ty];
 	const int W = t.mb_width;
@@ -630,8 +667,8 @@ __device__ __forceinline__ void reconstruct_block(const PARAMS &params, int ty, 
 		mb_col = c - second * W;
 		b = 4 + second;  // block 4 -> Cb plane, block 5 -> Cr plane (mpeg1.js:829-834, SURVEY Q8)
 	}
-	uint2 unused[8];
-	reconstruct_at<false, BIDIR, RES>(params, ty, mb_row, mb_col, b, in_picture, tid & 31, stage + (tid >> 5) * WARP_STAGE, unused);
+	uint2 rows[8];  // (used under FRAME only)
+	reconstruct_at<false, BIDIR, RES, FRAME>(params, ty, mb_row, mb_col, b, in_picture, tid & 31, stage + (tid >> 5) * WARP_STAGE, rows);
 }
 
 #ifndef JSMPEG_WALK_EMU  // (a CTA-wide barrier: outside what the one-warp host emulation runs)
@@ -658,7 +695,7 @@ __device__ __forceinline__ uint32_t rgba_px(int y, int r, int g, int b) {
 	return c(y + r) | (c(y - g) << 8) | (c(y + b) << 16) | 0xff000000u;
 }
 
-template <bool BIDIR = false, bool RES = false, class PARAMS>
+template <bool BIDIR = false, bool RES = false, bool FRAME = false, class PARAMS>
 __device__ __forceinline__ void reconstruct_rgba_block(const PARAMS &params, const RgbaTarget &out, int ty, int mb_row, int first_mb_col,
                                                        int tid, uint8_t *stage, uint8_t (*chroma)[8][RGBA_MBS * 8]) {
 	const auto &t = params.t[ty];
@@ -673,7 +710,7 @@ __device__ __forceinline__ void reconstruct_rgba_block(const PARAMS &params, con
 	uint2 rows[8];
 #pragma unroll
 	for (int r = 0; r < 8; r++) rows[r] = make_uint2(0u, 0u);
-	reconstruct_at<true, BIDIR, RES>(params, ty, mb_row, in_picture ? mb_col : 0, b, in_picture, lane, stage + warp * WARP_STAGE, rows);
+	reconstruct_at<true, BIDIR, RES, FRAME>(params, ty, mb_row, in_picture ? mb_col : 0, b, in_picture, lane, stage + warp * WARP_STAGE, rows);
 	if (warp == 2) {
 		// plane 0 = Cb (block 4), plane 1 = Cr (block 5)
 #pragma unroll
