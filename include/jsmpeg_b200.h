@@ -575,6 +575,36 @@ long jsmpeg_b200_batch_decode_frames(jsmpeg_b200_batch_t *b, int n_pictures, int
                                      void *const *rgba_dst, void *const *res_dst, void *const *mb_dst,
                                      jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out);
 
+/* EVERY COMPRESSED-DOMAIN INPUT OF decode(n) (CoViAR-style clip loaders, DCT-domain models): decode_frames_into is
+ * jsmpeg_b200_batch_decode_frames with two more kinds of frame, from the walk and expand decode() does anyway.  `dst`
+ * (not NULL) holds the four arrays of decode_frames, with their meaning, and per stream (any array or entry NULL: none)
+ *   coef[s] + j * mb_size * 768 bytes: byte for byte what decode_coefficients writes for frame j's picture (per
+ *       macroblock 6 blocks of 64 int16) -- I, P and B frames, damaged streams too, both reading the records of the walk
+ *       that starts at the picture's start code.  No flag is needed.
+ *   acc[s] + j * coded_size * 12 bytes: for an I/P frame, byte for byte what read_accumulated gives right after the
+ *       decode(1, flags) that reconstructs the picture, with OUT_ACCUMULATED's `prev` rules unchanged (a trace broken by
+ *       a call without the flag, reset, a seek without the flag or a start on a P picture stays untraced up to the next I
+ *       picture; maps of this call chain on into the next one); for a B frame all untraced {0, 0, 0, -1}.  A map
+ *       destination requires JSMPEG_B200_OUT_ACCUMULATED in `flags`, so that the batch state stays decode(n, flags)'s.
+ * Every frame below n_frames_out[s] is fully written; memory past it is left untouched.  Destinations of different
+ * streams or kinds must not overlap.  Per 1080p frame: coefficients 6,266,880 bytes, map 25,067,520 bytes -- so 64
+ * streams x 8 map frames take about 12.8 GB.
+ *
+ * Everything decode() observes afterwards is what decode(n, flags) leaves, maps included, but kernel_launches (one more
+ * coefficient export launch per reconstruct step with a coefficient frame).  decode_frames(b, n, flags, p, r, e, m, i,
+ * f) is decode_frames_into with {p, r, e, m, NULL, NULL}.
+ *
+ * Synchronous.  Returns what decode() returns; -1 for a dead batch; -2, before any work and with nothing changed, when
+ * dst is NULL, n_pictures < 0, a destination is not 16-byte aligned, or an acc entry is given without OUT_ACCUMULATED. */
+typedef struct jsmpeg_b200_frame_dst_t {
+	void *const *planes, *const *rgba, *const *res, *const *mb; /* decode_frames' four arrays */
+	void *const *coef;                                           /* per stream: frame j at + j * mb_size * 768 bytes */
+	void *const *acc;                                            /* per stream: frame j at + j * coded_size * 12 bytes */
+} jsmpeg_b200_frame_dst_t;
+
+long jsmpeg_b200_batch_decode_frames_into(jsmpeg_b200_batch_t *b, int n_pictures, int flags, const jsmpeg_b200_frame_dst_t *dst,
+                                          jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out);
+
 /* SEEK (players, video walls, clip loaders): move decode() of chosen streams to a chosen picture each, and play on from
  * there with decode() -- OUT_HOST, OUT_RGBA and the host ring as usual -- without stepping the other streams.  The
  * reference chains of all requests run side by side, as for decode_pictures, but into the streams' own plane sets.

@@ -38,6 +38,13 @@ class Frame(ctypes.Structure):
 
 
 _VP = ctypes.c_void_p
+
+
+class FrameDst(ctypes.Structure):
+    """jsmpeg_b200_frame_dst_t: decode_frames_into's destination arrays (one device pointer per stream each, NULL: none)."""
+    _fields_ = [("planes", _VP), ("rgba", _VP), ("res", _VP), ("mb", _VP), ("coef", _VP), ("acc", _VP)]
+
+
 _BATCH_ABI = {
     "jsmpeg_b200_batch_create": (_VP, [ctypes.c_int, ctypes.c_int, ctypes.c_uint]),
     "jsmpeg_b200_batch_destroy": (None, [_VP]),
@@ -72,6 +79,8 @@ _BATCH_ABI = {
     "jsmpeg_b200_batch_read_residuals": (ctypes.c_int, [_VP, ctypes.c_int, _VP]),
     "jsmpeg_b200_batch_decode_frames": (ctypes.c_long, [_VP, ctypes.c_int, ctypes.c_int, _VP, _VP, _VP, _VP,
                                                         ctypes.POINTER(Frame), _VP]),
+    "jsmpeg_b200_batch_decode_frames_into": (ctypes.c_long, [_VP, ctypes.c_int, ctypes.c_int, ctypes.POINTER(FrameDst),
+                                                             ctypes.POINTER(Frame), _VP]),
     "jsmpeg_b200_batch_last_picture": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_batch_intra_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
@@ -311,9 +320,10 @@ class BatchDecoder:
     def decode(self, n_pictures=1, flags=OUT_DEVICE):
         return self.lib.jsmpeg_b200_batch_decode(self.handle, n_pictures, flags)
 
-    _FRAME_KINDS = ("planes", "rgba", "residuals", "macroblocks")
+    _FRAME_KINDS = ("planes", "rgba", "residuals", "macroblocks", "coefficients", "accumulated")
 
-    def decode_frames(self, n_pictures, flags=OUT_DEVICE, planes=True, rgba=False, residuals=False, macroblocks=False):
+    def decode_frames(self, n_pictures, flags=OUT_DEVICE, planes=True, rgba=False, residuals=False, macroblocks=False,
+                      coefficients=False, accumulated=False):
         """decode(n_pictures, flags) that also hands back every picture it reconstructs (include/jsmpeg_b200.h,
         jsmpeg_b200_batch_decode_frames): frame j of a stream is the j-th picture the call reconstructs for it (I and P,
         and B under decode_b; skipped pictures have none), in coded order.  Returns per stream a dict with "n_frames",
@@ -323,21 +333,29 @@ class BatchDecoder:
         "macroblocks" uint8 [F, mb_height, mb_width, 16] (see macroblocks_view); None for a stream without a sequence
         header.  When every stream has one and all share one geometry, each kind is allocated as one [S, n_pictures,
         ...] tensor (last_frames_batch[kind]; RGBA only where a stream's n_pictures images are a multiple of 16 bytes) and
-        the per-stream tensors are views of it: a clip batch without a gather."""
+        the per-stream tensors are views of it: a clip batch without a gather.
+        coefficients=True and accumulated=True (jsmpeg_b200_batch_decode_frames_into) add "coefficients" int16 [F,
+        mb_height, mb_width, 6, 8, 8] (as decode_coefficients) and "accumulated" int16 [F, coded_size * 3 // 2, 4] (see
+        accumulated_view; a B frame's is all untraced); accumulated=True needs OUT_ACCUMULATED in `flags`."""
         import torch
         n = int(n_pictures)
         if n < 0:
             raise ValueError("n_pictures must be >= 0")
+        if accumulated and not int(flags) & OUT_ACCUMULATED:
+            raise ValueError("accumulated frames need OUT_ACCUMULATED in flags")
         dev = torch.device("cuda", self.device)
         infos = [self.stream_info(s) for s in range(self.n_streams)]
-        want = {"planes": planes, "rgba": rgba, "residuals": residuals, "macroblocks": macroblocks}
+        want = {"planes": planes, "rgba": rgba, "residuals": residuals, "macroblocks": macroblocks,
+                "coefficients": coefficients, "accumulated": accumulated}
 
         def shape(kind, info):
             cs, w, h = info["coded_size"], info["width"], info["height"]
             return {"planes": (cs * 3 // 2,), "rgba": (h, w, 4), "residuals": (cs * 3 // 2,),
-                    "macroblocks": ((h + 15) // 16, (w + 15) // 16, MACROBLOCK_BYTES)}[kind]
+                    "macroblocks": ((h + 15) // 16, (w + 15) // 16, MACROBLOCK_BYTES),
+                    "coefficients": ((h + 15) // 16, (w + 15) // 16, 6, 8, 8), "accumulated": (cs * 3 // 2, 4)}[kind]
 
-        dtype = {"planes": torch.uint8, "rgba": torch.uint8, "residuals": torch.int16, "macroblocks": torch.uint8}
+        dtype = {"planes": torch.uint8, "rgba": torch.uint8, "residuals": torch.int16, "macroblocks": torch.uint8,
+                 "coefficients": torch.int16, "accumulated": torch.int16}
         geometries = {(i["width"], i["height"]) for i in infos}
         shared = all(i["has_sequence_header"] for i in infos) and len(geometries) == 1
         full, self.last_frames_batch = {}, {}
@@ -357,8 +375,13 @@ class BatchDecoder:
         n_frames = (ctypes.c_int32 * S)()
         if full:
             torch.cuda.current_stream(dev).synchronize()  # the allocations are the caller's stream's; the call uses its own
-        got = self.lib.jsmpeg_b200_batch_decode_frames(self.handle, n, int(flags), dst.get("planes"), dst.get("rgba"),
-                                                       dst.get("residuals"), dst.get("macroblocks"), info_out, n_frames)
+        if coefficients or accumulated:
+            into = FrameDst(*[ctypes.addressof(dst[k]) if k in dst else None for k in
+                              ("planes", "rgba", "residuals", "macroblocks", "coefficients", "accumulated")])
+            got = self.lib.jsmpeg_b200_batch_decode_frames_into(self.handle, n, int(flags), ctypes.byref(into), info_out, n_frames)
+        else:
+            got = self.lib.jsmpeg_b200_batch_decode_frames(self.handle, n, int(flags), dst.get("planes"), dst.get("rgba"),
+                                                           dst.get("residuals"), dst.get("macroblocks"), info_out, n_frames)
         if got == -2:
             raise ValueError("decode_frames refused its arguments")
         if got < 0:

@@ -75,6 +75,9 @@ struct StreamSet {
 	// a call with the flag wrote `map` for the picture `planes` holds now; an unwritten map is never read as a trace's
 	// previous map
 	bool map_written = false;
+	// decode_frames_into (DESIGN 3.17): the map frame that holds that picture's map instead of `map`, while the call runs;
+	// nullptr: `map`
+	const uint2 *map_at = nullptr;
 };
 
 // One slot of a stream's host ring (OUT_HOST): a picture's planes and, under OUT_MACROBLOCKS, its entries (made zeroed on
@@ -192,6 +195,9 @@ struct jsmpeg_b200_batch_t {
 	// decode_coefficients: the coefficient export tasks of a wave (DESIGN 3.9)
 	PinnedBuffer<CoefExportTask> h_ctasks;
 	DeviceBuffer<CoefExportTask> d_ctasks;
+	// decode_frames_into's coefficient frames: the coefficient export tasks of a round's steps (DESIGN 3.17)
+	PinnedBuffer<CoefExportTask> h_ftasks;
+	DeviceBuffer<CoefExportTask> d_ftasks;
 	// decode_residuals: the residual export tasks of a wave (DESIGN 3.10)
 	PinnedBuffer<ResExportTask> h_rtasks;
 	DeviceBuffer<ResExportTask> d_rtasks;
@@ -643,13 +649,16 @@ void reserve_tasks(PinnedBuffer<T> &h, DeviceBuffer<T> &d, size_t n, cudaStream_
 // One step of stage 2 (run_steps): the reconstruct tasks of one step of decode() (or one depth of run_chains), queued
 // by launch_reconstruct; the export of their macroblock entries (OUT_MACROBLOCKS: `entries`, one launch of
 // export_macroblocks_kernel over `entry_mb` macroblocks); accumulated maps (OUT_ACCUMULATED, decode_accumulated:
-// `maps`, one launch of accumulate_kernel over `map_warps` warps); and the copies of its pictures that follow them
+// `maps`, one launch of accumulate_kernel over `map_warps` warps); coefficient frames (decode_frames_into: `coefs`, one
+// launch of export_coefficients_kernel over `coef_mb` macroblocks); and the copies of its pictures that follow them
 struct ReconStep {
 	std::vector<ReconTask> tasks;
 	std::vector<MbExportTask> entries;
 	uint32_t entry_mb = 0;
 	std::vector<AccTask> maps;
 	uint32_t map_warps = 0;
+	std::vector<CoefExportTask> coefs;
+	uint32_t coef_mb = 0;
 	std::vector<void *> dst, src;
 	std::vector<size_t> size;
 	void copy(void *to, void *from, size_t n) {
@@ -668,9 +677,14 @@ struct ReconStep {
 		maps.push_back(AccTask{sr.hdr, sr.coef, sr.compact, prev, to, map_warps, seq.mb_width, seq.mb_height});
 		map_warps += res_export_warps(seq.mb_size);
 	}
+	// the coefficients of the picture whose records are `sr` (`mb_size` macroblocks) into `to`
+	void coef(const SlotRecords &sr, int mb_size, void *to) {
+		coefs.push_back(CoefExportTask{sr.hdr, sr.coef, sr.compact, to, coef_mb, mb_size});
+		coef_mb += (uint32_t)mb_size;
+	}
 };
 
-// The tasks `list` of all `steps` (ReconStep::entries, ReconStep::maps) go up in one copy on the reconstruct stream,
+// The tasks `list` of all `steps` (ReconStep::entries, ReconStep::maps, ReconStep::coefs) go up in one copy on the reconstruct stream,
 // through the pinned table `h` into `d`; returns where each step's tasks begin in `d`.  The previous upload's readers are
 // done before the pinned table is written again: every call ends with its reconstruction complete, and run_chains'
 // next wave waits for ev_round.
@@ -702,12 +716,14 @@ void copy_out_step(Batch *b, ReconStep &r) {
 // Stage 2 of decode_round and of a run_chains wave: `steps`, one after the other on the reconstruct stream.  Every step's
 // export and accumulate tasks go up in one copy per table (upload_step_tasks, before ev_recon[0]); then, behind the
 // latest stage-1 wave (ev_b: the records are final; where the host waited for the wave, an ordering already met) and
-// between ev_recon[0] and ev_recon[1] (decode()'s recon_ms), each step's reconstruct, export and accumulate launch,
+// between ev_recon[0] and ev_recon[1] (decode()'s recon_ms), each step's reconstruct, export, accumulate and coefficient
+// export launch,
 // those it has tasks for, and its copies: with `copy_out` on the copy stream (copy_out_step), else on the reconstruct
 // stream.  The record slots stay until ev_round.  Returns the kernels launched.
 int run_steps(Batch *b, std::vector<ReconStep> &steps, bool copy_out) {
 	const std::vector<const MbExportTask *> entries = upload_step_tasks(b, steps, &ReconStep::entries, b->h_etasks, b->d_etasks);
 	const std::vector<const AccTask *> maps = upload_step_tasks(b, steps, &ReconStep::maps, b->h_atasks, b->d_atasks);
+	const std::vector<const CoefExportTask *> coefs = upload_step_tasks(b, steps, &ReconStep::coefs, b->h_ftasks, b->d_ftasks);
 	CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_b, 0));
 	CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
 	int launches = 0;
@@ -724,6 +740,10 @@ int run_steps(Batch *b, std::vector<ReconStep> &steps, bool copy_out) {
 		}
 		if (!r.maps.empty()) {  // (a map a step reads as `prev` was written by an earlier step)
 			launch_accumulate(maps[i], (int)r.maps.size(), r.map_warps, b->st_recon);
+			launches++;
+		}
+		if (!r.coefs.empty()) {
+			launch_export_coefficients(coefs[i], (int)r.coefs.size(), r.coef_mb, b->st_recon);
 			launches++;
 		}
 		if (r.dst.empty()) continue;
@@ -951,16 +971,24 @@ int16_t *reserve_residuals(Batch *b, Stream &s) {
 	return s.d_res.data();
 }
 
+// Every record of `n_rec` from `map` untraced {0, 0, 0, -1}, on `st`
+void fill_untraced(uint2 *map, size_t n_rec, cudaStream_t st) {
+	CUDA_CHECK(cudaMemsetAsync(map, 0, n_rec * 8, st));
+	CUDA_CHECK(cudaMemset2DAsync(reinterpret_cast<uint8_t *>(map) + 6, 8, 0xff, 2, n_rec, st));
+}
+
 // Where a task is in a list of steps: steps[step].tasks[task]; step -1: nowhere
 struct TaskAt {
 	int step = -1, task = 0;
 };
 
-// decode_frames (DESIGN 3.16): where one stream's frames go -- each destination nullptr or the stream's frame 0 in device
-// memory, `info` its row of the caller's info_out on the host -- and how many the call has given it so far
+// decode_frames (DESIGN 3.16) and decode_frames_into (DESIGN 3.17): where one stream's frames go -- each destination
+// nullptr or the stream's frame 0 in device memory, `info` its row of the caller's info_out on the host -- and how many
+// the call has given it so far
 struct FrameCursor {
 	uint8_t *planes = nullptr, *rgba = nullptr, *mb = nullptr;
-	int16_t *res = nullptr;
+	int16_t *res = nullptr, *coef = nullptr;
+	uint2 *acc = nullptr;
 	jsmpeg_b200_frame_t *info = nullptr;
 	int n = 0;
 };
@@ -972,8 +1000,10 @@ struct FrameCursor {
 // goes to the stream's RGBA under OUT_RGBA and, under OUT_HOST, with its entries to the next slot of its host ring.
 // `newest` gets where its task is (OUT_RESIDUALS: the caller's newest picture stores its residual).  With a `frame`
 // cursor (decode_frames) the picture is the stream's next frame: stage 2 also stores its planes, and its RGBA and
-// residual go to that frame instead of the stream's own, and its entries are also exported there.  Returns the bytes its
-// copies bring to the host.
+// residual go to that frame instead of the stream's own, and its entries are also exported there.  decode_frames_into
+// adds its coefficients, exported from its records, and its map: an I/P picture's map goes to the frame INSTEAD of the
+// set's map (the set's map_at says so; finish_frames brings the newest one back), a B picture's frame is untraced.
+// Returns the bytes its copies bring to the host.
 uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, size_t step, int slot, const picture_info_t &e,
                          int flags, bool visible, TaskAt &newest, FrameCursor *frame = nullptr) {
 	const bool is_b = e.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
@@ -1005,13 +1035,19 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 		r.entry(t, e.picture_type, set.entries.data());
 	}
 	if (frame && frame->mb) r.entry(t, e.picture_type, frame->mb + j * s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t));
-	if (!is_b) {  // the map beside the set, one depth step from the map beside the forward set
+	if (frame && frame->coef) r.coef(slot_records(b, slot), s.seq.mb_size, frame->coef + j * s.seq.mb_size * 384);
+	uint2 *acc = frame && frame->acc ? frame->acc + j * planes : nullptr;  // (only under OUT_ACCUMULATED)
+	if (!is_b) {  // the map beside the set (or in its map frame), one depth step from the forward set's picture's map
 		if (flags & JSMPEG_B200_OUT_ACCUMULATED) {
 			reserve_maps(s);
 			const StreamSet &fwd = s.sets[s.cur];  // (swapped above)
-			r.map(slot_records(b, slot), s.seq, fwd.map_written ? fwd.map.data() : nullptr, set.map.data());
+			const uint2 *prev = !fwd.map_written ? nullptr : fwd.map_at ? fwd.map_at : fwd.map.data();
+			r.map(slot_records(b, slot), s.seq, prev, acc ? acc : set.map.data());
 		}
 		set.map_written = (flags & JSMPEG_B200_OUT_ACCUMULATED) != 0;
+		set.map_at = acc;
+	} else if (acc) {  // (queued before the step's launches, which do not touch it)
+		fill_untraced(acc, planes, b->st_recon);
 	}
 	uint64_t host_bytes = 0;
 	if (visible && (flags & JSMPEG_B200_OUT_HOST)) {
@@ -1026,12 +1062,6 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 		}
 	}
 	return host_bytes;
-}
-
-// Every record of `n_rec` from `map` untraced {0, 0, 0, -1}, on `st`
-void fill_untraced(uint2 *map, size_t n_rec, cudaStream_t st) {
-	CUDA_CHECK(cudaMemsetAsync(map, 0, n_rec * 8, st));
-	CUDA_CHECK(cudaMemset2DAsync(reinterpret_cast<uint8_t *>(map) + 6, 8, 0xff, 2, n_rec, st));
 }
 
 // One round: parse ahead what is missing in one wave, then consume up to want[s] pictures per stream in decode()
@@ -1177,8 +1207,10 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 }
 
 // decode_frames, once the rounds are queued: the odd edge of every RGBA frame opaque white (the epilogue never writes
-// it), then the last RGBA frame into the stream's RGBA under OUT_RGBA and the last residual frame into its residual under
-// OUT_RESIDUALS, in one batched copy; all on the reconstruct stream, behind the frames' stage 2
+// it), then the last RGBA frame into the stream's RGBA under OUT_RGBA, the last residual frame into its residual under
+// OUT_RESIDUALS and the newest I/P picture's map frame into its set's map (decode_frames_into), in one batched copy; all
+// on the reconstruct stream, behind the frames' stage 2.  The older I/P set's map is never read again before that set is
+// rewritten (`prev` and get_accumulated read the newest), so one whose map is in a frame is left unwritten.
 void finish_frames(Batch *b, const std::vector<FrameCursor> &frames, int flags) {
 	std::vector<void *> dst, src;
 	std::vector<size_t> size;
@@ -1201,6 +1233,17 @@ void finish_frames(Batch *b, const std::vector<FrameCursor> &frames, int flags) 
 			dst.push_back(reserve_residuals(b, s));
 			src.push_back(f.res + (f.n - 1) * planes);
 			size.push_back(planes * sizeof(int16_t));
+		}
+		StreamSet &newest = s.sets[1 - s.cur], &older = s.sets[s.cur];
+		if (newest.map_at) {
+			dst.push_back(newest.map.data());
+			src.push_back(const_cast<uint2 *>(newest.map_at));
+			size.push_back((size_t)s.coded_size * 3 / 2 * sizeof(uint2));
+			newest.map_at = nullptr;
+		}
+		if (older.map_at) {
+			older.map_written = false;
+			older.map_at = nullptr;
 		}
 	}
 	if (!dst.empty()) copy_batch(b, dst, src, size, b->st_recon);
@@ -2343,22 +2386,36 @@ long jsmpeg_b200_batch_decode(jsmpeg_b200_batch_t *b, int n_pictures, int flags)
 long jsmpeg_b200_batch_decode_frames(jsmpeg_b200_batch_t *b, int n_pictures, int flags, void *const *planes_dst,
                                      void *const *rgba_dst, void *const *res_dst, void *const *mb_dst,
                                      jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out) {
+	const jsmpeg_b200_frame_dst_t dst{planes_dst, rgba_dst, res_dst, mb_dst, nullptr, nullptr};
+	return jsmpeg_b200_batch_decode_frames_into(b, n_pictures, flags, &dst, info_out, n_frames_out);
+}
+
+long jsmpeg_b200_batch_decode_frames_into(jsmpeg_b200_batch_t *b, int n_pictures, int flags, const jsmpeg_b200_frame_dst_t *dst,
+                                          jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out) {
 	return guarded<long>(b, -1, [&]() -> long {
+		if (!dst) return -2;
 		const size_t S = b->streams.size();
-		// every given destination 16-byte aligned (stage 2 stores 8 and 16 bytes at a time), checked before any work
-		auto aligned = [&](void *const *dst) {
-			for (size_t si = 0; dst && si < S; si++)
-				if ((uintptr_t)dst[si] & 15u) return false;
+		// every given destination 16-byte aligned (stage 2 and the exports store 8 and 16 bytes at a time), and map
+		// frames only where decode(n, flags) writes maps; checked before any work
+		auto aligned = [&](void *const *d) {
+			for (size_t si = 0; d && si < S; si++)
+				if ((uintptr_t)d[si] & 15u) return false;
 			return true;
 		};
-		if (n_pictures < 0 || !aligned(planes_dst) || !aligned(rgba_dst) || !aligned(res_dst) || !aligned(mb_dst)) return -2;
+		bool maps = false;
+		for (size_t si = 0; dst->acc && si < S; si++) maps |= dst->acc[si] != nullptr;
+		if (n_pictures < 0 || !aligned(dst->planes) || !aligned(dst->rgba) || !aligned(dst->res) || !aligned(dst->mb) ||
+		    !aligned(dst->coef) || !aligned(dst->acc) || (maps && !(flags & JSMPEG_B200_OUT_ACCUMULATED)))
+			return -2;
 		std::vector<FrameCursor> frames(S);
 		for (size_t si = 0; si < S; si++) {
 			FrameCursor &f = frames[si];
-			if (planes_dst) f.planes = static_cast<uint8_t *>(planes_dst[si]);
-			if (rgba_dst) f.rgba = static_cast<uint8_t *>(rgba_dst[si]);
-			if (res_dst) f.res = static_cast<int16_t *>(res_dst[si]);
-			if (mb_dst) f.mb = static_cast<uint8_t *>(mb_dst[si]);
+			if (dst->planes) f.planes = static_cast<uint8_t *>(dst->planes[si]);
+			if (dst->rgba) f.rgba = static_cast<uint8_t *>(dst->rgba[si]);
+			if (dst->res) f.res = static_cast<int16_t *>(dst->res[si]);
+			if (dst->mb) f.mb = static_cast<uint8_t *>(dst->mb[si]);
+			if (dst->coef) f.coef = static_cast<int16_t *>(dst->coef[si]);
+			if (dst->acc) f.acc = static_cast<uint2 *>(dst->acc[si]);
 			if (info_out) f.info = info_out + si * (size_t)n_pictures;
 		}
 		const long got = batch_decode(b, n_pictures, flags, &frames);
