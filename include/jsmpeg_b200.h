@@ -366,7 +366,8 @@ int jsmpeg_b200_batch_get_host_macroblocks(jsmpeg_b200_batch_t *b, int stream, v
  * mb_height * mb_width * 6 * 64 int16 (768 bytes per macroblock): macroblocks in raster order; per macroblock the
  * blocks 0-3 luma (top-left, top-right, bottom-left, bottom-right), 4 Cb, 5 Cr (the cbp bits' order); per block the
  * 64 values in RASTER (de-zig-zagged) order, row-major 8 x 8.  Each value is dequantised, made odd toward zero and
- * clipped to [-2048, 2047], the intra DC as 8 * dc: ISO 11172-2's dct_recon, with ONE deviation, kept because these
+ * clipped to [-2048, 2047], the intra DC as sat16(8 * dc) (8 * dc saturated to int16: exact while |dc| <= 4095, which
+ * a conforming stream never leaves; the planes use the exact DC): ISO 11172-2's dct_recon, with ONE deviation, kept because these
  * are the values the pictures' samples are made from: the product level * quantiser_scale * Q is shifted right
  * arithmetically by 4, so a negative product is rounded toward minus infinity where ISO truncates toward zero.
  * Every value of a block whose cbp bit is clear, and of a macroblock without PRESENT, is 0: every byte of
@@ -405,8 +406,11 @@ long jsmpeg_b200_batch_decode_coefficients(jsmpeg_b200_batch_t *b, int n, const 
  * block (the reference's shortcut, which the transform equals), and a damaged picture follows decode_coefficients'
  * rule (the block with the bad code, and those after it, are 0).  For a clean stream, the residual of an intra
  * macroblock is its samples before the clamp (its prediction is 0), that of any other PRESENT macroblock what stage 2
- * adds to its prediction when decode() reconstructs the picture.  Coefficients are clipped to [-2048, 2047], which
- * bounds every value well inside int16 (|r| <= 14,314; tests/test_residual_export.py).  mb_dst may be NULL; otherwise
+ * adds to its prediction when decode() reconstructs the picture.  An intra block's DC enters the transform as dc * 256
+ * (the reference's dc << 8) with dc clamped to [-16000, 16255], a clamp that changes no sample (the transform of the
+ * rest of the block stays within +-14,315); while |dc| <= 4095 that is decode_coefficients' 8 * dc times 32.
+ * Coefficients are clipped to [-2048, 2047], so every value of a non-intra block satisfies |r| <= 14,314 and every
+ * value of an intra one lies in [-32,000, 32,255] (255 + 2 * 16000): inside int16 (tests/test_residual_export.py).  mb_dst may be NULL; otherwise
  * mb_dst[i] (16-byte aligned) gets exactly what decode_macroblocks writes for the request, from the same walk: its
  * INTRA / FORWARD / BACKWARD flags say how to read the residual.
  *

@@ -88,10 +88,10 @@ accumulate_kernel(const AccTask *__restrict__ tasks, int n_tasks, uint32_t total
 #pragma unroll
 			for (int i = 0; i < 8; i++) q[i] = make_uint4(0u, 0u, 0u, 0u);
 		}
-		idct_block(q, v);
+		idct_block(q, v, false);  // (intra blocks end a trace: `coded` leaves them out)
 	} else {
 		const int c0 = !coded ? 0 : (dense ? (int)__ldg(t.coef + ((size_t)mb * 6 + b) * 64) : coef_record_dc(cr));
-		const int dc = coded ? idct_dc(c0) : 0;
+		const int dc = coded ? idct_dc(c0, false) : 0;
 #pragma unroll
 		for (int i = 0; i < 64; i++) v[i] = dc;
 	}

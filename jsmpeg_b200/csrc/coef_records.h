@@ -6,7 +6,7 @@
  * slot mb * 6 + b:
  *     uint64_t mask       bit k set <=> zig-zag position k was written by the block's codes
  *     int16_t  level[12]  the written values in zig-zag order: the k-th set bit of `mask` goes with level[k]
- * The values are exactly those of the dense record: dequantised, oddified, clipped, intra DC as dc * 8.  Positions
+ * The values are exactly those of the dense record: dequantised, oddified, clipped, intra DC as dc (records.h).  Positions
  * inside a block only increase (run >= 0; a store past position 63 is dropped), so the order is well defined.
  * A block with more than COEF_RECORD_LEVELS positions has mask == COEF_RECORD_DENSE: its dense 128-byte record
  * holds it, at its usual place in the coefficient plane.  Uncoded blocks write and read nothing.

@@ -63,6 +63,10 @@ export_coefficients_kernel(const CoefExportTask *__restrict__ tasks, int n_tasks
 			coef_record_row(cr, row, v);
 			memcpy(&out, v, sizeof out);
 		}
+		if (row == 0 && (rec & MBF_INTRA)) {  // an intra DC leaves in its public form, sat16(8 * dc) (records.h)
+			const int dc8 = max(-32768, min(32767, 8 * (int)(int16_t)(out.x & 0xffffu)));
+			out.x = (out.x & 0xffff0000u) | ((uint32_t)dc8 & 0xffffu);
+		}
 	}
 	__stcs(reinterpret_cast<uint4 *>(t.dst) + (size_t)mb * ROWS_PER_MB + r, out);
 }

@@ -60,7 +60,7 @@ struct ParseTask {
 	mb_record_t *hdr;      // [mb_size]
 	int16_t *coef;         // [mb_size][6][64]
 	picture_info_t *info;  // out
-	uint2 *park;           // [mb_size][6]: per coded block {bit offset of its first coefficient code, intra dc * 8},
+	uint2 *park;           // [mb_size][6]: per coded block {bit offset of its first coefficient code, intra dc},
 	                       // the walk's hand-over to stage 1b (a dense side array, written and read as a stream)
 	int32_t mb_width, mb_size;  // copies of the sequence parameters (no dependent load in front of the walk)
 	// lane-parallel walk: staging area for relative macroblock records (walk.cuh, WALK_STAGE): stage_entries

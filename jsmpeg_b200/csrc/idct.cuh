@@ -59,13 +59,21 @@ __device__ __forceinline__ void idct_rows(int (&v)[64]) {
 	}
 }
 
+// The premultiplied coefficient 0: an intra block's is its dc (records.h), x 256 = the reference's dc << 8
+// (src/mpeg1.js:747); any other block's is a level, x PREMULTIPLIER[0].  `lo` holds it in its low 16 bits.
+__device__ __forceinline__ int premultiplied_c0(uint32_t lo, bool intra) {
+	return intra ? (int)(lo << 16) >> 8 : __dp2a_lo((int)lo, PM[0], 0);
+}
+
 // The residual of one block from its 64 coefficients in raster order, eight per uint4 (int16 pairs, low half first):
 // each times its premultiplier (dp2a: lo16 * byte 0 + hi16 * byte 1, one instruction per coefficient), then the
-// column and the row passes -- px[] of the reference before the add or clamp (src/mpeg1.js:916-983).
-__device__ __forceinline__ void idct_block(const uint4 (&q)[8], int (&v)[64]) {
+// column and the row passes -- px[] of the reference before the add or clamp (src/mpeg1.js:916-983).  `intra`: the
+// block is an intra one, whose coefficient 0 is its dc (premultiplied_c0); without it, a level like any other.
+__device__ __forceinline__ void idct_block(const uint4 (&q)[8], int (&v)[64], bool intra = false) {
 #pragma unroll
 	for (int i = 0; i < 8; i++) {
-		v[i * 8 + 0] = __dp2a_lo((int)q[i].x, PM[i * 8 + 0], 0); v[i * 8 + 1] = __dp2a_lo((int)q[i].x, PM[i * 8 + 1] << 8, 0);
+		v[i * 8 + 0] = i ? __dp2a_lo((int)q[i].x, PM[i * 8 + 0], 0) : premultiplied_c0(q[0].x, intra);
+		v[i * 8 + 1] = __dp2a_lo((int)q[i].x, PM[i * 8 + 1] << 8, 0);
 		v[i * 8 + 2] = __dp2a_lo((int)q[i].y, PM[i * 8 + 2], 0); v[i * 8 + 3] = __dp2a_lo((int)q[i].y, PM[i * 8 + 3] << 8, 0);
 		v[i * 8 + 4] = __dp2a_lo((int)q[i].z, PM[i * 8 + 4], 0); v[i * 8 + 5] = __dp2a_lo((int)q[i].z, PM[i * 8 + 5] << 8, 0);
 		v[i * 8 + 6] = __dp2a_lo((int)q[i].w, PM[i * 8 + 6], 0); v[i * 8 + 7] = __dp2a_lo((int)q[i].w, PM[i * 8 + 7] << 8, 0);
@@ -75,7 +83,8 @@ __device__ __forceinline__ void idct_block(const uint4 (&q)[8], int (&v)[64]) {
 }
 
 // The residual of a DC-only block, every sample: the reference's shortcut (mpeg1.js:838-853), which the full
-// transform of such a block equals (column 0 comes out as eight copies of c0 * PM[0], every other term of a row is 0)
-__device__ __forceinline__ int idct_dc(int c0) { return (c0 * PM[0] + 128) >> 8; }
+// transform of such a block equals (column 0 comes out as eight copies of the premultiplied c0, every other term of a
+// row is 0): (c0 * 256 + 128) >> 8 = c0 for an intra block
+__device__ __forceinline__ int idct_dc(int c0, bool intra = false) { return intra ? c0 : (c0 * PM[0] + 128) >> 8; }
 
 }  // namespace

@@ -514,7 +514,8 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 			memcpy(&q, wstage + lane * ROW_PITCH + i * 16, 16);
 #endif
 			// dp2a: (lo16 * b0 + hi16 * b1): one instruction per coefficient, no unpacking on the ALU pipe
-			v[i * 8 + 0] = __dp2a_lo((int)q.x, PM[i * 8 + 0], 0); v[i * 8 + 1] = __dp2a_lo((int)q.x, PM[i * 8 + 1] << 8, 0);
+			v[i * 8 + 0] = i ? __dp2a_lo((int)q.x, PM[i * 8 + 0], 0) : premultiplied_c0(q.x, intra);
+			v[i * 8 + 1] = __dp2a_lo((int)q.x, PM[i * 8 + 1] << 8, 0);
 			v[i * 8 + 2] = __dp2a_lo((int)q.y, PM[i * 8 + 2], 0); v[i * 8 + 3] = __dp2a_lo((int)q.y, PM[i * 8 + 3] << 8, 0);
 			v[i * 8 + 4] = __dp2a_lo((int)q.z, PM[i * 8 + 4], 0); v[i * 8 + 5] = __dp2a_lo((int)q.z, PM[i * 8 + 5] << 8, 0);
 			v[i * 8 + 6] = __dp2a_lo((int)q.w, PM[i * 8 + 6], 0); v[i * 8 + 7] = __dp2a_lo((int)q.w, PM[i * 8 + 7] << 8, 0);
@@ -530,9 +531,9 @@ __device__ __forceinline__ void reconstruct_at(const PARAMS &params, int ty, int
 #else
 			memcpy(&d0, wstage + lane * ROW_PITCH, 2);
 #endif
-			dc = ((int)d0 * PM[0] + 128) >> 8;
+			dc = idct_dc(d0, intra);
 		} else if (c0.x & 1u) {  // a compact record's first value is coefficient 0 when zig-zag position 0 is written
-			dc = ((int)(int16_t)(c0.z & 0xffffu) * PM[0] + 128) >> 8;
+			dc = idct_dc((int)(int16_t)(c0.z & 0xffffu), intra);
 		}
 #pragma unroll
 		for (int i = 0; i < 64; i++) v[i] = dc;

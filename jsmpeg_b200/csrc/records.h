@@ -22,8 +22,15 @@
  * Coefficient values: the reference keeps `level * PREMULTIPLIER_MATRIX[i]` in int32
  * (src/mpeg1.js:810); that does not fit int16 (2047*62), so the record holds the dequantised,
  * oddified, clipped level in [-2048, 2047] (src/mpeg1.js:794-807) and stage 2 applies the
- * premultiplier in int32.  Intra DC is stored as dc*8, so that dc*8*PREMULTIPLIER[0](=32) equals
- * the reference's `dc << 8` (src/mpeg1.js:747).
+ * premultiplier in int32.  Intra DC is stored as dc itself, and stage 2 multiplies an intra block's coefficient 0
+ * by 256 instead of PREMULTIPLIER[0] (= 32): the reference's `dc << 8` (src/mpeg1.js:747).  The predictor is an
+ * unbounded sum of differentials (up to +-255 per block), so the record clamps it to
+ * [-INTRA_DC_BOUND, 255 + INTRA_DC_BOUND], and that is exact: in the reference's transform the DC term is only ever
+ * added (src/mpeg1.js:916-983), so every intra sample is clamp255(dc + ac(x)), ac being the transform of the block with
+ * its DC set to 0, and |ac(x)| <= 14,315 (DESIGN 3.10's bound for any block of coefficients in [-2048, 2047]) <
+ * INTRA_DC_BOUND.  A DC past either end therefore gives 0 or 255 in every sample, clamped or not.  The range fits
+ * int16, and so does every residual of an intra block: |dc + ac(x)| <= 255 + 2 * INTRA_DC_BOUND = 32,255.
+ * (decode_coefficients still reports an intra DC as sat16(8 * dc): the export converts it.)
  */
 #ifndef JSMPEG_B200_RECORDS_H
 #define JSMPEG_B200_RECORDS_H
@@ -50,7 +57,8 @@ typedef struct mb_record_t {
 	uint32_t mv_bwd;    /* B pictures: backward vector, (uint16)h | (uint16)v << 16, same units; else 0 */
 } mb_record_t;
 
-#define MB_COEF_INT16 (6 * 64) /* int16 per macroblock in the coefficient plane */
+#define MB_COEF_INT16 (6 * 64)
+#define INTRA_DC_BOUND 16000   /* intra DC in the records: clamped to [-INTRA_DC_BOUND, 255 + INTRA_DC_BOUND] */ /* int16 per macroblock in the coefficient plane */
 
 /* Picture-level result of stage 1 (one per picture start code that decode() consumes). */
 #define PIC_DECODED 1 /* I or P picture: reconstruct + swap (mpeg1.js:216-246)                  */

@@ -65,6 +65,7 @@ export_residuals_kernel(const ResExportTask *__restrict__ tasks, int n_tasks, ui
 	const uint32_t bit = 0x20u >> b;
 	const bool coded = (rec & MBF_PRESENT) && ((rec >> 8) & bit);
 	const bool full = coded && !((rec >> 16) & bit);
+	const bool intra = rec & MBF_INTRA;
 	coef_record_t cr;
 	cr.mask = 0;
 	if (coded) {
@@ -93,10 +94,10 @@ export_residuals_kernel(const ResExportTask *__restrict__ tasks, int n_tasks, ui
 #pragma unroll
 			for (int i = 0; i < 8; i++) q[i] = make_uint4(0u, 0u, 0u, 0u);
 		}
-		idct_block(q, v);
+		idct_block(q, v, intra);
 	} else {
 		const int c0 = !coded ? 0 : (dense ? (int)__ldg(t.coef + ((size_t)mb * 6 + b) * 64) : coef_record_dc(cr));
-		const int dc = coded ? idct_dc(c0) : 0;
+		const int dc = coded ? idct_dc(c0, intra) : 0;
 #pragma unroll
 		for (int i = 0; i < 64; i++) v[i] = dc;
 	}

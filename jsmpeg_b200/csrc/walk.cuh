@@ -282,14 +282,14 @@ __device__ __forceinline__ uint16_t walk_entry(uint16_t e) {
 }
 
 // One coded block (bitstream side of src/mpeg1.js:698-811): intra DC with its predictor, then only
-// code lengths.  Leaves {bit offset of the first coefficient code, dc * 8} in the block's slot.
+// code lengths.  Leaves {bit offset of the first coefficient code, intra dc clamped as records.h says} in the block's slot.
 // head: DC size VLC + differential + predictor (mpeg1.js:705-751), the parked pair, dct_coeff_first
-// RAW_DC (staging): the pair holds the DC predictor's value itself (possibly relative) instead of dc * 8
+// RAW_DC (staging): the pair holds the DC predictor's value itself (possibly relative), not yet clamped
 template <bool DEFER, bool RAW_DC = false, class BR>
 __device__ __forceinline__ bool walk_block_head(BR &br, uint32_t sbase, PictureState &ps, bool intra, int block,
                                                 uint2 *__restrict__ park, bool store, int &n, bool &defer_first) {
 	n = 0;
-	int dc8 = 0, dc_raw = 0;
+	int dc_rec = 0, dc_raw = 0;
 	if (intra) {
 		const uint32_t w = br.peek32();
 		const uint32_t e = block < 4 ? lds_u16(sbase + OFF_DC_LUMA + (w >> 25) * 2u)
@@ -315,10 +315,10 @@ __device__ __forceinline__ bool walk_block_head(BR &br, uint32_t sbase, PictureS
 		}
 		*pred = dc;
 		dc_raw = dc;
-		dc8 = max(-32768, min(32767, dc * 8));  // x PREMULTIPLIER[0] = dc << 8 in stage 2 (mpeg1.js:747)
+		dc_rec = max(-INTRA_DC_BOUND, min(255 + INTRA_DC_BOUND, dc));  // x 256 = dc << 8 in stage 2 (mpeg1.js:747)
 		n = 1;
 	}
-	if (store) *park = make_uint2(br.bitpos(), RAW_DC ? (uint32_t)dc_raw : (uint32_t)dc8 & 0xffffu);
+	if (store) *park = make_uint2(br.bitpos(), RAW_DC ? (uint32_t)dc_raw : (uint32_t)dc_rec & 0xffffu);
 	if (DEFER) {
 		defer_first = !intra;  // the caller's first look-up resolves dct_coeff_first (ac_step)
 	} else if (!intra && (br.peek32() >> 31)) {  // dct_coeff_first: a leading '1' is (0, +-1), never end_of_block
@@ -1028,13 +1028,13 @@ __device__ bool walk_slice_lanes(BR &br, uint32_t sbase, PictureState &ps, const
 					if (!(flags & 4u)) { ph = wrap_mv(x.mvh + ph, ps.f); pv = wrap_mv(x.mvv + pv, ps.f); }
 					const int cbp = (int)((w.y >> 8) & 0xffu);
 					uint4 pr[3] = {e[1], e[2], e[3]};  // six {bit offset, DC predictor} pairs; uncoded blocks' are stale, never read
-					if (flags & 1u) {  // intra: predictor value -> dc * 8 (x PREMULTIPLIER[0] = dc << 8 in stage 2, mpeg1.js:747)
+					if (flags & 1u) {  // intra: predictor value -> the record's clamped dc (x 256 = dc << 8 in stage 2, mpeg1.js:747)
 						uint32_t *v = reinterpret_cast<uint32_t *>(pr);
 #pragma unroll
 						for (int block = 0; block < 6; block++) {
 							int dc = (int)v[block * 2 + 1];
 							if (!(flags & 8u)) dc += block < 4 ? x.dcy : (block == 4 ? x.dc4 : x.dc5);
-							v[block * 2 + 1] = (uint32_t)max(-32768, min(32767, dc * 8)) & 0xffffu;
+							v[block * 2 + 1] = (uint32_t)max(-INTRA_DC_BOUND, min(255 + INTRA_DC_BOUND, dc)) & 0xffffu;
 						}
 					} else {
 						pr[0].y = pr[0].w = pr[1].y = pr[1].w = pr[2].y = pr[2].w = 0u;
@@ -1199,7 +1199,7 @@ __device__ void walk_picture(const ParseTask &t, uint32_t sbase, int lane, uint3
 // ==================================================================================================
 // 1b: coded blocks, from the offset the walk parked to the finished record.
 // rec = the macroblock record's second word (flags | cbp << 8 | dc_only << 16 | quantiser scale << 24),
-// parked = {bit offset of the block's first coefficient code, intra dc * 8} from the walk's dense side array.
+// parked = {bit offset of the block's first coefficient code, intra dc (clamped, records.h)} from the walk's dense side array.
 //
 // Run/level codes arrive in zig-zag order, and the compact record (coef_records.h) IS the position mask plus the
 // values in zig-zag order: the k-th value a block's codes give is level[k].  So a block is built as its compact

@@ -162,6 +162,9 @@ typedef struct {
 } parse_t;
 
 static int g_decode_b = 0;
+/* test hook: the least and the greatest intra DC predictor of the last picture parsed (before the records' clamp) */
+static int g_dc_lo, g_dc_hi;
+void oracle_last_dc_range(int *lo, int *hi) { *lo = g_dc_lo; *hi = g_dc_hi; }
 /* the B-picture extension: 0 (default) = B pictures are skipped like the reference does */
 void oracle_set_decode_b(int on) { g_decode_b = on; }
 
@@ -170,8 +173,6 @@ static void reset_mv(parse_t *p) {
 	p->mv_h = p->mv_v = p->mv_h_prev = p->mv_v_prev = 0;
 	p->mvb_h = p->mvb_v = p->mvb_h_prev = p->mvb_v_prev = 0; /* (unused outside B pictures) */
 }
-
-static int16_t sat16(int v) { return (int16_t)(v > 32767 ? 32767 : (v < -32768 ? -32768 : v)); }
 
 /* mpeg1.js:698-811 decodeBlock, bitstream part only.  Returns false on an invalid code. */
 static bool parse_block(parse_t *p, int mb, int block, bool intra, uint8_t *dc_only_mask) {
@@ -192,7 +193,11 @@ static bool parse_block(parse_t *p, int mb, int block, bool intra, uint8_t *dc_o
 			else dc += (int)((~0u << size) | (uint32_t)(diff + 1));
 		}
 		*pred = dc;
-		out[0] = sat16(dc * 8); /* x PREMULTIPLIER[0]=32 in stage 2 gives dc<<8, mpeg1.js:747 */
+		if (dc < g_dc_lo) g_dc_lo = dc;
+		if (dc > g_dc_hi) g_dc_hi = dc;
+		/* stage 2 takes coefficient 0 of an intra block x 256 = the reference's dc << 8 (mpeg1.js:747); clamped to the
+		 * range in which that is exact (records.h: INTRA_DC_BOUND) */
+		out[0] = (int16_t)(dc < -INTRA_DC_BOUND ? -INTRA_DC_BOUND : (dc > 255 + INTRA_DC_BOUND ? 255 + INTRA_DC_BOUND : dc));
 		q = p->seq->intra_q;
 		n = 1;
 	} else {
@@ -387,6 +392,7 @@ void oracle_parse_picture(const uint8_t *es, uint32_t es_len, uint32_t start_bit
 	p.bits.bytes = es; p.bits.length = es_len; p.bits.index = start_bit;
 	p.seq = seq; p.info = info; p.hdr = hdr; p.coef = coef;
 	info->start_byte = start_bit >> 3;
+	g_dc_lo = g_dc_hi = 128;
 
 	bits_skip(&p.bits, 10);
 	p.picture_type = bits_read(&p.bits, 3);
@@ -547,11 +553,12 @@ static void reconstruct_picture(const seq_params_t *seq, int coded_width, int co
 				dst = (block == 4 ? cur->cb : cur->cr) + row * 8 * hw + col * 8;
 			}
 			int px[64];
+			const int pm0 = intra ? 256 : ORACLE_PREMULTIPLIER[0]; /* an intra block's coefficient 0 is dc itself */
 			if (r->dc_only & (0x20 >> block)) { /* mpeg1.js:838-841, 850-853 */
-				int v = (c[0] * ORACLE_PREMULTIPLIER[0] + 128) >> 8;
+				int v = (c[0] * pm0 + 128) >> 8;
 				for (int k = 0; k < 64; k++) px[k] = v;
 			} else {
-				for (int k = 0; k < 64; k++) px[k] = c[k] * ORACLE_PREMULTIPLIER[k];
+				for (int k = 0; k < 64; k++) px[k] = c[k] * (k ? ORACLE_PREMULTIPLIER[k] : pm0);
 				for (int k = 0; k < 8; k++) idct_pass(px + k, 8, false);
 				for (int k = 0; k < 8; k++) idct_pass(px + 8 * k, 1, true);
 			}

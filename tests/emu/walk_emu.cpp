@@ -159,7 +159,7 @@ extern "C" void emu_set_quant(const uint8_t *intra_q, const uint8_t *non_intra_q
 	memcpy(emu_non_intra_q, non_intra_q, 64);
 }
 
-// park: [mb_size][6] x {bit offset, dc * 8}, the walk's dense hand-over to stage 1b.
+// park: [mb_size][6] x {bit offset, intra dc (clamped, records.h)}, the walk's dense hand-over to stage 1b.
 // lanes: 0 serial walk, 1 lane-parallel walk with its staging area (stage_entries_for(mb_size) entries, the
 // product's size), 2 lane-parallel walk with a staging area of 40 entries (lanes run out: second-pass
 // fall-back), 3 lane-parallel walk without staging area (always the second pass), 4 the slice walk (walk_slices.cuh:
@@ -298,7 +298,8 @@ extern "C" int emu_reconstruct_picture_b(const mb_record_t *hdr, const int16_t *
 }
 
 // Stage 1b's sign-magnitude dequantisation (dequant_sm, walk.cuh) against the reference's statements
-// (src/mpeg1.js:794-807, src/wasm/mpeg1.c decode_block), every level an escape or a table code can carry,
+// (src/mpeg1.js:794-807, src/wasm/mpeg1.c decode_block), every level an escape or a table code can carry
+// (-256 included: the escape (128, 0)),
 // every quantiser scale (0 included: a corrupt stream can carry it), every matrix entry, intra and not.
 // Returns the number of mismatches; first_bad = {level, qs, Q, intra, got, want} of the first one.
 extern "C" long emu_check_dequant(int *first_bad) {
@@ -306,7 +307,7 @@ extern "C" long emu_check_dequant(int *first_bad) {
 	for (int intra = 0; intra < 2; intra++)
 		for (int qs = 0; qs < 32; qs++)
 			for (int Q = 0; Q < 256; Q++)
-				for (int lv = -255; lv <= 255; lv++) {
+				for (int lv = -256; lv <= 255; lv++) {
 					int level = lv;  // the reference, statement for statement
 					level <<= 1;
 					if (!intra) level += (level < 0 ? -1 : 1);

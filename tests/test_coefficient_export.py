@@ -113,16 +113,19 @@ def test_fresh_coefficients_equal_the_sequential_decode(name):
     assert checked == len(by_pos) > 0 and coded > 0, name
 
 
-def test_the_model_zeroes_uncoded_blocks_and_absent_macroblocks():
+def test_the_model_zeroes_uncoded_blocks_and_absent_macroblocks_and_reports_intra_dc_as_8_dc():
     rec = np.zeros((3, 16), np.uint8)
     rec[0, 4], rec[0, 5] = macroblock_model.MBF_PRESENT, 0b100001  # blocks 0 and 5 coded
     rec[1, 4], rec[1, 5] = 0, 0x3F                                  # absent: cbp ignored
     rec[2, 4], rec[2, 5] = macroblock_model.MBF_PRESENT | macroblock_model.MBF_INTRA, 0x3F
     coef = np.arange(3 * 6 * 64, dtype=np.int16) + 1
+    coef[(2 * 6 + 1) * 64], coef[(2 * 6 + 2) * 64] = 5000, -4097  # records' intra DCs whose 8 * dc leaves int16
     got = macroblock_model.coefficients(rec, coef)
     want = coef.reshape(3, 6, 64).copy()
     want[0, 1:5] = 0
     want[1] = 0
+    want[2, :, 0] = np.clip(8 * want[2, :, 0].astype(np.int64), -32768, 32767)  # an intra DC leaves as sat16(8 * dc)
+    assert (want[2, 1, 0], want[2, 2, 0]) == (32767, -32768)
     assert got.dtype == np.int16 and np.array_equal(got, want)
 
 

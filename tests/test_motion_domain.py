@@ -144,7 +144,7 @@ def test_model_idct_is_the_references():
         assert np.array_equal(recon_model.idct(stored[kind + "_in"]), stored[kind + "_out"]), kind
 
 
-def test_model_rules_on_hand_made_records():
+def test_model_rules_on_hand_made_records_with_the_intra_dc_x_256():
     """One macroblock of 2 x 2 on a ramp, each rule in isolation: flat-index wrap, the four roundings, a tap out, chroma
     truncation toward zero, B averaging, absent and intra macroblocks, dc_only."""
     mbw, mbh = 2, 2
@@ -195,7 +195,9 @@ def test_model_rules_on_hand_made_records():
     out = recon_model.reconstruct(r, coef, ref, cur, mbw, mbh)
     blk = np.zeros(64, np.int64)
     blk[0], blk[5] = 100, 7
-    want = np.clip(recon_model.idct(blk * recon_model.mm.PREMULTIPLIER), 0, 255).reshape(8, 8)
+    pm = recon_model.mm.PREMULTIPLIER.copy()
+    pm[0] = 256  # an intra block's coefficient 0 is its dc itself, x 256 (jsmpeg_b200/csrc/records.h)
+    want = np.clip(recon_model.idct(blk * pm), 0, 255).reshape(8, 8)
     assert np.array_equal(out[:ysz].reshape(-1, cw)[:8, 16:24], want)
     assert (out[:ysz].reshape(-1, cw)[:8, 24:32] == 0).all()  # an intra block without coefficients: 0
 

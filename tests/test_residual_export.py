@@ -113,6 +113,30 @@ def test_every_residual_fits_int16():
     assert np.abs(got).max() <= limit and np.abs(got).max() > limit - 64, (np.abs(got).max(), limit)
 
 
+def test_the_intra_dc_clamp_is_exact_and_keeps_intra_residuals_in_int16():
+    """records.h clamps an intra DC to [-C, 255 + C], C = INTRA_DC_BOUND, and stage 2 takes it x 256.  The DC term of
+    the transform is only added, so an intra sample is clamp255(dc + ac(x)) with ac the transform of the block with its
+    DC at 0; |ac(x)| is below the bound above (any coefficients in [-2048, 2047]), which is below C: the clamp changes no
+    sample.  And every intra residual dc + ac(x) stays within [-2C, 255 + 2C], inside int16."""
+    import re
+    c = int(re.search(r"#define INTRA_DC_BOUND (\d+)",
+                      open(os.path.join(helpers.ROOT, "jsmpeg_b200", "csrc", "records.h")).read()).group(1))
+    limit = max(b.magnitude() for b in transform_bounds())
+    assert limit < c and 255 + 2 * c <= 32767, (limit, c)
+    # the DC term is additive: dc x 256 moves every output of the transform by exactly dc
+    rng = np.random.default_rng(5)
+    ac = rng.integers(LO, HI + 1, size=(200, 64))
+    ac[:, 0] = 0
+    ac = np.concatenate([ac, extreme_blocks(transform_bounds())])
+    ac[:, 0] = 0
+    base = macroblock_model.idct(ac * PM)
+    for dc in (-c, -4097, -1, 0, 255, 4096, 255 + c):
+        blk = ac * PM
+        blk[:, 0] = dc * 256
+        assert np.array_equal(macroblock_model.idct(blk), base + dc), dc
+    assert np.abs(base).max() < c
+
+
 def test_the_numpy_transform_equals_the_reference_and_the_oracle():
     stored = np.load(os.path.join(helpers.REFERENCE_DATA, "idct.npz"))
     for name in ("random", "sparse_extreme"):

@@ -59,7 +59,7 @@ def picture_starts(es):
 def walk(lib, buf, n, start, mbw, mbh, lanes):
     mb = mbw * mbh
     hdr = np.zeros(mb * 4, dtype=np.uint32)
-    park = np.full(mb * 6 * 2, 0xDEADBEEF, dtype=np.uint32)  # 8 bytes per coded block: {bit offset, dc * 8}
+    park = np.full(mb * 6 * 2, 0xDEADBEEF, dtype=np.uint32)  # 8 bytes per coded block: {bit offset, intra dc}
     info = np.zeros(12, dtype=np.int32)
     lib.emu_walk_picture(buf.ctypes.data, n, start, mbw, mbh, hdr.ctypes.data, park.ctypes.data, info.ctypes.data, lanes)
     return hdr.reshape(mb, 4), park.reshape(mb * 6, 2), info

@@ -82,8 +82,18 @@ def export(records, picture_type):
 def coefficients(records, coef):
     """What decode_coefficients gives (int16 [n, 6, 64], each block in raster order) for n mb_record_t (any 16-byte-
     per-record buffer) and the int16 coefficient plane of the same picture ([n * 6 * 64] values in the oracle's layout,
-    which is the public one): the plane, with every value 0 where the macroblock is not PRESENT or the block's cbp bit
-    (bit 5 - block) is clear."""
+    whose intra DC is the clamped dc of the records, jsmpeg_b200/csrc/records.h): the plane, with every value 0 where the
+    macroblock is not PRESENT or the block's cbp bit (bit 5 - block) is clear, and an intra block's coefficient 0 in its
+    public form sat16(8 * dc)."""
+    c = records_coefficients(records, coef).astype(np.int64)
+    intra = (np.frombuffer(np.ascontiguousarray(records).tobytes(), RECORD)["flags"] & MBF_INTRA) != 0
+    c[:, :, 0] = np.where(intra[:, None], np.clip(8 * c[:, :, 0], -32768, 32767), c[:, :, 0])
+    return c.astype(np.int16)
+
+
+def records_coefficients(records, coef):
+    """The coefficient plane as the records hold it (intra DC = the clamped dc itself), int16 [n, 6, 64], every value 0
+    where the macroblock is not PRESENT or the block's cbp bit is clear"""
     r = np.frombuffer(np.ascontiguousarray(records).tobytes(), RECORD)
     c = np.frombuffer(np.ascontiguousarray(coef).tobytes(), np.int16).reshape(len(r), 6, 64)
     coded = ((r["flags"] & MBF_PRESENT) != 0)[:, None] & ((r["cbp"][:, None] >> (5 - np.arange(6))) & 1).astype(bool)
@@ -138,16 +148,23 @@ def idct(blocks):
 
 def residuals(records, coef, mb_width, mb_height):
     """What decode_residuals gives (int16 [coded_size * 3 // 2]: Y | Cr | Cb) for the records and coefficient plane of
-    a picture of mb_width x mb_height macroblocks: residual_planes() of its coefficients()."""
-    return residual_planes(coefficients(records, coef), mb_width, mb_height)
+    a picture of mb_width x mb_height macroblocks: residual_planes() of the records' coefficients, an intra block's
+    coefficient 0 (its clamped dc) premultiplied by 256."""
+    intra = (np.frombuffer(np.ascontiguousarray(records).tobytes(), RECORD)["flags"] & MBF_INTRA) != 0
+    return residual_planes(records_coefficients(records, coef), mb_width, mb_height, intra)
 
 
-def residual_planes(blocks, mb_width, mb_height):
-    """The residual of a picture from what decode_coefficients gives for it (int16 [mb_size, 6, 64] or any shape of as
-    many values): every block premultiplied and transformed (idct), placed where stage 2 writes it -- blocks 0-3 the
-    luma quadrants, 4 Cb (the third plane), 5 Cr (the second).  int16 [coded_size * 3 // 2]: Y | Cr | Cb."""
-    c = np.asarray(blocks).reshape(-1, 64).astype(np.int64)
-    px = idct(c * PREMULTIPLIER).astype(np.int16).reshape(mb_height, mb_width, 6, 8, 8)
+def residual_planes(blocks, mb_width, mb_height, intra=None):
+    """The residual of a picture from its coefficient blocks (int16 [mb_size, 6, 64] or any shape of as many values):
+    every block premultiplied and transformed (idct), placed where stage 2 writes it -- blocks 0-3 the luma quadrants,
+    4 Cb (the third plane), 5 Cr (the second).  int16 [coded_size * 3 // 2]: Y | Cr | Cb.  Without `intra` (bool per
+    macroblock) every coefficient 0 is x PREMULTIPLIER[0], which is what decode_coefficients' sat16(8 * dc) needs while
+    |dc| <= 4095; with it, an intra macroblock's coefficient 0 is its records' dc, x 256."""
+    c = np.asarray(blocks).reshape(-1, 6, 64).astype(np.int64)
+    pm = np.broadcast_to(PREMULTIPLIER, c.shape).copy()
+    if intra is not None:
+        pm[:, :, 0] = np.where(np.asarray(intra).reshape(-1)[:, None], 256, PREMULTIPLIER[0])
+    px = idct((c * pm).reshape(-1, 64)).astype(np.int16).reshape(mb_height, mb_width, 6, 8, 8)
     y = px[:, :, :4].reshape(mb_height, mb_width, 2, 2, 8, 8).transpose(0, 2, 4, 1, 3, 5)
     cb = px[:, :, 4].transpose(0, 2, 1, 3)
     cr = px[:, :, 5].transpose(0, 2, 1, 3)

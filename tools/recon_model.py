@@ -8,7 +8,9 @@ Planes are flat uint8 arrays Y | Cr | Cb (coded_size * 3 // 2), records mb_recor
   * an intra block is its residual, saturated;
   * a predicted block is its prediction plus its residual, saturated;
   * the residual of a coded block is the reference's integer inverse transform of the premultiplied block, or for a
-    dc_only block (c0 * 32 + 128) >> 8 in every sample; an uncoded block's residual is 0;
+    dc_only block (c0 * 32 + 128) >> 8 in every sample; an intra block's c0 is its dc (the records' clamped one,
+    jsmpeg_b200/csrc/records.h) and is premultiplied by 256 instead, so its dc_only block is c0 itself; an uncoded
+    block's residual is 0;
   * prediction addresses by flat index: the block's first tap is origin + (v >> 1) * stride + (h >> 1), so a tap past a
     row's end is the next row's first sample; the half-sample flags h & 1, v & 1 choose the copy, (a + b + 1) >> 1
     horizontally or vertically, or (a + b + c + d + 2) >> 2;
@@ -83,8 +85,10 @@ def residual_planes(records, coef, mb_width, mb_height):
     bits = 0x20 >> np.arange(6)
     coded = (((r["flags"] & MBF_PRESENT) != 0)[:, None] & ((r["cbp"][:, None] & bits) != 0))
     dc_only = coded & ((r["dc_only"][:, None] & bits) != 0)
-    px = idct(c * mm.PREMULTIPLIER)
-    px = np.where(dc_only[:, :, None], ((c[:, :, :1] * mm.PREMULTIPLIER[0] + 128) >> 8), px)
+    pc = c * mm.PREMULTIPLIER
+    pc[:, :, 0] = np.where(((r["flags"] & MBF_INTRA) != 0)[:, None], c[:, :, 0] * 256, pc[:, :, 0])
+    px = idct(pc)
+    px = np.where(dc_only[:, :, None], ((pc[:, :, :1] + 128) >> 8), px)
     px = np.where(coded[:, :, None], px, 0).reshape(mb_height, mb_width, 6, 8, 8)
     y = px[:, :, :4].reshape(mb_height, mb_width, 2, 2, 8, 8).transpose(0, 2, 4, 1, 3, 5).reshape(-1)
     cb = px[:, :, 4].transpose(0, 2, 1, 3).reshape(-1)  # block 4 -> Cb, the third plane

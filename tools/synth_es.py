@@ -115,7 +115,28 @@ class Knobs:
         #   "mixed"    one of the four per macroblock
         # "inside" draws exactly what it always drew: the streams of the committed cases stay byte-identical.
         self.vectors = "inside"
+        # The value domain (VALUE_CASES).  None / 0 / "canonical" draw exactly what they always drew: the streams of
+        # the committed cases stay byte-identical.
+        #   dc_walk        None: every intra DC target in 0..255.  Else one mode per DC predictor (Y, the one of block
+        #                  4, the one of block 5): "keep" (a target in 0..255), "climb" / "descend" (every differential
+        #                  +-dc_step, turning back at +-dc_limit), "wander" (runs of dc_run blocks in one direction)
+        #   ac_cross_prob  of the intra blocks, the share whose AC coefficients are escapes of level +-255 signed like the
+        #                  transform's basis at one sample: |ac(x)| of several thousand, so that dc + ac(x) crosses 0 and
+        #                  255 when the DC is far outside 0..255
+        #   escape_forms   "all": besides the canonical escapes, the two-byte forms of small levels, (0, 0) = level 0
+        #                  and (128, 0) = level -256
+        #   qscales        None: quantiser scales 1..31; else the scales the slice and macroblock headers draw from
+        #   matrix_entries None: the default custom matrices; else the values every entry (intra Q[0] included) draws from
+        self.dc_walk = None
+        self.dc_step = (128, 255)
+        self.dc_limit = 300_000
+        self.dc_run = 24
+        self.ac_cross_prob = 0.0
+        self.escape_forms = "canonical"
+        self.qscales = None
+        self.matrix_entries = None
         self.__dict__.update(kw)
+        assert self.dc_limit + 255 < 1 << 23  # the reference keeps dc << 8 in an int
 
 
 class SynthStream:
@@ -138,7 +159,12 @@ class SynthStream:
         w.put(1, 1)          # marker
         w.put(20, 10)        # vbv buffer size
         w.put(0, 1)          # constrained
-        if self.k.custom_matrices:
+        if self.k.custom_matrices and self.k.matrix_entries is not None:
+            for _ in range(2):
+                w.put(1, 1)
+                for i in range(64):
+                    w.put(int(self.rng.choice(self.k.matrix_entries)), 8)
+        elif self.k.custom_matrices:
             w.put(1, 1)
             for i in range(64):
                 w.put(8 if i == 0 else int(self.rng.integers(4, 64)), 8)
@@ -178,12 +204,16 @@ class SynthStream:
                 w.put(int(self.rng.integers(1, 256)) | 0x40, 8)
 
     # ---------------------------------------------------------------- blocks
-    def block(self, w, intra, luma, dc_pred):
-        """One coded block.  Returns the new DC predictor (intra)."""
+    def block(self, w, intra, luma, dc_pred, which=0):
+        """One coded block (`which`: its DC predictor, 0 = Y, 1 = block 4's, 2 = block 5's).  Returns the new DC
+        predictor (intra)."""
         rng = self.rng
         if intra:
-            # keep the reconstructed DC in 0..255
-            target = int(rng.integers(0, 256)) if rng.random() < 0.7 else dc_pred
+            if self.k.dc_walk is None or self.k.dc_walk[which] == "keep":
+                # keep the reconstructed DC in 0..255
+                target = int(rng.integers(0, 256)) if rng.random() < 0.7 else dc_pred
+            else:
+                target = dc_pred + self.dc_step(which, dc_pred)
             diff = target - dc_pred
             size = 0 if diff == 0 else int(abs(diff)).bit_length()
             w.code((DC_LUMA_CODE if luma else DC_CHROMA_CODE)[size])
@@ -191,6 +221,9 @@ class SynthStream:
                 w.put(diff if diff > 0 else diff + (1 << size) - 1, size)
             dc_pred = target
             n = 1
+            if self.k.ac_cross_prob and rng.random() < self.k.ac_cross_prob:
+                self.crossing_ac(w)
+                return dc_pred
         else:
             n = 0
         if intra and rng.random() < self.k.dc_only_prob:
@@ -198,6 +231,7 @@ class SynthStream:
         else:
             count = int(rng.integers(1, self.k.max_coefs + 1))
         first = not intra
+        zero_tail = False  # the last escape ended in a zero byte: the next code is an escape too (5 leading zeros)
         for c in range(count):
             remaining = 63 - n
             if remaining < 0:
@@ -206,8 +240,8 @@ class SynthStream:
                 run = remaining  # land exactly on index 63
             else:
                 run = int(min(remaining, rng.geometric(0.35) - 1))
-            if rng.random() < self.k.escape_prob:
-                self.escape(w, run)
+            if zero_tail or rng.random() < self.k.escape_prob:
+                zero_tail = self.escape(w, run)
             else:
                 run_t = min(run, 31)
                 level = int(rng.integers(1, MAX_LEVEL_FOR_RUN[run_t] + 1))
@@ -232,8 +266,67 @@ class SynthStream:
         w.code(V.DCT_EOB_CODE)
         return dc_pred
 
+    def dc_step(self, which, dc_pred):
+        """The next DC differential of predictor `which` under Knobs.dc_walk: +-1..255, turning back at +-dc_limit"""
+        rng, k = self.rng, self.k
+        mode = k.dc_walk[which]
+        if mode == "wander":
+            self.wander = getattr(self, "wander", [1, 1, 1])
+            if rng.random() < 1.0 / k.dc_run:
+                self.wander[which] = -self.wander[which]
+            sign = self.wander[which]
+        else:
+            sign = 1 if mode == "climb" else -1
+        step = sign * int(rng.integers(k.dc_step[0], k.dc_step[1] + 1))
+        if abs(dc_pred + step) > k.dc_limit:
+            step = -step
+            if mode == "wander":
+                self.wander[which] = -self.wander[which]
+        return step
+
+    def crossing_ac(self, w):
+        """The AC coefficients of an intra block as escapes of level +-255 at zig-zag positions 1..K, each signed like
+        the 2-D cosine basis at one sample (y, x) -- all of them the same way or all the opposite way -- so that the
+        transform moves that sample by thousands; then end_of_block"""
+        rng = self.rng
+        y, x = int(rng.integers(0, 8)), int(rng.integers(0, 8))
+        s = 1 if rng.random() < 0.5 else -1
+        count = int(rng.integers(11, 64))
+        for n in range(1, count + 1):
+            r = V.ZIG_ZAG[n]
+            basis = np.cos((2 * x + 1) * (r % 8) * np.pi / 16) * np.cos((2 * y + 1) * (r // 8) * np.pi / 16)
+            level = 255 if s * basis > 0 else -255
+            if level < 0 and self.k.escape_forms == "all" and rng.random() < 0.3:
+                level = -256
+            self.escape_level(w, 0, level)
+        w.code(V.DCT_EOB_CODE)
+
+    def escape_level(self, w, run, level):
+        """An escape of `level` in -256..255 (0 and -256 only in their two-byte forms (0, 0) and (128, 0))"""
+        w.code(V.DCT_ESCAPE_CODE)
+        w.put(run, 6)
+        if 0 < abs(level) < 128:
+            w.put(level & 255, 8)
+        elif level >= 0:
+            w.put(0, 8)
+            w.put(level, 8)
+        else:
+            w.put(128, 8)
+            w.put(level + 256, 8)
+
     def escape(self, w, run):
         rng = self.rng
+        if self.k.escape_forms == "all" and rng.random() < 0.5:
+            # the two-byte forms of any level (0 and -256 only have those); level 0 only behind an odd run, and a
+            # level ending in a zero byte is followed by an escape or end_of_block, so that the zeros of the escape,
+            # the run, the level and the next code never make 23 in a row.  Returns whether it ends in a zero byte.
+            form = int(rng.integers(0, 4))
+            level = (0 if run & 1 else -256, -256, int(rng.integers(1, 128)), -int(rng.integers(1, 128)))[form]
+            w.code(V.DCT_ESCAPE_CODE)
+            w.put(run, 6)
+            w.put(0 if level >= 0 else 128, 8)
+            w.put(level & 255, 8)
+            return level in (0, -256)
         w.code(V.DCT_ESCAPE_CODE)
         w.put(run, 6)
         if rng.random() < self.k.big_escape_prob:
@@ -247,6 +340,10 @@ class SynthStream:
         else:
             level = int(rng.integers(1, 128))
             w.put(level if rng.random() < 0.5 else 256 - level, 8)
+        return False
+
+    def qscale(self):
+        return int(self.rng.integers(1, 32)) if self.k.qscales is None else int(self.rng.choice(self.k.qscales))
 
     # ---------------------------------------------------------------- motion
     def motion_component(self, w, target, prev, f, r_size):
@@ -410,7 +507,7 @@ class SynthStream:
         mbw = self.mbw
         row = first_mb // mbw
         w.start_code(row + 1)
-        qscale = int(rng.integers(1, 32))
+        qscale = self.qscale()
         w.put(qscale, 5)
         if rng.random() < 0.1:          # extra_information_slice
             w.put(1, 1)
@@ -447,7 +544,7 @@ class SynthStream:
                     mtype = int(rng.choice([0x0A, 0x02, 0x08, 0x1A, 0x12]))
                 w.code(TYPE_P_CODE[mtype])
             if mtype & 0x10:
-                qscale = int(rng.integers(1, 32))
+                qscale = self.qscale()
                 w.put(qscale, 5)
             intra = mtype & 0x01
             if intra:
@@ -468,7 +565,7 @@ class SynthStream:
             for blk in range(6):
                 if cbp & (0x20 >> blk):
                     which = 0 if blk < 4 else blk - 3
-                    dc[which] = self.block(w, intra, blk < 4, dc[which])
+                    dc[which] = self.block(w, intra, blk < 4, dc[which], which)
             mb += 1
         w.align()
         return w.tobytes()
@@ -479,7 +576,7 @@ class SynthStream:
         mbw = self.mbw
         row = first_mb // mbw
         w.start_code(row + 1)
-        qscale = int(rng.integers(1, 32))
+        qscale = self.qscale()
         w.put(qscale, 5)
         w.put(0, 1)
         f, r_size = 1 << (f_code - 1), f_code - 1
@@ -517,7 +614,7 @@ class SynthStream:
                 mtype = int(rng.choice([0x0C, 0x0E, 0x04, 0x06, 0x08, 0x0A, 0x1E, 0x1A, 0x16]))
             w.code(TYPE_B_CODE[mtype])
             if mtype & 0x10:
-                qscale = int(rng.integers(1, 32))
+                qscale = self.qscale()
                 w.put(qscale, 5)
             intra = mtype & 0x01
             if intra:
@@ -543,7 +640,7 @@ class SynthStream:
             for blk in range(6):
                 if cbp & (0x20 >> blk):
                     which = 0 if blk < 4 else blk - 3
-                    dc[which] = self.block(w, intra, blk < 4, dc[which])
+                    dc[which] = self.block(w, intra, blk < 4, dc[which], which)
             mb += 1
         w.align()
         return w.tobytes()
@@ -669,8 +766,82 @@ VECTOR_CASES = {
 }
 
 
+# Streams over the value domain of intra DC and coefficients (the Knobs after `vectors`): DC predictors far outside
+# 0..255 -- past +-4095 (where 8 * dc leaves int16), past the intra DC clamp of stage 2's records (+-16,000) and up to
+# about +-300,000 -- next to AC coefficients that make dc + ac(x) cross 0 and 255; every escape form, quantiser scales 0
+# and 31, matrix entries 0 and 255.  Every DC walk is reset in between by slice starts, non-intra macroblocks or skips,
+# depending on the case.  The compiled reference decodes every I and P picture of them: tests/golden/reference/decodes.json
+# holds its decodes.
+_CROSS = dict(ac_cross_prob=0.35, escape_forms="all", qscales=(31,))
+VALUE_CASES = {
+    "val_repro_96x16": None,  # value_repro(): the smallest stream that shows the 8 * dc saturation
+    "val_i_one_slice_300k": dict(knobs=dict(width=320, height=240, pictures=2, gop=1, slices="one", dc_walk=("climb", "descend", "wander"),
+                                            dc_step=(250, 255), dc_only_prob=0.1, **_CROSS), seed=41),
+    "val_i_one_slice_down": dict(knobs=dict(width=320, height=240, pictures=1, gop=1, slices="one", dc_walk=("descend", "wander", "climb"),
+                                            dc_step=(250, 255), dc_only_prob=0.1, **_CROSS), seed=42),
+    "val_i_rows_wander": dict(knobs=dict(width=352, height=96, pictures=3, gop=1, slices="rows", dc_walk=("wander", "wander", "wander"),
+                                         dc_run=12, dc_limit=20_000, **_CROSS), seed=43),
+    "val_i_random_slices": dict(knobs=dict(width=176, height=144, pictures=3, gop=1, slices="random", dc_walk=("wander", "climb", "descend"),
+                                           dc_limit=40_000, **_CROSS), seed=44),
+    "val_p_intra_resets": dict(knobs=dict(width=352, height=64, pictures=6, gop=3, slices="one", dc_walk=("wander", "climb", "descend"),
+                                          dc_limit=24_000, intra_in_p_prob=0.85, skip_prob=0.04, max_skip=3, **_CROSS), seed=45),
+    "val_lanes_640x480": dict(knobs=dict(width=640, height=480, pictures=2, gop=2, slices="one", dc_walk=("wander", "wander", "wander"),
+                                         dc_run=40, dc_limit=30_000, intra_in_p_prob=0.6, skip_prob=0.02, max_skip=2, ac_cross_prob=0.2,
+                                         escape_forms="all", qscales=(31,)), seed=46),
+    "val_quant_matrices": dict(knobs=dict(width=96, height=64, pictures=6, gop=3, slices="rows", custom_matrices=True,
+                                          matrix_entries=(0, 1, 255, 255, 37), qscales=(0, 31, 31, 1), escape_prob=0.5,
+                                          big_escape_prob=0.5, escape_forms="all", max_coefs=20, dc_walk=("wander", "wander", "wander"),
+                                          dc_run=8, dc_limit=9_000, ac_cross_prob=0.2), seed=47),
+    "val_quant_default": dict(knobs=dict(width=112, height=48, pictures=6, gop=2, slices="one", qscales=(0, 31), escape_prob=0.6,
+                                         escape_forms="all", max_coefs=24, dc_walk=("climb", "keep", "descend"), dc_limit=12_000), seed=48),
+}
+
+# B-picture streams over the same value domain: intra macroblocks of B pictures (decode_b).  No reference decodes of the
+# B pictures (the reference skips them); their expected values come from the oracle.
+VALUE_B_CASES = {
+    "val_b_intra": dict(knobs=dict(width=320, height=96, pictures=7, gop=2, slices="one", b_frames=2, b_intra_prob=0.85, b_skip_prob=0.05,
+                                   intra_in_p_prob=0.5, dc_walk=("climb", "wander", "descend"), dc_limit=60_000, **_CROSS), seed=49),
+    "val_b_rows": dict(knobs=dict(width=176, height=64, pictures=7, gop=2, slices="rows", b_frames=1, b_intra_prob=0.9,
+                                  dc_walk=("wander", "climb", "wander"), dc_run=10, dc_limit=20_000, **_CROSS), seed=50),
+}
+
+
+def value_repro():
+    """A 96x16 I picture, one slice, quantiser scale 31, six intra macroblocks whose luma DC differentials are all
+    +255: the Y predictor is 128 + 17 * 255 = 4463 at block 0 of macroblock 4, which also carries escapes of level -255
+    at zig-zag positions 1-11.  Saturating 8 * dc at 32767 changes its samples (255 in the reference)."""
+    s = SynthStream(Knobs(width=96, height=16, pictures=1, gop=1, slices="one"), 0)
+    s.sequence_header()
+    s.gop_header()
+    s.picture_header(0, 1)
+    s.out.align()
+    w = BitWriter()
+    w.start_code(1)
+    w.put(31, 5)
+    w.put(0, 1)
+    for mb in range(6):
+        w.code(MBA_CODE[1])
+        w.code(TYPE_I_CODE[0x01])
+        for blk in range(6):
+            if blk < 4:
+                w.code(DC_LUMA_CODE[8])
+                w.put(255, 8)
+            else:
+                w.code(DC_CHROMA_CODE[0])
+            if mb == 4 and blk == 0:
+                for _ in range(11):
+                    s.escape_level(w, 0, -255)
+            w.code(V.DCT_EOB_CODE)
+    w.align()
+    s.out.bits.extend(w.bits)
+    s.out.start_code(0xB7)
+    return s.out.tobytes()
+
+
 def make_case(name):
-    spec = CASES[name] if name in CASES else (B_CASES[name] if name in B_CASES else VECTOR_CASES[name])
+    if name == "val_repro_96x16":
+        return value_repro()
+    spec = next(c[name] for c in (CASES, B_CASES, VECTOR_CASES, VALUE_CASES, VALUE_B_CASES) if name in c)
     return SynthStream(Knobs(**spec["knobs"]), spec["seed"]).generate()
 
 
