@@ -609,6 +609,47 @@ typedef struct jsmpeg_b200_frame_dst_t {
 long jsmpeg_b200_batch_decode_frames_into(jsmpeg_b200_batch_t *b, int n_pictures, int flags, const jsmpeg_b200_frame_dst_t *dst,
                                           jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out);
 
+/* EVERY PICTURE OF decode(n) IN DISPLAY ORDER (clip loaders, video walls on IBBP content): decode_frames_display does to
+ * the batch exactly what decode_frames_into(b, n_pictures, flags, dst, ...) does and returns the same value, but hands
+ * the frames over in presentation order, each stored by stage 2 straight into its place.
+ *
+ * PRESENTATION, per stream, over the pictures the call reconstructs (PIC_DECODED), in consumption order -- the rule of
+ * MPEG1Video's displayOrder (jsmpeg_b200/decoder.py): a B picture is presented at once; an I/P picture first presents
+ * the I/P picture the stream holds, if any, and is then held itself; skipped pictures present nothing.  A held picture
+ * carries over into the next call (which presents it when its successor reference arrives) or is presented by
+ * jsmpeg_b200_batch_flush_frames (end of clip).  Without decode_b a stream has no B pictures, and every I/P picture is
+ * presented at once: the frames are decode_frames_into's, in its order, and nothing is held.  With decode_b, a stream
+ * without B pictures lags one held picture behind, as MPEG1Video does.
+ *
+ * FRAME j of stream s is the j-th picture the call presents, a held one of an earlier call included, so n_frames_out[s]
+ * may be n_pictures + 1: size each destination for n_pictures + 1 frames (at the offsets of decode_frames_into), and
+ * info_out (NULL: none) for n_streams * (n_pictures + 1) entries, stream s's frame j at s * (n_pictures + 1) + j.  Each
+ * frame of each kind is byte for byte what decode_frames_into writes for that picture (the map rule of I/P frames,
+ * untraced B maps included); memory past frame n_frames_out[s] - 1 is left untouched.
+ *
+ * HELD PICTURES live in a per-stream store of one frame of each kind the holding call asked for, made on first use.  A
+ * held picture is dropped, never presented, by reset, rewind, set_index, seek_pictures, and by decode(), decode_frames,
+ * decode_frames_into or any other call that reconstructs a picture into the stream's plane sets; emptying the stream's
+ * buffer (EVICT) keeps it.
+ *
+ * Everything decode() observes afterwards is what decode(n, flags) leaves, as for decode_frames_into; with OUT_RGBA /
+ * OUT_RESIDUALS the stream's RGBA and residual end as those of the last RECONSTRUCTED picture (held or presented).
+ *
+ * Synchronous.  Returns what decode() returns; -1 for a dead batch; -2, before any work and with nothing changed, for
+ * decode_frames_into's reasons, or when a stream holds a picture and the call asks for a kind (a non-NULL entry) the
+ * holding call did not. */
+long jsmpeg_b200_batch_decode_frames_display(jsmpeg_b200_batch_t *b, int n_pictures, int flags,
+                                             const jsmpeg_b200_frame_dst_t *dst, jsmpeg_b200_frame_t *info_out,
+                                             int32_t *n_frames_out);
+
+/* End of clip: presents every stream's held picture (decode_frames_display) as its frame 0 -- each kind `dst` asks for,
+ * at frame 0's place -- with n_frames_out[s] 0 or 1 and info_out (NULL: none) of n_streams entries, and releases the
+ * holds.  It reconstructs nothing and changes nothing else decode() observes.  Synchronous.  Returns the number of
+ * pictures presented; -1 for a dead batch; -2, before any work and with nothing changed, when dst is NULL, a destination
+ * is not 16-byte aligned, or a stream holds a picture without a kind the call asks for. */
+long jsmpeg_b200_batch_flush_frames(jsmpeg_b200_batch_t *b, const jsmpeg_b200_frame_dst_t *dst, jsmpeg_b200_frame_t *info_out,
+                                    int32_t *n_frames_out);
+
 /* SEEK (players, video walls, clip loaders): move decode() of chosen streams to a chosen picture each, and play on from
  * there with decode() -- OUT_HOST, OUT_RGBA and the host ring as usual -- without stepping the other streams.  The
  * reference chains of all requests run side by side, as for decode_pictures, but into the streams' own plane sets.

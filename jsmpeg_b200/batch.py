@@ -81,6 +81,9 @@ _BATCH_ABI = {
                                                         ctypes.POINTER(Frame), _VP]),
     "jsmpeg_b200_batch_decode_frames_into": (ctypes.c_long, [_VP, ctypes.c_int, ctypes.c_int, ctypes.POINTER(FrameDst),
                                                              ctypes.POINTER(Frame), _VP]),
+    "jsmpeg_b200_batch_decode_frames_display": (ctypes.c_long, [_VP, ctypes.c_int, ctypes.c_int, ctypes.POINTER(FrameDst),
+                                                                ctypes.POINTER(Frame), _VP]),
+    "jsmpeg_b200_batch_flush_frames": (ctypes.c_long, [_VP, ctypes.POINTER(FrameDst), ctypes.POINTER(Frame), _VP]),
     "jsmpeg_b200_batch_last_picture": (ctypes.c_int, [_VP, ctypes.c_int, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]),
     "jsmpeg_b200_batch_intra_index": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, ctypes.c_long]),
     "jsmpeg_b200_batch_decode_intra": (ctypes.c_long, [_VP, ctypes.c_int, _VP, _VP, _VP, _VP, ctypes.c_int, _VP, _VP]),
@@ -323,7 +326,7 @@ class BatchDecoder:
     _FRAME_KINDS = ("planes", "rgba", "residuals", "macroblocks", "coefficients", "accumulated")
 
     def decode_frames(self, n_pictures, flags=OUT_DEVICE, planes=True, rgba=False, residuals=False, macroblocks=False,
-                      coefficients=False, accumulated=False):
+                      coefficients=False, accumulated=False, display_order=False):
         """decode(n_pictures, flags) that also hands back every picture it reconstructs (include/jsmpeg_b200.h,
         jsmpeg_b200_batch_decode_frames): frame j of a stream is the j-th picture the call reconstructs for it (I and P,
         and B under decode_b; skipped pictures have none), in coded order.  Returns per stream a dict with "n_frames",
@@ -336,17 +339,57 @@ class BatchDecoder:
         the per-stream tensors are views of it: a clip batch without a gather.
         coefficients=True and accumulated=True (jsmpeg_b200_batch_decode_frames_into) add "coefficients" int16 [F,
         mb_height, mb_width, 6, 8, 8] (as decode_coefficients) and "accumulated" int16 [F, coded_size * 3 // 2, 4] (see
-        accumulated_view; a B frame's is all untraced); accumulated=True needs OUT_ACCUMULATED in `flags`."""
-        import torch
+        accumulated_view; a B frame's is all untraced); accumulated=True needs OUT_ACCUMULATED in `flags`.
+        display_order=True (jsmpeg_b200_batch_decode_frames_display) hands the frames over in presentation order: frame
+        j of a stream is the j-th picture the call presents (a B picture at once, an I/P picture when the next I/P
+        picture arrives, one held by an earlier call included; see flush_frames), "info" in that order, each tensor
+        allocated for n_pictures + 1 frames ([S, n_pictures + 1, ...] in last_frames_batch) and cut to n_frames."""
         n = int(n_pictures)
         if n < 0:
             raise ValueError("n_pictures must be >= 0")
         if accumulated and not int(flags) & OUT_ACCUMULATED:
             raise ValueError("accumulated frames need OUT_ACCUMULATED in flags")
-        dev = torch.device("cuda", self.device)
-        infos = [self.stream_info(s) for s in range(self.n_streams)]
         want = {"planes": planes, "rgba": rgba, "residuals": residuals, "macroblocks": macroblocks,
                 "coefficients": coefficients, "accumulated": accumulated}
+        cap = n + 1 if display_order else n  # frames per stream
+        full, dst, into = self._frame_destinations(cap, want)
+        info_out = (Frame * max(self.n_streams * cap, 1))()
+        n_frames = (ctypes.c_int32 * max(self.n_streams, 1))()
+        if display_order:
+            got = self.lib.jsmpeg_b200_batch_decode_frames_display(self.handle, n, int(flags), ctypes.byref(into), info_out, n_frames)
+        elif coefficients or accumulated:
+            got = self.lib.jsmpeg_b200_batch_decode_frames_into(self.handle, n, int(flags), ctypes.byref(into), info_out, n_frames)
+        else:
+            got = self.lib.jsmpeg_b200_batch_decode_frames(self.handle, n, int(flags), dst.get("planes"), dst.get("rgba"),
+                                                           dst.get("residuals"), dst.get("macroblocks"), info_out, n_frames)
+        if got == -2:
+            raise ValueError("decode_frames refused its arguments")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_frames failed")
+        return self._frames_out(full, info_out, n_frames, cap)
+
+    def flush_frames(self, planes=True, rgba=False, residuals=False, macroblocks=False, coefficients=False, accumulated=False):
+        """End of clip for decode_frames(display_order=True) (jsmpeg_b200_batch_flush_frames): every stream's held I/P
+        picture, as decode_frames' result of one frame (n_frames 0 or 1), and the holds released.  A stream that holds a
+        picture must have been asked for every kind asked for here (ValueError otherwise, with nothing changed)."""
+        want = {"planes": planes, "rgba": rgba, "residuals": residuals, "macroblocks": macroblocks,
+                "coefficients": coefficients, "accumulated": accumulated}
+        full, _, into = self._frame_destinations(1, want)
+        info_out = (Frame * max(self.n_streams, 1))()
+        n_frames = (ctypes.c_int32 * max(self.n_streams, 1))()
+        got = self.lib.jsmpeg_b200_batch_flush_frames(self.handle, ctypes.byref(into), info_out, n_frames)
+        if got == -2:
+            raise ValueError("flush_frames refused its arguments")
+        if got < 0:
+            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_flush_frames failed")
+        return self._frames_out(full, info_out, n_frames, 1)
+
+    def _frame_destinations(self, n, want):
+        """Room for n frames per stream of each kind in `want` (decode_frames' tensor rules): the tensors per kind, the
+        per-stream pointer arrays per kind, and a FrameDst over them"""
+        import torch
+        dev = torch.device("cuda", self.device)
+        infos = [self.stream_info(s) for s in range(self.n_streams)]
 
         def shape(kind, info):
             cs, w, h = info["coded_size"], info["width"], info["height"]
@@ -371,21 +414,13 @@ class BatchDecoder:
                               for i in infos]
         S = max(self.n_streams, 1)
         dst = {kind: (_VP * S)(*[t.data_ptr() if t is not None and n else None for t in full[kind]]) for kind in full}
-        info_out = (Frame * max(self.n_streams * n, 1))()
-        n_frames = (ctypes.c_int32 * S)()
         if full:
             torch.cuda.current_stream(dev).synchronize()  # the allocations are the caller's stream's; the call uses its own
-        if coefficients or accumulated:
-            into = FrameDst(*[ctypes.addressof(dst[k]) if k in dst else None for k in
-                              ("planes", "rgba", "residuals", "macroblocks", "coefficients", "accumulated")])
-            got = self.lib.jsmpeg_b200_batch_decode_frames_into(self.handle, n, int(flags), ctypes.byref(into), info_out, n_frames)
-        else:
-            got = self.lib.jsmpeg_b200_batch_decode_frames(self.handle, n, int(flags), dst.get("planes"), dst.get("rgba"),
-                                                           dst.get("residuals"), dst.get("macroblocks"), info_out, n_frames)
-        if got == -2:
-            raise ValueError("decode_frames refused its arguments")
-        if got < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_frames failed")
+        into = FrameDst(*[ctypes.addressof(dst[k]) if k in dst else None for k in self._FRAME_KINDS])
+        return full, dst, into
+
+    def _frames_out(self, full, info_out, n_frames, n):
+        """Per stream: decode_frames' dict of the frames the call wrote (info rows n apart)"""
         out = []
         for s in range(self.n_streams):
             f = n_frames[s]

@@ -86,6 +86,29 @@ struct HostSlot {
 	PinnedBuffer<uint8_t> planes, entries;
 };
 
+// decode_frames_display (DESIGN 3.18): one frame of each kind of one stream -- where one picture's planes, RGBA,
+// residual, entries, coefficients and map go (nullptr: that kind not at all)
+struct FrameAt {
+	uint8_t *planes = nullptr, *rgba = nullptr, *mb = nullptr;
+	int16_t *res = nullptr, *coef = nullptr;
+	uint2 *acc = nullptr;
+};
+
+// The kinds of frame, as bits of FrameStore::kinds and FrameCursor::kinds
+enum : unsigned { KIND_PLANES = 1, KIND_RGBA = 2, KIND_RES = 4, KIND_MB = 8, KIND_COEF = 16, KIND_ACC = 32 };
+
+// decode_frames_display: the I/P picture a stream holds back until its successor reference (or flush_frames) presents
+// it, in a store of one frame per kind made on first use.  `kinds`: the kinds the holding call wrote into the store;
+// `info`: the picture's frame info.
+struct FrameStore {
+	DeviceBuffer<uint8_t> planes, rgba, mb;
+	DeviceBuffer<int16_t> res, coef;
+	DeviceBuffer<uint2> acc;
+	bool held = false;
+	unsigned kinds = 0;
+	jsmpeg_b200_frame_t info{};
+};
+
 struct Stream {
 	bitbuffer::Buffer bb;  // host bit buffer (pinned) -- src/wasm/buffer.c
 	// sequence header
@@ -124,6 +147,9 @@ struct Stream {
 	bool ps_in_sync = false;           // ... and whether they continue the item chain (else: look for a pack header)
 	// parsed-ahead pictures, consecutive, front = next picture decode() consumes
 	std::deque<Parsed> cache;
+	// decode_frames_display's held picture: dropped by reset, rewind, set_index, a seek and every other call that
+	// reconstructs into the stream's sets (DESIGN 3.18)
+	FrameStore hold;
 };
 
 struct ScratchDeleter {
@@ -984,13 +1010,33 @@ struct TaskAt {
 
 // decode_frames (DESIGN 3.16) and decode_frames_into (DESIGN 3.17): where one stream's frames go -- each destination
 // nullptr or the stream's frame 0 in device memory, `info` its row of the caller's info_out on the host -- and how many
-// the call has given it so far
+// the call has given it so far.  decode_frames_display (DESIGN 3.18, `display`) presents them: frame j is the j-th
+// picture the call presents, and `n` counts those.
 struct FrameCursor {
 	uint8_t *planes = nullptr, *rgba = nullptr, *mb = nullptr;
 	int16_t *res = nullptr, *coef = nullptr;
 	uint2 *acc = nullptr;
 	jsmpeg_b200_frame_t *info = nullptr;
 	int n = 0;
+	bool display = false;
+	unsigned kinds = 0;  // (display) the KIND_* bits of the destinations given
+	int made = 0;        // pictures reconstructed
+	int reserved = -1;   // (display) the frame the stream's held I/P picture was written to, its successor in the round
+	bool stored = false;  // (display) a picture of the call went to the stream's store
+	uint8_t *last_rgba = nullptr;  // where the newest reconstructed picture's RGBA and residual went
+	int16_t *last_res = nullptr;
+	// frame j of the stream `s`
+	FrameAt at(const Stream &s, size_t j) const {
+		const size_t planes_n = (size_t)s.coded_size * 3 / 2, mb_n = (size_t)s.seq.mb_size;
+		FrameAt f;
+		if (planes) f.planes = planes + j * planes_n;
+		if (rgba) f.rgba = rgba + j * s.width * s.height * 4;
+		if (mb) f.mb = mb + j * mb_n * sizeof(jsmpeg_b200_macroblock_t);
+		if (res) f.res = res + j * planes_n;
+		if (coef) f.coef = coef + j * mb_n * 384;
+		if (acc) f.acc = acc + j * planes_n;
+		return f;
+	}
 };
 
 // Picture `e` of stream `s`, records in `slot`, consumed by decode() or by a seek, reconstructed by step `step` of
@@ -998,18 +1044,17 @@ struct FrameCursor {
 // every picture it consumes, a seek: each chain's last).  Beside its planes go, under OUT_MACROBLOCKS, its entries and,
 // for an I/P picture, under OUT_ACCUMULATED its map (else the set's map no longer matches it); the visible picture also
 // goes to the stream's RGBA under OUT_RGBA and, under OUT_HOST, with its entries to the next slot of its host ring.
-// `newest` gets where its task is (OUT_RESIDUALS: the caller's newest picture stores its residual).  With a `frame`
-// cursor (decode_frames) the picture is the stream's next frame: stage 2 also stores its planes, and its RGBA and
-// residual go to that frame instead of the stream's own, and its entries are also exported there.  decode_frames_into
-// adds its coefficients, exported from its records, and its map: an I/P picture's map goes to the frame INSTEAD of the
-// set's map (the set's map_at says so; finish_frames brings the newest one back), a B picture's frame is untraced.
-// Returns the bytes its copies bring to the host.
+// `newest` gets where its task is (OUT_RESIDUALS: the caller's newest picture stores its residual).  With a frame `to`
+// (decode_frames: the stream's next frame; decode_frames_display: its presentation frame or the stream's store) stage 2
+// also stores its planes there, and its RGBA and residual go there instead of the stream's own, and its entries are also
+// exported there.  decode_frames_into adds its coefficients, exported from its records, and its map: an I/P picture's map
+// goes to the frame INSTEAD of the set's map (the set's map_at says so; finish_frames brings the newest one back), a B
+// picture's frame is untraced.  Returns the bytes its copies bring to the host.
 uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, size_t step, int slot, const picture_info_t &e,
-                         int flags, bool visible, TaskAt &newest, FrameCursor *frame = nullptr) {
+                         int flags, bool visible, TaskAt &newest, const FrameAt *to = nullptr) {
 	const bool is_b = e.picture_type == 3;  // (only the extension's walk answers PIC_DECODED for one)
-	const size_t j = frame ? (size_t)frame->n++ : 0, planes = (size_t)s.coded_size * 3 / 2;
-	uint8_t *rgba = frame && frame->rgba ? frame->rgba + j * s.width * s.height * 4
-	                : visible && (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
+	const size_t planes = (size_t)s.coded_size * 3 / 2;
+	uint8_t *rgba = to && to->rgba ? to->rgba : visible && (flags & JSMPEG_B200_OUT_RGBA) ? stream_rgba(b, s) : nullptr;
 	ReconTask t;
 	if (is_b) {
 		// `cur` holds the older and `1 - cur` the newer of the two most recent I/P pictures: the B picture's forward
@@ -1023,8 +1068,8 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 		t = recon_task(b, s, slot, s.sets[s.cur].planes.data(), s.sets[1 - s.cur].planes.data(), nullptr, rgba);
 		s.cur ^= 1;  // mpeg1.js:221-246: the picture just decoded becomes `forward`
 	}
-	if (frame && frame->planes) t.frame = frame->planes + j * planes;
-	if (frame && frame->res) t.res = frame->res + j * planes;
+	if (to && to->planes) t.frame = to->planes;
+	if (to && to->res) t.res = to->res;
 	StreamSet &set = s.sets[s.last];
 	if (steps.size() <= step) steps.emplace_back();
 	ReconStep &r = steps[step];
@@ -1034,9 +1079,9 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 		reserve_entries(b, s);
 		r.entry(t, e.picture_type, set.entries.data());
 	}
-	if (frame && frame->mb) r.entry(t, e.picture_type, frame->mb + j * s.seq.mb_size * sizeof(jsmpeg_b200_macroblock_t));
-	if (frame && frame->coef) r.coef(slot_records(b, slot), s.seq.mb_size, frame->coef + j * s.seq.mb_size * 384);
-	uint2 *acc = frame && frame->acc ? frame->acc + j * planes : nullptr;  // (only under OUT_ACCUMULATED)
+	if (to && to->mb) r.entry(t, e.picture_type, to->mb);
+	if (to && to->coef) r.coef(slot_records(b, slot), s.seq.mb_size, to->coef);
+	uint2 *acc = to ? to->acc : nullptr;  // (only under OUT_ACCUMULATED)
 	if (!is_b) {  // the map beside the set (or in its map frame), one depth step from the forward set's picture's map
 		if (flags & JSMPEG_B200_OUT_ACCUMULATED) {
 			reserve_maps(s);
@@ -1062,6 +1107,101 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 		}
 	}
 	return host_bytes;
+}
+
+// How many of the stream's parsed-ahead pictures a round that wants `want` of them consumes: decode_round's consumption
+// loop over the cache, run ahead without consuming (its stop rules, in its order)
+size_t consumable(const Stream &s, int want) {
+	uint64_t index = s.bb.index;
+	size_t k = 0;
+	for (; (int)k < want && k < s.cache.size(); k++) {
+		auto it = std::lower_bound(s.pics.begin(), s.pics.end(), (uint32_t)((index + 7) >> 3));
+		const Parsed &e = s.cache[k];
+		if (it == s.pics.end() || e.pos != *it || entry_stale(s, e)) break;
+		index = e.info.end_bit;
+	}
+	return k;
+}
+
+// The stream's store, with room for one frame of each kind `f` asks for
+FrameAt store_frame(Stream &s, const FrameCursor &f) {
+	const size_t planes = (size_t)s.coded_size * 3 / 2, mb = (size_t)s.seq.mb_size;
+	FrameStore &h = s.hold;
+	FrameAt to;
+	if (f.planes) { h.planes.reserve(planes); to.planes = h.planes.data(); }
+	if (f.rgba) { h.rgba.reserve((size_t)s.width * s.height * 4); to.rgba = h.rgba.data(); }
+	if (f.mb) { h.mb.reserve(mb * sizeof(jsmpeg_b200_macroblock_t)); to.mb = h.mb.data(); }
+	if (f.res) { h.res.reserve(planes); to.res = h.res.data(); }
+	if (f.coef) { h.coef.reserve(mb * 384); to.coef = h.coef.data(); }
+	if (f.acc) { h.acc.reserve(planes); to.acc = h.acc.data(); }
+	return to;
+}
+
+// The held picture's frame of each kind in `kinds` into `to`, queued as copies (copy_batch)
+void copy_held(const Stream &s, unsigned kinds, const FrameAt &to, std::vector<void *> &dst, std::vector<void *> &src,
+               std::vector<size_t> &size) {
+	const FrameStore &h = s.hold;
+	const size_t planes = (size_t)s.coded_size * 3 / 2, mb = (size_t)s.seq.mb_size;
+	auto add = [&](unsigned kind, void *d, const void *from, size_t n) {
+		if (!(kinds & kind) || !d) return;
+		dst.push_back(d);
+		src.push_back(const_cast<void *>(from));
+		size.push_back(n);
+	};
+	add(KIND_PLANES, to.planes, h.planes.data(), planes);
+	add(KIND_RGBA, to.rgba, h.rgba.data(), (size_t)s.width * s.height * 4);
+	add(KIND_MB, to.mb, h.mb.data(), mb * sizeof(jsmpeg_b200_macroblock_t));
+	add(KIND_RES, to.res, h.res.data(), planes * sizeof(int16_t));
+	add(KIND_COEF, to.coef, h.coef.data(), mb * 384 * sizeof(int16_t));
+	add(KIND_ACC, to.acc, h.acc.data(), planes * sizeof(uint2));
+}
+
+// decode_frames_display (DESIGN 3.18): where the reconstructed picture `e` of stream `s`, frame info `info`, goes, by the
+// presentation rule.  A B picture is presented at once: the next frame.  An I/P picture first presents the picture the
+// stream holds, then is held itself (without decode_b: presented at once).  `left`: the cache entries after it that
+// the round consumes.  If its successor reference is among them, its frame is known now -- after the B pictures
+// between -- and it goes there directly (f.reserved); else it goes to the stream's store, and a later round, call or
+// flush_frames copies it to its frame.  Such a copy (held from an earlier round or call) is queued into `dst`, `src`,
+// `size`, for the reconstruct stream ahead of the round's launches: behind the store's writer, before its next one.
+FrameAt present_picture(Stream &s, FrameCursor &f, const Parsed &e, const jsmpeg_b200_frame_t &info, size_t left,
+                        bool decode_b, std::vector<void *> &dst, std::vector<void *> &src, std::vector<size_t> &size) {
+	auto frame = [&](int j) {
+		if (f.info) f.info[j] = info;
+		return f.at(s, (size_t)j);
+	};
+	if (!f.display) return frame(f.n++);
+	if (e.info.picture_type == 3) return frame(f.n++);
+	if (f.reserved >= 0) {  // the held picture went to its frame directly, and the B pictures before it have theirs
+		if (f.reserved != f.n) throw std::logic_error("jsmpeg_b200: display order: a held frame out of place");
+		f.reserved = -1;
+		f.n++;
+	} else if (s.hold.held) {
+		const FrameAt at = f.at(s, (size_t)f.n);
+		copy_held(s, s.hold.kinds, at, dst, src, size);
+		if (f.info) f.info[f.n] = s.hold.info;
+		// the map_at invariant (finish_frames): the held picture's map is in its frame once the copy has run, and the
+		// store may be rewritten by this round -- the next I/P picture reads its `prev` from the frame
+		for (int i = 0; i < 2; i++)
+			if (s.sets[i].map_at && s.sets[i].map_at == s.hold.acc.data()) s.sets[i].map_at = at.acc;
+		s.hold.held = false;
+		f.n++;
+	}
+	if (!decode_b) return frame(f.n++);
+	int n_b = 0;
+	for (size_t k = 0; k < left; k++) {
+		const picture_info_t &q = s.cache[k].info;
+		if (q.status != PIC_DECODED) continue;
+		if (q.picture_type != 3) {
+			f.reserved = f.n + n_b;
+			return frame(f.reserved);
+		}
+		n_b++;
+	}
+	s.hold.held = true;
+	s.hold.kinds = f.kinds;
+	s.hold.info = info;
+	f.stored = true;
+	return store_frame(s, f);
 }
 
 // One round: parse ahead what is missing in one wave, then consume up to want[s] pictures per stream in decode()
@@ -1124,10 +1264,13 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 	// ---- 3. consume in decode() order; the j-th reconstructed picture of a stream goes to step j
 	long consumed = 0;
 	std::vector<ReconStep> steps;
+	std::vector<void *> held_dst, held_src;  // decode_frames_display: held pictures this round presents (present_picture)
+	std::vector<size_t> held_size;
 	for (int si = 0; si < S; si++) {
 		if (!more[si]) continue;
 		Stream &s = b->streams[si];
 		FrameCursor *frame = frames ? &(*frames)[si] : nullptr;
+		const size_t ahead = frame && frame->display ? consumable(s, want[si]) : 0;
 		size_t step = 0;
 		TaskAt newest;
 		while (progress[si] < want[si]) {
@@ -1153,10 +1296,18 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 			// (0 unless both of its bytes are in the buffer)
 			s.last_temporal = (uint64_t)e.pos + 5 < s.bb.length ? picture_header(s, e.pos).temporal_reference : 0;
 			if (e.info.status == PIC_DECODED) {
-				b->stats.d2h_bytes += consume_picture(b, s, steps, step++, e.slot, e.info, flags, true, newest, frame);
-				if (frame && frame->info)
-					frame->info[frame->n - 1] = jsmpeg_b200_frame_t{e.pos, (int16_t)e.info.picture_type, (int16_t)s.last_temporal,
-					                                                 e.info.n_present, e.info.error};
+				FrameAt to;
+				if (frame) {
+					const jsmpeg_b200_frame_t info{e.pos, (int16_t)e.info.picture_type, (int16_t)s.last_temporal, e.info.n_present,
+					                               e.info.error};
+					const size_t left = ahead > (size_t)progress[si] ? ahead - progress[si] : 0;
+					to = present_picture(s, *frame, e, info, left, b->decode_b, held_dst, held_src, held_size);
+					frame->made++;
+					frame->last_rgba = to.rgba;
+					frame->last_res = to.res;
+				}
+				if (!(frame && frame->display)) s.hold.held = false;
+				b->stats.d2h_bytes += consume_picture(b, s, steps, step++, e.slot, e.info, flags, true, newest, frame ? &to : nullptr);
 				const bool is_b = e.info.picture_type == 3;
 				const uint64_t planes = (uint64_t)s.coded_size * 3 / 2;
 				b->stats.pictures_decoded++;
@@ -1173,7 +1324,10 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 		// round could not be observed.  (With residual frames the last one is copied at the end of the call: finish_frames.)
 		if ((flags & JSMPEG_B200_OUT_RESIDUALS) && newest.step >= 0 && !(frame && frame->res))
 			steps[newest.step].tasks[newest.task].res = reserve_residuals(b, s);
+		// (consumable() foresaw this loop: a picture whose successor it saw has been presented)
+		if (frame && frame->reserved >= 0) throw std::logic_error("jsmpeg_b200: display order: a successor not consumed");
 	}
+	if (!held_dst.empty()) copy_batch(b, held_dst, held_src, held_size, b->st_recon);
 	lap(b->trace.consume, t);
 	// ---- 4. reconstruction, behind the wave's expand: the host has consumed the infos and queues the launches while the
 	// expand of the biggest pictures is still running.  Every step reconstructs.
@@ -1211,27 +1365,36 @@ long decode_round(Batch *b, const std::vector<int> &want, std::vector<int> &prog
 // OUT_RESIDUALS and the newest I/P picture's map frame into its set's map (decode_frames_into), in one batched copy; all
 // on the reconstruct stream, behind the frames' stage 2.  The older I/P set's map is never read again before that set is
 // rewritten (`prev` and get_accumulated read the newest), so one whose map is in a frame is left unwritten.
+// decode_frames_display: the edge fill covers the store too, and the newest reconstructed picture's RGBA and residual are
+// wherever it went, frame or store.  The map_at invariant: while the call runs, an I/P set's map_at is where that set's
+// picture's map is now -- its frame, or the store while the picture is held there and until present_picture has queued
+// its copy to its frame (the store is then free for the next held picture's map, and the next I/P picture's `prev` is
+// read from the frame); so the newest set's map_at is what this copies back.
 void finish_frames(Batch *b, const std::vector<FrameCursor> &frames, int flags) {
 	std::vector<void *> dst, src;
 	std::vector<size_t> size;
 	for (size_t si = 0; si < frames.size(); si++) {
 		const FrameCursor &f = frames[si];
 		Stream &s = b->streams[si];
-		if (f.n == 0) continue;
+		if (f.made == 0) continue;
 		if (f.rgba) {
 			const size_t row = (size_t)s.width * 4, image = row * s.height;
-			if (s.width & 1) CUDA_CHECK(cudaMemset2DAsync(f.rgba + row - 4, row, 0xff, 4, (size_t)f.n * s.height, b->st_recon));
-			if (s.height & 1) CUDA_CHECK(cudaMemset2DAsync(f.rgba + image - row, image, 0xff, row, f.n, b->st_recon));
+			auto fill = [&](uint8_t *rgba, size_t n) {  // the odd edge of `n` images from `rgba`
+				if (s.width & 1) CUDA_CHECK(cudaMemset2DAsync(rgba + row - 4, row, 0xff, 4, n * s.height, b->st_recon));
+				if (s.height & 1) CUDA_CHECK(cudaMemset2DAsync(rgba + image - row, image, 0xff, row, n, b->st_recon));
+			};
+			if (f.n) fill(f.rgba, (size_t)f.n);
+			if (f.stored) fill(s.hold.rgba.data(), 1);
 			if (flags & JSMPEG_B200_OUT_RGBA) {
 				dst.push_back(stream_rgba(b, s));
-				src.push_back(f.rgba + (f.n - 1) * image);
+				src.push_back(f.last_rgba);
 				size.push_back(image);
 			}
 		}
 		if (f.res && (flags & JSMPEG_B200_OUT_RESIDUALS)) {
 			const size_t planes = (size_t)s.coded_size * 3 / 2;
 			dst.push_back(reserve_residuals(b, s));
-			src.push_back(f.res + (f.n - 1) * planes);
+			src.push_back(f.last_res);
 			size.push_back(planes * sizeof(int16_t));
 		}
 		StreamSet &newest = s.sets[1 - s.cur], &older = s.sets[s.cur];
@@ -1929,6 +2092,7 @@ void seek_pictures(Batch *b, std::vector<PictureRequest> &req, int flags, int32_
 		}
 		s.cur = s.b_cur = 0;
 		s.last = 1;
+		s.hold.held = false;
 		if (flags & JSMPEG_B200_OUT_RESIDUALS) {  // 0 unless the chain reconstructs a picture, like the entries
 			reserve_residuals(b, s);
 			CUDA_CHECK(cudaMemsetAsync(s.d_res.data(), 0, s.d_res.size() * sizeof(int16_t), b->st_recon));
@@ -2324,6 +2488,7 @@ void jsmpeg_b200_batch_set_index(jsmpeg_b200_batch_t *b, int stream, unsigned in
 	Stream &s = b->streams[stream];
 	s.bb.index = index;
 	flush_cache(b, s);
+	s.hold.held = false;
 }
 
 int jsmpeg_b200_batch_stream_info(jsmpeg_b200_batch_t *b, int stream, int *width, int *height, int *coded_size, float *frame_rate) {
@@ -2351,6 +2516,7 @@ void jsmpeg_b200_batch_rewind(jsmpeg_b200_batch_t *b) {
 		s.codes_classified = 0;
 		s.scanned = 0;
 		s.bb.index = s.has_seq ? s.seq_end_index : 0;  // where did_write left it (mpeg1.c:812-819)
+		s.hold.held = false;
 	}
 }
 
@@ -2366,6 +2532,7 @@ void jsmpeg_b200_batch_reset(jsmpeg_b200_batch_t *b) {
 			s.last_type = s.last_temporal = 0;
 			s.h_head = -1;
 			s.seq_floor = 0;
+			s.hold.held = false;
 			for (StreamSet &set : s.sets) {  // (zeroed sets: no picture, no map)
 				if (set.planes.data()) CUDA_CHECK(cudaMemsetAsync(set.planes.data(), 0, (size_t)s.coded_size * 3 / 2, b->st_main));
 				if (set.entries.data()) CUDA_CHECK(cudaMemsetAsync(set.entries.data(), 0, set.entries.size(), b->st_main));
@@ -2390,37 +2557,92 @@ long jsmpeg_b200_batch_decode_frames(jsmpeg_b200_batch_t *b, int n_pictures, int
 	return jsmpeg_b200_batch_decode_frames_into(b, n_pictures, flags, &dst, info_out, n_frames_out);
 }
 
+namespace {
+
+// The frame cursors of decode_frames_into, decode_frames_display and flush_frames for `dst`, info rows `stride` apart,
+// or false -- before any work -- when dst is NULL, n_pictures < 0, a destination is not 16-byte aligned (stage 2 and the
+// exports store 8 and 16 bytes at a time), a map destination is given where decode(n, flags) writes no maps, or
+// (`display`) a stream holds a picture without a kind the call asks for
+bool frame_cursors(const Batch *b, int n_pictures, int flags, const jsmpeg_b200_frame_dst_t *dst, jsmpeg_b200_frame_t *info_out,
+                   size_t stride, bool display, std::vector<FrameCursor> &frames) {
+	if (!dst || n_pictures < 0) return false;
+	const size_t S = b->streams.size();
+	auto aligned = [&](void *const *d) {
+		for (size_t si = 0; d && si < S; si++)
+			if ((uintptr_t)d[si] & 15u) return false;
+		return true;
+	};
+	bool maps = false;
+	for (size_t si = 0; dst->acc && si < S; si++) maps |= dst->acc[si] != nullptr;
+	if (!aligned(dst->planes) || !aligned(dst->rgba) || !aligned(dst->res) || !aligned(dst->mb) || !aligned(dst->coef) ||
+	    !aligned(dst->acc) || (maps && !(flags & JSMPEG_B200_OUT_ACCUMULATED)))
+		return false;
+	frames.assign(S, FrameCursor{});
+	for (size_t si = 0; si < S; si++) {
+		FrameCursor &f = frames[si];
+		if (dst->planes) f.planes = static_cast<uint8_t *>(dst->planes[si]);
+		if (dst->rgba) f.rgba = static_cast<uint8_t *>(dst->rgba[si]);
+		if (dst->res) f.res = static_cast<int16_t *>(dst->res[si]);
+		if (dst->mb) f.mb = static_cast<uint8_t *>(dst->mb[si]);
+		if (dst->coef) f.coef = static_cast<int16_t *>(dst->coef[si]);
+		if (dst->acc) f.acc = static_cast<uint2 *>(dst->acc[si]);
+		if (info_out) f.info = info_out + si * stride;
+		f.display = display;
+		f.kinds = (f.planes ? KIND_PLANES : 0) | (f.rgba ? KIND_RGBA : 0) | (f.res ? KIND_RES : 0) | (f.mb ? KIND_MB : 0) |
+		          (f.coef ? KIND_COEF : 0) | (f.acc ? KIND_ACC : 0);
+		const FrameStore &h = b->streams[si].hold;
+		if (display && h.held && (f.kinds & ~h.kinds)) return false;
+	}
+	return true;
+}
+
+}  // namespace
+
 long jsmpeg_b200_batch_decode_frames_into(jsmpeg_b200_batch_t *b, int n_pictures, int flags, const jsmpeg_b200_frame_dst_t *dst,
                                           jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out) {
 	return guarded<long>(b, -1, [&]() -> long {
-		if (!dst) return -2;
-		const size_t S = b->streams.size();
-		// every given destination 16-byte aligned (stage 2 and the exports store 8 and 16 bytes at a time), and map
-		// frames only where decode(n, flags) writes maps; checked before any work
-		auto aligned = [&](void *const *d) {
-			for (size_t si = 0; d && si < S; si++)
-				if ((uintptr_t)d[si] & 15u) return false;
-			return true;
-		};
-		bool maps = false;
-		for (size_t si = 0; dst->acc && si < S; si++) maps |= dst->acc[si] != nullptr;
-		if (n_pictures < 0 || !aligned(dst->planes) || !aligned(dst->rgba) || !aligned(dst->res) || !aligned(dst->mb) ||
-		    !aligned(dst->coef) || !aligned(dst->acc) || (maps && !(flags & JSMPEG_B200_OUT_ACCUMULATED)))
-			return -2;
-		std::vector<FrameCursor> frames(S);
-		for (size_t si = 0; si < S; si++) {
-			FrameCursor &f = frames[si];
-			if (dst->planes) f.planes = static_cast<uint8_t *>(dst->planes[si]);
-			if (dst->rgba) f.rgba = static_cast<uint8_t *>(dst->rgba[si]);
-			if (dst->res) f.res = static_cast<int16_t *>(dst->res[si]);
-			if (dst->mb) f.mb = static_cast<uint8_t *>(dst->mb[si]);
-			if (dst->coef) f.coef = static_cast<int16_t *>(dst->coef[si]);
-			if (dst->acc) f.acc = static_cast<uint2 *>(dst->acc[si]);
-			if (info_out) f.info = info_out + si * (size_t)n_pictures;
-		}
+		std::vector<FrameCursor> frames;
+		if (!frame_cursors(b, n_pictures, flags, dst, info_out, (size_t)n_pictures, false, frames)) return -2;
 		const long got = batch_decode(b, n_pictures, flags, &frames);
-		for (size_t si = 0; n_frames_out && si < S; si++) n_frames_out[si] = frames[si].n;
+		for (size_t si = 0; n_frames_out && si < frames.size(); si++) n_frames_out[si] = frames[si].n;
 		return got;
+	});
+}
+
+long jsmpeg_b200_batch_decode_frames_display(jsmpeg_b200_batch_t *b, int n_pictures, int flags, const jsmpeg_b200_frame_dst_t *dst,
+                                             jsmpeg_b200_frame_t *info_out, int32_t *n_frames_out) {
+	return guarded<long>(b, -1, [&]() -> long {
+		std::vector<FrameCursor> frames;
+		if (!frame_cursors(b, n_pictures, flags, dst, info_out, (size_t)n_pictures + 1, true, frames)) return -2;
+		const long got = batch_decode(b, n_pictures, flags, &frames);
+		for (size_t si = 0; n_frames_out && si < frames.size(); si++) n_frames_out[si] = frames[si].n;
+		return got;
+	});
+}
+
+long jsmpeg_b200_batch_flush_frames(jsmpeg_b200_batch_t *b, const jsmpeg_b200_frame_dst_t *dst, jsmpeg_b200_frame_t *info_out,
+                                    int32_t *n_frames_out) {
+	return guarded<long>(b, -1, [&]() -> long {
+		std::vector<FrameCursor> frames;
+		if (!frame_cursors(b, 0, JSMPEG_B200_OUT_ACCUMULATED, dst, info_out, 1, true, frames)) return -2;
+		use_device(b);
+		std::vector<void *> to, from;
+		std::vector<size_t> size;
+		long presented = 0;
+		for (size_t si = 0; si < frames.size(); si++) {
+			Stream &s = b->streams[si];
+			FrameCursor &f = frames[si];
+			if (!s.hold.held) continue;
+			copy_held(s, s.hold.kinds, f.at(s, 0), to, from, size);
+			if (f.info) f.info[0] = s.hold.info;
+			s.hold.held = false;
+			f.n = 1;
+			presented++;
+		}
+		if (!to.empty()) copy_batch(b, to, from, size, b->st_recon);
+		CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+		for (size_t si = 0; n_frames_out && si < frames.size(); si++) n_frames_out[si] = frames[si].n;
+		return presented;
 	});
 }
 
