@@ -38,6 +38,8 @@ class Frame(ctypes.Structure):
 
 
 _VP = ctypes.c_void_p
+# decode_macroblocks', decode_coefficients' and decode_residuals' refusal (-2)
+_NOT_IN_MACROBLOCK_INDEX = "a request names a picture that is not in the stream's macroblock index"
 
 
 class FrameDst(ctypes.Structure):
@@ -628,18 +630,9 @@ class BatchDecoder:
         {"n_present", "error"} per request.  The tensors are views of one allocation per picture size (thousands of
         requests cost a few allocations, not thousands)."""
         import torch
-        reqs = [(int(s), int(p)) for s, p in requests]
-        n = len(reqs)
-        out = self._per_picture_views(reqs, lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8)
-        streams, pictures, n_present, errors = self._request_arrays(reqs)
-        dst = (_VP * max(n, 1))(*[t.data_ptr() for t in out])
-        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # the allocations are the caller's stream's; the call uses its own
-        got = self.lib.jsmpeg_b200_batch_decode_macroblocks(self.handle, n, streams, pictures, dst, n_present, errors)
-        if got == -2:
-            raise ValueError("a request names a picture that is not in the stream's macroblock index")
-        if got < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_macroblocks failed")
-        self.last_macroblocks_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
+        (out,), self.last_macroblocks_info = self._export_requests(
+            self.lib.jsmpeg_b200_batch_decode_macroblocks, requests,
+            [(lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8)], [], _NOT_IN_MACROBLOCK_INDEX)
         return out
 
     def decode_coefficients(self, requests, macroblocks=False):
@@ -651,21 +644,10 @@ class BatchDecoder:
         decode_macroblocks returns them, from the same walk.  last_coefficients_info gets {"n_present", "error"} per
         request.  The tensors are views of one allocation per picture size."""
         import torch
-        reqs = [(int(s), int(p)) for s, p in requests]
-        n = len(reqs)
-        coefs = self._per_picture_views(reqs, lambda h, w: (h, w, 6, 8, 8), torch.int16)
-        entries = self._per_picture_views(reqs, lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8) if macroblocks else None
-        streams, pictures, n_present, errors = self._request_arrays(reqs)
-        coef_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in coefs])
-        mb_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in entries]) if macroblocks else None
-        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # as in decode_macroblocks
-        got = self.lib.jsmpeg_b200_batch_decode_coefficients(self.handle, n, streams, pictures, coef_dst, mb_dst,
-                                                             n_present, errors)
-        if got == -2:
-            raise ValueError("a request names a picture that is not in the stream's macroblock index")
-        if got < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_coefficients failed")
-        self.last_coefficients_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
+        entries = (lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8) if macroblocks else None
+        (coefs, entries), self.last_coefficients_info = self._export_requests(
+            self.lib.jsmpeg_b200_batch_decode_coefficients, requests,
+            [(lambda h, w: (h, w, 6, 8, 8), torch.int16), entries], [], _NOT_IN_MACROBLOCK_INDEX)
         return list(zip(coefs, entries)) if macroblocks else coefs
 
     def decode_residuals(self, requests, macroblocks=False):
@@ -678,21 +660,10 @@ class BatchDecoder:
         last_residuals_info gets {"n_present", "error"} per request.  The tensors are views of one allocation per
         picture size."""
         import torch
-        reqs = [(int(s), int(p)) for s, p in requests]
-        n = len(reqs)
-        res = self._per_picture_views(reqs, lambda h, w: (h * w * 384,), torch.int16)
-        entries = self._per_picture_views(reqs, lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8) if macroblocks else None
-        streams, pictures, n_present, errors = self._request_arrays(reqs)
-        res_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in res])
-        mb_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in entries]) if macroblocks else None
-        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # as in decode_macroblocks
-        got = self.lib.jsmpeg_b200_batch_decode_residuals(self.handle, n, streams, pictures, res_dst, mb_dst,
-                                                          n_present, errors)
-        if got == -2:
-            raise ValueError("a request names a picture that is not in the stream's macroblock index")
-        if got < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_residuals failed")
-        self.last_residuals_info = [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
+        entries = (lambda h, w: (h, w, MACROBLOCK_BYTES), torch.uint8) if macroblocks else None
+        (res, entries), self.last_residuals_info = self._export_requests(
+            self.lib.jsmpeg_b200_batch_decode_residuals, requests,
+            [(lambda h, w: (h * w * 384,), torch.int16), entries], [], _NOT_IN_MACROBLOCK_INDEX)
         return list(zip(res, entries)) if macroblocks else res
 
     def decode_accumulated(self, requests):
@@ -705,20 +676,11 @@ class BatchDecoder:
         then all untraced).  The tensors are views of one allocation per picture size."""
         import torch
         reqs = [(int(s), int(p)) for s, p in requests]
-        n = len(reqs)
-        maps = self._per_picture_views(reqs, lambda h, w: (h * w * 384, 4), torch.int16)
-        streams, pictures, n_present, errors = self._request_arrays(reqs)
-        status = (ctypes.c_int32 * max(n, 1))()
-        acc_dst = (_VP * max(n, 1))(*[t.data_ptr() for t in maps])
-        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # as in decode_macroblocks
-        got = self.lib.jsmpeg_b200_batch_decode_accumulated(self.handle, n, streams, pictures, acc_dst, status,
-                                                            n_present, errors)
-        if got == -2:
-            raise ValueError("a request names a picture that is not an I or P picture of the stream's picture index")
-        if got < 0:
-            raise RuntimeError(self.last_error() or "jsmpeg_b200_batch_decode_accumulated failed")
-        self.last_accumulated_info = [{"status": status[i], "n_present": n_present[i], "error": errors[i]}
-                                      for i in range(n)]
+        status = (ctypes.c_int32 * max(len(reqs), 1))()
+        (maps,), info = self._export_requests(
+            self.lib.jsmpeg_b200_batch_decode_accumulated, reqs, [(lambda h, w: (h * w * 384, 4), torch.int16)],
+            [status], "a request names a picture that is not an I or P picture of the stream's picture index")
+        self.last_accumulated_info = [{"status": status[i], **row} for i, row in enumerate(info)]
         return maps
 
     def seek_pictures(self, requests, flags=OUT_DEVICE):
@@ -776,6 +738,26 @@ class BatchDecoder:
         if not info["has_sequence_header"]:
             raise ValueError(f"stream {s} has no sequence header yet")
         return info
+
+    def _export_requests(self, fn, requests, kinds, extra_out, refused):
+        """Allocate the destinations of (stream, picture) `requests` and call `fn` (decode_macroblocks,
+        decode_coefficients, decode_residuals or decode_accumulated) with one pointer array per kind, then `extra_out`,
+        n_present and error.  `kinds`: per destination array of fn, (shape, dtype) as _per_picture_views takes them, or
+        None for an array not given (NULL).  Returns (per kind its tensors or None, [{"n_present", "error"} per
+        request])."""
+        import torch
+        reqs = [(int(s), int(p)) for s, p in requests]
+        n = len(reqs)
+        out = [self._per_picture_views(reqs, *kind) if kind else None for kind in kinds]
+        streams, pictures, n_present, errors = self._request_arrays(reqs)
+        dst = [(_VP * max(n, 1))(*[t.data_ptr() for t in views]) if views is not None else None for views in out]
+        torch.cuda.current_stream(torch.device("cuda", self.device)).synchronize()  # the allocations are the caller's stream's; the call uses its own
+        got = fn(self.handle, n, streams, pictures, *dst, *extra_out, n_present, errors)
+        if got == -2:
+            raise ValueError(refused)
+        if got < 0:
+            raise RuntimeError(self.last_error() or f"{fn.__name__} failed")
+        return out, [{"n_present": n_present[i], "error": errors[i]} for i in range(n)]
 
     def _decode_requests(self, fn, reqs, rgba, extra_out, refused):
         """Allocate the destinations of (stream, picture) requests and call `fn` (decode_intra / decode_pictures) with

@@ -27,7 +27,8 @@
 // Cutting the wave into chunks to overlap stage 1 with stage 2 was measured not to pay (DESIGN 8).
 // decode_macroblocks runs the same waves walk-only (no expand, no reconstruct) and exports the records (DESIGN 3.8);
 // decode_coefficients runs them with expand and exports the coefficients too (DESIGN 3.9), decode_residuals their
-// inverse transform (DESIGN 3.10).
+// inverse transform (DESIGN 3.10).  Each wave's exports are a stage-2 step without reconstruct tasks, queued by the
+// same step runner (run_steps) on the reconstruct stream.
 #include <sched.h>
 
 #include <algorithm>
@@ -212,26 +213,20 @@ struct jsmpeg_b200_batch_t {
 	// (DESIGN 3.6); and the pool of the other chains' plane sets, zeroed per chain group (DESIGN 3.7)
 	DeviceBuffer<uint8_t> d_intra_fwd;
 	DeviceBuffer<uint8_t> d_chain_sets;
-	// decode_macroblocks: the export tasks of a wave (DESIGN 3.8)
-	PinnedBuffer<MbExportTask> h_xtasks;
-	DeviceBuffer<MbExportTask> d_xtasks;
-	// decode() and seek_pictures under OUT_MACROBLOCKS: the export tasks of a round's (a wave's) steps (DESIGN 3.13)
+	// the export and accumulate tasks of a call's steps (run_steps: a decode() round, a wave of the others), one table
+	// per task type, read on st_recon: macroblock entries (decode_macroblocks, OUT_MACROBLOCKS and macroblock frames,
+	// DESIGN 3.8, 3.13), coefficients (decode_coefficients and coefficient frames, DESIGN 3.9, 3.17), residuals
+	// (decode_residuals, DESIGN 3.10) and accumulated maps (decode_accumulated and OUT_ACCUMULATED, DESIGN 3.11, 3.14)
 	PinnedBuffer<MbExportTask> h_etasks;
 	DeviceBuffer<MbExportTask> d_etasks;
-	// decode_coefficients: the coefficient export tasks of a wave (DESIGN 3.9)
 	PinnedBuffer<CoefExportTask> h_ctasks;
 	DeviceBuffer<CoefExportTask> d_ctasks;
-	// decode_frames_into's coefficient frames: the coefficient export tasks of a round's steps (DESIGN 3.17)
-	PinnedBuffer<CoefExportTask> h_ftasks;
-	DeviceBuffer<CoefExportTask> d_ftasks;
-	// decode_residuals: the residual export tasks of a wave (DESIGN 3.10)
 	PinnedBuffer<ResExportTask> h_rtasks;
 	DeviceBuffer<ResExportTask> d_rtasks;
-	// decode_accumulated: the pool of the chains' two scratch map sets, and the tasks of a wave's depths (DESIGN 3.11)
-	DeviceBuffer<uint8_t> d_map_sets;
-	// (and under OUT_ACCUMULATED, the accumulate tasks of a decode() round's or a seek wave's steps, DESIGN 3.14)
 	PinnedBuffer<AccTask> h_atasks;
 	DeviceBuffer<AccTask> d_atasks;
+	// decode_accumulated: the pool of the chains' two scratch map sets (DESIGN 3.11)
+	DeviceBuffer<uint8_t> d_map_sets;
 	jsmpeg_b200_stats_t stats{};
 	// JSMPEG_B200_HOST_TRACE=1: decode() prints where the host's time of the call went (tools/time_stages.py), in ms:
 	// upload_all | planning the waves | building and queueing stage 1 | waiting for the infos | consuming them |
@@ -673,10 +668,12 @@ void reserve_tasks(PinnedBuffer<T> &h, DeviceBuffer<T> &d, size_t n, cudaStream_
 }
 
 // One step of stage 2 (run_steps): the reconstruct tasks of one step of decode() (or one depth of run_chains), queued
-// by launch_reconstruct; the export of their macroblock entries (OUT_MACROBLOCKS: `entries`, one launch of
-// export_macroblocks_kernel over `entry_mb` macroblocks); accumulated maps (OUT_ACCUMULATED, decode_accumulated:
-// `maps`, one launch of accumulate_kernel over `map_warps` warps); coefficient frames (decode_frames_into: `coefs`, one
-// launch of export_coefficients_kernel over `coef_mb` macroblocks); and the copies of its pictures that follow them
+// by launch_reconstruct; the export of macroblock entries (OUT_MACROBLOCKS, decode_macroblocks: `entries`, one launch
+// of export_macroblocks_kernel over `entry_mb` macroblocks); accumulated maps (OUT_ACCUMULATED, decode_accumulated:
+// `maps`, one launch of accumulate_kernel over `map_warps` warps); coefficients (decode_frames_into,
+// decode_coefficients: `coefs`, one launch of export_coefficients_kernel over `coef_mb` macroblocks); residuals
+// (decode_residuals: `residuals`, one launch of export_residuals_kernel over `res_warps` warps); and the copies of its
+// pictures that follow them.  A step of decode_macroblocks' wave has exports and no reconstruct task.
 struct ReconStep {
 	std::vector<ReconTask> tasks;
 	std::vector<MbExportTask> entries;
@@ -685,6 +682,8 @@ struct ReconStep {
 	uint32_t map_warps = 0;
 	std::vector<CoefExportTask> coefs;
 	uint32_t coef_mb = 0;
+	std::vector<ResExportTask> residuals;
+	uint32_t res_warps = 0;
 	std::vector<void *> dst, src;
 	std::vector<size_t> size;
 	void copy(void *to, void *from, size_t n) {
@@ -692,10 +691,10 @@ struct ReconStep {
 		src.push_back(from);
 		size.push_back(n);
 	}
-	// the entries of task t's picture (picture_coding_type `type`) into `to`
-	void entry(const ReconTask &t, int type, void *to) {
-		entries.push_back(MbExportTask{t.hdr, to, entry_mb, t.mb_size, type, 0});
-		entry_mb += (uint32_t)t.mb_size;
+	// the entries of the picture whose records are `sr` (`mb_size` macroblocks, picture_coding_type `type`) into `to`
+	void entry(const SlotRecords &sr, int mb_size, int type, void *to) {
+		entries.push_back(MbExportTask{sr.hdr, to, entry_mb, mb_size, type, 0});
+		entry_mb += (uint32_t)mb_size;
 	}
 	// the map of the I/P picture whose records are `sr` (of a stream with sequence parameters `seq`) into `to`, one depth
 	// step from `prev` (nullptr: no previous map)
@@ -708,12 +707,17 @@ struct ReconStep {
 		coefs.push_back(CoefExportTask{sr.hdr, sr.coef, sr.compact, to, coef_mb, mb_size});
 		coef_mb += (uint32_t)mb_size;
 	}
+	// the residual of the picture whose records are `sr` (of a stream with sequence parameters `seq`) into `to`
+	void residual(const SlotRecords &sr, const SeqParams &seq, int16_t *to) {
+		residuals.push_back(ResExportTask{sr.hdr, sr.coef, sr.compact, to, res_warps, seq.mb_width, seq.mb_height, 0});
+		res_warps += res_export_warps(seq.mb_size);
+	}
 };
 
-// The tasks `list` of all `steps` (ReconStep::entries, ReconStep::maps, ReconStep::coefs) go up in one copy on the reconstruct stream,
-// through the pinned table `h` into `d`; returns where each step's tasks begin in `d`.  The previous upload's readers are
-// done before the pinned table is written again: every call ends with its reconstruction complete, and run_chains'
-// next wave waits for ev_round.
+// The tasks `list` of all `steps` (ReconStep::entries, maps, coefs, residuals) go up in one copy on the reconstruct
+// stream, through the pinned table `h` into `d`; returns where each step's tasks begin in `d`.  The previous upload's
+// readers are done before the pinned table is written again: every call ends with its reconstruction complete, and the
+// next wave of run_chains or decode_macroblocks waits for ev_round.
 template <typename T>
 std::vector<const T *> upload_step_tasks(Batch *b, const std::vector<ReconStep> &steps, std::vector<T> ReconStep::*list,
                                          PinnedBuffer<T> &h, DeviceBuffer<T> &d) {
@@ -739,17 +743,19 @@ void copy_out_step(Batch *b, ReconStep &r) {
 	b->copy_steps++;
 }
 
-// Stage 2 of decode_round and of a run_chains wave: `steps`, one after the other on the reconstruct stream.  Every step's
-// export and accumulate tasks go up in one copy per table (upload_step_tasks, before ev_recon[0]); then, behind the
-// latest stage-1 wave (ev_b: the records are final; where the host waited for the wave, an ordering already met) and
-// between ev_recon[0] and ev_recon[1] (decode()'s recon_ms), each step's reconstruct, export, accumulate and coefficient
-// export launch,
-// those it has tasks for, and its copies: with `copy_out` on the copy stream (copy_out_step), else on the reconstruct
-// stream.  The record slots stay until ev_round.  Returns the kernels launched.
+// Stage 2 of decode_round and of a run_chains or decode_macroblocks wave: `steps`, one after the other on the
+// reconstruct stream.  Every step's export and accumulate tasks go up in one copy per table (upload_step_tasks, before
+// ev_recon[0]); then, behind the latest stage-1 wave (ev_b: the records are final; where the host waited for the wave,
+// an ordering already met) and between ev_recon[0] and ev_recon[1] (decode()'s recon_ms), each step's reconstruct,
+// entry export, accumulate, coefficient export and residual export launch, those it has tasks for, and its copies:
+// with `copy_out` on the copy stream (copy_out_step), else on the reconstruct stream.  The record slots stay until
+// ev_round.  Returns the kernels launched.
 int run_steps(Batch *b, std::vector<ReconStep> &steps, bool copy_out) {
 	const std::vector<const MbExportTask *> entries = upload_step_tasks(b, steps, &ReconStep::entries, b->h_etasks, b->d_etasks);
 	const std::vector<const AccTask *> maps = upload_step_tasks(b, steps, &ReconStep::maps, b->h_atasks, b->d_atasks);
-	const std::vector<const CoefExportTask *> coefs = upload_step_tasks(b, steps, &ReconStep::coefs, b->h_ftasks, b->d_ftasks);
+	const std::vector<const CoefExportTask *> coefs = upload_step_tasks(b, steps, &ReconStep::coefs, b->h_ctasks, b->d_ctasks);
+	const std::vector<const ResExportTask *> residuals =
+	    upload_step_tasks(b, steps, &ReconStep::residuals, b->h_rtasks, b->d_rtasks);
 	CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_b, 0));
 	CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
 	int launches = 0;
@@ -770,6 +776,10 @@ int run_steps(Batch *b, std::vector<ReconStep> &steps, bool copy_out) {
 		}
 		if (!r.coefs.empty()) {
 			launch_export_coefficients(coefs[i], (int)r.coefs.size(), r.coef_mb, b->st_recon);
+			launches++;
+		}
+		if (!r.residuals.empty()) {
+			launch_export_residuals(residuals[i], (int)r.residuals.size(), r.res_warps, b->st_recon);
 			launches++;
 		}
 		if (r.dst.empty()) continue;
@@ -1075,19 +1085,20 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 	ReconStep &r = steps[step];
 	r.tasks.push_back(t);
 	newest = {(int)step, (int)r.tasks.size() - 1};
+	const SlotRecords sr = slot_records(b, slot);
 	if (flags & JSMPEG_B200_OUT_MACROBLOCKS) {
 		reserve_entries(b, s);
-		r.entry(t, e.picture_type, set.entries.data());
+		r.entry(sr, s.seq.mb_size, e.picture_type, set.entries.data());
 	}
-	if (to && to->mb) r.entry(t, e.picture_type, to->mb);
-	if (to && to->coef) r.coef(slot_records(b, slot), s.seq.mb_size, to->coef);
+	if (to && to->mb) r.entry(sr, s.seq.mb_size, e.picture_type, to->mb);
+	if (to && to->coef) r.coef(sr, s.seq.mb_size, to->coef);
 	uint2 *acc = to ? to->acc : nullptr;  // (only under OUT_ACCUMULATED)
 	if (!is_b) {  // the map beside the set (or in its map frame), one depth step from the forward set's picture's map
 		if (flags & JSMPEG_B200_OUT_ACCUMULATED) {
 			reserve_maps(s);
 			const StreamSet &fwd = s.sets[s.cur];  // (swapped above)
 			const uint2 *prev = !fwd.map_written ? nullptr : fwd.map_at ? fwd.map_at : fwd.map.data();
-			r.map(slot_records(b, slot), s.seq, prev, acc ? acc : set.map.data());
+			r.map(sr, s.seq, prev, acc ? acc : set.map.data());
 		}
 		set.map_written = (flags & JSMPEG_B200_OUT_ACCUMULATED) != 0;
 		set.map_at = acc;
@@ -1807,11 +1818,16 @@ uint32_t seek_start(const Batch *b, const Stream &s, const IndexEntry &e) {
 	return e.pic;
 }
 
-// The checks of a random-access call's requests that name no destination, all before anything changes: the arrays
-// are there; every request names a stream with a sequence header and a picture of its `what` listing.  Fills `req`
-// (with the chain starts) and returns true, or returns false.
+// The checks of a random-access call's requests, all before anything changes: the arrays are there; every request
+// names a stream with a sequence header and a picture of its `what` listing; and the first `n_dst` of the destination
+// arrays -- `dst` (seek_pictures has none) and an optional second one, `dst2` (decode_intra and decode_pictures under
+// OUT_RGBA: the images; the exports: mb_dst) -- are there with every destination 16-byte aligned (stage 2 and the
+// exports store 8 and 16 bytes at a time).  Fills `req` (with the chain starts) and returns true, or returns false.
 bool check_requests(Batch *b, Listing what, int n, const int *streams, const uint32_t *pictures,
-                    std::vector<PictureRequest> &req) {
+                    std::vector<PictureRequest> &req, int n_dst = 0, void *const *dst = nullptr, void *const *dst2 = nullptr) {
+	void *const *const arrays[2] = {dst, dst2};
+	for (int k = 0; k < n_dst; k++)
+		if (n > 0 && !arrays[k]) return false;
 	use_device(b);
 	if (n < 0 || (n > 0 && (!streams || !pictures))) return false;
 	upload_all(b);
@@ -1830,18 +1846,9 @@ bool check_requests(Batch *b, Listing what, int n, const int *streams, const uin
 		if (e == listed[si].end() || e->pic != pictures[i]) return false;
 		req[i] = {si, pictures[i], e->chain_start};
 	}
-	return true;
-}
-
-// ... and of those that name one: besides, `dst` is there and every destination, and with `rgba` its image, is
-// 16-byte aligned (stage 2 stores 8 and 16 bytes at a time)
-bool check_requests(Batch *b, Listing what, int n, const int *streams, const uint32_t *pictures, void *const *dst,
-                    void *const *rgba_dst, bool rgba, std::vector<PictureRequest> &req) {
-	if (n > 0 && (!dst || (rgba && !rgba_dst))) return false;
-	if (!check_requests(b, what, n, streams, pictures, req)) return false;
-	auto aligned = [](const void *p) { return p && ((uintptr_t)p & 15u) == 0; };
-	for (int i = 0; i < n; i++)
-		if (!aligned(dst[i]) || (rgba && !aligned(rgba_dst[i]))) return false;
+	for (int k = 0; k < n_dst; k++)
+		for (int i = 0; i < n; i++)
+			if (!arrays[k][i] || ((uintptr_t)arrays[k][i] & 15u) != 0) return false;
 	return true;
 }
 
@@ -1850,23 +1857,29 @@ long batch_decode_chosen(Batch *b, bool intra, int n, const int *streams, const 
                          void *const *rgba_dst, int flags, int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
 	const bool rgba = (flags & JSMPEG_B200_OUT_RGBA) != 0;
 	std::vector<PictureRequest> req;
-	if (!check_requests(b, intra ? Listing::Intra : Listing::Pictures, n, streams, pictures, planes_dst, rgba_dst, rgba, req))
-		return -2;
+	const Listing what = intra ? Listing::Intra : Listing::Pictures;
+	if (!check_requests(b, what, n, streams, pictures, req, rgba ? 2 : 1, planes_dst, rgba_dst)) return -2;
 	if (n == 0) return 0;
 	decode_chains(b, req, planes_dst, rgba_dst, rgba, status_out, n_present_out, error_out);
 	return n;
 }
 
-// ---- decode_macroblocks: the walks' records of chosen pictures of any streams, in the public layout (DESIGN 3.8) ----
+// ---- decode_macroblocks, decode_coefficients, decode_residuals: the walks' records of chosen pictures of any streams,
+// in the public layouts (DESIGN 3.8, 3.9, 3.10) ----
+
+// What an export call writes into its required destinations
+enum class Export { Macroblocks, Coefficients, Residuals };
 
 // Each unique (stream, picture) of the requests takes a record slot; waves of as many as there are free slots (after
-// flushing the look-ahead when they do not cover the call) run the walks alone -- or, with `coef_dst` (decode_coefficients,
-// DESIGN 3.9) or `res_dst` (decode_residuals, DESIGN 3.10), the walks and the expand -- and one export launch per wave
-// and destination kind, on the main stream behind stage 1 and before the slots are released, writes every request of
-// the wave to its destination: `dst` (may be nullptr) gets the macroblock entries, `coef_dst` (nullptr: none) the
-// coefficients, `res_dst` (nullptr: none) the residuals.  The requests are valid (the caller checked them).
-void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *const *dst, void *const *coef_dst,
-                        void *const *res_dst, int32_t *n_present_out, int32_t *error_out) {
+// flushing the look-ahead when they do not cover the call) run the walks alone -- or, for coefficients and residuals,
+// the walks and the expand.  Each wave is then one stage-2 step without reconstruct tasks (run_steps): one export
+// launch per destination kind, on the reconstruct stream behind the wave (ev_b), writes every request of the wave to
+// its destination.  `dst` gets what `what` names; `mb_dst` (nullptr: none) gets the macroblock entries too.  The
+// slots go back right after: the next wave's stage 1 waits for ev_round, so it rewrites them (records, dense records
+// and -- through its walks and expands -- the compact planes) only after the exports read them.  The requests are
+// valid (the caller checked them).
+void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, Export what, void *const *dst,
+                        void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
 	const int n = (int)req.size();
 	ensure_pool(b);
 	std::vector<std::pair<int, uint32_t>> uniq(n);
@@ -1877,87 +1890,42 @@ void decode_macroblocks(Batch *b, const std::vector<PictureRequest> &req, void *
 	for (int i = 0; i < n; i++)
 		uniq_of[i] = std::lower_bound(uniq.begin(), uniq.end(), std::make_pair(req[i].stream, req[i].pic)) - uniq.begin();
 	free_slots_for(b, uniq.size());
-	if (dst) reserve_tasks(b->h_xtasks, b->d_xtasks, n, b->st_main);
-	if (coef_dst) reserve_tasks(b->h_ctasks, b->d_ctasks, n, b->st_main);
-	if (res_dst) reserve_tasks(b->h_rtasks, b->d_rtasks, n, b->st_main);
+	void *const *entries_dst = what == Export::Macroblocks ? dst : mb_dst;
 	const size_t wave_max = b->free_slots.size();
 	RequestInfo out(n);
 	for (size_t lo = 0; lo < uniq.size(); lo += wave_max) {
 		const size_t hi = std::min(uniq.size(), lo + wave_max);
 		std::vector<WaveItem> wave;
 		for (size_t u = lo; u < hi; u++) wave.push_back(take_slot(b, uniq[u].first, uniq[u].second, true));
-		// (parse_wave waits for the infos, which also means the previous wave's task uploads have read the task tables)
-		parse_wave(b, wave, coef_dst != nullptr || res_dst != nullptr);
-		int m = 0;
-		uint32_t total = 0, res_warps = 0;
-		for (int i = 0; i < n; i++) {
+		parse_wave(b, wave, what != Export::Macroblocks);
+		std::vector<ReconStep> steps(1);
+		for (int i = 0; i < n; i++) {  // in request order: a duplicate gets tasks of its own
 			if (uniq_of[i] < lo || uniq_of[i] >= hi) continue;
 			const WaveItem &w = wave[uniq_of[i] - lo];
 			const picture_info_t &info = b->h_info[uniq_of[i] - lo];
 			out.set(i, info);
 			const SeqParams &seq = b->streams[w.stream].seq;
-			const int mb_size = seq.mb_size;
 			const SlotRecords sr = slot_records(b, w.slot);
-			if (dst) b->h_xtasks[m] = MbExportTask{sr.hdr, dst[i], total, mb_size, info.picture_type, 0};
-			if (coef_dst) b->h_ctasks[m] = CoefExportTask{sr.hdr, sr.coef, sr.compact, coef_dst[i], total, mb_size};
-			if (res_dst) {
-				b->h_rtasks[m] = ResExportTask{sr.hdr, sr.coef, sr.compact, static_cast<int16_t *>(res_dst[i]), res_warps,
-				                               seq.mb_width, seq.mb_height, 0};
-				res_warps += res_export_warps(mb_size);
-			}
-			m++;
-			total += (uint32_t)mb_size;
+			if (entries_dst) steps[0].entry(sr, seq.mb_size, info.picture_type, entries_dst[i]);
+			if (what == Export::Coefficients) steps[0].coef(sr, seq.mb_size, dst[i]);
+			if (what == Export::Residuals) steps[0].residual(sr, seq, static_cast<int16_t *>(dst[i]));
 		}
-		if (dst) {
-			CUDA_CHECK(cudaMemcpyAsync(b->d_xtasks.data(), b->h_xtasks.data(), m * sizeof(MbExportTask), cudaMemcpyHostToDevice, b->st_main));
-			launch_export_macroblocks(b->d_xtasks.data(), m, total, b->st_main);
-		}
-		if (coef_dst) {
-			CUDA_CHECK(cudaMemcpyAsync(b->d_ctasks.data(), b->h_ctasks.data(), m * sizeof(CoefExportTask), cudaMemcpyHostToDevice, b->st_main));
-			launch_export_coefficients(b->d_ctasks.data(), m, total, b->st_main);
-		}
-		if (res_dst) {
-			CUDA_CHECK(cudaMemcpyAsync(b->d_rtasks.data(), b->h_rtasks.data(), m * sizeof(ResExportTask), cudaMemcpyHostToDevice, b->st_main));
-			launch_export_residuals(b->d_rtasks.data(), m, res_warps, b->st_main);
-		}
-		// Released right behind the exports, which read the slots on st_main: the next wave's stage 1 rewrites them
-		// (records, dense records and -- through its walks and expands -- the compact planes) only after them.  Its
-		// kernels on st_main queue behind the exports; those on the side streams (parse_wave's st_side, and the size
-		// groups of launch_parse_pictures) start from an event recorded on st_main after them (ev_sfork, fork.fork).
+		run_steps(b, steps, false);
 		for (const WaveItem &w : wave) release_slot(b, w.slot);
 	}
-	CUDA_CHECK(cudaStreamSynchronize(b->st_main));
+	CUDA_CHECK(cudaStreamSynchronize(b->st_recon));
+	b->recon_pending = false;
 	out.copy_out(nullptr, n_present_out, error_out);
 }
 
-long batch_decode_macroblocks(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *mb_dst,
-                              int32_t *n_present_out, int32_t *error_out) {
+// The export calls' requests: pictures of the macroblock index, with the required destinations `dst` and the optional
+// `mb_dst` (decode_coefficients, decode_residuals) checked as decode_pictures' are
+long batch_decode_macroblocks(Batch *b, Export what, int n, const int *streams, const uint32_t *pictures, void *const *dst,
+                              void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
 	std::vector<PictureRequest> req;
-	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, mb_dst, nullptr, false, req)) return -2;
+	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, req, mb_dst ? 2 : 1, dst, mb_dst)) return -2;
 	if (n == 0) return 0;
-	decode_macroblocks(b, req, mb_dst, nullptr, nullptr, n_present_out, error_out);
-	return n;
-}
-
-// decode_coefficients: decode_macroblocks' requests and schedule with stage 1b on and the coefficient export
-// (DESIGN 3.9); mb_dst, when given, is checked as decode_macroblocks' destinations are
-long batch_decode_coefficients(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *coef_dst,
-                               void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
-	std::vector<PictureRequest> req;
-	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, coef_dst, mb_dst, mb_dst != nullptr, req)) return -2;
-	if (n == 0) return 0;
-	decode_macroblocks(b, req, mb_dst, coef_dst, nullptr, n_present_out, error_out);
-	return n;
-}
-
-// decode_residuals: decode_coefficients' requests and schedule with the residual export in place of the coefficient
-// export (DESIGN 3.10)
-long batch_decode_residuals(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *res_dst,
-                            void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
-	std::vector<PictureRequest> req;
-	if (!check_requests(b, Listing::Macroblocks, n, streams, pictures, res_dst, mb_dst, mb_dst != nullptr, req)) return -2;
-	if (n == 0) return 0;
-	decode_macroblocks(b, req, mb_dst, nullptr, res_dst, n_present_out, error_out);
+	decode_macroblocks(b, req, what, dst, mb_dst, n_present_out, error_out);
 	return n;
 }
 
@@ -2020,7 +1988,7 @@ void decode_accumulated(Batch *b, const std::vector<PictureRequest> &req, void *
 long batch_decode_accumulated(Batch *b, int n, const int *streams, const uint32_t *pictures, void *const *acc_dst,
                               int32_t *status_out, int32_t *n_present_out, int32_t *error_out) {
 	std::vector<PictureRequest> req;
-	if (!check_requests(b, Listing::Accumulated, n, streams, pictures, acc_dst, nullptr, false, req)) return -2;
+	if (!check_requests(b, Listing::Accumulated, n, streams, pictures, req, 1, acc_dst)) return -2;
 	std::map<std::pair<int, uint32_t>, uint32_t> chain_last;  // per (stream, chain start): the last picture requested
 	for (const PictureRequest &r : req) {
 		uint32_t &last = chain_last[{r.stream, r.from}];
@@ -2682,14 +2650,16 @@ long jsmpeg_b200_batch_macroblock_index(jsmpeg_b200_batch_t *b, int stream, uint
 
 long jsmpeg_b200_batch_decode_macroblocks(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
                                           void *const *mb_dst, int32_t *n_present_out, int32_t *error_out) {
-	return guarded<long>(b, -1, [&] { return batch_decode_macroblocks(b, n, streams, pictures, mb_dst, n_present_out, error_out); });
+	return guarded<long>(b, -1, [&] {
+		return batch_decode_macroblocks(b, Export::Macroblocks, n, streams, pictures, mb_dst, nullptr, n_present_out, error_out);
+	});
 }
 
 long jsmpeg_b200_batch_decode_coefficients(jsmpeg_b200_batch_t *b, int n, const int *streams, const uint32_t *pictures,
                                            void *const *coef_dst, void *const *mb_dst, int32_t *n_present_out,
                                            int32_t *error_out) {
 	return guarded<long>(b, -1, [&] {
-		return batch_decode_coefficients(b, n, streams, pictures, coef_dst, mb_dst, n_present_out, error_out);
+		return batch_decode_macroblocks(b, Export::Coefficients, n, streams, pictures, coef_dst, mb_dst, n_present_out, error_out);
 	});
 }
 
@@ -2697,7 +2667,7 @@ long jsmpeg_b200_batch_decode_residuals(jsmpeg_b200_batch_t *b, int n, const int
                                         void *const *res_dst, void *const *mb_dst, int32_t *n_present_out,
                                         int32_t *error_out) {
 	return guarded<long>(b, -1, [&] {
-		return batch_decode_residuals(b, n, streams, pictures, res_dst, mb_dst, n_present_out, error_out);
+		return batch_decode_macroblocks(b, Export::Residuals, n, streams, pictures, res_dst, mb_dst, n_present_out, error_out);
 	});
 }
 
