@@ -60,7 +60,8 @@ def describe(lib, es):
 # the CPU tests that compare with the reference record their own streams when run with JSMPEG_RECORD_REFERENCE=1
 RECORDING_TESTS = ["test_oracle_vs_reference.py", "test_unit_parity.py", "test_vlc_tables.py", "test_rgba_cases.py",
                    "test_bench_contract.py", "test_b_pictures.py::test_extension_off_b_pictures_are_consumed_and_not_decoded",
-                   "test_motion_domain.py::test_oracle_equals_the_compiled_reference"]
+                   "test_motion_domain.py::test_oracle_equals_the_compiled_reference",
+                   "test_geometry_domain.py::test_oracle_equals_the_compiled_reference"]
 
 
 def gpu_test_streams():

@@ -40,6 +40,7 @@ CBP_CODE = _inv(V.CODE_BLOCK_PATTERN)
 MOTION_CODE = _inv(V.MOTION)
 DC_LUMA_CODE = _inv(V.DCT_DC_SIZE_LUMINANCE)
 DC_CHROMA_CODE = _inv(V.DCT_DC_SIZE_CHROMINANCE)
+MAX_SLICE_ROW = 0xAF - 1  # the last macroblock row a slice start code (0x01..0xAF) names
 MAX_LEVEL_FOR_RUN = {}
 for (_r, _l) in V.DCT_RUN_LEVEL_CODE:
     MAX_LEVEL_FOR_RUN[_r] = max(MAX_LEVEL_FOR_RUN.get(_r, 0), _l)
@@ -135,6 +136,13 @@ class Knobs:
         self.escape_forms = "canonical"
         self.qscales = None
         self.matrix_entries = None
+        # How the bits spread over the picture (GEOMETRY_CASES).  None draws exactly what it always drew.
+        #   "letterbox"  the first and last `bar` of the macroblock rows (a (top, bottom) pair: each its own share) are
+        #                black bars: DC-only intra macroblocks of about 30 bits in I pictures, skipped runs and
+        #                zero-vector uncoded macroblocks in P pictures
+        #   "flat"       the whole picture is bar (a fade to black)
+        self.profile = None
+        self.bar = 0.12
         self.__dict__.update(kw)
         assert self.dc_limit + 255 < 1 << 23  # the reference keeps dc << 8 in an int
 
@@ -497,6 +505,10 @@ class SynthStream:
             else:
                 data = self._slice_once(w, ptype, first_mb, last_mb, f_code, full_pel)
             body = data[4:]
+            # the decoder ends a slice where the next whole byte starts a start code (buffer.c:101-110): a last
+            # macroblock that begins in the slice's final byte would never be read
+            if (self.last_mb_bit + 7) // 8 >= len(data):
+                continue
             bad = any(body[i] == 0 and body[i + 1] == 0 and body[i + 2] <= 1 for i in range(len(body) - 2))
             if not bad and not (len(body) >= 2 and body[-1] == 0 and body[-2] == 0) and not (len(body) >= 1 and body[-1] == 0):
                 return data
@@ -523,13 +535,20 @@ class SynthStream:
         while mb <= last_mb:
             inc = mb - addr
             skipped = 0
+            if self.in_bar(mb):
+                mb, addr, first, dc, prev_h, prev_v = self._bar_macroblock(w, ptype, mb, addr, first, last_mb, dc, prev_h,
+                                                                          prev_v, f, r_size)
+                continue
             if not first and ptype == 2 and rng.random() < self.k.skip_prob and mb < last_mb:
                 skipped = int(min(rng.integers(1, self.k.max_skip + 1), last_mb - mb))
+                while skipped and self.in_bar(mb + skipped):  # (a bar's macroblocks are coded as bars)
+                    skipped -= 1
                 mb += skipped
                 inc = mb - addr
             if skipped:
                 dc = [128, 128, 128]
                 prev_h = prev_v = 0
+            self.last_mb_bit = len(w.bits)
             self.address_increment(w, inc)
             addr = mb
             first = False
@@ -570,6 +589,48 @@ class SynthStream:
         w.align()
         return w.tobytes()
 
+    def in_bar(self, mb):
+        """Whether macroblock `mb` lies in a black bar of Knobs.profile"""
+        if self.k.profile is None:
+            return False
+        if self.k.profile == "flat":
+            return True
+        top, bottom = self.k.bar if isinstance(self.k.bar, tuple) else (self.k.bar, self.k.bar)
+        row = mb // self.mbw
+        return row < round(top * self.mbh) or row >= self.mbh - round(bottom * self.mbh)
+
+    def _bar_macroblock(self, w, ptype, mb, addr, first, last_mb, dc, prev_h, prev_v, f, r_size):
+        """A black-bar macroblock at `mb` (after a skipped run through the bar in P pictures): intra and DC-only near
+        black in I pictures, a zero vector without coded blocks in P pictures.  Returns the slice state after it."""
+        rng = self.rng
+        if ptype == 2 and not first and mb < last_mb and rng.random() < 0.8:
+            run = 1
+            while run < 4 * self.mbw and mb + run < last_mb and self.in_bar(mb + run):
+                run += 1
+            mb += int(rng.integers(1, run + 1))
+            dc = [128, 128, 128]
+            prev_h = prev_v = 0
+        self.last_mb_bit = len(w.bits)
+        self.address_increment(w, mb - addr)
+        if ptype == 1:
+            w.code(TYPE_I_CODE[0x01])
+            for blk in range(6):
+                which = 0 if blk < 4 else blk - 3
+                target = (16 if blk < 4 else 128) + (int(rng.integers(0, 3)) if rng.random() < 0.2 else 0)
+                diff = target - dc[which]
+                size = 0 if diff == 0 else abs(diff).bit_length()
+                w.code((DC_LUMA_CODE if blk < 4 else DC_CHROMA_CODE)[size])
+                if size:
+                    w.put(diff if diff > 0 else diff + (1 << size) - 1, size)
+                dc[which] = target
+                w.code(V.DCT_EOB_CODE)
+        else:
+            w.code(TYPE_P_CODE[0x08])
+            prev_h = self.motion_component(w, 0, prev_h, f, r_size)
+            prev_v = self.motion_component(w, 0, prev_v, f, r_size)
+            dc = [128, 128, 128]
+        return mb + 1, mb, False, dc, prev_h, prev_v
+
     def _slice_once_b(self, w, first_mb, last_mb, f_code, full_pel, f_code_b, full_pel_b):
         """A slice of a B picture (ISO 11172-2 2.4.3.6, 2.4.4.2, 2.4.4.3; types: table B.2d)."""
         rng = self.rng
@@ -604,6 +665,7 @@ class SynthStream:
                 mb += skipped
             if skipped:
                 dc = [128, 128, 128]
+            self.last_mb_bit = len(w.bits)
             self.address_increment(w, mb - addr)
             addr = mb
             first = False
@@ -693,6 +755,11 @@ class SynthStream:
                 at = end + 1
                 if at < total and index >= k.gap_from_picture and rng.random() < k.slice_gap_prob:
                     at = min(total, at + int(rng.integers(1, self.mbw)))
+        if self.mbh > MAX_SLICE_ROW + 1:
+            # slice start codes end at 0xAF (row 174): the slice that starts in the last row a code can name runs to
+            # the picture's end, and a slice that would start further down is not written
+            spans = [s for s in spans if s[0] // self.mbw <= MAX_SLICE_ROW]
+            spans[-1] = (spans[-1][0], total - 1)
         self.out.align()
         for (a, b) in spans:
             self.out.bits.extend(BitWriter_bits(self.slice(ptype, a, b, f_code, full_pel, f_code_b, full_pel_b)))
@@ -806,6 +873,41 @@ VALUE_B_CASES = {
 }
 
 
+# Streams over the picture's geometry and the spread of its bits, I/P and every macroblock coded: from one macroblock
+# (one lane of the lane walk) and a 1x1 display to 4095x4095 (256 x 256 macroblocks, the bit fields' whole range);
+# 256 one-macroblock rows; 250 rows, where the slice that starts in row 174 (code 0xAF, the last) spans the rest; and
+# letterboxed pictures whose black bars -- many short macroblocks -- overflow a lane's share of the lane walk's staging
+# area, so that it stores its records in a second pass.  The compiled reference decodes the cases whose taps all stay
+# inside the planes (GEOMETRY_REFERENCE_CASES): tests/golden/reference/decodes.json holds its decodes of them.
+_LETTERBOX = dict(pictures=3, gop=2, slices="one", profile="letterbox", bar=0.12)
+GEOMETRY_CASES = {
+    "geo_1mb": dict(knobs=dict(width=16, height=16, pictures=8, gop=4, slices="one", f_codes=(1, 2, 3), vectors="mixed"), seed=61),
+    "geo_1x1": dict(knobs=dict(width=1, height=1, pictures=6, gop=3, slices="one"), seed=62),
+    "geo_column": dict(knobs=dict(width=16, height=4095, pictures=4, gop=2, slices="rows", f_codes=(1, 2, 3), vectors="wrap"), seed=63),
+    "geo_row": dict(knobs=dict(width=4095, height=16, pictures=6, gop=3, slices="random", f_codes=(1, 3, 5)), seed=64),
+    "geo_max": dict(knobs=dict(width=4095, height=4095, pictures=2, gop=2, slices="one", max_coefs=4, skip_prob=0.05), seed=65),
+    "geo_tall_rows": dict(knobs=dict(width=336, height=4000, pictures=3, gop=2, slices="rows", max_coefs=6), seed=66),
+    "geo_odd_4k": dict(knobs=dict(width=4070, height=2303, pictures=2, gop=2, slices="random", max_coefs=4, skip_prob=0.05), seed=67),
+    "geo_letterbox_720p": dict(knobs=dict(width=1280, height=720, **_LETTERBOX), seed=68),
+    "geo_letterbox_1080p": dict(knobs=dict(width=1920, height=1088, **_LETTERBOX), seed=69),
+    # all the detail in the first macroblock row, dense enough that the bars below fill whole lanes
+    "geo_letterbox_qcif": dict(knobs=dict(width=176, height=144, **dict(_LETTERBOX, bar=(0.0, 0.9)), max_coefs=63,
+                                          dc_only_prob=0.0), seed=70),
+    "geo_flat_1080p": dict(knobs=dict(width=1920, height=1080, pictures=3, gop=2, slices="one", profile="flat"), seed=71),
+}
+# B-picture twins (decode_b) of the smallest and the most lopsided pictures
+GEOMETRY_B_CASES = {
+    "geo_1mb_b": dict(knobs=dict(width=16, height=16, pictures=10, gop=2, slices="one", b_frames=2, f_codes=(1, 2, 3),
+                                 b_f_codes=(1, 2, 3), vectors="mixed"), seed=72),
+    "geo_column_b": dict(knobs=dict(width=16, height=4095, pictures=7, gop=2, slices="rows", b_frames=2, f_codes=(1, 2),
+                                    b_f_codes=(1, 2), vectors="wrap", b_skip_prob=0.35), seed=73),
+    "geo_row_b": dict(knobs=dict(width=4095, height=16, pictures=7, gop=2, slices="random", b_frames=2, f_codes=(1, 3),
+                                 b_f_codes=(2, 4)), seed=74),
+}
+# the I/P cases the compiled reference decodes: every tap inside its planes ("outside" taps read the reference's heap)
+GEOMETRY_REFERENCE_CASES = sorted(n for n, c in GEOMETRY_CASES.items() if c["knobs"].get("vectors") != "mixed")
+
+
 def value_repro():
     """A 96x16 I picture, one slice, quantiser scale 31, six intra macroblocks whose luma DC differentials are all
     +255: the Y predictor is 128 + 17 * 255 = 4463 at block 0 of macroblock 4, which also carries escapes of level -255
@@ -841,7 +943,8 @@ def value_repro():
 def make_case(name):
     if name == "val_repro_96x16":
         return value_repro()
-    spec = next(c[name] for c in (CASES, B_CASES, VECTOR_CASES, VALUE_CASES, VALUE_B_CASES) if name in c)
+    spec = next(c[name] for c in (CASES, B_CASES, VECTOR_CASES, VALUE_CASES, VALUE_B_CASES, GEOMETRY_CASES, GEOMETRY_B_CASES)
+                if name in c)
     return SynthStream(Knobs(**spec["knobs"]), spec["seed"]).generate()
 
 
