@@ -160,6 +160,17 @@ static napi_value js_set_export_macroblocks(napi_env env, napi_callback_info inf
 	jsmpeg_b200_decoder_set_option(d, "macroblocks", (int)on);
 	return NULL;
 }
+/* Extension: setConceal(decoder, on) switches the decoder's "conceal" option: each macroblock a damaged picture lacks
+ * gets the co-located samples of the picture it predicts from. */
+static napi_value js_set_conceal(napi_env env, napi_callback_info info) {
+	napi_value argv[2];
+	uint32_t on = 0;
+	mpeg1_decoder_t *d = decoder_arg(env, info, 2, argv);
+	if (!d) return NULL;
+	napi_get_value_uint32(env, argv[1], &on);
+	jsmpeg_b200_decoder_set_option(d, "conceal", (int)on);
+	return NULL;
+}
 static napi_value js_macroblocks(napi_env env, napi_callback_info info) {
 	napi_value argv[1];
 	mpeg1_decoder_t *d = decoder_arg(env, info, 1, argv);
@@ -181,6 +192,7 @@ static napi_value init(napi_env env, napi_value exports) {
 		{"decode", js_decode}, {"planes", js_planes},
 		{"setDecodeB", js_set_decode_b}, {"lastPictureType", js_last_picture_type},
 		{"setExportMacroblocks", js_set_export_macroblocks}, {"macroblocks", js_macroblocks},
+		{"setConceal", js_set_conceal},
 	};
 	for (size_t i = 0; i < sizeof(table) / sizeof(table[0]); i++) {
 		napi_value fn;

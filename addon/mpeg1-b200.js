@@ -28,6 +28,10 @@ var MPEG1B200 = function(options) {
 	// last decode() rendered (motion detection, overlays) without walking the picture a second time
 	this.exportMacroblocks = !!options.exportMacroblocks;
 	if (this.exportMacroblocks) { native.setExportMacroblocks(this.decoder, 1); }
+	// extension: with concealErrors, each macroblock a damaged picture lacks gets the co-located samples of the picture
+	// it predicts from, instead of keeping what the plane held two pictures ago
+	this.concealErrors = !!options.concealErrors;
+	if (this.concealErrors) { native.setConceal(this.decoder, 1); }
 	this.held = null;
 	this.decodeFirstFrame = options.decodeFirstFrame !== false;
 	this.hasSequenceHeader = false;

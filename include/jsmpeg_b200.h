@@ -123,7 +123,23 @@ const char *jsmpeg_b200_batch_last_error(jsmpeg_b200_batch_t *b);
  * decoded after ISO/IEC 11172-2 from the two most recent I/P pictures; decode() still consumes pictures in
  * CODED order, the planes of a B picture are what get_planes / get_host_planes / the reference ABI's
  * get_{y,cr,cb}_ptr return after it, and jsmpeg_b200_batch_last_picture tells type and temporal_reference so
- * that a player can put pictures into display order.  No reference implementation exists for this part. */
+ * that a player can put pictures into display order.  No reference implementation exists for this part.
+ * "conceal" (default 0): ERROR CONCEALMENT.  When a picture's walk stops at an invalid code, or a slice is lost, the
+ * macroblocks it did not reach are not decoded; by default (like the reference) they keep whatever their plane set
+ * held, which is the picture two references back (for a B picture: the B picture two B pictures back).  With 1,
+ * before a picture is reconstructed every macroblock whose record is not PRESENT gets the co-located samples of the
+ * picture's forward reference -- 16x16 luma and 8x8 Cr and Cb, zero motion, a plain copy: for an I or P picture the
+ * stream's newest I/P picture before it (for an I picture, what a P picture in its place would predict from), for a
+ * B picture its forward (past) reference.  A PRESENT macroblock, even one whose walk stopped inside a block, is not
+ * touched.  What follows from the planes follows the concealed content: get_planes, the host ring, RGBA, frames of
+ * decode_frames*, decode_pictures and seek_pictures, and every picture predicted from it later.  A picture of
+ * decode_pictures / decode_intra that is its own chain has no forward reference (a zeroed set), so its absent
+ * macroblocks stay 0 either way.  The records define the exports, so these do NOT change: macroblock entries
+ * (OUT_MACROBLOCKS, decode_macroblocks), coefficients, residuals (0 for an absent macroblock) and accumulated maps
+ * (absent samples stay untraced).  A picture whose walk met no invalid code, counted the picture's macroblocks and
+ * whose slices never go back to an earlier row adds no work; for the others one copy launch per reconstruct step runs
+ * before it (counted in kernel_launches).  Records do not
+ * depend on the option: it takes effect from the next reconstruct step.  jsmpeg_b200_decoder_set_option forwards it. */
 int jsmpeg_b200_batch_set_option(jsmpeg_b200_batch_t *b, const char *name, int value);
 
 /* per-stream twins of the reference ABI */
@@ -711,7 +727,8 @@ long jsmpeg_b200_debug_read_es(jsmpeg_b200_batch_t *b, int stream, void *dst, si
 const char *jsmpeg_b200_decoder_last_error(mpeg1_decoder_t *self);
 
 /* jsmpeg_b200_batch_set_option / jsmpeg_b200_batch_last_picture for a decoder of the reference ABI (which has no
- * option call): "decode_b" switches the B-picture extension on, "lookahead" sets the pictures parsed ahead.  The
+ * option call): "decode_b" switches the B-picture extension on, "conceal" error concealment, "lookahead" sets the
+ * pictures parsed ahead.  The
  * decoder's own option "macroblocks" (default 0): with 1, mpeg1_decoder_decode decodes with JSMPEG_B200_OUT_MACROBLOCKS
  * and jsmpeg_b200_decoder_get_macroblocks returns the entries of the picture it rendered (what get_y_ptr shows). */
 int jsmpeg_b200_decoder_set_option(mpeg1_decoder_t *self, const char *name, int value);

@@ -159,7 +159,8 @@ def bind_batch_abi(lib):
 class BatchDecoder:
     """``n_streams`` independent MPEG-1 video decoders on one GPU."""
 
-    def __init__(self, n_streams, device=0, max_slots=0, lib=None, decode_b=None, slice_walk=None):
+    def __init__(self, n_streams, device=0, max_slots=0, lib=None, decode_b=None, slice_walk=None,
+                 conceal=None):
         from . import capi
         self.lib = lib if lib is not None else capi.product_library()
         self.n_streams = n_streams
@@ -182,6 +183,8 @@ class BatchDecoder:
             self.set_option("slice_walk", slice_walk)
         if decode_b is not None:  # the B-picture extension (the reference skips B pictures, and so does the default)
             self.set_option("decode_b", decode_b)
+        if conceal is not None:  # the macroblocks a damaged picture lacks are copied from its forward reference
+            self.set_option("conceal", conceal)
 
     def close(self):
         if self.handle:

@@ -13,7 +13,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["engine.cu", "parse.cu", "recon.cu", "scan.cu", "tsdemux.cu", "psdemux.cu", "macroblocks.cu", "coefficients.cu", "residuals.cu", "accumulate.cu"]
+SOURCES = ["engine.cu", "parse.cu", "recon.cu", "scan.cu", "tsdemux.cu", "psdemux.cu", "macroblocks.cu", "coefficients.cu", "residuals.cu", "accumulate.cu", "conceal.cu"]
 OUT = os.path.join(HERE, "libjsmpeg_b200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 

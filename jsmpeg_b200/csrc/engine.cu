@@ -43,6 +43,7 @@
 #include "bitbuffer.h"
 #include "buffers.h"
 #include "common.cuh"
+#include "conceal.cuh"
 #include "demux.h"
 #include "psdemux.cuh"
 #include "tsdemux.cuh"
@@ -193,6 +194,7 @@ struct jsmpeg_b200_batch_t {
 	int lookahead = 1;
 	bool decode_b = false;       // the B-picture extension: off = B pictures are skipped like the reference does (mpeg1.js:181-184)
 	bool slice_walk = false;     // I/P pictures of >= SLICE_WALK_MIN_SLICES slices go to the one-lane-per-slice walk (walk_slices.cuh)
+	bool conceal = false;        // the macroblocks a decoded picture lacks are copied from its forward set (DESIGN 3.19)
 	// pictures with a walk kernel of their own (B pictures; with "slice_walk", I/P pictures of many slices) are
 	// walked beside the others, on these streams
 	cudaStream_t st_side[2] = {nullptr, nullptr};
@@ -225,6 +227,9 @@ struct jsmpeg_b200_batch_t {
 	DeviceBuffer<ResExportTask> d_rtasks;
 	PinnedBuffer<AccTask> h_atasks;
 	DeviceBuffer<AccTask> d_atasks;
+	// the conceal option's copies (DESIGN 3.19), read on st_recon like the tables above
+	PinnedBuffer<ConcealTask> h_ktasks;
+	DeviceBuffer<ConcealTask> d_ktasks;
 	// decode_accumulated: the pool of the chains' two scratch map sets (DESIGN 3.11)
 	DeviceBuffer<uint8_t> d_map_sets;
 	jsmpeg_b200_stats_t stats{};
@@ -667,15 +672,41 @@ void reserve_tasks(PinnedBuffer<T> &h, DeviceBuffer<T> &d, size_t n, cudaStream_
 	d.reserve(n);
 }
 
+// Whether picture `e` of `s` may lack a macroblock, for the conceal option (DESIGN 3.19).  Every walk counts one per
+// record it writes, so a picture whose walk met no invalid code and counted mb_size lacks one only if it wrote one
+// twice.  A slice that goes back to an earlier row (a slice start code below the one before it) does that; a picture
+// no longer in the stream's listing (its bytes were evicted since it was walked) is taken as one that may.
+bool may_lack_macroblocks(const Stream &s, const picture_info_t &e) {
+	if (e.error != 0 || e.n_present != s.seq.mb_size) return true;
+	const auto at = std::lower_bound(s.pics.begin(), s.pics.end(), e.start_byte - 4);
+	if (at == s.pics.end() || *at != e.start_byte - 4) return true;
+	const size_t pic = at - s.pics.begin();
+	const uint32_t hi = pic + 1 < s.pic_code.size() ? s.pic_code[pic + 1] : (uint32_t)s.codes.size();
+	int last = 0;  // the slice start code before (0: none yet)
+	for (uint32_t k = s.pic_code[pic] + 1; k < hi; k++) {
+		const uint32_t q = s.codes[k];
+		if (q + 3u >= s.bb.length) break;
+		const int code = s.bb.bytes[q + 3u];
+		if (!last && (code == 0xB2 || code == 0xB5)) continue;  // extension and user data before the first slice
+		if (code < 0x01 || code > 0xAF) break;                   // (the picture ends at any other start code)
+		if (code < last) return true;
+		last = code;
+	}
+	return false;
+}
+
 // One step of stage 2 (run_steps): the reconstruct tasks of one step of decode() (or one depth of run_chains), queued
 // by launch_reconstruct; the export of macroblock entries (OUT_MACROBLOCKS, decode_macroblocks: `entries`, one launch
 // of export_macroblocks_kernel over `entry_mb` macroblocks); accumulated maps (OUT_ACCUMULATED, decode_accumulated:
 // `maps`, one launch of accumulate_kernel over `map_warps` warps); coefficients (decode_frames_into,
 // decode_coefficients: `coefs`, one launch of export_coefficients_kernel over `coef_mb` macroblocks); residuals
 // (decode_residuals: `residuals`, one launch of export_residuals_kernel over `res_warps` warps); and the copies of its
-// pictures that follow them.  A step of decode_macroblocks' wave has exports and no reconstruct task.
+// pictures that follow them.  A step of decode_macroblocks' wave has exports and no reconstruct task.  With the conceal
+// option, `conceals` (one launch of conceal_kernel over `conceal_mb` macroblocks) runs before the step's reconstruct.
 struct ReconStep {
 	std::vector<ReconTask> tasks;
+	std::vector<ConcealTask> conceals;
+	uint32_t conceal_mb = 0;
 	std::vector<MbExportTask> entries;
 	uint32_t entry_mb = 0;
 	std::vector<AccTask> maps;
@@ -712,9 +743,17 @@ struct ReconStep {
 		residuals.push_back(ResExportTask{sr.hdr, sr.coef, sr.compact, to, res_warps, seq.mb_width, seq.mb_height, 0});
 		res_warps += res_export_warps(seq.mb_size);
 	}
+	// With the conceal option `on`, the copy of the macroblocks picture `e` of `s` lacks from the forward set of its
+	// reconstruct task `t` into its destination set (DESIGN 3.19), queued only for a picture that may lack one
+	// (may_lack_macroblocks): a clean picture costs nothing.
+	void conceal(const ReconTask &t, const Stream &s, const picture_info_t &e, bool on) {
+		if (!on || !may_lack_macroblocks(s, e)) return;
+		conceals.push_back(ConcealTask{t.hdr, t.cur, t.fwd, t.mb_width, t.mb_size, conceal_mb, 0});
+		conceal_mb += (uint32_t)t.mb_size;
+	}
 };
 
-// The tasks `list` of all `steps` (ReconStep::entries, maps, coefs, residuals) go up in one copy on the reconstruct
+// The tasks `list` of all `steps` (ReconStep::entries, maps, coefs, residuals, conceals) go up in one copy on the reconstruct
 // stream, through the pinned table `h` into `d`; returns where each step's tasks begin in `d`.  The previous upload's
 // readers are done before the pinned table is written again: every call ends with its reconstruction complete, and the
 // next wave of run_chains or decode_macroblocks waits for ev_round.
@@ -756,6 +795,7 @@ int run_steps(Batch *b, std::vector<ReconStep> &steps, bool copy_out) {
 	const std::vector<const CoefExportTask *> coefs = upload_step_tasks(b, steps, &ReconStep::coefs, b->h_ctasks, b->d_ctasks);
 	const std::vector<const ResExportTask *> residuals =
 	    upload_step_tasks(b, steps, &ReconStep::residuals, b->h_rtasks, b->d_rtasks);
+	const std::vector<const ConcealTask *> conceals = upload_step_tasks(b, steps, &ReconStep::conceals, b->h_ktasks, b->d_ktasks);
 	CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_b, 0));
 	CUDA_CHECK(cudaEventRecord(b->ev_recon[0], b->st_recon));
 	int launches = 0;
@@ -765,6 +805,10 @@ int run_steps(Batch *b, std::vector<ReconStep> &steps, bool copy_out) {
 		// at least two copy-out launches back: the copy-out recorded two launches ago must be done (the copy stream is
 		// in order, so that covers every earlier one).  The same holds for the set's entries.
 		if (copy_out && b->copy_steps >= 2) CUDA_CHECK(cudaStreamWaitEvent(b->st_recon, b->ev_copied[b->copy_steps & 1], 0));
+		if (!r.conceals.empty()) {  // (it writes the destination sets the reconstruct launch then leaves alone there)
+			launch_conceal(conceals[i], (int)r.conceals.size(), r.conceal_mb, b->st_recon);
+			launches++;
+		}
 		if (!r.tasks.empty()) launches += launch_reconstruct(r.tasks.data(), (int)r.tasks.size(), b->st_recon);
 		if (!r.entries.empty()) {
 			launch_export_macroblocks(entries[i], (int)r.entries.size(), r.entry_mb, b->st_recon);
@@ -1083,6 +1127,7 @@ uint64_t consume_picture(Batch *b, Stream &s, std::vector<ReconStep> &steps, siz
 	StreamSet &set = s.sets[s.last];
 	if (steps.size() <= step) steps.emplace_back();
 	ReconStep &r = steps[step];
+	r.conceal(t, s, e, b->conceal);
 	r.tasks.push_back(t);
 	newest = {(int)step, (int)r.tasks.size() - 1};
 	const SlotRecords sr = slot_records(b, slot);
@@ -1749,6 +1794,7 @@ struct PlaneWork : ChainWork {
 			t = recon_task(b, s, slot, ch.set[ch.cur], ch.set[1 - ch.cur], nullptr, out_rgba);
 		if (steps.size() <= d) steps.emplace_back();
 		ReconStep &dp = steps[d];
+		dp.conceal(t, s, e, b->conceal && !leaf);  // (a leaf's forward set is the zeroed scratch and its destination is zeroed)
 		dp.tasks.push_back(t);
 		for (int q = q_lo; q < q_hi; q++) {  // the first request gets the picture, duplicates a copy of it
 			if (!leaf || q > q_lo) dp.copy(planes_dst[order[q]], t.cur.y, (size_t)s.coded_size * 3 / 2);
@@ -2423,6 +2469,7 @@ int jsmpeg_b200_batch_set_option(jsmpeg_b200_batch_t *b, const char *name, int v
 	if (!b || !name) return -1;
 	if (!strcmp(name, "lookahead")) { b->lookahead = std::max(1, value); return 0; }
 	if (!strcmp(name, "slice_walk")) { b->slice_walk = value != 0; return 0; }  // (same records either way: nothing to flush)
+	if (!strcmp(name, "conceal")) { b->conceal = value != 0; return 0; }  // (stage 2 only: from the next reconstruct step)
 	if (!strcmp(name, "decode_b")) {
 		if (b->decode_b != (value != 0))
 			for (auto &st : b->streams) flush_cache(b, st);  // what was parsed ahead was parsed under the other rule

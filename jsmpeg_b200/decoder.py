@@ -9,7 +9,9 @@
                    temporal_reference; with `displayOrder` the destination gets them in DISPLAY order: an I/P
                    picture is held back (a copy) until the next I/P picture arrives, `flush()` renders the last;
                    `exportMacroblocks`: `macroblocks()` gives the macroblock types and motion vectors of the
-                   picture the last decode() rendered)
+                   picture the last decode() rendered; `concealErrors`: each macroblock a damaged picture lacks
+                   gets the co-located samples of the picture it predicts from, instead of keeping what the plane
+                   held two pictures ago)
     connect(destination) / destroy()
     bufferGetIndex() / bufferSetIndex(i) / bufferWrite(buffers)
     write(pts, buffers) / seek(time) / decode() -> bool
@@ -80,6 +82,12 @@ class MPEG1Video:
             if not hasattr(self.functions, "jsmpeg_b200_decoder_get_macroblocks"):
                 raise ValueError("exportMacroblocks: this library has no macroblock export")
             self.functions.jsmpeg_b200_decoder_set_option(self.decoder, b"macroblocks", 1)
+        self.concealErrors = bool(options.get("concealErrors"))
+        if self.concealErrors:
+            if not hasattr(self.functions, "jsmpeg_b200_decoder_set_option") or \
+                    self.functions.jsmpeg_b200_decoder_set_option(self.decoder, b"conceal", 1) != 0:
+                self.destroy()
+                raise ValueError("concealErrors: this library has no error concealment")
 
     # ---- src/decoder.js:19-35 / src/mpeg1-wasm.js:32-50
     def destroy(self):

@@ -14,7 +14,7 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "jsmpeg_b200", "csrc")
-FILES = ("parse.cu", "recon.cu", "scan.cu", "tsdemux.cu", "psdemux.cu", "macroblocks.cu", "coefficients.cu", "residuals.cu", "accumulate.cu")
+FILES = ("parse.cu", "recon.cu", "scan.cu", "tsdemux.cu", "psdemux.cu", "macroblocks.cu", "coefficients.cu", "residuals.cu", "accumulate.cu", "conceal.cu")
 
 
 def kernel_hashes(cu, csrc=CSRC, flags=()):
